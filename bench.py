@@ -1,6 +1,6 @@
-"""bench.py - frame-pairs/sec of the adversarial train step at 256x448 (BASELINE.json metric) on N B200s.
+"""bench.py - frame-pairs/sec of the adversarial train step at 256x448 (BASELINE.json metric) on N H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload train|gen_fwd|ensemble]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload train|gen_fwd|ensemble] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 Headline workload `train` (BASELINE.json configs[1]/[2]): DAVIS2016-shaped adversarial training, 4 frame pairs per GPU, PWC-Net at
@@ -13,6 +13,8 @@ Other arms (not the headline; BASELINE.json configs[0] and configs[4]):
   --workload ensemble   multi-crop ensemble inference (test_generator_ensemble.py / generate_buffer_DAVIS2016.sh): per frame pair the
                         four central crops -> PWC-Net 384x640 -> generator at the default 192x384; frames sharded over the ranks
 `--impl reference` times the CPU restatement of the same graph (oracle/; TF 1.13 cannot be installed here) on the host cores.
+`--dump-outputs DIR` writes, after the timed steps, what the timed path computed in its last step as DIR/<name>.npy (float32 /
+float64, a fixed seeded sample where an output is large); inputs and weights are seeded, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -37,7 +39,25 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense bf16; no sustained figure has been measured
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0, 'bf16_tflops_sustained': 989.0}, 'H100 SXM data sheet'
+
+
+def dump_outputs(d, arrays):
+    """--dump-outputs: one .npy per array (float32 / float64), at most 64 MB in all."""
+    import numpy as np
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.ascontiguousarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(d, name + '.npy'), a)
+
+
+def param_sample(params, n=1 << 20, seed=0):
+    """A fixed, seeded sample of n values of every parameter (sorted names, concatenated): 4 MB instead of the 76 MB of all weights."""
+    flat = torch.cat([params[k].detach().float().reshape(-1).cpu() for k in sorted(params)])
+    idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(seed))[:n].sort().values
+    return flat[idx].numpy()
 
 
 class ClockSampler(threading.Thread):
@@ -133,7 +153,7 @@ def run_reference(args):
 
 # ---------------------------------------------------------------------------------------------------- our arm
 def conv_roofline(graph, reps=5):
-    """Dominant kernel FAMILY = the tcgen05 implicit-GEMM convolutions (cis_conv_igemm forward / data gradient and cis_conv_wgrad):
+    """Dominant kernel FAMILY = the wgmma implicit-GEMM convolutions (cis_conv_igemm forward / data gradient and cis_conv_wgrad):
     algorithmic FLOPs of every conv launch of one 1R:3G cycle / CUDA-event time of those launches replayed back to back on the
     launching stream.  Returns (FLOPs per step, ms per step, launches per step)."""
     CONV = ('cis_conv_igemm', 'cis_conv_wgrad')
@@ -245,6 +265,12 @@ def run_ours(args):
     smp = ClockSampler(L.local_rank)
     smp.start()
     ms_dev = timed(dev_step, K)
+    if args.dump_outputs and rank == 0:
+        g.pipeline_drain()
+        torch.cuda.synchronize()
+        full = g.losses(full=True)
+        dump_outputs(args.dump_outputs, {'losses': __import__('numpy').array([full[k] for k in sorted(full)], dtype='float64'),
+                                         'mask': g.mask.float().cpu().numpy(), 'params_sample': param_sample(g.export_params())})
     # ---- end-to-end arm through the public API: pinned host batch -> H2D -> step -> D2H losses
     for i in range(Wm):
         L.step(pool[i % 2], fetch_losses=True, next_batch=pool[(i + 1) % 2])
@@ -276,11 +302,6 @@ def run_ours(args):
     dfl, dms, ddesc = dominant_launch_roofline(g)
     dach = dfl / (dms * 1e-3) / 1e12
     traffic = None
-    try:   # DRAM bytes of the best launch from the committed ncu --set full capture (profiles/r02_ncu_full_summary.json)
-        prof = json.load(open(os.path.join(ROOT, 'profiles', 'r02_ncu_full_summary.json')))['prof_halo128_dominant'][-1]
-        traffic = (float(prof['dram__bytes_read.sum'].split()[0]) + float(prof['dram__bytes_write.sum'].split()[0])) * 1e6
-    except Exception:
-        pass
     try:
         cv, cores, cms = cpu_reference(4, 0)[:3] if not args.no_cpu else (None, 0, 0)
     except Exception as e:  # the CPU leg must never take the GPU number down
@@ -290,20 +311,19 @@ def run_ours(args):
     line = {'metric': METRIC, 'value': value, 'unit': 'frame-pairs/s', 'n_gpus': world, 'steps': K, 'warmup': Wm, 'ms_per_step': step_ms,
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'bf16', 'data': 'synthetic',
             'config': {'workload': WORKLOAD_TRAIN,
-                       'global_batch': gb, 'parallelism': 'dp%d' % world, 'l2': 'per-step working set (activations) exceeds the 126 MB L2',
+                       'global_batch': gb, 'parallelism': 'dp%d' % world, 'l2': 'per-step working set (activations) exceeds the 50 MB L2',
                        'cuda_graph': True, 'ms_per_step_by_kind': by_kind,
                        'flow_net_pipelined': bool(PIPE)},
             'e2e': {'value': e2e, 'unit': 'frame-pairs/s', 'h2d_bytes_per_step': 2 * BPG * 384 * 640 * 3 * 4, 'd2h_bytes_per_step': 32,
                     'ms_per_step': ms_e2e / K},
             'gpu_launches': launches,
             'clocks': smp.summary(),
-            # the dominant kernel family BY TIME SHARE (every tcgen05 conv launch of the step), against the sustained measured peak
-            'roofline': {'bound': 'tensor', 'kernel': 'tcgen05 implicit-GEMM conv family: cis::conv_halo_kernel / conv_igemm_kernel / '
+            # the dominant kernel family BY TIME SHARE (every wgmma conv launch of the step), against the sustained peak
+            'roofline': {'bound': 'tensor', 'kernel': 'wgmma implicit-GEMM conv family: cis::conv_halo_kernel / conv_igemm_kernel / '
                                                       'conv_wgrad_kernel, every launch of a 1R:3G cycle',
                          'achieved': ach, 'peak': pk['bf16_tflops_sustained'], 'unit': 'TFLOP/s', 'frac': ach / pk['bf16_tflops_sustained'],
                          'peak_source': src + ' bf16_tflops_sustained (family timed inside a long replay)', 'traffic': None,
                          'algorithmic_gflop_per_step': fl / 1e9, 'ms_per_step': ms_conv, 'launches_per_step': nconv,
-                         'share_of_summed_kernel_time': 'see profiles/r02_per_op_gpu_times.txt (the step overlaps two streams, so shares of the wall-clock step are not additive)',
                          'whole_step': {'algorithmic_gflop_per_pair_step': GFLOP_PER_PAIR_STEP, 'achieved': step_tflops,
                                         'frac_of_sustained_peak': step_tflops / pk['bf16_tflops_sustained']},
                          'best_launch': {'kernel': ddesc, 'achieved': dach, 'peak': pk['bf16_tflops'], 'frac': dach / pk['bf16_tflops'],
@@ -382,6 +402,9 @@ def run_ours_other(args):
         smp = ClockSampler(local)
         smp.start()
         ms_dev = _timed_events(dev_step, K, barrier)
+        if args.dump_outputs and rank == 0:
+            torch.cuda.synchronize()
+            dump_outputs(args.dump_outputs, {'mask': g.mask.float().cpu().numpy()})
         ms_e2e = _timed_events(e2e_step, K, barrier)
         smp.stop_flag = True
         smp.join(timeout=2)
@@ -405,7 +428,7 @@ def run_ours_other(args):
                 'e2e': {'value': world * K / (ms_e2e / 1e3), 'unit': 'frame-pairs/s', 'h2d_bytes_per_step': GEN_H * GEN_W * 5 * 4,
                         'd2h_bytes_per_step': GEN_H * GEN_W * 4, 'ms_per_step': ms_e2e / K},
                 'gpu_launches': nl * K, 'clocks': smp.summary(),
-                'roofline': {'bound': 'tensor', 'kernel': 'tcgen05 conv family, generator forward (17 layers, batch 1)',
+                'roofline': {'bound': 'tensor', 'kernel': 'wgmma conv family, generator forward (17 layers, batch 1)',
                              'achieved': gflop / (ms_dev / K), 'peak': pk['bf16_tflops_sustained'], 'unit': 'TFLOP/s',
                              'frac': gflop / (ms_dev / K) / pk['bf16_tflops_sustained'], 'peak_source': src, 'traffic': None},
                 'cpu_baseline': {'value': cv, 'unit': 'frame-pairs/s', 'cores': cores, 'kind': 'port',
@@ -431,6 +454,9 @@ def run_ours_other(args):
     smp = ClockSampler(L.local_rank)
     smp.start()
     ms_dev = _timed_events(lambda i: g.forward_masks(use_graph=True), K, barrier)       # crops already resident
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        dump_outputs(args.dump_outputs, {'mask': g.mask.float().cpu().numpy()})
     ms_e2e = _timed_events(lambda i: L.inference(batch=pool[i % 2]), K, barrier)        # H2D + device crops + forward + D2H masks/images
     smp.stop_flag = True
     smp.join(timeout=2)
@@ -451,13 +477,13 @@ def run_ours_other(args):
             'config': {'workload': 'generate_buffer ensemble inference: 4 central crops per frame pair, PWC-Net 384x640 + generator 192x384 '
                                    '(configs[4])', 'global_batch': world, 'crops_per_frame': ncrop,
                        'parallelism': 'frames sharded over %d rank(s), no data-path collective' % world, 'cuda_graph': True,
-                       'l2': 'per-step working set exceeds the 126 MB L2'},
+                       'l2': 'per-step working set exceeds the 50 MB L2'},
             'e2e': {'value': world * K / (ms_e2e / 1e3), 'unit': 'frame-pairs/s', 'h2d_bytes_per_step': (2 * 3 + 1) * 384 * 640 * 4,
                     'd2h_bytes_per_step': ncrop * ENS_H * ENS_W * (1 + 1 + 3) * 4, 'ms_per_step': ms_e2e / K,
                     'note': 'one frame pair + ground truth uploaded per step; the 4 central crops and their resizes run on the device '
                             '(cis_crop_resize_bilinear_f32); masks, resized ground truth and the network input image are read back'},
             'gpu_launches': g._mask_plan.count() * K, 'clocks': smp.summary(),
-            'roofline': {'bound': 'tensor', 'kernel': 'tcgen05 conv family, PWC-Net + generator forward, 4 crops', 'achieved': gflop / (ms_dev / K),
+            'roofline': {'bound': 'tensor', 'kernel': 'wgmma conv family, PWC-Net + generator forward, 4 crops', 'achieved': gflop / (ms_dev / K),
                          'peak': pk['bf16_tflops_sustained'], 'unit': 'TFLOP/s', 'frac': gflop / (ms_dev / K) / pk['bf16_tflops_sustained'],
                          'peak_source': src, 'traffic': None},
             'cpu_baseline': {'value': cv, 'unit': 'frame-pairs/s', 'cores': cores, 'kind': 'port',
@@ -528,6 +554,8 @@ def main():
     ap.add_argument('--no-cpu', action='store_true', help='skip the cpu_baseline leg')
     ap.add_argument('--workload', default='train', choices=['train', 'gen_fwd', 'ensemble'],
                     help='train = the headline metric; gen_fwd = BASELINE configs[0]; ensemble = BASELINE configs[4]')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write what the timed path computed in its last step to DIR/<name>.npy')
     args = ap.parse_args()
     if args.impl == 'reference':
         run_reference(args)

@@ -1,4 +1,4 @@
-/* cis_b200.h - C ABI of libcis_b200.so: the sm_100a kernels behind the adversarial motion-segmentation hot path.
+/* cis_b200.h - C ABI of libcis_b200.so: the sm_90a kernels behind the adversarial motion-segmentation hot path.
  *
  * The reference (antonilo/unsupervised_detection @ 46cae6e) has no FFI layer: its "operators" are TensorFlow 1.13 graph
  * ops called from Python (SURVEY.md section 8b).  Each entry point below replaces the TF op class used at the cited
@@ -32,7 +32,7 @@ typedef struct {
   int32_t n_mod;   /* >0: batch index taken modulo n_mod (features shared by the 3 recover_net calls) */
 } CisSrc;
 
-/* Implicit-GEMM convolution on tcgen05 tensor cores: D[rows=(n,oh,ow)][BN] = sum_k A[row][k] * Wp[n][k],
+/* Implicit-GEMM convolution on the tensor cores (wgmma): D[rows=(n,oh,ow)][BN] = sum_k A[row][k] * Wp[n][k],
  * A[row][(t,c)] = src[n, oh*sh + dh[t], ow*sw + dw[t], c] (zero outside the image = TF 'SAME' padding).
  * With suitable tap tables this one kernel is: tf.layers.conv2d / tf.nn.conv2d forward (convolution_utils.py:46,81;
  * model_pwcnet.py:161-165,484-504,562-574), its data gradient (stride 1: flipped taps; stride 2: four parity launches),
@@ -69,10 +69,10 @@ typedef struct {
   int32_t mode;      /* 0 normal; 1: outf[pix] = sigmoid((l0 - l1)/10)  (nets.py:38-41) */
   /* halo-resident variant (stride-1 gathers only): the CTA tile is MT stacked 16x8-pixel blocks of dilation phase (a,b);
    * the (16*MT+ey) x (8+ex) input halo of a 64-channel chunk is staged ONCE in shared memory and all taps read it through
-   * shifted UMMA descriptors.  dh/dw then hold tap offsets >= 0 relative to the halo origin, in units of `dil` pixels. */
+   * shifted wgmma descriptors.  dh/dw then hold tap offsets >= 0 relative to the halo origin, in units of `dil` pixels. */
   int32_t halo;      /* 0: generic per-tap gather kernel, 1: halo-resident kernel */
   int32_t dil;       /* dilation = phase period (1 for undilated) */
-  int32_t MT;        /* 1..4 stacked M tiles (MT*BN <= 512 TMEM columns) */
+  int32_t MT;        /* 1..4 stacked M tiles (MT*BN <= 128 register accumulator columns) */
   int32_t hoy, hox;  /* halo origin relative to the tile origin (phase units, <= 0) */
   int32_t ey, ex;    /* halo extent beyond the tile (max tap offset) */
   /* Split-K for launches that cover only a few SMs (low-resolution layers): grid.z = splits CTAs share one output tile, each reduces a

@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 implicit-GEMM conv engine (forward, data gradient, weight gradient) against a plain torch
+"""GPU parity of the wgmma implicit-GEMM conv engine (forward, data gradient, weight gradient) against a plain torch
 fp32 reference of the same op on the same bf16-rounded operands.  Tolerances: the product accumulates in fp32 from bf16
 operands exactly like the reference's inputs, so only summation order and the final bf16 rounding of stored activations
 differ: |err| <= 2^-8 * |ref|_max + small absolute slack."""

@@ -31,7 +31,7 @@ def _check_conv(d):
     if d.out:
         assert d.out_pitch > 0 and d.out_ch >= 1     # unaligned channel offsets are legal (scalar store path), e.g. PWC up_flow slices
     if d.halo:
-        assert d.sh == 1 and d.sw == 1 and 1 <= d.MT <= 4 and d.MT * d.BN <= 512 and d.dil >= 1
+        assert d.sh == 1 and d.sw == 1 and 1 <= d.MT <= 4 and d.MT * d.BN <= engine.MAX_ACC_COLS and d.dil >= 1
         hp = (8 + d.ex) * (16 * d.MT + d.ey)
         assert 2 * ((hp * 128 + 1023) // 1024 * 1024) + hp * 4 + 1024 + d.BN * 128 <= 227 * 1024      # at least one weight stage fits
         hp0, wp0 = -(-d.OH // d.dil), -(-d.OW // d.dil)
@@ -42,7 +42,7 @@ def _check_conv(d):
         if d.MT > 1 and d.nsub <= 1 and engine.PLAN_MODEL == 4:
             # planner rule measured in r02: a taller tile stack only on big grids of short tiles (MMA loop < a CTA's fixed costs)
             n1 = d.N * d.dil * d.dil * (-(-wp0 // 8)) * (-(-hp0 // 16)) * d.n_tiles
-            assert 2.0 * d.BN * d.ntaps * (-(-chunks // 8)) < 6000.0 and n1 > 4 * 148
+            assert 2.0 * d.BN * d.ntaps * (-(-chunks // 8)) < 6000.0 and n1 > 4 * engine.NUM_SMS
     if d.splits > 1:                                  # two-launch split-K (default): private slices, no ticket counters, every split owns work
         assert d.sk_scratch and not d.sk_counters and 2 <= d.splits <= 16
         units = -(-chunks // 8) if d.halo else d.K_pad // 64

@@ -1,10 +1,10 @@
-"""Index-level model of the experimental halo-resident wgrad kernel (csrc/conv_igemm.cu: conv_wgrad_halo_kernel, CisWgrad.tma = 2).
+"""Index-level model of the halo-resident wgrad kernel (csrc/conv_igemm.cu: conv_wgrad_halo_kernel, CisWgrad.tma = 2).
 
-The kernel has not run on a GPU yet; what CAN be checked without one is its addressing scheme: this test replays, in numpy, exactly
+What CAN be checked without a GPU is its addressing scheme: this test replays, in numpy, exactly
 the data movement the kernel programs -- the zero-filled TMA halo box, the tap origins `s_off`, the per-K-step descriptor start
 (two halo rows per 16 pixels), the LBO hop from tap 2q to tap 2q+1 inside one M = 128 operand, the accumulator column ranges and
 the epilogue's (tap, chunk, channel) -> packed column map -- and compares the result with a direct weight-gradient sum.
-What it cannot check is the hardware's treatment of those descriptors (tools/umma_probe_mn.cu does that on a B200)."""
+What it cannot check is the hardware's treatment of those descriptors (tests/test_conv_engine_gpu.py runs the kernel)."""
 import numpy as np
 import pytest
 
@@ -27,7 +27,7 @@ def model_wgrad_halo(x, g, taps, cout):
     tiles_y, tiles_x = -(-OH // 8), -(-OW // 8)
     for c64 in range(nch64):
         for half in range(nhalf):
-            acc = np.zeros((npair, 128, Nh), np.float64)                      # TMEM: pair q -> columns [q*Nh, (q+1)*Nh)
+            acc = np.zeros((npair, 128, Nh), np.float64)                      # accumulator: pair q -> columns [q*Nh, (q+1)*Nh)
             for n in range(N):
                 for ty in range(tiles_y):
                     for tx in range(tiles_x):
@@ -109,5 +109,5 @@ def test_halo_wgrad_eligibility_rules():
     assert wgrad_halo_fits(t3, 128, 1) and not wgrad_halo_fits(t3, 128, 2)
     assert not wgrad_halo_fits(t3[::-1], 16, 1)                                   # pairs need increasing row-major origins
     t5 = [(a, b) for a in range(-2, 3) for b in range(-2, 3)]
-    assert wgrad_halo_fits(t5, 32, 1) and not wgrad_halo_fits(t5, 128, 1)         # 13 pairs x 64 columns exceed TMEM
+    assert wgrad_halo_fits(t5, 32, 1) and not wgrad_halo_fits(t5, 128, 1)         # 13 pairs x 64 columns exceed the 512 the planner allows
     assert not wgrad_halo_fits([(a * 16, b * 16) for a in (-1, 0, 1) for b in (-1, 0, 1)], 128, 1)   # 40x40 halo: no 2 stages

@@ -21,6 +21,11 @@ int cis_check_launch(const char* where) {
   if (e != cudaSuccess) return cis_set_cuda_error(e, where);
   return CIS_OK;
 }
+int cis_num_sms() {
+  int dev = 0, n = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n < 1) return 132;
+  return n;
+}
 extern "C" const char* cis_last_error(void) { return g_err; }
 extern "C" int cis_version(void) { return 100; }
 

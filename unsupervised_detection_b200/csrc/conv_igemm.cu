@@ -1,4 +1,4 @@
-// tcgen05 implicit-GEMM convolution engine for sm_100a (forward / data-gradient / transposed conv / weight-gradient).
+// wgmma implicit-GEMM convolution engine for sm_90a (forward / data-gradient / transposed conv / weight-gradient).
 //
 // Replaces the TF1 op classes K1/K3/K5/K6 of SURVEY.md section 2.2 (tf.layers.conv2d, tf.nn.conv2d,
 // tf.layers.conv2d_transpose and their tf.gradients twins; reference call sites
@@ -6,10 +6,10 @@
 //
 // Design (see DESIGN.md): one CTA = one 128-row tile of the GEMM (rows = output pixels).  Four producer warps gather the
 // im2col A tile (128 rows x 64 bf16 of K) and the packed-weight B tile straight into the canonical SWIZZLE_128B K-major
-// shared-memory layout with 16-byte cp.async (zero-fill = SAME padding); one thread of a fifth warp issues
-// tcgen05.mma.kind::f16 (M=128, N=BN, K=16) with the fp32 accumulator in TMEM; smem stages are recycled with
-// tcgen05.commit -> mbarrier.  The producer warps then become the epilogue: tcgen05.ld the accumulator, apply
-// bias / residuals / activation and store bf16 and/or fp32 NHWC.
+// shared-memory layout with 16-byte cp.async (zero-fill = SAME padding); an MMA warpgroup issues wgmma (two m64nBNk16 per
+// 128-row K=16 step) with the fp32 accumulator in its registers and releases each smem stage through an mbarrier once its
+// wgmma group has completed.  After the last K block it stores the accumulator to shared memory (acc_store) and the producer
+// warps become the epilogue: read the accumulator rows, apply bias / residuals / activation and store bf16 and/or fp32 NHWC.
 #include "ptx.cuh"
 #include "../../include/cis_b200.h"
 #include "common.cuh"
@@ -17,7 +17,7 @@
 #include <stdlib.h>
 #include <string.h>
 
-// cp.async (LDGSTS) writes shared memory through the generic proxy while tcgen05.mma reads it through the async proxy.  Every
+// cp.async (LDGSTS) writes shared memory through the generic proxy while wgmma reads it through the async proxy.  Every
 // cp.async producer therefore publishes a stage itself: commit_group, wait_group<lag> (its own copies of the stage landed),
 // fence.proxy.async, then a plain mbarrier.arrive -- the MMA warp needs no fence.  The lag keeps (stages - 1) groups in flight.
 
@@ -39,16 +39,18 @@ __device__ int g_trace_cap = 0;
 static constexpr int kBM = 128;       // GEMM rows per CTA
 static constexpr int kBK = 64;        // bf16 K elements per stage (128-byte swizzled rows)
 static constexpr int kAStage = kBM * 128;
-static constexpr int kThreads = 160;  // halo / wgrad kernels: 4 producer/epilogue warps + 1 MMA warp
+static constexpr int kThreads = 256;  // halo / wgrad kernels: 4 producer/epilogue warps + 1 MMA warpgroup
 // conv_halo_kernel<BN>: warps 0-3 producers + epilogue; BN >= 64 adds warps 4-7 (epilogue only: the wide epilogue is instruction-bound on its
-// warps); last warp = MMA issuer / TMEM owner.  BN <= 32 keeps 160 threads: there the number of co-resident CTAs matters more (measured).
+// warps); the last four warps = the MMA warpgroup.
 template <int BN> struct HaloCfg {
-  static constexpr int kMmaWarp = BN >= 64 ? 8 : 4;
-  static constexpr int kThreads = (kMmaWarp + 1) * 32;
-  static constexpr int kMinCtas = BN >= 64 ? 2 : (BN == 32 ? 3 : 4);
+  static constexpr int kMmaWarp = BN >= 64 ? 8 : 4;     // first warp of the MMA warpgroup
+  static constexpr int kThreads = (kMmaWarp + 4) * 32;
+  // accumulator registers per MMA thread: MT * BN <= kMaxAccCols (the host never stacks more tiles than that)
+  static constexpr int kMaxMT = (128 / BN) < 4 ? (128 / BN) : 4;
 };
+static constexpr int kMaxAccCols = 128;   // fp32 accumulator columns one MMA warpgroup holds in registers (128 per thread)
 static constexpr int kGProducers = 256;   // gather kernel: 8 producer/epilogue warps (its cp.async address arithmetic is the bottleneck)
-static constexpr int kGThreads = 288;     // + 1 MMA warp
+static constexpr int kGThreads = 384;     // + 1 MMA warpgroup
 
 struct SrcS {
   const __nv_bfloat16* ptr;
@@ -125,8 +127,8 @@ __device__ __forceinline__ void epi_chunk(const CisConv& p, float (&v)[16], cons
 
 
 
-// Latency-batched epilogue for NC x 16 accumulator columns of one row: residual loads are issued first, then all TMEM loads,
-// ONE wait, then the arithmetic and the stores (the per-chunk version paid a full TMEM + global-load round trip per 16 columns).
+// Latency-batched epilogue for NC x 16 accumulator columns of one row: residual loads are issued first, then the accumulator reads,
+// then the arithmetic and the stores.  taddr = accumulator tile + row * 16 + first column * kAccColBytes.
 template <int NC>
 __device__ __forceinline__ void epi_group(const CisConv& p, const uint32_t taddr, const int cg0, const size_t dpix, const bool valid,
                                           const float* __restrict__ sbias) {
@@ -145,17 +147,16 @@ __device__ __forceinline__ void epi_group(const CisConv& p, const uint32_t taddr
       if (has_res && cg + 8 * h < p.out_ch) rres[c][h] = __ldg(reinterpret_cast<const uint4*>(rp + roff + cg) + h);
     }
   }
-  uint32_t raw[NC][16];
-#pragma unroll
-  for (int c = 0; c < NC; ++c) tmem_ld16_nowait(taddr + 16 * c, raw[c]);
-  tmem_ld_wait();
   if (!valid) return;
+  float raw[NC][16];
+#pragma unroll
+  for (int c = 0; c < NC; ++c) acc_ld16(taddr + (uint32_t)(16 * c) * kAccColBytes, raw[c]);
 #pragma unroll
   for (int c = 0; c < NC; ++c) {
     const int cg = cg0 + 16 * c;
     float v[16];
 #pragma unroll
-    for (int e = 0; e < 16; ++e) v[e] = __uint_as_float(raw[c][e]);
+    for (int e = 0; e < 16; ++e) v[e] = raw[c][e];
     if (p.bias) {
       const float4* sb = reinterpret_cast<const float4*>(sbias + (cg - cg0));   // sbias = this group's first column; 16-float aligned: 4 x LDS.128
 #pragma unroll
@@ -225,8 +226,8 @@ __device__ __forceinline__ void epi_cols(const CisConv& p, const uint32_t t_row,
                                          const float* __restrict__ sbias, const int c_lo, const int c_hi) {
   int c0 = c_lo;
 #pragma unroll 1
-  for (; c0 + 32 <= c_hi; c0 += 32) epi_group<2>(p, t_row + c0, cbase + c0, dpix, valid, sbias + c0);
-  if (c0 < c_hi) epi_group<1>(p, t_row + c0, cbase + c0, dpix, valid, sbias + c0);
+  for (; c0 + 32 <= c_hi; c0 += 32) epi_group<2>(p, t_row + (uint32_t)c0 * kAccColBytes, cbase + c0, dpix, valid, sbias + c0);
+  if (c0 < c_hi) epi_group<1>(p, t_row + (uint32_t)c0 * kAccColBytes, cbase + c0, dpix, valid, sbias + c0);
 }
 // all BN columns of one row
 template <int BN>
@@ -240,13 +241,13 @@ __device__ __forceinline__ void epi_row(const CisConv& p, const uint32_t t_row, 
 template <int BN>
 __device__ __forceinline__ void splitk_store_partial(float* slice, uint32_t t_row, int row, int c_lo = 0, int c_hi = BN) {
   // slice = this split's private fp32 tile, stored as float4 COLUMNS: element (row, c) at ((c / 4) * 128 + row) * 4 + c % 4.  A warp
-  // (32 consecutive accumulator rows, same columns) then writes 512 contiguous bytes per store instruction; the row-major layout of
-  // r01/r02 made every st.v4 touch 32 different 128-byte lines and the LSU, not HBM, bounded the epilogue (~10k clk per 128x128 tile
-  // in the CIS_TRACE build -- as long as the whole MMA loop of a split).  No atomics, fixed summation order later.
+  // (32 consecutive accumulator rows, same columns) then writes 512 contiguous bytes per store instruction; a row-major layout would
+  // make every st.v4 touch 32 different 128-byte lines and the LSU, not HBM, would bound the epilogue.  No atomics, fixed summation
+  // order later.
 #pragma unroll 1
   for (int c0 = c_lo; c0 < c_hi; c0 += 16) {
     float v[16];
-    tmem_ld16(t_row + c0, v);
+    acc_ld16(t_row + (uint32_t)c0 * kAccColBytes, v);
     float4* o = reinterpret_cast<float4*>(slice) + (size_t)(c0 / 4) * kBM + row;
     o[0] = make_float4(v[0], v[1], v[2], v[3]);
     o[kBM] = make_float4(v[4], v[5], v[6], v[7]);
@@ -255,7 +256,7 @@ __device__ __forceinline__ void splitk_store_partial(float* slice, uint32_t t_ro
   }
 }
 // sum of the nsplit private slices of one tile for (row, c0..c0+15); loads are plain L2 loads (__ldcg) issued in batches of
-// 4 slices x 4 float4 so their latencies overlap (a volatile-asm version serialised ~150 round trips per thread: ncu r01d)
+// 4 slices x 4 float4 so their latencies overlap (volatile-asm loads would serialise the round trips)
 template <int BN>
 __device__ __forceinline__ void splitk_reduce16(const float* tile0, int nsplit, int row, int c0, float* v) {
 #pragma unroll
@@ -313,29 +314,16 @@ __device__ __forceinline__ void cluster_reduce_rows(const CisConv& p, const uint
     if (valid) epi_chunk(p, v, cbase + c0, dpix);
   }
 }
-// this warp's 32 accumulator rows x columns [c_lo, c_hi) -> shared-memory stage in the layout above
-__device__ __forceinline__ void tmem_to_stage(const uint32_t t_row, const int row, const uint32_t stage, const int c_lo, const int c_hi) {
-#pragma unroll 1
-  for (int c0 = c_lo; c0 < c_hi; c0 += 16) {
-    float v[16];
-    tmem_ld16(t_row + c0, v);
-#pragma unroll
-    for (int h = 0; h < 4; ++h)
-      asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(stage + (uint32_t)(((c0 / 4 + h) * kBM + row) * 16)), "f"(v[4 * h]),
-                   "f"(v[4 * h + 1]), "f"(v[4 * h + 2]), "f"(v[4 * h + 3])
-                   : "memory");
-  }
-}
 
 template <int BN>
 struct FwdCfg {
-  // kLag + 1 K blocks of gathers are in flight per producer thread (the im2col loads are L2 round trips of ~1 us).  A deeper ring
-  // (5-6 stages for BN <= 32) was measured SLOWER: it drops the thin layers from 3 to 2 co-resident CTAs per SM.
+  // kLag + 1 K blocks of gathers are in flight per producer thread (the im2col loads are L2 round trips).  A deeper ring costs
+  // co-resident CTAs on the thin layers.
   static constexpr int kStages = (BN == 128) ? 3 : 4;
   static constexpr int kLag = kStages - 2;
   static constexpr int kBStage = BN * 128;
   static constexpr int kSmem = kStages * (kAStage + kBStage) + 1024;
-  static constexpr int kTmemCols = BN < 32 ? 32 : BN;
+  static_assert(kStages * (kAStage + kBStage) >= kBM * BN * 4, "the accumulator tile reuses the operand ring");
 };
 
 template <int BN>
@@ -345,7 +333,6 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
   constexpr int kMmaWarp = kGProducers / 32;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * S + 1];
-  __shared__ uint32_t tmem_slot;
   __shared__ int s_dh[CIS_MAX_TAPS], s_dw[CIS_MAX_TAPS];
   __shared__ SrcS s_src[CIS_MAX_SRC];
 
@@ -384,24 +371,17 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     s_src[tid].chunks = p.src[tid].chunks;
     s_src[tid].n_mod = p.src[tid].n_mod;
   }
-  if (warp == kMmaWarp) {
-    if (lane == 0) {
-      for (int s = 0; s < S; ++s) {
-        mbar_init(bar_full + 8 * s, kGProducers);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      mbar_init(bar_accum, 1);
-      fence_mbar_init();
+  if (tid == kMmaWarp * 32) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(bar_full + 8 * s, kGProducers);
+      mbar_init(bar_empty + 8 * s, 1);
     }
-    __syncwarp();
-    tmem_alloc<Cfg::kTmemCols>(smem_u32(&tmem_slot));
+    mbar_init(bar_accum, 128);    // every thread of the MMA warpgroup, after storing its accumulator fragment
+    fence_mbar_init();
   }
-  pdl_wait();   // everything above touched only kernel parameters / shared memory / TMEM
+  pdl_wait();   // everything above touched only kernel parameters / shared memory
   if (tid < BN) s_bias[tid] = p.bias ? p.bias[ny * BN + tid] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   if (tid == 0) CIS_TRACE_AT(0);
 
   if (warp < kMmaWarp) {
@@ -410,8 +390,8 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     const int rl = tid >> 3;        // 0..31
     const uint32_t sw_off = (uint32_t)((j ^ (rl & 7)) << 4);
     // Per-row constants (this thread's 4 rows): top-left input pixel, and the linear pixel index of it in the plain and in the
-    // batch-broadcast (n % n_mod) view of the sources.  The K loop below is division-free: r02's ncu source view showed the producer
-    // warps issue-bound on the integer divisions / 64-bit address arithmetic of every (K block, row), not on the loads.
+    // batch-broadcast (n % n_mod) view of the sources.  The K loop below is division-free: with integer divisions / 64-bit address
+    // arithmetic per (K block, row) the producer warps are issue-bound, not bound by the loads.
     int hb[4], wb[4], pre[4], prem[4];
     int nm0 = 0;                          // the batch-broadcast modulus (sources with n_mod > 0 share one; others: slow path)
     for (int i = 0; i < p.nsrc; ++i)
@@ -502,9 +482,8 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
       mbar_arrive(bar_full + 8 * ((nkb - 1 - i) % S));
     }
 
-    // ------------------------------------------------------------------ epilogue: warps w and w + 4 share a TMEM lane quarter and split the columns
+    // ------------------------------------------------------------------ epilogue: warps w and w + 4 share 32 accumulator rows and split the columns
     mbar_wait(bar_accum, 0);
-    tc_fence_after();
     if (tid == 0) CIS_TRACE_AT(2);
     const int qtr = warp & 3, half = warp >> 2;
     const int row = qtr * 32 + lane;
@@ -518,13 +497,12 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
       const int n = t / p.OH;
       dpix = (size_t)(n * p.DH + oh * p.osh + p.oa) * p.DW + ow * p.osw + p.ob;
     }
-    const uint32_t t_row = tmem + ((uint32_t)(qtr * 32) << 16);
+    const uint32_t t_row = tile_base + (uint32_t)row * 16;          // the accumulator tile overlays the (dead) operand ring
     const int cbase = ny * BN;
     constexpr int kHalf = BN >= 32 ? BN / 2 : BN;                 // BN = 16: the first warp group does it all
     const int c_lo = half * kHalf, c_hi = (BN >= 32 || half == 0) ? c_lo + kHalf : c_lo;
     if (nsplit > 1 && p.sk_cluster) {
-      // cluster split-K: partial tile -> own shared memory (the operand ring is dead: every MMA has completed); reduced below
-      tmem_to_stage(t_row, row, tile_base, c_lo, c_hi);
+      // cluster split-K: the partial tile already sits in this CTA's shared memory in the layout the reduction below reads
     } else if (nsplit > 1) {
       // two-launch split-K: this split's private fp32 slice; splitk_finish_kernel reduces the slices and runs the fused epilogue
       const int tile_id = blockIdx.x * gridDim.y + ny;
@@ -534,25 +512,27 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
       epi_cols<BN>(p, t_row, cbase, dpix, valid, s_bias, c_lo, c_hi);
     }
   } else {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, 0, 0);
+    // ------------------------------------------------------------------ MMA warpgroup
+    const int wtid = tid - kMmaWarp * 32;
+    float acc[BN];
+    const uint32_t dhi = desc_hi(1024);
+    constexpr uint32_t a_half = (8 * 1024) >> 4;     // rows 64..127: 8 core-matrix groups of SBO = 1024 B further
     for (int kb = 0; kb < nkb; ++kb) {
       const int s = kb % S;
-      const uint32_t ph = (uint32_t)((kb / S) & 1);
-      mbar_wait(bar_full + 8 * s, ph);
-      tc_fence_after();
-      if (elect_one()) {
-        CIS_TRACE_AT(8 + 2 * kb);
-        const uint32_t alo = desc_lo(a_base + s * kAStage, 16), blo = desc_lo(b_base + s * Cfg::kBStage, 16);
-        const uint32_t dhi = desc_hi(1024);
+      mbar_wait(bar_full + 8 * s, (uint32_t)((kb / S) & 1));
+      if (wtid == 0) CIS_TRACE_AT(8 + 2 * kb);
+      const uint32_t alo = desc_lo(a_base + s * kAStage, 16), blo = desc_lo(b_base + s * Cfg::kBStage, 16);
+      wg_fence();
 #pragma unroll
-        for (int k = 0; k < kBK / 16; ++k) umma_bf16_lh(tmem, alo + 2 * k, dhi, blo + 2 * k, dhi, idesc, (uint32_t)((kb | k) != 0));
-        umma_commit(bar_empty + 8 * s);
-        if (kb == nkb - 1) umma_commit(bar_accum);
-        CIS_TRACE_AT(9 + 2 * kb);
-      }
-      __syncwarp();
+      for (int k = 0; k < kBK / 16; ++k) mma128<BN, 0, 0>(acc, alo + 2 * k, dhi, blo + 2 * k, dhi, a_half, (uint32_t)((kb | k) != 0));
+      wg_commit();
+      wg_wait<1>();                 // block kb-1 has been consumed: release its stage while block kb runs
+      if (wtid == 0 && kb > 0) mbar_arrive(bar_empty + 8 * ((kb - 1) % S));
+      if (wtid == 0) CIS_TRACE_AT(9 + 2 * kb);
     }
+    wg_wait<0>();
+    acc_store<BN>(acc, tile_base, wtid);   // every operand stage has been consumed: the ring is dead
+    mbar_arrive(bar_accum);
   }
   if (nsplit > 1 && p.sk_cluster) {
     cluster_sync_all();                       // every CTA's partial tile is in its shared memory
@@ -571,10 +551,7 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     }
     cluster_sync_all();                       // peers may still be reading this CTA's shared memory
   }
-  tc_fence_before();
-  __syncthreads();
   if (tid == 0) CIS_TRACE_AT(3);
-  if (warp == kMmaWarp) tmem_dealloc<Cfg::kTmemCols>(tmem);
 }
 
 
@@ -583,7 +560,7 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
 // of the 4x4 s2 transposed convs).  The CTA owns MT stacked tiles of 16x8 output pixels of one dilation phase; per 64-channel
 // chunk the (16*MT+ey) x (8+ex) input halo is copied ONCE into shared memory (SWIZZLE_128B rows of 128 B = one pixel x 64 ch)
 // and every tap (dy,dx) reads it in place: A descriptor start = halo + ((16*m+dy)*Wh + dx)*128, SBO = Wh*128.  The hardware
-// applies the 128B swizzle on absolute shared-memory address bits (tools/umma_probe.cu), so 128-byte-granular starts and a
+// applies the 128B swizzle on absolute shared-memory address bits, so 128-byte-granular starts and a
 // non-1024 SBO are legal with base_offset = 0.  im2col traffic drops from k*k x to ~1.3 x and the packed weights of a
 // (tap, chunk) are reused by the MT tiles.
 static constexpr int kHaloMaxBStages = 8;
@@ -592,101 +569,70 @@ struct HaloMaps {
   CUtensorMap m[CIS_MAX_SRC * 4];
 };
 
-// MMAs of one weight stage (gt taps of one 64-channel chunk, MT stacked tiles, NK K=16 steps each), issued by ONE thread.  The tap
-// offsets come from a shared-memory table; the next tap's offset is fetched BEFORE the current tap's MMAs are issued so the
-// LDS -> R2UR -> descriptor chain (~100 clk, measured 220 clk per single-MMA tap in r02) overlaps the previous issue.
-// MT == 1 (every thin layer): straight-line groups of four taps -- the four tap offsets of the NEXT group are loaded before this group's
-// MMAs are issued, no per-tap branch or tile loop.  (r02 trace: the generic loop below cost 105-157 clk per single-MMA tap, 3-4x the
-// 36 clk the tensor pipe needs for a 128x16x16 MMA; the thin layers were bound by this thread, not by shared memory.)
-template <int NK>
-__device__ __forceinline__ void halo_issue_mt1(const uint32_t tmem, const uint32_t hlo, uint32_t blo, const uint32_t* s_aoff, const int gt,
-                                               const uint32_t bstep, const uint32_t ahi, const uint32_t bhi, const uint32_t idesc,
-                                               const bool first) {
-  int tt = 0;
-  uint32_t acc = first ? 0u : 1u;
-  uint32_t o0 = 0, o1 = 0, o2 = 0, o3 = 0;
-  if (gt >= 4) {
-    o0 = s_aoff[0];
-    o1 = s_aoff[1];
-    o2 = s_aoff[2];
-    o3 = s_aoff[3];
-  }
-  for (; tt + 4 <= gt; tt += 4) {
-    const uint32_t a0 = hlo + o0, a1 = hlo + o1, a2 = hlo + o2, a3 = hlo + o3;
-    if (tt + 8 <= gt) {
-      o0 = s_aoff[tt + 4];
-      o1 = s_aoff[tt + 5];
-      o2 = s_aoff[tt + 6];
-      o3 = s_aoff[tt + 7];
-    }
-#pragma unroll
-    for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, a0 + 2 * k, ahi, blo + 2 * k, bhi, idesc, k ? 1u : acc);
-#pragma unroll
-    for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, a1 + 2 * k, ahi, blo + bstep + 2 * k, bhi, idesc, 1u);
-#pragma unroll
-    for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, a2 + 2 * k, ahi, blo + 2 * bstep + 2 * k, bhi, idesc, 1u);
-#pragma unroll
-    for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, a3 + 2 * k, ahi, blo + 3 * bstep + 2 * k, bhi, idesc, 1u);
-    acc = 1u;
-    blo += 4 * bstep;
-  }
-  if (tt < gt) {              // 1-3 left-over taps
-    const uint32_t r0 = s_aoff[tt], r1 = tt + 1 < gt ? s_aoff[tt + 1] : 0u, r2 = tt + 2 < gt ? s_aoff[tt + 2] : 0u;
-#pragma unroll
-    for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, hlo + r0 + 2 * k, ahi, blo + 2 * k, bhi, idesc, k ? 1u : acc);
-    if (tt + 1 < gt) {
-#pragma unroll
-      for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, hlo + r1 + 2 * k, ahi, blo + bstep + 2 * k, bhi, idesc, 1u);
-    }
-    if (tt + 2 < gt) {
-#pragma unroll
-      for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, hlo + r2 + 2 * k, ahi, blo + 2 * bstep + 2 * k, bhi, idesc, 1u);
-    }
-  }
-}
-
-template <int NK>
-__device__ __forceinline__ void halo_issue_stage(const uint32_t tmem, const uint32_t hlo, uint32_t blo, const uint32_t* s_aoff, const int gt,
-                                                 const int MT, const int BN, const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep,
-                                                 const uint32_t idesc, const bool first) {
+// wgmma of one weight stage (gt taps of one 64-channel chunk, MT stacked tiles, NK K=16 steps each), issued by the MMA warpgroup into
+// the register accumulators acc[m] of the MT tiles.  The tap offsets come from a shared-memory table (a broadcast read); the offset
+// two taps ahead is fetched before the current tap's wgmma are issued.  Every tap is its own straight-line fence .. commit group:
+// with a branch or a loop between wgmma.fence and wgmma.commit_group ptxas serialises every wgmma of the kernel (C7520).
+template <int NK, int MT, int BN, int MTM>
+__device__ __forceinline__ void halo_issue_stage(float (&acc)[MTM][BN], const uint32_t hlo, uint32_t blo, const uint32_t* s_aoff, const int gt,
+                                                 const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep, const uint32_t a_half,
+                                                 const bool first) {
   const uint32_t bstep = (uint32_t)(BN * 128) >> 4;
-  if (NK == 1 && MT == 1) {      // single-MMA taps: the loop overhead below would dominate
-    halo_issue_mt1<NK>(tmem, hlo, blo, s_aoff, gt, bstep, ahi, bhi, idesc, first);
-    return;
-  }
   uint32_t off0 = s_aoff[0], off1 = gt > 1 ? s_aoff[1] : 0u;
-#pragma unroll 2
-  for (int tt = 0; tt < gt; ++tt, blo += bstep) {
+  int tt = 0;
+#pragma unroll 1
+  do {
     const uint32_t off2 = tt + 2 < gt ? s_aoff[tt + 2] : 0u;    // two taps ahead
-    uint32_t alo = hlo + off0;
+    const uint32_t alo = hlo + off0;
     const uint32_t acc0 = (uint32_t)(!(first && tt == 0));
-    if (MT == 1) {
+    wg_fence();
 #pragma unroll
-      for (int k = 0; k < NK; ++k) umma_bf16_lh(tmem, alo + 2 * k, ahi, blo + 2 * k, bhi, idesc, k ? 1u : acc0);
-    } else {
-      for (int m = 0; m < MT; ++m, alo += a_mstep) {
-        const uint32_t td = tmem + m * BN;
+    for (int m = 0; m < MT; ++m) {
 #pragma unroll
-        for (int k = 0; k < NK; ++k) umma_bf16_lh(td, alo + 2 * k, ahi, blo + 2 * k, bhi, idesc, k ? 1u : acc0);
-      }
+      for (int k = 0; k < NK; ++k) mma128<BN, 0, 0>(acc[m], alo + m * a_mstep + 2 * k, ahi, blo + 2 * k, bhi, a_half, k ? 1u : acc0);
     }
+    wg_commit();
     off0 = off1;
     off1 = off2;
+    blo += bstep;
+  } while (++tt < gt);
+}
+// one weight stage with the K depth of the chunk (nk16 = 1..4 K=16 steps: the last chunk of a layer may be partial)
+template <int MT, int BN, int MTM>
+__device__ __forceinline__ void halo_issue_nk(const int nk16, float (&acc)[MTM][BN], const uint32_t hlo, const uint32_t blo, const uint32_t* s_aoff,
+                                              const int gt, const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep, const uint32_t a_half,
+                                              const bool first) {
+  if (nk16 == 4) halo_issue_stage<4, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+  else if (nk16 == 1) halo_issue_stage<1, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+  else if (nk16 == 2) halo_issue_stage<2, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+  else halo_issue_stage<3, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+}
+template <int BN, int MTM>
+__device__ __forceinline__ void halo_issue_any(const int nk16, float (&acc)[MTM][BN], const uint32_t hlo, const uint32_t blo, const uint32_t* s_aoff,
+                                               const int gt, const int MT, const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep,
+                                               const uint32_t a_half, const bool first) {
+  static_assert(MTM >= 1 && MTM <= 4, "1..4 stacked tiles");
+  if (MT == 1) halo_issue_nk<1>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+  else if constexpr (MTM >= 2) {
+    if (MT == 2) halo_issue_nk<2>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+    else if constexpr (MTM >= 3) {
+      if (MT == 3) halo_issue_nk<3>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+      else if constexpr (MTM >= 4) halo_issue_nk<4>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+    }
   }
+  wg_wait<0>();
 }
 
 template <int BN>
-__global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
+__global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
                                                         const __grid_constant__ HaloMaps maps, const int use_tma, const int G) {
   // One weight pipeline stage = the tiles of G consecutive taps of one 64-channel chunk (contiguous in the pre-tiled operand, ONE
-  // bulk copy): the single MMA-issuing thread then pays the per-stage cost (mbarrier wait, tcgen05 fence, election, commits: several
-  // hundred clocks of dependent single-thread latency, measured with the CIS_TRACE build) once per 4*MT*G MMAs instead of once per
-  // 4*MT -- that cost, not the tensor pipe, bounded every launch of round 1.
+  // bulk copy): the MMA warpgroup pays the per-stage cost (mbarrier wait, wgmma fence / commit / wait, release) once per 4*MT*G
+  // MMAs instead of once per 4*MT.
   constexpr int kBStage = BN * 128;
   constexpr int kHMmaWarp_ = HaloCfg<BN>::kMmaWarp, kHThreads_ = HaloCfg<BN>::kThreads;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * 2 + 2 * kHaloMaxBStages + 1];
-  __shared__ uint32_t tmem_slot;
   __shared__ uint32_t s_aoff[CIS_MAX_TAPS];   // tap origin inside the halo, in descriptor start-field units (16 B)
   __shared__ SrcS s_src[CIS_MAX_SRC];
 
@@ -730,7 +676,6 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
   const int nchunks = min(cper, nchunks_all - cc_lo);   // chunks handled by this CTA (host guarantees >= 1)
   __shared__ __align__(16) float s_bias[BN];
   pdl_launch_dependents();
-  const uint32_t ncols = (MT * BN <= 32) ? 32u : (MT * BN <= 64) ? 64u : (MT * BN <= 128) ? 128u : (MT * BN <= 256) ? 256u : 512u;
 
   if (tid < ntaps) s_aoff[tid] = (uint32_t)((p.dh[tap0 + tid] * Wh + p.dw[tap0 + tid]) * 8);   // * 128 B / 16
   if (tid < p.nsrc) {
@@ -746,29 +691,22 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
     const int y = pa + d * gy, x = pb + d * gx;
     pixtab[q] = (gy >= 0 && gx >= 0 && y < p.H && x < p.W) ? (y * p.W + x) : -1;
   }
-  if (warp == kHMmaWarp_) {
-    if (lane == 0) {
-      for (int s = 0; s < 2; ++s) {
-        mbar_init(bar_hfull + 8 * s, use_tma ? 1 : 96);
-        mbar_init(bar_hempty + 8 * s, 1);
-      }
-      for (int s = 0; s < BS; ++s) {
-        mbar_init(bar_bfull + 8 * s, 1);   // one expect_tx arrival; the bulk copy completes the transaction bytes
-        mbar_init(bar_bempty + 8 * s, 1);  // one commit by the MMA thread
-      }
-      mbar_init(bar_accum, 1);
-      fence_mbar_init();
+  if (tid == kHMmaWarp_ * 32) {
+    for (int s = 0; s < 2; ++s) {
+      mbar_init(bar_hfull + 8 * s, use_tma ? 1 : 96);
+      mbar_init(bar_hempty + 8 * s, 1);
     }
-    __syncwarp();
-    tmem_alloc_dyn(smem_u32(&tmem_slot), ncols);
+    for (int s = 0; s < BS; ++s) {
+      mbar_init(bar_bfull + 8 * s, 1);   // one expect_tx arrival; the bulk copy completes the transaction bytes
+      mbar_init(bar_bempty + 8 * s, 1);  // one release by the MMA warpgroup
+    }
+    mbar_init(bar_accum, 128);           // every thread of the MMA warpgroup, after storing its accumulator fragments
+    fence_mbar_init();
   }
   if (use_tma && tid < p.nsrc) tma_prefetch_desc(&maps.m[tid]);   // descriptors live in the kernel parameters: fetch them before the grid dependency resolves
   pdl_wait();
   if (tid < BN) s_bias[tid] = p.bias ? p.bias[ny * BN + tid] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   if (tid == 0) CIS_TRACE_AT(0);
 
   if (warp < kHMmaWarp_) {
@@ -872,44 +810,43 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
     __syncwarp();
    }
 
-    // ------------------------------------------------------------------ epilogue: warps w and w + 4 share TMEM lane quarter w % 4 and
-    // split the columns (the epilogue is instruction-bound on its warps: ~6k clk per 128x128 tile with four of them, r02 trace)
+    // ------------------------------------------------------------------ epilogue: warps w and w + 4 share accumulator rows
+    // 32 (w % 4) .. 32 (w % 4) + 31 and split the columns (the epilogue is instruction-bound on its warps)
     mbar_wait(bar_accum, 0);
-    tc_fence_after();
     if (tid == 0) CIS_TRACE_AT(2);
     const int qtr = warp & 3, half = warp >> 2;
     const int r = qtr * 32 + lane;
     const int c_lo = (kHMmaWarp_ == 8) ? half * (BN / 2) : 0, c_hi = (kHMmaWarp_ == 8) ? c_lo + BN / 2 : BN;
-    const uint32_t t_qtr = tmem + ((uint32_t)(qtr * 32) << 16);
+    const uint32_t t_qtr = tile_base + (uint32_t)r * 16;            // tile m at + m * BN columns (the operand buffers are dead)
     const int cbase = ny * BN;
     const int tile_id = blockIdx.x * gridDim.y + ny;
     if (nsplit > 1 && p.sk_cluster) {
-      // cluster split-K: the MT partial tiles -> own shared memory (operand buffers are dead: every MMA has completed); reduced below
-      for (int m = 0; m < MT; ++m)
-        if (c_lo < c_hi) tmem_to_stage(t_qtr + m * BN, r, tile_base + (uint32_t)m * (kBM * BN * 4), c_lo, c_hi);
+      // cluster split-K: the MT partial tiles already sit in this CTA's shared memory in the layout the reduction below reads
     } else if (nsplit > 1) {
       // two-launch split-K: this split's private fp32 slices; splitk_finish_kernel reduces them and runs the fused epilogue
       for (int m = 0; m < MT; ++m)
         if (c_lo < c_hi)
-          splitk_store_partial<BN>(p.sk_scratch + (((size_t)tile_id * MT + m) * nsplit + blockIdx.z) * kBM * BN, t_qtr + m * BN, r, c_lo, c_hi);
+          splitk_store_partial<BN>(p.sk_scratch + (((size_t)tile_id * MT + m) * nsplit + blockIdx.z) * kBM * BN,
+                                   t_qtr + (uint32_t)(m * BN) * kAccColBytes, r, c_lo, c_hi);
     } else if (c_lo < c_hi) {
       for (int m = 0; m < MT; ++m) {
         const int gy = ty * 16 * MT + 16 * m + (r >> 3), gx = tx * 8 + (r & 7);
         const int oy = pa + d * gy, ox = pb + d * gx;
         const bool valid = oy < OHs && ox < OWs;
         const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + oa) * p.DW + ox * p.osw + ob) : 0;
-        epi_cols<BN>(p, t_qtr + m * BN, cbase, dpix, valid, s_bias, c_lo, c_hi);
+        epi_cols<BN>(p, t_qtr + (uint32_t)(m * BN) * kAccColBytes, cbase, dpix, valid, s_bias, c_lo, c_hi);
       }
     }
   } else {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, 0, 0);
+    // ------------------------------------------------------------------ MMA warpgroup
+    const int wtid = tid - kHMmaWarp_ * 32;
+    constexpr int MTM = HaloCfg<BN>::kMaxMT;
+    float acc[MTM][BN];
     const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
     const uint32_t a_mstep = (uint32_t)(16 * Wh * 128) >> 4;   // descriptor start-field step between stacked M tiles
+    const uint32_t a_half = (uint32_t)(8 * Wh * 128) >> 4;     // rows 64..127 of a tile: 8 halo rows further
     int bs = 0, hs = 0, it = 0;
     uint32_t bph = 0, hph = 0;
-    int vlast = nchunks * nph - 1;                       // last virtual chunk that has taps
-    while (nph > 1 && vlast > 0 && p.ph_tap[vlast % nph + 1] == p.ph_tap[vlast % nph]) --vlast;
     bool any = false;
     for (int vc = 0; vc < nchunks * nph; ++vc) {
       const int cc = vc / nph, ph = vc - cc * nph;
@@ -918,28 +855,19 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
       const int rem = m_chunks - (cc_lo + cc) * 8;
       const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
       mbar_wait(bar_hfull + 8 * hs, hph);
-      if (vc == 0 && lane == 0) CIS_TRACE_AT(1);
+      if (vc == 0 && wtid == 0) CIS_TRACE_AT(1);
       const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16);
       for (int t0 = tlo; t0 < thi; t0 += G, ++it) {
         const int gt = min(G, thi - t0);
         mbar_wait(bar_bfull + 8 * bs, bph);
-        tc_fence_after();
-        if (elect_one()) {
-          CIS_TRACE_AT(8 + 2 * it);
-          const uint32_t blo = desc_lo(b_base + bs * stage_bytes, 16);
-          const bool first = !any;
-          if (nk16 == 4) halo_issue_stage<4>(tmem, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-          else if (nk16 == 1) halo_issue_stage<1>(tmem, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-          else if (nk16 == 2) halo_issue_stage<2>(tmem, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-          else halo_issue_stage<3>(tmem, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-          umma_commit(bar_bempty + 8 * bs);
-          if (t0 + G >= thi) {
-            umma_commit(bar_hempty + 8 * hs);
-            if (vc == vlast) umma_commit(bar_accum);
-          }
+        if (wtid == 0) CIS_TRACE_AT(8 + 2 * it);
+        const uint32_t blo = desc_lo(b_base + bs * stage_bytes, 16);
+        halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, !any);
+        if (wtid == 0) {
+          mbar_arrive(bar_bempty + 8 * bs);
+          if (t0 + G >= thi) mbar_arrive(bar_hempty + 8 * hs);
           CIS_TRACE_AT(9 + 2 * it);
         }
-        __syncwarp();
         any = true;
         if (++bs == BS) {
           bs = 0;
@@ -951,6 +879,11 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
         hph ^= 1u;
       }
     }
+    // every operand stage has been consumed: the accumulator tiles overlay the operand buffers
+#pragma unroll
+    for (int m = 0; m < MTM; ++m)
+      if (m < MT) acc_store<BN>(acc[m], tile_base + (uint32_t)(m * BN) * kAccColBytes, wtid);
+    mbar_arrive(bar_accum);
   }
   if (nsplit > 1 && p.sk_cluster) {
     cluster_sync_all();                       // every CTA's partial tiles are in its shared memory
@@ -967,15 +900,12 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, HaloCfg<BN>::kMinCtas) 
     }
     cluster_sync_all();                       // peers may still be reading this CTA's shared memory
   }
-  tc_fence_before();
-  __syncthreads();
   if (tid == 0) CIS_TRACE_AT(3);
-  if (warp == kHMmaWarp_) tmem_dealloc_dyn(tmem, ncols);
 }
 
 // ======================================================================================================= split-K finish
-// Second launch of split-K.  (Round 1 let the last-arriving CTA of a tile read all nsplit x 64 KB slices by itself -- one SM pulling up
-// to 1 MB through L2 -- which cost more than the split saved on the low-resolution layers it is meant for.)  Here the reduction + fused
+// Second launch of split-K (letting the last-arriving CTA of a tile read all nsplit x 64 KB slices by itself would pull up to 1 MB
+// through one SM).  Here the reduction + fused
 // epilogue of a tile is spread over 128 * BN/16 threads of several CTAs: thread = (accumulator row, 16-column group), row fastest so
 // the reads of the float4-column slices coalesce (the bf16 output is 1 / (2 * nsplit) of the bytes: its 32-byte pieces matter less).
 template <int BN>
@@ -1031,25 +961,24 @@ __global__ void __launch_bounds__(256) splitk_finish_kernel(const __grid_constan
 }
 // ======================================================================================================= persistent halo conv
 // Same math as conv_halo_kernel (TMA halo path only) for layers with MANY output tiles per SM (high-resolution thin layers), where the
-// per-CTA prologue (barrier init, TMEM allocation, first TMA round trip: ~3k clk) and epilogue (TMEM read-back + stores on one warp
-// per scheduler: 2-17k clk) of the one-tile-per-CTA kernel cost more than its MMA loop (CIS_TRACE build, r02).  Here a CTA is
-// persistent and fully warp-specialised so those phases of neighbouring tiles overlap:
-//   warp 0: halo TMA producer (NHS stages) | warp 1: weight producer | warp 2: MMA issuer | warp 3: TMEM owner
-//   warps 4-7 / 8-11: two epilogue groups (TMEM lane quarter = warp % 4); tile i uses accumulator stage i % AS and group i % AS.
+// per-CTA prologue (barrier init, first TMA round trip) and epilogue (accumulator read-back + stores) of the one-tile-per-CTA kernel
+// cost more than its MMA loop.  Here a CTA is persistent and fully warp-specialised so those phases of neighbouring tiles overlap:
+//   warps 0-3: MMA warpgroup | warps 4-7 / 8-11: two epilogue groups (accumulator rows 32 (warp % 4) ..) | warp 12: halo TMA
+//   producer (NHS stages) | warp 13: weight producer.  Tile i is handed over in shared-memory accumulator stage i % AS to group i % AS.
 // Weights: resident (ws = 1: the whole set of nchunks*ntaps tiles is fetched once per CTA and stays in shared memory while the CTA
 // walks its tiles) when it fits, else re-streamed per tile in stages of G taps through a ring of BS stages.
 // Every role walks the same static work list  w = blockIdx.x, blockIdx.x + gridDim.x, ...  of output tiles.
-static constexpr int kPThreads = 384;
+static constexpr int kPThreads = 448;
+static constexpr int kPMaxAccCols = 64;    // MT * BN limit of the persistent kernel (register accumulators next to 13 other warps)
 
 template <int BN>
-__global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes,
+__global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes,
                                                                        const int BS, const int NHS, const int AS, const int G,
                                                                        const __grid_constant__ HaloMaps maps, const int ws) {
   constexpr int kBStage = BN * 128;
   constexpr int kMaxHS = 4;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * kMaxHS + 2 * kHaloMaxBStages + 4];
-  __shared__ uint32_t tmem_slot;
   __shared__ uint32_t s_aoff[CIS_MAX_TAPS];
   __shared__ __align__(16) float s_bias[BN];
 
@@ -1058,7 +987,8 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
   const int Wh = 8 + p.ex, Hh = 16 * MT + p.ey, HP = Wh * Hh;
   const uint32_t stage_bytes = (uint32_t)G * kBStage;
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  const uint32_t h_base = tile_base, b_base = tile_base + NHS * halo_stage_bytes;
+  const uint32_t acc_bytes = (uint32_t)(MT * BN) * kAccColBytes;     // one accumulator stage (a multiple of 8 KB)
+  const uint32_t acc_base = tile_base, h_base = tile_base + AS * acc_bytes, b_base = h_base + NHS * halo_stage_bytes;
   const uint32_t bar_hfull = smem_u32(&bars[0]), bar_hempty = smem_u32(&bars[kMaxHS]);
   const uint32_t bar_bfull = smem_u32(&bars[2 * kMaxHS]), bar_bempty = smem_u32(&bars[2 * kMaxHS + kHaloMaxBStages]);
   const uint32_t bar_tfull = smem_u32(&bars[2 * kMaxHS + 2 * kHaloMaxBStages]), bar_tempty = smem_u32(&bars[2 * kMaxHS + 2 * kHaloMaxBStages + 2]);
@@ -1068,44 +998,34 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
   int m_chunks = 0;
   for (int i = 0; i < p.nsrc; ++i) m_chunks += p.src[i].chunks;
   const int nchunks = (m_chunks + 7) / 8;
-  const uint32_t acc_cols = (uint32_t)(MT * BN);
-  const uint32_t want = acc_cols * AS;
-  const uint32_t ncols = want <= 32 ? 32u : want <= 64 ? 64u : want <= 128 ? 128u : want <= 256 ? 256u : 512u;
 
   pdl_launch_dependents();
   if (tid < p.ntaps) s_aoff[tid] = (uint32_t)((p.dh[tid] * Wh + p.dw[tid]) * 8);
-  if (warp == 3) {
-    if (lane == 0) {
-      for (int s = 0; s < NHS; ++s) {
-        mbar_init(bar_hfull + 8 * s, 1);
-        mbar_init(bar_hempty + 8 * s, 1);
-      }
-      for (int s = 0; s < BS; ++s) {
-        mbar_init(bar_bfull + 8 * s, 1);
-        mbar_init(bar_bempty + 8 * s, 1);
-      }
-      for (int s = 0; s < AS; ++s) {
-        mbar_init(bar_tfull + 8 * s, 1);
-        mbar_init(bar_tempty + 8 * s, 4);   // one arrival per warp of the epilogue group that drained the stage
-      }
-      fence_mbar_init();
+  if (tid == 0) {
+    for (int s = 0; s < NHS; ++s) {
+      mbar_init(bar_hfull + 8 * s, 1);
+      mbar_init(bar_hempty + 8 * s, 1);
     }
-    __syncwarp();
-    tmem_alloc_dyn(smem_u32(&tmem_slot), ncols);
+    for (int s = 0; s < BS; ++s) {
+      mbar_init(bar_bfull + 8 * s, 1);
+      mbar_init(bar_bempty + 8 * s, 1);
+    }
+    for (int s = 0; s < AS; ++s) {
+      mbar_init(bar_tfull + 8 * s, 128);  // every thread of the MMA warpgroup, after storing its fragments
+      mbar_init(bar_tempty + 8 * s, 4);   // one arrival per warp of the epilogue group that drained the stage
+    }
+    fence_mbar_init();
   }
   if (tid < p.nsrc) tma_prefetch_desc(&maps.m[tid]);
   pdl_wait();
   if (tid < BN) s_bias[tid] = p.bias ? p.bias[tid] : 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
   if (tid == 0) {
     CIS_TRACE_AT(0);
     CIS_TRACE_AT(4);      // slot 4 marks a persistent-kernel trace (tools/trace_persist.py)
   }
 
-  if (warp == 0) {
+  if (warp == 12) {
     // ------------------------------------------------------------------ halo producer
     if (lane == 0) {
       int hs = 0;
@@ -1133,7 +1053,7 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
         }
       }
     }
-  } else if (warp == 1) {
+  } else if (warp == 13) {
     // ------------------------------------------------------------------ weight producer
     if (lane == 0) {
       const uint8_t* wt = reinterpret_cast<const uint8_t*>(p.wpack);
@@ -1165,52 +1085,36 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
         }
       }
     }
-  } else if (warp == 2) {
-    // ------------------------------------------------------------------ MMA issuer
-    constexpr uint32_t idesc = make_idesc_bf16(kBM, BN, 0, 0);
+  } else if (warp < 4) {
+    // ------------------------------------------------------------------ MMA warpgroup
+    const int wtid = tid;
+    constexpr int MTM = (kPMaxAccCols / BN) < 4 ? kPMaxAccCols / BN : 4;
+    float acc[MTM][BN];
     const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
     const uint32_t a_mstep = (uint32_t)(16 * Wh * 128) >> 4;
+    const uint32_t a_half = (uint32_t)(8 * Wh * 128) >> 4;
     int hs = 0, bs = 0, as = 0;
     uint32_t hph = 0, bph = 0, tph = 1;
-    if (ws && (int)blockIdx.x < total) {
-      mbar_wait(bar_bfull, 0u);      // the resident weight set; never released
-      tc_fence_after();
-    }
+    if (ws && (int)blockIdx.x < total) mbar_wait(bar_bfull, 0u);      // the resident weight set; never released
     int wi = 0;
     for (int w = blockIdx.x; w < total; w += gridDim.x, ++wi) {
-      if (lane == 0) CIS_TRACE_AT(8 + 5 * wi);
-      mbar_wait(bar_tempty + 8 * as, tph);
-      tc_fence_after();
-      if (lane == 0) CIS_TRACE_AT(9 + 5 * wi);
-      const uint32_t tacc = tmem + as * acc_cols;
+      if (wtid == 0) CIS_TRACE_AT(8 + 5 * wi);
       for (int cc = 0; cc < nchunks; ++cc) {
         const int rem = m_chunks - cc * 8;
         const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
         mbar_wait(bar_hfull + 8 * hs, hph);
-        if (cc == 0 && lane == 0) CIS_TRACE_AT(10 + 5 * wi);
+        if (cc == 0 && wtid == 0) CIS_TRACE_AT(10 + 5 * wi);
         const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16);
         const int gstep = ws ? p.ntaps : G;
         for (int t0 = 0; t0 < p.ntaps; t0 += gstep) {
           const int gt = min(gstep, p.ntaps - t0);
           if (!ws) mbar_wait(bar_bfull + 8 * bs, bph);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(cc * p.ntaps) * kBStage : b_base + bs * stage_bytes, 16);
-            const bool first = (cc | t0) == 0;
-            if (nk16 == 4) halo_issue_stage<4>(tacc, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-            else if (nk16 == 1) halo_issue_stage<1>(tacc, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-            else if (nk16 == 2) halo_issue_stage<2>(tacc, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-            else halo_issue_stage<3>(tacc, hlo, blo, s_aoff + t0, gt, MT, BN, ahi, bhi, a_mstep, idesc, first);
-            if (!ws) umma_commit(bar_bempty + 8 * bs);
-            if (t0 + gstep >= p.ntaps) {
-              umma_commit(bar_hempty + 8 * hs);
-              if (cc == nchunks - 1) {
-                umma_commit(bar_tfull + 8 * as);
-                CIS_TRACE_AT(11 + 5 * wi);
-              }
-            }
+          const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(cc * p.ntaps) * kBStage : b_base + bs * stage_bytes, 16);
+          halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, (cc | t0) == 0);
+          if (wtid == 0) {
+            if (!ws) mbar_arrive(bar_bempty + 8 * bs);
+            if (t0 + gstep >= p.ntaps) mbar_arrive(bar_hempty + 8 * hs);
           }
-          __syncwarp();
           if (!ws && ++bs == BS) {
             bs = 0;
             bph ^= 1u;
@@ -1221,6 +1125,14 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
           hph ^= 1u;
         }
       }
+      // hand the tile to epilogue group `as` once that group has drained the stage's previous tile
+      mbar_wait(bar_tempty + 8 * as, tph);
+      if (wtid == 0) CIS_TRACE_AT(9 + 5 * wi);
+#pragma unroll
+      for (int m = 0; m < MTM; ++m)
+        if (m < MT) acc_store<BN>(acc[m], acc_base + as * acc_bytes + (uint32_t)(m * BN) * kAccColBytes, wtid);
+      mbar_arrive(bar_tfull + 8 * as);
+      if (wtid == 0) CIS_TRACE_AT(11 + 5 * wi);
       if (++as == AS) {
         as = 0;
         tph ^= 1u;
@@ -1238,23 +1150,18 @@ __global__ void __launch_bounds__(kPThreads, 2) conv_halo_persist_kernel(const _
         const int tx = w % tiles_x, r1 = w / tiles_x, ty = r1 % tiles_y, n = r1 / tiles_y;
         mbar_wait(bar_tfull + 8 * grp, tph);
         tph ^= 1u;
-        tc_fence_after();
         for (int m = 0; m < MT; ++m) {
           const int oy = ty * 16 * MT + 16 * m + (r >> 3), ox = tx * 8 + (r & 7);
           const bool valid = oy < p.OH && ox < p.OW;
           const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + p.oa) * p.DW + ox * p.osw + p.ob) : 0;
-          epi_row<BN>(p, tmem + ((uint32_t)(q * 32) << 16) + grp * acc_cols + m * BN, 0, dpix, valid, s_bias);
+          epi_row<BN>(p, acc_base + grp * acc_bytes + (uint32_t)r * 16 + (uint32_t)(m * BN) * kAccColBytes, 0, dpix, valid, s_bias);
         }
-        tc_fence_before();
         __syncwarp();
         if (lane == 0) mbar_arrive(bar_tempty + 8 * grp);
         if (q == 0 && lane == 0) CIS_TRACE_AT(12 + 5 * wi);
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 3) tmem_dealloc_dyn(tmem, ncols);
 }
 
 // ======================================================================================================= wgrad
@@ -1274,16 +1181,15 @@ __global__ void __launch_bounds__(kGThreads) conv_wgrad_kernel(const __grid_cons
   constexpr int S = kWStages;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * S + 1];
-  __shared__ uint32_t tmem_slot;
   __shared__ int s_dh[CIS_MAX_TAPS], s_dw[CIS_MAX_TAPS];
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_full = smem_u32(&bars[0]);
   const uint32_t bar_empty = smem_u32(&bars[S]);
   const uint32_t bar_accum = smem_u32(&bars[2 * S]);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // blockDim = producer/epilogue warps + 1 MMA warp: 4 + 1 on the TMA operand path (one thread issues the loads), 8 + 1 on the
+  // blockDim = producer/epilogue warps + 1 MMA warpgroup: 4 + 4 on the TMA operand path (one thread issues the loads), 8 + 4 on the
   // cp.async gather path, whose address arithmetic is the bottleneck (thin or strided layers)
-  const int nprod = (int)blockDim.x - 32, mma_warp = nprod >> 5;
+  const int nprod = (int)blockDim.x - 128, mma_warp = nprod >> 5;
   pdl_launch_dependents();
   if (tid < p.ntaps) {
     s_dh[tid] = p.dh[tid];
@@ -1301,23 +1207,16 @@ __global__ void __launch_bounds__(kGThreads) conv_wgrad_kernel(const __grid_cons
   const int nkb = kb1 - kb0;
   if (nkb <= 0) return;  // never taken: cis_conv_wgrad rejects split counts that leave a split without work (its slice would be garbage)
 
-  if (warp == mma_warp) {
-    if (lane == 0) {
-      for (int s = 0; s < S; ++s) {
-        mbar_init(bar_full + 8 * s, p.tma ? 1 : nprod);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      mbar_init(bar_accum, 1);
-      fence_mbar_init();
+  if (tid == mma_warp * 32) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(bar_full + 8 * s, p.tma ? 1 : nprod);
+      mbar_init(bar_empty + 8 * s, 1);
     }
-    __syncwarp();
-    tmem_alloc<128>(smem_u32(&tmem_slot));
+    mbar_init(bar_accum, 128);
+    fence_mbar_init();
   }
   pdl_wait();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
   if (warp < mma_warp) {
     if (p.tma) {
@@ -1449,15 +1348,14 @@ __global__ void __launch_bounds__(kGThreads) conv_wgrad_kernel(const __grid_cons
     }
     // epilogue: row = output channel co, columns = packed K columns of this n-tile
     mbar_wait(bar_accum, 0);
-    tc_fence_after();
-    const int co = (warp & 3) * 32 + lane;          // warps w and w + 4 share a TMEM lane quarter and split the 128 columns
-    const uint32_t t_row = tmem + ((uint32_t)((warp & 3) * 32) << 16);
+    const int co = (warp & 3) * 32 + lane;          // warps w and w + 4 share 32 accumulator rows and split the 128 columns
+    const uint32_t t_row = tile_base + (uint32_t)co * 16;
     const int c_lo = mma_warp == 8 ? (warp >> 2) * 64 : 0, c_hi = mma_warp == 8 ? c_lo + 64 : 128;
     const int kcol0 = blockIdx.x * 128;
 #pragma unroll 1
     for (int c0 = c_lo; c0 < c_hi; c0 += 16) {
       float v[16];
-      tmem_ld16(t_row + c0, v);
+      acc_ld16(t_row + (uint32_t)c0 * kAccColBytes, v);
       if (co < p.Cout && kcol0 + c0 < p.K_pad) {     // K_pad % 64 == 0: a 16-column group is inside or outside as a whole
         // this split's private slice, float4-COLUMN layout [K_pad / 4][Cout][4]: the warp's 32 consecutive output channels write 512
         // contiguous bytes per store (row-major [Cout][K_pad] made every store touch 32 lines, the LSU-bound pattern of the split-K slices)
@@ -1469,40 +1367,39 @@ __global__ void __launch_bounds__(kGThreads) conv_wgrad_kernel(const __grid_cons
       }
     }
   } else {
-    constexpr uint32_t idesc = make_idesc_bf16(128, 128, 1, 1);
+    // ------------------------------------------------------------------ MMA warpgroup (both operands MN-major)
+    const int wtid = tid - mma_warp * 32;
+    float acc[128];
     for (int it = 0; it < nkb; ++it) {
       const int s = it % S;
-      const uint32_t ph = (uint32_t)((it / S) & 1);
-      mbar_wait(bar_full + 8 * s, ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t st = tile_base + s * kWStage;
-        // 16 pixels (K) per MMA = 16 rows x 128 B; MN atoms (64 channels) are kWTile apart (LBO), 8-row K groups 1024 B (SBO)
-        const uint32_t alo = desc_lo(st, kWTile), blo = desc_lo(st + 2 * kWTile, kWTile), dhi = desc_hi(1024);
+      mbar_wait(bar_full + 8 * s, (uint32_t)((it / S) & 1));
+      const uint32_t st = tile_base + s * kWStage;
+      // 16 pixels (K) per MMA = 16 rows x 128 B; MN atoms (64 channels) are kWTile apart (LBO), 8-row K groups 1024 B (SBO)
+      const uint32_t alo = desc_lo(st, kWTile), blo = desc_lo(st + 2 * kWTile, kWTile), dhi = desc_hi(1024);
+      wg_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) umma_bf16_lh(tmem, alo + 128 * k, dhi, blo + 128 * k, dhi, idesc, (uint32_t)((it | k) != 0));
-        umma_commit(bar_empty + 8 * s);
-        if (it == nkb - 1) umma_commit(bar_accum);
-      }
-      __syncwarp();
+      for (int k = 0; k < 4; ++k) mma128<128, 1, 1>(acc, alo + 128 * k, dhi, blo + 128 * k, dhi, (uint32_t)kWTile >> 4, (uint32_t)((it | k) != 0));
+      wg_commit();
+      wg_wait<0>();
+      if (wtid == 0) mbar_arrive(bar_empty + 8 * s);
     }
+    acc_store<128>(acc, tile_base, wtid);     // every operand stage has been consumed: the accumulator overlays the ring
+    mbar_arrive(bar_accum);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == mma_warp) tmem_dealloc<128>(tmem);
 }
 
 
 // ======================================================================================================= halo-resident wgrad
-// EXPERIMENTAL (CisWgrad.tma == 2; written after round 1's GPU budget was spent: compiled, never run -- DESIGN.md section 6, E4).
-// Swapped roles: D[kcol][co] = sum_pix x[pix + tap][c] * g[pix][co].  Per 8x8 pixel tile the CTA fetches ONE activation halo
+// CisWgrad.tma == 2.  Swapped roles: D[kcol][co] = sum_pix x[pix + tap][c] * g[pix][co].  Per 8x8 pixel tile the CTA fetches ONE activation halo
 // ((8+ex) x (8+ey) pixels x 64 channels, TMA, SWIZZLE_128B) and ONE gradient tile (8x8 pixels x 64 channels) and reads every tap
 // in place: A = MN-major operand whose two 64-channel atoms are the taps 2q and 2q+1 (descriptor start = origin of tap 2q shifted
 // by two tile rows per K step, LBO = distance between the two tap origins, SBO = Wh*128 between the 8-pixel rows), B = the gradient
-// tile (N = Nh output channels), accumulator columns [q*Nh, (q+1)*Nh).  Relies on the tensor core applying the 128B swizzle on
-// absolute address bits for MN-major operands too (tools/umma_probe_mn.cu checks exactly these descriptor forms).
-// grid = (64-channel chunks of the input, pixel-tile splits, 64-channel halves of Cout); dwp layout = the tma == 1 layout.
+// tile (N = 64 output channels), one 128 x 64 register accumulator per tap pair.  Relies on the tensor core applying the 128B swizzle
+// on absolute address bits for MN-major operands too.  A CTA owns kWHPairs tap pairs (the register budget of its MMA warpgroup).
+// grid = (64-channel chunks of the input, pixel-tile splits, 64-channel halves of Cout x groups of kWHPairs tap pairs); dwp layout =
+// the tma == 1 layout.
 static constexpr int kWHMaxStages = 6;
+static constexpr int kWHPairs = 2;           // tap pairs per CTA: 2 x 64 accumulator columns
 struct WgradHaloMaps {
   CUtensorMap g;                 // (C8, OW, OH, N) gradient slice, box (64, 8, 8, 1)
   CUtensorMap x[CIS_MAX_SRC];    // (C8, W, H, N) activation slices, box (64, Wh, Hh, 1)
@@ -1510,10 +1407,10 @@ struct WgradHaloMaps {
 
 __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_constant__ CisWgrad p, const __grid_constant__ WgradHaloMaps maps,
                                                                     const int Wh, const int Hh, const int hoy, const int hox,
-                                                                    const int stage_bytes, const int S, const int Nh, const int ncols) {
+                                                                    const int stage_bytes, const int S) {
+  constexpr int Nh = 64;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * kWHMaxStages + 1];
-  __shared__ uint32_t tmem_slot;
   __shared__ int s_off[CIS_MAX_TAPS + 1];   // tap origin inside the halo, in pixel rows of 128 B
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t bar_full = smem_u32(&bars[0]);
@@ -1529,30 +1426,25 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
   const int per = (nkb_total + (int)gridDim.y - 1) / (int)gridDim.y;
   const int kb0 = blockIdx.y * per;
   const int nkb = min(per, nkb_total - kb0);
-  if (nkb <= 0) return;   // uniform per CTA: before any barrier / TMEM allocation
+  if (nkb <= 0) return;   // uniform per CTA: before any barrier
   int m_chunks = 0;
   for (int i = 0; i < p.nsrc; ++i) m_chunks += p.src[i].chunks;
   const int nch64 = (m_chunks + 7) / 8;
-  const int c64 = blockIdx.x, half = blockIdx.z;
-  const int npair = (p.ntaps + 1) / 2;
+  const int nhalf = p.Cout > 64 ? 2 : 1;
+  const int c64 = blockIdx.x, half = blockIdx.z % nhalf;
+  const int q0 = (blockIdx.z / nhalf) * kWHPairs;                 // first tap pair of this CTA
+  const int npair = min(kWHPairs, (p.ntaps + 1) / 2 - q0);
 
-  if (warp == 4) {
-    if (lane == 0) {
-      for (int s = 0; s < S; ++s) {
-        mbar_init(bar_full + 8 * s, 1);
-        mbar_init(bar_empty + 8 * s, 1);
-      }
-      mbar_init(bar_accum, 1);
-      fence_mbar_init();
+  if (tid == 128) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, 1);
     }
-    __syncwarp();
-    tmem_alloc_dyn(smem_u32(&tmem_slot), (uint32_t)ncols);
+    mbar_init(bar_accum, 128);
+    fence_mbar_init();
   }
   pdl_wait();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = tmem_slot;
 
   if (warp < 4) {
     if (tid == 0) {
@@ -1582,19 +1474,18 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
     __syncwarp();
     // ---- epilogue: accumulator row r = (tap parity r / 64, input channel r % 64) of every tap pair; columns = output channels
     mbar_wait(bar_accum, 0);
-    tc_fence_after();
     const int r = warp * 32 + lane;
     const int cch = r & 63;
-    const uint32_t t_row = tmem + ((uint32_t)(warp * 32) << 16);
+    const uint32_t t_row = tile_base + (uint32_t)r * 16;
     for (int q = 0; q < npair; ++q) {
-      const int t = 2 * q + (r >> 6);
+      const int t = 2 * (q0 + q) + (r >> 6);
       const bool tv = t < p.ntaps;
       const size_t kcol = ((size_t)t * nch64 + c64) * 64 + cch;
 #pragma unroll 1
       for (int c0 = 0; c0 < Nh; c0 += 16) {
-        float v[16];
-        tmem_ld16(t_row + q * Nh + c0, v);     // whole-warp collective: no early exit before it
         if (!tv) continue;
+        float v[16];
+        acc_ld16(t_row + (uint32_t)(q * Nh + c0) * kAccColBytes, v);
         for (int e = 0; e < 16; ++e) {
           const int co = half * 64 + c0 + e;
           if (co < p.Cout) p.dwp[((size_t)blockIdx.y * p.Cout + co) * p.K_pad + kcol] = v[e];   // private slice; lanes = consecutive kcol: coalesced
@@ -1602,33 +1493,37 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
       }
     }
   } else {
-    const uint32_t idesc = make_idesc_bf16(128, Nh, 1, 1);
+    // ------------------------------------------------------------------ MMA warpgroup (warps 4-7)
+    const int wtid = tid - 128;
+    float acc[kWHPairs][Nh];
     const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
+    const uint32_t kstep = (uint32_t)(2 * Wh * 128) >> 4;                    // 16 pixels = two tile rows of the halo
     for (int it = 0; it < nkb; ++it) {
       const int s = it % S;
       mbar_wait(bar_full + 8 * s, (uint32_t)((it / S) & 1));
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t st = tile_base + s * stage_bytes;
-        const uint32_t blo0 = desc_lo(st + halo_bytes, 8192);
-        for (int q = 0; q < npair; ++q) {
-          const int o0 = s_off[2 * q], o1 = s_off[2 * q + 1];
+      const uint32_t st = tile_base + s * stage_bytes;
+      const uint32_t blo0 = desc_lo(st + halo_bytes, 8192);
+      wg_fence();
+#pragma unroll
+      for (int q = 0; q < kWHPairs; ++q) {
+        if (q < npair) {
+          const int o0 = s_off[2 * (q0 + q)], o1 = s_off[2 * (q0 + q) + 1];
           const uint32_t lbo = (uint32_t)((o1 > o0 ? o1 - o0 : 1) * 128);      // distance between the two tap origins
           const uint32_t alo0 = desc_lo(st + (uint32_t)(o0 * 128), lbo);
-          const uint32_t kstep = (uint32_t)(2 * Wh * 128) >> 4;                // 16 pixels = two tile rows of the halo
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            umma_bf16_lh(tmem + q * Nh, alo0 + k * kstep, ahi, blo0 + 128 * k, bhi, idesc, (uint32_t)((it | k) != 0));
+            mma128<Nh, 1, 1>(acc[q], alo0 + k * kstep, ahi, blo0 + 128 * k, bhi, lbo >> 4, (uint32_t)((it | k) != 0));
         }
-        umma_commit(bar_empty + 8 * s);
-        if (it == nkb - 1) umma_commit(bar_accum);
       }
-      __syncwarp();
+      wg_commit();
+      wg_wait<0>();
+      if (wtid == 0) mbar_arrive(bar_empty + 8 * s);
     }
+#pragma unroll
+    for (int q = 0; q < kWHPairs; ++q)
+      if (q < npair) acc_store<Nh>(acc[q], tile_base + (uint32_t)(q * Nh) * kAccColBytes, wtid);
+    mbar_arrive(bar_accum);
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc_dyn(tmem, (uint32_t)ncols);
 }
 
 }  // namespace cis
@@ -1803,21 +1698,22 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   if (G > ntaps_max) G = ntaps_max;
   const int fixed = nhs * halo_stage + HP * 4 + 1024;
   // two co-resident CTAs per SM overlap one CTA's epilogue with the other's main loop -- when the grid has that many CTAs
-  static const int lim_small_kb = getenv("CIS_HALO_SMALL_KB") ? atoi(getenv("CIS_HALO_SMALL_KB")) : 226;   // grids of <= 148 CTAs
+  static const int lim_small_kb = getenv("CIS_HALO_SMALL_KB") ? atoi(getenv("CIS_HALO_SMALL_KB")) : 226;   // grids of <= one CTA per SM
   static const int lim_kb_wide = getenv("CIS_HALO_LIMIT_KB") ? atoi(getenv("CIS_HALO_LIMIT_KB")) : 113;
   static const int lim_kb_thin = getenv("CIS_HALO_LIMIT_THIN_KB") ? atoi(getenv("CIS_HALO_LIMIT_THIN_KB")) : 113;   // BN <= 32
   const int lim_kb = BN <= 32 ? lim_kb_thin : lim_kb_wide;
-  int limit = (ncta_all > 148 && fixed + 2 * kB <= lim_kb * 1024) ? lim_kb * 1024 : 226 * 1024;
-  if (ncta_all <= 148 && fixed + 2 * kB <= lim_small_kb * 1024) limit = lim_small_kb * 1024;
+  const int nsm = cis_num_sms();
+  int limit = (ncta_all > nsm && fixed + 2 * kB <= lim_kb * 1024) ? lim_kb * 1024 : 226 * 1024;
+  if (ncta_all <= nsm && fixed + 2 * kB <= lim_small_kb * 1024) limit = lim_small_kb * 1024;
   while (G > 1 && fixed + 2 * G * kB > limit) --G;
   const int groups = cper * ((nsub > 1 ? 1 : (ntaps_max + G - 1) / G));   // pipeline stages one CTA walks (grouped: at least one per chunk)
   int BS = (limit - fixed) / (G * kB);
-  if (BS > (ncta_all > 148 ? 4 : kHaloMaxBStages)) BS = ncta_all > 148 ? 4 : kHaloMaxBStages;
+  if (BS > (ncta_all > nsm ? 4 : kHaloMaxBStages)) BS = ncta_all > nsm ? 4 : kHaloMaxBStages;
   if (BS > groups) BS = groups;
   if (BS < 1) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): tile does not fit shared memory");
   int smem = fixed + BS * G * kB;
-  if (nsp > 1 && d->sk_cluster && smem < d->MT * kBM * BN * 4 + 1024) smem = d->MT * kBM * BN * 4 + 1024;   // fp32 staging tiles of the cluster reduction
-  if (smem > 226 * 1024) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): cluster split-K staging does not fit shared memory");
+  if (smem < d->MT * kBM * BN * 4 + 1024) smem = d->MT * kBM * BN * 4 + 1024;   // the fp32 accumulator tiles overlay the operand buffers
+  if (smem > 226 * 1024) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): accumulator tiles do not fit shared memory");
   static int attr_smem = 0;
   if (smem > attr_smem) {
     cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -1852,23 +1748,26 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   const int persist_mode = g_persist_mode >= 0 ? g_persist_mode : (getenv("CIS_PERSIST_MODE") ? atoi(getenv("CIS_PERSIST_MODE")) : 1);
   static const int p_min_tiles = getenv("CIS_PERSIST_MIN_TILES") ? atoi(getenv("CIS_PERSIST_MIN_TILES")) : 296;
   static const int p_ws_kb = getenv("CIS_PERSIST_WS_KB") ? atoi(getenv("CIS_PERSIST_WS_KB")) : 112;
-  if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && nsub == 1 && dd == 1) {
+  if constexpr (BN <= kPMaxAccCols) {
+   if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && nsub == 1 && dd == 1 && d->MT * BN <= kPMaxAccCols) {
     const int total = tiles * d->N;
     const int per_tile = nchunks * d->ntaps;
-    const int AS = (2 * d->MT * BN <= 512) ? 2 : 1;
+    const int acc_stage = d->MT * BN * (int)kAccColBytes;           // one shared-memory accumulator stage
+    const int AS = 2;
+    const int fixed_p = AS * acc_stage + 1024;
     const int ws_bytes = per_tile * kB;
     int p_nhs = nchunks >= 3 ? 4 : 3;
-    while (p_nhs > 2 && p_nhs * halo_stage + 1024 + (ws_bytes <= p_ws_kb * 1024 ? ws_bytes : 2 * G * kB) > 226 * 1024) --p_nhs;
-    const bool ws_fits = ws_bytes <= p_ws_kb * 1024 && p_nhs * halo_stage + 1024 + ws_bytes <= 226 * 1024;
+    while (p_nhs > 2 && p_nhs * halo_stage + fixed_p + (ws_bytes <= p_ws_kb * 1024 ? ws_bytes : 2 * G * kB) > 226 * 1024) --p_nhs;
+    const bool ws_fits = ws_bytes <= p_ws_kb * 1024 && p_nhs * halo_stage + fixed_p + ws_bytes <= 226 * 1024;
     const bool take = persist_mode == 2 || (persist_mode == 3 && ws_fits) || (persist_mode == 1 && ws_fits && total >= p_min_tiles);
     int p_bs = 0, p_smem = 0;
     if (ws_fits) {
       p_bs = 1;
-      p_smem = p_nhs * halo_stage + 1024 + ws_bytes;
+      p_smem = p_nhs * halo_stage + fixed_p + ws_bytes;
     } else {
-      p_bs = (226 * 1024 - p_nhs * halo_stage - 1024) / (G * kB);
+      p_bs = (226 * 1024 - p_nhs * halo_stage - fixed_p) / (G * kB);
       if (p_bs > 4) p_bs = 4;
-      p_smem = p_nhs * halo_stage + 1024 + p_bs * G * kB;
+      p_smem = p_nhs * halo_stage + fixed_p + p_bs * G * kB;
     }
     if (take && p_bs >= (ws_fits ? 1 : 2)) {
       static int attr_p = 0;   // largest dynamic-smem limit set so far on conv_halo_persist_kernel<BN>
@@ -1877,19 +1776,17 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
         if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(conv_halo_persist)");
         attr_p = p_smem;
       }
-      const int want = AS * d->MT * BN;
-      const int tcols = want <= 32 ? 32 : want <= 64 ? 64 : want <= 128 ? 128 : want <= 256 ? 256 : 512;
-      int cps = (227 * 1024) / (p_smem + 1024);          // co-resident persistent CTAs per SM: shared memory, TMEM columns, threads
-      if (cps > 512 / tcols) cps = 512 / tcols;
-      if (cps > 2048 / kPThreads) cps = 2048 / kPThreads;
-      if (cps > 2) cps = 2;
+      int cps = 0;                 // co-resident persistent CTAs per SM (shared memory, registers, threads)
+      cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cps, conv_halo_persist_kernel<BN>, kPThreads, p_smem);
+      if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaOccupancyMaxActiveBlocksPerMultiprocessor(conv_halo_persist)");
       if (cps < 1) cps = 1;
-      int g = total < 148 * cps ? total : 148 * cps;
+      int g = total < nsm * cps ? total : nsm * cps;
       cudaError_t le = launch_pdl(conv_halo_persist_kernel<BN>, dim3(g), dim3(kPThreads), p_smem, st, *d, halo_stage, p_bs, p_nhs, AS, G, maps,
                                   ws_fits ? 1 : 0);
       if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_halo_persist)");
       return cis_check_launch("conv_halo_persist");
     }
+   }
   }
   cudaError_t le = (splits > 1 && d->sk_cluster)
                        ? launch_pdl_zcluster(conv_halo_kernel<BN>, grid, dim3(HaloCfg<BN>::kThreads), smem, st, splits, *d, halo_stage, BS, nhs, maps, use_tma, G)
@@ -1917,7 +1814,7 @@ extern "C" int cis_conv_igemm(const CisConv* d, cis_stream_t stream) {
     return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm: residual slices must be 8-channel aligned");
   cudaStream_t st = (cudaStream_t)stream;
   if (d->halo) {
-    if (d->MT < 1 || d->MT > 4 || d->MT * d->BN > 512 || d->dil < 1 || d->sh != 1 || d->sw != 1 || d->ey < 0 || d->ex < 0 ||
+    if (d->MT < 1 || d->MT > 4 || d->MT * d->BN > kMaxAccCols || d->dil < 1 || d->sh != 1 || d->sw != 1 || d->ey < 0 || d->ex < 0 ||
         (d->dil > 1 && (d->OH != d->H || d->OW != d->W)) || (d->nph > 1 && (d->nph != 4 || d->dil != 1 || d->ph_tap[0] != 0 || d->ph_tap[4] != d->ntaps)))
       return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): bad tile parameters");
     switch (d->BN) {
@@ -1960,16 +1857,12 @@ static int launch_wgrad_halo(const CisWgrad* d, cudaStream_t st) {
   const int halo_bytes = (Wh * Hh * 128 + 1023) & ~1023;
   const int stage = halo_bytes + 8192;
   const int nhalf = d->Cout > 64 ? 2 : 1;
-  int Nh = d->Cout > 64 ? 64 : ((d->Cout + 15) & ~15);
-  const int npair = (d->ntaps + 1) / 2;
-  const int want = npair * Nh;
-  if (want > 512) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_wgrad(halo): accumulators exceed TMEM");
-  const int ncols = want <= 32 ? 32 : want <= 64 ? 64 : want <= 128 ? 128 : want <= 256 ? 256 : 512;
+  const int npg = ((d->ntaps + 1) / 2 + kWHPairs - 1) / kWHPairs;      // groups of kWHPairs tap pairs
   int S = (200 * 1024) / stage;
   if (S > kWHMaxStages) S = kWHMaxStages;
-  if (S > 4 && ncols <= 256) S = 4;       // leave room for a second co-resident CTA when TMEM allows one
   if (S < 2) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_wgrad(halo): halo does not fit shared memory");
-  const int smem = S * stage + 1024;
+  int smem = S * stage + 1024;
+  if (smem < kWHPairs * 64 * (int)kAccColBytes + 1024) smem = kWHPairs * 64 * (int)kAccColBytes + 1024;   // accumulators overlay the stages
   static int attr_smem = 0;
   if (smem > attr_smem) {
     cudaError_t e = cudaFuncSetAttribute(conv_wgrad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
@@ -1984,8 +1877,8 @@ static int launch_wgrad_halo(const CisWgrad* d, cudaStream_t st) {
   bool ok = encode_src_map(&maps.g, gs, d->N, d->OH, d->OW, 8, 8);
   for (int i = 0; ok && i < d->nsrc; ++i) ok = encode_src_map(&maps.x[i], d->src[i], d->N, d->H, d->W, Wh, Hh);
   if (!ok) return cis_set_error(CIS_ERR_CUDA, "cis_conv_wgrad(halo): cuTensorMapEncodeTiled failed / unavailable");
-  dim3 grid(nch64, d->splits, nhalf);
-  cudaError_t le = launch_pdl(conv_wgrad_halo_kernel, grid, dim3(kThreads), (size_t)smem, st, *d, maps, Wh, Hh, hoy, hox, stage, S, Nh, ncols);
+  dim3 grid(nch64, d->splits, nhalf * npg);
+  cudaError_t le = launch_pdl(conv_wgrad_halo_kernel, grid, dim3(kThreads), (size_t)smem, st, *d, maps, Wh, Hh, hoy, hox, stage, S);
   if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_wgrad_halo)");
   return cis_check_launch("conv_wgrad_halo");
 }

@@ -42,7 +42,7 @@ __device__ __forceinline__ void pack_weights_body(size_t i, const float* __restr
   wp[i] = __float2bfloat16(v);
 }
 // Pre-swizzled weight tiles for the halo kernel: block (ny, cc, t) = BN rows x 128 B, row n holds K = 64 channels of chunk cc for
-// tap t with the SWIZZLE_128B pattern already applied (16-byte chunk index ^= n & 7), so a plain bulk copy lands the UMMA layout.
+// tap t with the SWIZZLE_128B pattern already applied (16-byte chunk index ^= n & 7), so a plain bulk copy lands the wgmma operand layout.
 __device__ __forceinline__ void pack_weights_tiled_body(size_t i, const float* __restrict__ w, const int* __restrict__ kmap, int cin8, int ntaps,
                                                         int n_tiles, int BN, int cout, int sn, const int* __restrict__ nmap,
                                                         bf16* __restrict__ out) {
@@ -144,8 +144,8 @@ __device__ __forceinline__ void bn_fold_body(size_t i, const float* __restrict__
   if (i < (size_t)cout) b_eff[i] = bias[i] * gamma[i] * BN_RSQRT + beta[i];
 }
 // one 256-thread block per 8 output channels: thread = (channel co0 + tid % 8, row lane tid / 8), so a row of 8 channels is one 32-byte
-// sector and every byte fetched is used.  (r02: one block per channel walked a column of the [rows][cout] matrix -- 4 useful bytes per
-// sector, 96 us for the generator's 1.45 M parameters; this form moves the same data in ~10 us.)  Fixed summation order.
+// sector and every byte fetched is used (one block per channel walking a column of the [rows][cout] matrix would use 4 bytes of every
+// 32-byte sector).  Fixed summation order.
 static constexpr int kBnChainCo = 8;
 __device__ __forceinline__ void bn_chain_body(int blk, const float* __restrict__ w, const float* __restrict__ bias, const float* __restrict__ gamma,
                                               float* __restrict__ dwe, const float* __restrict__ dbe, size_t nw, int cout,
@@ -1004,8 +1004,8 @@ __global__ void cis_loss_fwd_kernel(const float* __restrict__ flow, const float*
     a[3] += m * e[2];           // den_red       :179
     a[4] += (1.f - m) * e[2];   // den_red_compl :186
   }
-  // block-level reduction first: one fp64 atomic per (block, sum) instead of one per warp -- 23.7 k atomics on 20 addresses serialised
-  // in L2 for ~25 us of this kernel's 31 us, between the forward and the backward pass of every step
+  // block-level reduction first: one fp64 atomic per (block, sum) instead of one per warp -- tens of thousands of atomics on 20
+  // addresses would serialise in L2 between the forward and the backward pass of every step
   __shared__ float red[8][5];
 #pragma unroll
   for (int k = 0; k < 5; ++k) {
@@ -1102,8 +1102,8 @@ __global__ void mask_bwd_kernel(const float* __restrict__ flow, const float* __r
 __global__ void grad_avg_abs_kernel(const float* __restrict__ g, const long long* __restrict__ seg, int nseg, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
-  // grid = (variables, kAvgAbsChunks): a variable of 2.4 M elements walked by ONE block took 82 us (r02 launch list) -- on the critical
-  // path between the backward pass and the optimiser of every generator step
+  // grid = (variables, kAvgAbsChunks): a variable of 2.4 M elements walked by ONE block is slow -- and on the critical path between
+  // the backward pass and the optimiser of every generator step
   const int s = blockIdx.x;
   const long long a = seg[2 * s], e = seg[2 * s + 1];
   const long long per = (e - a + gridDim.y - 1) / gridDim.y;
@@ -1410,7 +1410,7 @@ int cis_charbonnier_sum(const float* gt, const float* pred, const float* mask, i
 }
 int cis_cis_loss_fwd(const float* flow, const float* mask, const float* flow1, int32_t B, int32_t H, int32_t W, int32_t h1, int32_t w1, float cbn,
                      double* sums, float* pred_out, cis_stream_t stream) {
-  dim3 grid(148, B);
+  dim3 grid(cis_num_sms(), B);
   CIS_LAUNCH(cis_loss_fwd_kernel, grid, 256, 0, ST, flow, mask, flow1, B, H, W, h1, w1, cbn, sums, pred_out);
   return cis_check_launch("cis_loss_fwd");
 }

@@ -1,10 +1,10 @@
-"""Frozen PWC-Net 'lg-6-2' (dense + residual/context) forward on the sm_100a kernels.
+"""Frozen PWC-Net 'lg-6-2' (dense + residual/context) forward on the sm_90a kernels.
 
 Mirrors models/PWCNet/model_pwcnet.py of the reference: extract_features :149-168, warp :173-245 (core_warp.py:153-202),
 corr :291-340 (core_costvol.py:20-40), predict_flow :476-506, refine_flow :559-576, deconv :283-286, nn :581-649,
 predict_from_img_pairs :61-76.  Forward only: the optimiser var_lists exclude 'pwcnet' (adversarial_learner.py:211-234).
 
-B200 layout: each pyramid level owns ONE NHWC bf16 buffer that holds the whole DenseNet concat
+Buffer layout: each pyramid level owns ONE NHWC bf16 buffer that holds the whole DenseNet concat
 [act4 32|act3 64|act2 96|act1 128|act0 128|corr 81(+7)|c1 C|up_flow 2,up_feat 2(+4)]; every conv writes its output straight
 into its channel slice (tf.concat never materialises), the fused warp+cost-volume kernel writes the 81 correlation
 channels, and the 4x4 stride-2 transposed convs of the level above write up_flow/up_feat into the tail.

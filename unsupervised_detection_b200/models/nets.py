@@ -1,4 +1,4 @@
-"""Generator (mask) and recover (flow-inpainter) networks on the sm_100a conv engine.
+"""Generator (mask) and recover (flow-inpainter) networks on the sm_90a conv engine.
 
 Mirrors models/nets.py of the reference (generator_net :4-42, recover_net :45-110) and the layer primitives of
 models/utils/convolution_utils.py (gen_conv :26-53, gen_deconv :55-75, conv :77-85, deconv :87-90); same layer names,
