@@ -72,7 +72,7 @@ typedef struct {
    * shifted wgmma descriptors.  dh/dw then hold tap offsets >= 0 relative to the halo origin, in units of `dil` pixels. */
   int32_t halo;      /* 0: generic per-tap gather kernel, 1: halo-resident kernel */
   int32_t dil;       /* dilation = phase period (1 for undilated) */
-  int32_t MT;        /* 1..4 stacked M tiles (MT*BN <= 128 register accumulator columns) */
+  int32_t MT;        /* 1..4 stacked M tiles per MMA warpgroup (MT*BN <= 128 register accumulator columns); see nwg */
   int32_t hoy, hox;  /* halo origin relative to the tile origin (phase units, <= 0) */
   int32_t ey, ex;    /* halo extent beyond the tile (max tap offset) */
   /* Split-K for launches that cover only a few SMs (low-resolution layers): grid.z = splits CTAs share one output tile, each reduces a
@@ -80,7 +80,7 @@ typedef struct {
    * tile to a private slice of sk_scratch; a second kernel launched by the same call sums the slices in a fixed order
    * (deterministic) and runs the fused epilogue spread over many CTAs. */
   int32_t splits;        /* 0/1 = off */
-  float* sk_scratch;     /* >= tiles * splits * 128 * BN floats (tiles = grid.x * grid.y * MT); need not be initialised */
+  float* sk_scratch;     /* >= tiles * splits * 128 * BN floats (tiles = grid.x * grid.y * MT * max(nwg, 1)); need not be initialised */
   int32_t* sk_counters;  /* must be NULL (the single-launch ticket mode of round 1 was removed; the field keeps the struct layout) */
   /* Stride-2 forward convolution on the halo kernel (halo = 1, sh = sw = 1 in this descriptor, H x W = the INPUT size): the input is
    * read as nph = 4 space-to-depth phases in(2y + py, 2x + px), phase index py*2 + px; taps are listed phase by phase in PHASE
@@ -102,6 +102,9 @@ typedef struct {
     int32_t OH, OW, oa, ob;   /* output extent and offset inside the (DH, DW) destination grid (stride osh / osw) */
     const void* wpack;        /* pre-tiled weights of this sub-problem */
   } sub[4];
+  /* halo kernel, BN >= 64: 2 = two MMA warpgroups share every weight stage, each owning MT stacked tiles, so the CTA covers 2*MT tiles
+   * (16*2*MT output rows per column of tiles; split-K scratch and the grid count CTAs of that height).  0/1: one warpgroup. */
+  int32_t nwg;
 } CisConv;
 
 /* Weight gradient of the same convolution: dWp[co][(t,c)] = sum_rows g[row][co] * A[row][(t,c)]  (fp32).  The reduction over rows

@@ -15,7 +15,8 @@ def conv_row(d):
     if d.halo:
         dd = d.dil
         hp0, wp0 = -(-d.OH // dd), -(-d.OW // dd)
-        tiles = (-(-wp0 // 8)) * (-(-hp0 // (16 * d.MT))) * dd * dd * d.N
+        mtc = d.MT * max(d.nwg, 1)          # 16x8 tiles per CTA (nwg MMA warpgroups of MT tiles each)
+        tiles = (-(-wp0 // 8)) * (-(-hp0 // (16 * mtc))) * dd * dd * d.N
         nchunks = -(-chunks // 8)
         steps = nchunks * d.ntaps
         kind = 'halo'
@@ -27,10 +28,10 @@ def conv_row(d):
         wtile = d.BN * 128
     splits = max(1, d.splits)
     ncta = tiles * d.n_tiles * splits
-    return dict(kind=kind, BN=d.BN, nt=d.n_tiles, MT=d.MT if d.halo else 1, N=d.N, OH=d.OH, OW=d.OW, taps=d.ntaps, cin=chunks * 8,
+    return dict(kind=kind, BN=d.BN, nt=d.n_tiles, MT=d.MT if d.halo else 1, nwg=max(d.nwg, 1) if d.halo else 1, N=d.N, OH=d.OH, OW=d.OW, taps=d.ntaps, cin=chunks * 8,
                 tiles=tiles, ncta=ncta, steps=-(-steps // splits), splits=splits, two_launch=bool(splits > 1 and not d.sk_counters),
                 ws_fit=bool(d.halo and d.dil == 1 and d.n_tiles == 1 and d.BN <= 32 and steps >= 2 and
-                            2 * (((8 + d.ex) * (16 * d.MT + d.ey) * 128 + 1023) // 1024 * 1024) + 1024 + steps * wtile <= 200 * 1024),
+                            2 * (((8 + d.ex) * (16 * mtc + d.ey) * 128 + 1023) // 1024 * 1024) + 1024 + steps * wtile <= 200 * 1024),
                 cluster=bool(d.halo and d.BN >= 64 and (tiles % 2 == 0)))
 
 
@@ -45,11 +46,11 @@ def main():
                 r.update(plan=pname, w=w, flops=fl)
                 rows.append(r)
     print('%d conv launches in the three plans; per step (1R:3G): %.1f' % (len(rows), sum(r['w'] for r in rows) / 4.0))
-    print('%-5s %-4s %4s %3s %3s %3s %9s %5s %6s %6s %6s %6s  %s' % ('plan', 'kern', 'BN', 'nt', 'MT', 'N', 'OHxOW', 'taps', 'cin', 'CTAs',
+    print('%-5s %-4s %4s %3s %3s %3s %3s %9s %5s %6s %6s %6s %6s  %s' % ('plan', 'kern', 'BN', 'nt', 'MT', 'nwg', 'N', 'OHxOW', 'taps', 'cin', 'CTAs',
                                                                   'steps', 'split', 'flags'))
     for r in sorted(rows, key=lambda r: (r['ncta'], -r['steps'])):
         flags = ' '.join(k for k in ('two_launch', 'ws_fit', 'cluster') if r[k])
-        print('%-5s %-4s %4d %3d %3d %3d %4dx%-4d %5d %6d %6d %6d %6d  %s' % (r['plan'], r['kind'], r['BN'], r['nt'], r['MT'], r['N'], r['OH'],
+        print('%-5s %-4s %4d %3d %3d %3d %3d %4dx%-4d %5d %6d %6d %6d %6d  %s' % (r['plan'], r['kind'], r['BN'], r['nt'], r['MT'], r['nwg'], r['N'], r['OH'],
                                                                            r['OW'], r['taps'], r['cin'], r['ncta'], r['steps'], r['splits'], flags))
     few = [r for r in rows if r['ncta'] <= 32]
     print('\nlaunches with <= 32 CTAs: %.1f per step, serial steps per CTA: median %d, max %d' %

@@ -47,7 +47,7 @@ class CisConv(C.Structure):
                 ('ey', C.c_int32), ('ex', C.c_int32),
                 ('splits', C.c_int32), ('sk_scratch', C.c_void_p), ('sk_counters', C.c_void_p),
                 ('nph', C.c_int32), ('ph_tap', C.c_int32 * 5), ('sk_cluster', C.c_int32),
-                ('nsub', C.c_int32), ('sub', CisSub * 4)]
+                ('nsub', C.c_int32), ('sub', CisSub * 4), ('nwg', C.c_int32)]
 
 
 class CisWgrad(C.Structure):

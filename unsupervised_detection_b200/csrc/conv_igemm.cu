@@ -40,11 +40,17 @@ static constexpr int kBM = 128;       // GEMM rows per CTA
 static constexpr int kBK = 64;        // bf16 K elements per stage (128-byte swizzled rows)
 static constexpr int kAStage = kBM * 128;
 static constexpr int kThreads = 256;  // halo / wgrad kernels: 4 producer/epilogue warps + 1 MMA warpgroup
-// conv_halo_kernel<BN>: warps 0-3 producers + epilogue; BN >= 64 adds warps 4-7 (epilogue only: the wide epilogue is instruction-bound on its
-// warps); the last four warps = the MMA warpgroup.
-template <int BN> struct HaloCfg {
-  static constexpr int kMmaWarp = BN >= 64 ? 8 : 4;     // first warp of the MMA warpgroup
-  static constexpr int kThreads = (kMmaWarp + 4) * 32;
+// conv_halo_kernel<BN, NWG>: warps 0-3 producers + epilogue, then NWG MMA warpgroups.
+//   NWG = 1: BN >= 64 adds warps 4-7 (epilogue only: the wide epilogue is instruction-bound on its warps) before the MMA warpgroup.
+//   NWG = 2 (BN >= 64): two MMA warpgroups (warps 4-11) consume every weight stage, so each weight byte fetched from L2 feeds twice
+//   the output rows; no epilogue-only warps (384 threads keep the 168-register budget of one warpgroup's 128 accumulator columns),
+//   the MMA warps join the epilogue once their accumulators are in shared memory.
+template <int BN, int NWG> struct HaloCfg {
+  static_assert(NWG == 1 || (NWG == 2 && BN >= 64), "two MMA warpgroups only for BN >= 64");
+  static constexpr int kMmaWarp = (NWG == 1 && BN >= 64) ? 8 : 4;     // first warp of the first MMA warpgroup
+  static constexpr int kThreads = (kMmaWarp + 4 * NWG) * 32;
+  static constexpr int kEpiWarps = NWG == 1 ? kMmaWarp : kThreads / 32;   // warps 0 .. kEpiWarps-1 run the epilogue
+  static constexpr int kEpiParts = NWG == 1 ? (BN >= 64 ? 2 : 1) : BN / 32;   // column parts of a 32-row epilogue unit
   // accumulator registers per MMA thread: MT * BN <= kMaxAccCols (the host never stacks more tiles than that)
   static constexpr int kMaxMT = (128 / BN) < 4 ? (128 / BN) : 4;
 };
@@ -623,23 +629,25 @@ __device__ __forceinline__ void halo_issue_any(const int nk16, float (&acc)[MTM]
   wg_wait<0>();
 }
 
-template <int BN>
-__global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
+template <int BN, int NWG>
+__global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
                                                         const __grid_constant__ HaloMaps maps, const int use_tma, const int G) {
   // One weight pipeline stage = the tiles of G consecutive taps of one 64-channel chunk (contiguous in the pre-tiled operand, ONE
   // bulk copy): the MMA warpgroup pays the per-stage cost (mbarrier wait, wgmma fence / commit / wait, release) once per 4*MT*G
-  // MMAs instead of once per 4*MT.
+  // MMAs instead of once per 4*MT.  With NWG = 2 MMA warpgroups the CTA is MTC = 2 * MT tiles tall: warpgroup w owns tiles
+  // w * MT .. w * MT + MT - 1 of the one shared halo and both consume every weight stage.
+  using Cfg = HaloCfg<BN, NWG>;
   constexpr int kBStage = BN * 128;
-  constexpr int kHMmaWarp_ = HaloCfg<BN>::kMmaWarp, kHThreads_ = HaloCfg<BN>::kThreads;
+  constexpr int kHMmaWarp_ = Cfg::kMmaWarp, kHThreads_ = Cfg::kThreads;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * 2 + 2 * kHaloMaxBStages + 1];
   __shared__ uint32_t s_aoff[CIS_MAX_TAPS];   // tap origin inside the halo, in descriptor start-field units (16 B)
   __shared__ SrcS s_src[CIS_MAX_SRC];
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int MT = p.MT, d = p.dil;
+  const int MT = p.MT, MTC = NWG * MT, d = p.dil;   // MT tiles per MMA warpgroup, MTC per CTA
   const int nph = p.nph > 1 ? p.nph : 1;       // stride-2 forward conv: 4 space-to-depth phases, each with its own halo and tap range
-  const int Wh = 8 + p.ex, Hh = 16 * MT + p.ey, HP = Wh * Hh;
+  const int Wh = 8 + p.ex, Hh = 16 * MTC + p.ey, HP = Wh * Hh;
   const uint32_t stage_bytes = (uint32_t)G * kBStage;
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t h_base = tile_base;                                // NHS halo stages
@@ -658,7 +666,7 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
   const void* const wpack = grouped ? p.sub[blockIdx.z].wpack : p.wpack;
   // ---- tile decode: blockIdx.x -> (tx, ty, phase, n)
   const int Hp0 = (OHs + d - 1) / d, Wp0 = (OWs + d - 1) / d;
-  const int tiles_x = (Wp0 + 7) / 8, tiles_y = (Hp0 + 16 * MT - 1) / (16 * MT);
+  const int tiles_x = (Wp0 + 7) / 8, tiles_y = (Hp0 + 16 * MTC - 1) / (16 * MTC);
   if (grouped && (int)blockIdx.x >= tiles_x * tiles_y * p.N) return;   // the grid is sized for the largest sub-problem (uniform per CTA)
   int bid = blockIdx.x;
   const int tx = bid % tiles_x; bid /= tiles_x;
@@ -687,20 +695,20 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
   }
   for (int q = tid; q < (use_tma ? 0 : HP); q += kHThreads_) {
     const int hy = q / Wh, hx = q - hy * Wh;
-    const int gy = ty * 16 * MT + hy + hoy, gx = tx * 8 + hx + hox;
+    const int gy = ty * 16 * MTC + hy + hoy, gx = tx * 8 + hx + hox;
     const int y = pa + d * gy, x = pb + d * gx;
     pixtab[q] = (gy >= 0 && gx >= 0 && y < p.H && x < p.W) ? (y * p.W + x) : -1;
   }
   if (tid == kHMmaWarp_ * 32) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(bar_hfull + 8 * s, use_tma ? 1 : 96);
-      mbar_init(bar_hempty + 8 * s, 1);
+      mbar_init(bar_hempty + 8 * s, NWG);
     }
     for (int s = 0; s < BS; ++s) {
-      mbar_init(bar_bfull + 8 * s, 1);   // one expect_tx arrival; the bulk copy completes the transaction bytes
-      mbar_init(bar_bempty + 8 * s, 1);  // one release by the MMA warpgroup
+      mbar_init(bar_bfull + 8 * s, 1);     // one expect_tx arrival; the bulk copy completes the transaction bytes
+      mbar_init(bar_bempty + 8 * s, NWG);  // one release per MMA warpgroup
     }
-    mbar_init(bar_accum, 128);           // every thread of the MMA warpgroup, after storing its accumulator fragments
+    mbar_init(bar_accum, 128 * NWG);       // every thread of the MMA warpgroups, after storing its accumulator fragments
     fence_mbar_init();
   }
   if (use_tma && tid < p.nsrc) tma_prefetch_desc(&maps.m[tid]);   // descriptors live in the kernel parameters: fetch them before the grid dependency resolves
@@ -733,7 +741,7 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
           mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
           // dilated layer: the map strides by d pixels from any start, the start carries this CTA's phase (pa, pb)
           tma_load_4d(h_base + hs * halo_stage_bytes, &maps.m[si * nph + ph], bar_hfull + 8 * hs, c * 8, pb + d * (tx * 8 + hox),
-                      pa + d * (ty * 16 * MT + hoy), nmod ? (n % nmod) : n);
+                      pa + d * (ty * 16 * MTC + hoy), nmod ? (n % nmod) : n);
         }
       }
       __syncwarp();
@@ -810,41 +818,16 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
     __syncwarp();
    }
 
-    // ------------------------------------------------------------------ epilogue: warps w and w + 4 share accumulator rows
-    // 32 (w % 4) .. 32 (w % 4) + 31 and split the columns (the epilogue is instruction-bound on its warps)
-    mbar_wait(bar_accum, 0);
-    if (tid == 0) CIS_TRACE_AT(2);
-    const int qtr = warp & 3, half = warp >> 2;
-    const int r = qtr * 32 + lane;
-    const int c_lo = (kHMmaWarp_ == 8) ? half * (BN / 2) : 0, c_hi = (kHMmaWarp_ == 8) ? c_lo + BN / 2 : BN;
-    const uint32_t t_qtr = tile_base + (uint32_t)r * 16;            // tile m at + m * BN columns (the operand buffers are dead)
-    const int cbase = ny * BN;
-    const int tile_id = blockIdx.x * gridDim.y + ny;
-    if (nsplit > 1 && p.sk_cluster) {
-      // cluster split-K: the MT partial tiles already sit in this CTA's shared memory in the layout the reduction below reads
-    } else if (nsplit > 1) {
-      // two-launch split-K: this split's private fp32 slices; splitk_finish_kernel reduces them and runs the fused epilogue
-      for (int m = 0; m < MT; ++m)
-        if (c_lo < c_hi)
-          splitk_store_partial<BN>(p.sk_scratch + (((size_t)tile_id * MT + m) * nsplit + blockIdx.z) * kBM * BN,
-                                   t_qtr + (uint32_t)(m * BN) * kAccColBytes, r, c_lo, c_hi);
-    } else if (c_lo < c_hi) {
-      for (int m = 0; m < MT; ++m) {
-        const int gy = ty * 16 * MT + 16 * m + (r >> 3), gx = tx * 8 + (r & 7);
-        const int oy = pa + d * gy, ox = pb + d * gx;
-        const bool valid = oy < OHs && ox < OWs;
-        const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + oa) * p.DW + ox * p.osw + ob) : 0;
-        epi_cols<BN>(p, t_qtr + (uint32_t)(m * BN) * kAccColBytes, cbase, dpix, valid, s_bias, c_lo, c_hi);
-      }
-    }
   } else {
-    // ------------------------------------------------------------------ MMA warpgroup
-    const int wtid = tid - kHMmaWarp_ * 32;
-    constexpr int MTM = HaloCfg<BN>::kMaxMT;
+    // ------------------------------------------------------------------ MMA warpgroup(s)
+    const int wg = NWG > 1 ? (warp - kHMmaWarp_) >> 2 : 0;
+    const int wtid = tid - (kHMmaWarp_ + 4 * wg) * 32;
+    constexpr int MTM = Cfg::kMaxMT;
     float acc[MTM][BN];
     const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
     const uint32_t a_mstep = (uint32_t)(16 * Wh * 128) >> 4;   // descriptor start-field step between stacked M tiles
     const uint32_t a_half = (uint32_t)(8 * Wh * 128) >> 4;     // rows 64..127 of a tile: 8 halo rows further
+    const uint32_t a_wg = (uint32_t)(wg * MT) * a_mstep;        // this warpgroup's first tile inside the halo
     int bs = 0, hs = 0, it = 0;
     uint32_t bph = 0, hph = 0;
     bool any = false;
@@ -855,18 +838,18 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
       const int rem = m_chunks - (cc_lo + cc) * 8;
       const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
       mbar_wait(bar_hfull + 8 * hs, hph);
-      if (vc == 0 && wtid == 0) CIS_TRACE_AT(1);
-      const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16);
+      if (vc == 0 && wtid == 0 && wg == 0) CIS_TRACE_AT(1);
+      const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16) + a_wg;
       for (int t0 = tlo; t0 < thi; t0 += G, ++it) {
         const int gt = min(G, thi - t0);
         mbar_wait(bar_bfull + 8 * bs, bph);
-        if (wtid == 0) CIS_TRACE_AT(8 + 2 * it);
+        if (wtid == 0 && wg == 0) CIS_TRACE_AT(8 + 2 * it);
         const uint32_t blo = desc_lo(b_base + bs * stage_bytes, 16);
         halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, !any);
-        if (wtid == 0) {
+        if (wtid == 0) {   // one release per warpgroup
           mbar_arrive(bar_bempty + 8 * bs);
           if (t0 + G >= thi) mbar_arrive(bar_hempty + 8 * hs);
-          CIS_TRACE_AT(9 + 2 * it);
+          if (wg == 0) CIS_TRACE_AT(9 + 2 * it);
         }
         any = true;
         if (++bs == BS) {
@@ -879,20 +862,51 @@ __global__ void __launch_bounds__(HaloCfg<BN>::kThreads, 1) conv_halo_kernel(con
         hph ^= 1u;
       }
     }
-    // every operand stage has been consumed: the accumulator tiles overlay the operand buffers
+    // every operand stage has been consumed: the accumulator tiles overlay the operand buffers.  Two warpgroups: the other one may
+    // still be reading the last stages, so both finish their wgmma before either overwrites them.
+    if constexpr (NWG > 1) asm volatile("bar.sync 1, %0;" ::"n"(128 * NWG) : "memory");
 #pragma unroll
     for (int m = 0; m < MTM; ++m)
-      if (m < MT) acc_store<BN>(acc[m], tile_base + (uint32_t)(m * BN) * kAccColBytes, wtid);
+      if (m < MT) acc_store<BN>(acc[m], tile_base + (uint32_t)((wg * MT + m) * BN) * kAccColBytes, wtid);
     mbar_arrive(bar_accum);
+  }
+
+  if (warp < Cfg::kEpiWarps) {
+    // ------------------------------------------------------------------ epilogue: unit u = (tile m, 32-row quarter, column part); warp w
+    // takes units w, w + kEpiWarps, ...  (NWG = 1, BN >= 64: warps w and w + 4 share accumulator rows 32 (w % 4) .. 32 (w % 4) + 31 and
+    // split the columns -- the epilogue is instruction-bound on its warps)
+    mbar_wait(bar_accum, 0);
+    if (tid == 0) CIS_TRACE_AT(2);
+    constexpr int kParts = Cfg::kEpiParts, kCols = BN / kParts, kUnits = 4 * kParts;
+    const int cbase = ny * BN;
+    const int tile_id = blockIdx.x * gridDim.y + ny;
+    // cluster split-K: the MTC partial tiles already sit in this CTA's shared memory in the layout the reduction below reads
+    if (!(nsplit > 1 && p.sk_cluster)) {
+#pragma unroll 1
+      for (int u = warp; u < MTC * kUnits; u += Cfg::kEpiWarps) {
+        const int m = u / kUnits, r = (u & 3) * 32 + lane, c_lo = ((u >> 2) % kParts) * kCols, c_hi = c_lo + kCols;
+        const uint32_t t_row = tile_base + (uint32_t)(m * BN) * kAccColBytes + (uint32_t)r * 16;   // the operand buffers are dead
+        if (nsplit > 1) {
+          // two-launch split-K: this split's private fp32 slices; splitk_finish_kernel reduces them and runs the fused epilogue
+          splitk_store_partial<BN>(p.sk_scratch + (((size_t)tile_id * MTC + m) * nsplit + blockIdx.z) * kBM * BN, t_row, r, c_lo, c_hi);
+        } else {
+          const int gy = ty * 16 * MTC + 16 * m + (r >> 3), gx = tx * 8 + (r & 7);
+          const int oy = pa + d * gy, ox = pb + d * gx;
+          const bool valid = oy < OHs && ox < OWs;
+          const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + oa) * p.DW + ox * p.osw + ob) : 0;
+          epi_cols<BN>(p, t_row, cbase, dpix, valid, s_bias, c_lo, c_hi);
+        }
+      }
+    }
   }
   if (nsplit > 1 && p.sk_cluster) {
     cluster_sync_all();                       // every CTA's partial tiles are in its shared memory
     if (warp < 4) {
       const int cbase = ny * BN;
-      for (int m = 0; m < MT; ++m)
+      for (int m = 0; m < MTC; ++m)
         cluster_reduce_rows<BN>(p, tile_base + (uint32_t)m * (kBM * BN * 4), nsplit, (int)cluster_ctarank(), tid, 128, cbase,
                                 [&](int row, bool& valid) -> size_t {
-                                  const int gy = ty * 16 * MT + 16 * m + (row >> 3), gx = tx * 8 + (row & 7);
+                                  const int gy = ty * 16 * MTC + 16 * m + (row >> 3), gx = tx * 8 + (row & 7);
                                   const int oy = pa + d * gy, ox = pb + d * gx;
                                   valid = oy < OHs && ox < OWs;
                                   return valid ? ((size_t)(n * p.DH + oy * p.osh + oa) * p.DW + ox * p.osw + ob) : 0;
@@ -927,7 +941,7 @@ __global__ void __launch_bounds__(256) splitk_finish_kernel(const __grid_constan
   size_t dpix = 0;
   const float* tile0;
   if (p.halo) {
-    const int MT = p.MT, d = p.dil;
+    const int MT = p.MT * (p.nwg > 1 ? p.nwg : 1), d = p.dil;   // tiles per CTA
     const int Hp0 = (p.OH + d - 1) / d, Wp0 = (p.OW + d - 1) / d;
     const int tiles_x = (Wp0 + 7) / 8, tiles_y = (Hp0 + 16 * MT - 1) / (16 * MT);
     int bid = blockIdx.x;
@@ -1578,7 +1592,7 @@ static cudaError_t launch_splitk_finish(const CisConv* d, dim3 main_grid, cudaSt
   constexpr int G = BN / 16;
   constexpr int kBlock = (128 * G < 256) ? 128 * G : 256;
   constexpr int kSub = 128 * G / kBlock;
-  const int mt = d->halo ? d->MT : 1;
+  const int mt = d->halo ? d->MT * (d->nwg > 1 ? d->nwg : 1) : 1;
   return launch_pdl(splitk_finish_kernel<BN>, dim3(main_grid.x, main_grid.y, mt * kSub), dim3(kBlock), 0, st, *d);
 }
 
@@ -1659,9 +1673,10 @@ extern "C" int cis_set_persist_mode(int mode) {
   return CIS_OK;
 }
 
-template <int BN>
+template <int BN, int NWG>
 static int launch_halo(const CisConv* d, cudaStream_t st) {
-  const int Wh = 8 + d->ex, Hh = 16 * d->MT + d->ey, HP = Wh * Hh;
+  const int MTC = d->MT * NWG;                                 // stacked 16x8 tiles per CTA
+  const int Wh = 8 + d->ex, Hh = 16 * MTC + d->ey, HP = Wh * Hh;
   const int halo_stage = (HP * 128 + 1023) & ~1023;
   int chunks = 0;
   for (int i = 0; i < d->nsrc; ++i) chunks += d->src[i].chunks;
@@ -1677,7 +1692,7 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
     ntaps_max = 0;
     int tsum = 0;
     for (int i = 0; i < nsub; ++i) {
-      const int t = ((d->sub[i].OW + 7) / 8) * ((d->sub[i].OH + 16 * d->MT - 1) / (16 * d->MT));
+      const int t = ((d->sub[i].OW + 7) / 8) * ((d->sub[i].OH + 16 * MTC - 1) / (16 * MTC));
       if (t > tiles) tiles = t;
       if (d->sub[i].ntaps > ntaps_max) ntaps_max = d->sub[i].ntaps;
       if (d->sub[i].ntaps < 1 || d->sub[i].tap0 != tsum || !d->sub[i].wpack) return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): bad sub-problem");
@@ -1686,7 +1701,7 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
     if (tsum != d->ntaps) return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): sub-problem taps must add up to ntaps");
   } else {
     const int Hp0 = (d->OH + dd - 1) / dd, Wp0 = (d->OW + dd - 1) / dd;
-    tiles = ((Wp0 + 7) / 8) * ((Hp0 + 16 * d->MT - 1) / (16 * d->MT));
+    tiles = ((Wp0 + 7) / 8) * ((Hp0 + 16 * MTC - 1) / (16 * MTC));
   }
   const long ncta_all = (long)tiles * dd * dd * d->N * d->n_tiles * nsp * nsub;
   // ---- weight pipeline: G taps per stage (one bulk copy, one wait / commit of the MMA thread), BS stages
@@ -1712,11 +1727,11 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   if (BS > groups) BS = groups;
   if (BS < 1) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): tile does not fit shared memory");
   int smem = fixed + BS * G * kB;
-  if (smem < d->MT * kBM * BN * 4 + 1024) smem = d->MT * kBM * BN * 4 + 1024;   // the fp32 accumulator tiles overlay the operand buffers
+  if (smem < MTC * kBM * BN * 4 + 1024) smem = MTC * kBM * BN * 4 + 1024;   // the fp32 accumulator tiles overlay the operand buffers
   if (smem > 226 * 1024) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): accumulator tiles do not fit shared memory");
   static int attr_smem = 0;
   if (smem > attr_smem) {
-    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(conv_halo_kernel<BN, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(conv_halo)");
     attr_smem = smem;
   }
@@ -1748,7 +1763,7 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   const int persist_mode = g_persist_mode >= 0 ? g_persist_mode : (getenv("CIS_PERSIST_MODE") ? atoi(getenv("CIS_PERSIST_MODE")) : 1);
   static const int p_min_tiles = getenv("CIS_PERSIST_MIN_TILES") ? atoi(getenv("CIS_PERSIST_MIN_TILES")) : 296;
   static const int p_ws_kb = getenv("CIS_PERSIST_WS_KB") ? atoi(getenv("CIS_PERSIST_WS_KB")) : 112;
-  if constexpr (BN <= kPMaxAccCols) {
+  if constexpr (BN <= kPMaxAccCols && NWG == 1) {
    if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && nsub == 1 && dd == 1 && d->MT * BN <= kPMaxAccCols) {
     const int total = tiles * d->N;
     const int per_tile = nchunks * d->ntaps;
@@ -1789,8 +1804,9 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
    }
   }
   cudaError_t le = (splits > 1 && d->sk_cluster)
-                       ? launch_pdl_zcluster(conv_halo_kernel<BN>, grid, dim3(HaloCfg<BN>::kThreads), smem, st, splits, *d, halo_stage, BS, nhs, maps, use_tma, G)
-                       : launch_pdl(conv_halo_kernel<BN>, grid, dim3(HaloCfg<BN>::kThreads), smem, st, *d, halo_stage, BS, nhs, maps, use_tma, G);
+                       ? launch_pdl_zcluster(conv_halo_kernel<BN, NWG>, grid, dim3(HaloCfg<BN, NWG>::kThreads), smem, st, splits, *d, halo_stage, BS, nhs, maps,
+                                             use_tma, G)
+                       : launch_pdl(conv_halo_kernel<BN, NWG>, grid, dim3(HaloCfg<BN, NWG>::kThreads), smem, st, *d, halo_stage, BS, nhs, maps, use_tma, G);
   if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_halo)");
   if (splits > 1 && !d->sk_cluster) {
     le = launch_splitk_finish<BN>(d, grid, st);
@@ -1814,14 +1830,15 @@ extern "C" int cis_conv_igemm(const CisConv* d, cis_stream_t stream) {
     return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm: residual slices must be 8-channel aligned");
   cudaStream_t st = (cudaStream_t)stream;
   if (d->halo) {
-    if (d->MT < 1 || d->MT > 4 || d->MT * d->BN > kMaxAccCols || d->dil < 1 || d->sh != 1 || d->sw != 1 || d->ey < 0 || d->ex < 0 ||
+    if (d->MT < 1 || d->MT > 4 || d->MT * d->BN > kMaxAccCols || d->nwg < 0 || d->nwg > 2 || (d->nwg == 2 && d->BN < 64) || d->dil < 1 ||
+        d->sh != 1 || d->sw != 1 || d->ey < 0 || d->ex < 0 ||
         (d->dil > 1 && (d->OH != d->H || d->OW != d->W)) || (d->nph > 1 && (d->nph != 4 || d->dil != 1 || d->ph_tap[0] != 0 || d->ph_tap[4] != d->ntaps)))
       return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): bad tile parameters");
     switch (d->BN) {
-      case 16: return launch_halo<16>(d, st);
-      case 32: return launch_halo<32>(d, st);
-      case 64: return launch_halo<64>(d, st);
-      case 128: return launch_halo<128>(d, st);
+      case 16: return launch_halo<16, 1>(d, st);
+      case 32: return launch_halo<32, 1>(d, st);
+      case 64: return d->nwg == 2 ? launch_halo<64, 2>(d, st) : launch_halo<64, 1>(d, st);
+      case 128: return d->nwg == 2 ? launch_halo<128, 2>(d, st) : launch_halo<128, 1>(d, st);
       default: return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm: BN must be 16/32/64/128");
     }
   }

@@ -277,7 +277,7 @@ def small_bn_cap(level):
 
 
 NUM_SMS = 132        # H100 SXM
-# fp32 accumulator columns (MT stacked tiles x BN) one CTA of the halo kernel keeps in the registers of its MMA warpgroup
+# fp32 accumulator columns (MT stacked tiles x BN) one MMA warpgroup of the halo kernel keeps in its registers
 MAX_ACC_COLS = 128
 HALO_ENABLED = True
 WGRAD_TMA = True
@@ -327,6 +327,43 @@ HALO_SKIP_THIN = int(os.environ.get('CIS_HALO_SKIP_THIN', '0'))
 HALO_MIN_UTIL = float(os.environ.get('CIS_HALO_MIN_UTIL', '0.2'))
 
 
+# MMA warpgroups per halo-kernel CTA (CisConv.nwg): 2 = both warpgroups consume every weight stage, so the CTA pulls half the weight
+# bytes from L2 per output row.  CIS_HALO_NWG: 1 one warpgroup everywhere (A/B runs) | 2 (default) where halo_nwg's rule says it pays |
+# 3 every launch that can take two (tests)
+HALO_NWG = int(os.environ.get('CIS_HALO_NWG', '2'))
+# time of a two-warpgroup CTA relative to two one-warpgroup CTAs of the same rows: 0.78-0.80 measured on the 4x96x160 BN = 128 PWC-Net
+# layers (H100 SXM at a 400 W power limit, tools/time_ops.py)
+HALO_NWG2_COST = 0.8
+
+
+def halo_nwg(d, MT, Hp0, Wp0, dil, n_tiles, ntaps, nchunks, ey, ex):
+    """CisConv.nwg for a halo launch of MT tiles per warpgroup: 2 when the launch spans more than one wave of CTAs, so that half as
+    many CTAs of twice the height take fewer waves-times-cost, the taller tile wastes no more padded rows and the taller halo fits
+    shared memory; else 1."""
+    if HALO_NWG < 2 or d.BN < 64:
+        return 1
+    if HALO_NWG == 2 and n_tiles == 1 and dil == 1 and MT * d.BN <= 64 and nchunks * ntaps * d.BN * 128 <= 112 * 1024:
+        return 1           # a candidate of the persistent kernel (one warpgroup, whole weight set resident in shared memory)
+    tiles_x = -(-Wp0 // 8)
+    ty1, ty2 = -(-Hp0 // (16 * MT)), -(-Hp0 // (32 * MT))
+    HP = (8 + ex) * (32 * MT + ey)
+    nhs = 2 if nchunks > 1 else 1
+    if nhs * ru(HP * 128, 1024) + HP * 4 + 2048 + 3 * d.BN * 128 > 227 * 1024 or 2 * MT * 128 * d.BN * 4 + 1024 > 226 * 1024:
+        return 1
+    util1 = (Hp0 * Wp0) / float(ty1 * 16 * MT * tiles_x * 8)
+    util2 = (Hp0 * Wp0) / float(ty2 * 32 * MT * tiles_x * 8)
+    if util2 < (HALO_MIN_UTIL if dil == 1 else 0.5):
+        return 1
+    if HALO_NWG == 3:
+        return 2
+    if util2 < 0.95 * util1:
+        return 1
+    # one CTA per SM either way (register-bound): compare whole waves of CTAs, a two-warpgroup CTA costing 2 * HALO_NWG2_COST
+    ncta1 = d.N * dil * dil * tiles_x * ty1 * n_tiles
+    ncta2 = d.N * dil * dil * tiles_x * ty2 * n_tiles
+    return 2 if 2 * HALO_NWG2_COST * (-(-ncta2 // NUM_SMS)) <= -(-ncta1 // NUM_SMS) else 1
+
+
 def setup_splitk(d, device, keep):
     """Launches whose grid would cover well under the NUM_SMS SMs (low-resolution pyramid levels) split their K loop over grid.z;
     see CisConv.splits.  Scratch and ticket buffers are per launch (launches on different lanes may overlap)."""
@@ -335,8 +372,9 @@ def setup_splitk(d, device, keep):
     m_chunks = sum(d.src[i].chunks for i in range(d.nsrc))
     if d.halo:
         Hp0, Wp0 = -(-d.OH // d.dil), -(-d.OW // d.dil)
-        tiles = (-(-Wp0 // 8)) * (-(-Hp0 // (16 * d.MT))) * d.dil * d.dil * d.N
-        ncta, units, min_units, mt = tiles * d.n_tiles, -(-m_chunks // 8), 1, d.MT
+        mt = d.MT * max(d.nwg, 1)         # 16x8 tiles per CTA
+        tiles = (-(-Wp0 // 8)) * (-(-Hp0 // (16 * mt))) * d.dil * d.dil * d.N
+        ncta, units, min_units = tiles * d.n_tiles, -(-m_chunks // 8), 1
     else:
         ncta, units, min_units, mt = (-(-(d.N * d.OH * d.OW) // 128)) * d.n_tiles, d.K_pad // 64, 4, 1
     steps = units * (d.ntaps if d.halo else 1)     # serial pipeline steps of one CTA (halo: one per (chunk, tap); generic: one per 64-wide K block)
@@ -418,6 +456,7 @@ def setup_halo(d, taps, dil, n_tiles):
     if best is None:
         return False
     d.halo, d.dil, d.MT, d.hoy, d.hox, d.ey, d.ex = 1, dil, best[1], hoy, hox, ey, ex
+    d.nwg = halo_nwg(d, best[1], Hp0, Wp0, dil, n_tiles, ntaps, nchunks, ey, ex)
     _fill_taps(d, rel)
     return True
 
@@ -466,6 +505,7 @@ def setup_halo_s2(d, taps, n_tiles):
     if best is None:
         return None
     d.halo, d.dil, d.MT, d.hoy, d.hox, d.ey, d.ex = 1, 1, best[1], hoy, hox, ey, ex
+    d.nwg = halo_nwg(d, best[1], d.OH, d.OW, 1, n_tiles, len(taps), nchunks, ey, ex)
     d.sh = d.sw = 1                     # the phases absorb the stride; H x W stay the input size (tensor maps)
     _fill_taps(d, rel)
     d.nph = 4
@@ -502,6 +542,7 @@ def merge_parity_launches(descs):
         return None
     g = CisConv.from_buffer_copy(bytes(d0))
     g.MT, g.ey, g.ex = min(d.MT for d in descs), max(d.ey for d in descs), max(d.ex for d in descs)
+    g.nwg = min(max(d.nwg, 1) for d in descs)
     g.OH, g.OW = max(d.OH for d in descs), max(d.OW for d in descs)
     t = 0
     for i, d in enumerate(descs):
