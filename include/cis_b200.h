@@ -127,6 +127,11 @@ typedef struct {
   int32_t tma;       /* 2: experimental halo-resident variant of 1 (same dwp layout; one activation halo per pixel tile, taps read in place);
                         1: stride-1 layer, operands fetched as 8x8-pixel TMA tiles; dwp columns are then laid out per tap in
                         64-channel groups: col = (tap*ceil(Cin8/64) + chunk64)*64 + c, K_pad = that extent rounded to 128 */
+  /* tma == 2 tiling.  nh = MMA N (16 / 32 / 64; 0 = 64): at least Cout rounded up to 16, and 64 when Cout > 64; one MMA warpgroup
+   * holds 128 / nh tap pairs.  nwg = MMA warpgroups per CTA (0/1 = one, 2 = two on the same stages: the two 64-channel halves of
+   * Cout when Cout > 64, else twice the tap pairs). */
+  int32_t nh;
+  int32_t nwg;
 } CisWgrad;
 
 const char* cis_last_error(void);

@@ -7,6 +7,7 @@ import os
 import sys
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from unsupervised_detection_b200 import engine  # noqa: E402
 from unsupervised_detection_b200.step_graph import CISGraph  # noqa: E402
 
 
@@ -62,6 +63,33 @@ def main():
     print('launches per step by CTA count: <=8: %.1f | 9-32: %.1f | 33-148: %.1f | 149-592: %.1f | >592: %.1f' % tuple(hist[i] for i in range(1, 6)))
     print('weight-stationary-eligible (CIS_PERSIST_WS): %.1f per step; cluster-eligible (CIS_HALO_CLUSTER=2): %.1f per step; split: %.1f per step' %
           (sum(r['w'] for r in rows if r['ws_fit']) / 4.0, sum(r['w'] for r in rows if r['cluster']) / 4.0, sum(r['w'] for r in rows if r['splits'] > 1) / 4.0))
+    wgrad_report(g)
+
+
+def wgrad_report(g):
+    """Halo weight-gradient launches (CisWgrad.tma = 2): MMA N, MMA warpgroups, grid, and issued / useful MMA work per step."""
+    print('\nhalo wgrad launches (tma = 2)')
+    print('%-5s %3s %9s %5s %5s %5s %3s %3s %14s  %s' % ('plan', 'N', 'OHxOW', 'taps', 'cin', 'cout', 'nh', 'nwg', 'grid', 'GFLOP issued/useful'))
+    useful = issued = 0.0
+    for pname, plan, w in (('bwdG', g.bwd['G'], 3), ('bwdR', g.bwd['R'], 1)):
+        for fn, a, name, fl, lane in plan.ops:
+            if name != 'cis_conv_wgrad' or a[0]._obj.tma != 2:
+                continue
+            d = a[0]._obj
+            chunks = sum(d.src[i].chunks for i in range(d.nsrc))
+            nch64 = -(-chunks // 8)
+            nh, nwg, gz = d.nh or 64, max(d.nwg, 1), engine.wgrad_halo_tiling(d.ntaps, d.Cout)[2]
+            nblk = d.N * (-(-d.OH // 8)) * (-(-d.OW // 8))
+            # every CTA row of pairs along grid.z issues its real pairs; Cout > 64 on one warpgroup repeats them per Cout half
+            pairs = (d.ntaps + 1) // 2 * (2 if d.Cout > 64 else 1)
+            iss = nblk * nch64 * pairs * 2.0 * 128 * nh * 64
+            use = 2.0 * d.N * d.OH * d.OW * d.ntaps * chunks * 8 * d.Cout
+            useful += w * use / 4.0
+            issued += w * iss / 4.0
+            print('%-5s %3d %4dx%-4d %5d %5d %5d %3d %3d %14s  %.1f / %.1f' % (pname, d.N, d.OH, d.OW, d.ntaps, chunks * 8, d.Cout, nh, nwg,
+                                                                       '%dx%dx%d' % (nch64, d.splits, gz), iss / 1e9, use / 1e9))
+    if useful:
+        print('per step (1R:3G): %.1f GFLOP issued for %.1f useful (%.2fx)' % (issued / 1e9, useful / 1e9, issued / useful))
 
 
 if __name__ == '__main__':

@@ -47,6 +47,8 @@ for pname, plan, w in (('fwd', g.fwd, 4), ('bwdG', g.bwd['G'], 3), ('bwdR', g.bw
         elif name == 'cis_conv_wgrad':
             d = a[0]._obj
             info = 'tma%d N%d %dx%d taps%d cout%d K%d sp%d' % (d.tma, d.N, d.OH, d.OW, d.ntaps, d.Cout, d.K_pad, d.splits)
+            if d.tma == 2:
+                info += ' nh%d nwg%d' % (d.nh or 64, max(d.nwg, 1))
         rows.append((pname, w, name, us, fl, info))
 if os.environ.get('TIME_OPS_JSON'):
     # one row per launch, keyed by (plan, index-in-plan): lets tools/ab_diff.py line up the same layer across two configurations

@@ -56,7 +56,8 @@ class CisWgrad(C.Structure):
                 ('dh', C.c_int16 * MAX_TAPS), ('dw', C.c_int16 * MAX_TAPS),
                 ('nsrc', C.c_int32), ('src', CisSrc * MAX_SRC),
                 ('g', C.c_void_p), ('g_pitch', C.c_int32), ('g_coff', C.c_int32), ('g_chunks', C.c_int32),
-                ('dwp', C.c_void_p), ('Cout', C.c_int32), ('K_pad', C.c_int32), ('splits', C.c_int32), ('tma', C.c_int32)]
+                ('dwp', C.c_void_p), ('Cout', C.c_int32), ('K_pad', C.c_int32), ('splits', C.c_int32), ('tma', C.c_int32),
+                ('nh', C.c_int32), ('nwg', C.c_int32)]
 
 
 _i32, _i64, _f32, _p, _u64 = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_uint64

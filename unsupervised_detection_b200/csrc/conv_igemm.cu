@@ -1405,24 +1405,55 @@ __global__ void __launch_bounds__(kGThreads) conv_wgrad_kernel(const __grid_cons
 
 // ======================================================================================================= halo-resident wgrad
 // CisWgrad.tma == 2.  Swapped roles: D[kcol][co] = sum_pix x[pix + tap][c] * g[pix][co].  Per 8x8 pixel tile the CTA fetches ONE activation halo
-// ((8+ex) x (8+ey) pixels x 64 channels, TMA, SWIZZLE_128B) and ONE gradient tile (8x8 pixels x 64 channels) and reads every tap
+// ((8+ex) x (8+ey) pixels x 64 channels, TMA, SWIZZLE_128B) and the gradient tile(s) (8x8 pixels x NH channels) and reads every tap
 // in place: A = MN-major operand whose two 64-channel atoms are the taps 2q and 2q+1 (descriptor start = origin of tap 2q shifted
 // by two tile rows per K step, LBO = distance between the two tap origins, SBO = Wh*128 between the 8-pixel rows), B = the gradient
-// tile (N = 64 output channels), one 128 x 64 register accumulator per tap pair.  Relies on the tensor core applying the 128B swizzle
-// on absolute address bits for MN-major operands too.  A CTA owns kWHPairs tap pairs (the register budget of its MMA warpgroup).
-// grid = (64-channel chunks of the input, pixel-tile splits, 64-channel halves of Cout x groups of kWHPairs tap pairs); dwp layout =
-// the tma == 1 layout.
+// tile (N = NH output channels), one 128 x NH register accumulator per tap pair.  Relies on the tensor core applying the swizzle
+// on absolute address bits for MN-major operands too.
+// NH = min(64, Cout rounded to 16) is the MMA N: the gradient tile is exactly one MN-major swizzle atom wide (NH * 2 bytes: 128B / 64B /
+// 32B swizzle), so no zero channels are fetched or multiplied beyond the 16-channel granule.  Each MMA warpgroup holds P = 128 / NH tap
+// pairs (128 accumulator registers).  NWG = 2 adds a second MMA warpgroup on the same stages: Cout > 64 -> warpgroup w takes Cout half w
+// over the same P pairs (the stage holds both 64-channel gradient halves); Cout <= 64 -> the CTA owns 2P pairs, split between the two.
+// grid = (64-channel chunks of the input, pixel-tile splits, pair groups [x 64-channel halves of Cout when one warpgroup]);
+// dwp layout = [split][co][K_pad].
 static constexpr int kWHMaxStages = 6;
-static constexpr int kWHPairs = 2;           // tap pairs per CTA: 2 x 64 accumulator columns
 struct WgradHaloMaps {
-  CUtensorMap g;                 // (C8, OW, OH, N) gradient slice, box (64, 8, 8, 1)
+  CUtensorMap g;                 // (C8, OW, OH, N) gradient slice, box (NH, 8, 8, 1)
   CUtensorMap x[CIS_MAX_SRC];    // (C8, W, H, N) activation slices, box (64, Wh, Hh, 1)
 };
+template <int NH> struct WgradHaloCfg {
+  static_assert(NH == 16 || NH == 32 || NH == 64, "NH is 16, 32 or 64 output channels");
+  static constexpr int kPairs = kMaxAccCols / NH;                    // tap pairs per MMA warpgroup
+  static constexpr uint32_t kGRow = 2 * NH;                          // bytes per pixel of the gradient tile = its swizzle span
+  static constexpr uint32_t kGTile = 64 * kGRow;                     // 8x8 pixels
+  static constexpr uint32_t kLayout = NH == 64 ? 1u : NH == 32 ? 2u : 3u;   // descriptor layout type: SWIZZLE_128B / 64B / 32B
+};
 
-__global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_constant__ CisWgrad p, const __grid_constant__ WgradHaloMaps maps,
-                                                                    const int Wh, const int Hh, const int hoy, const int hox,
-                                                                    const int stage_bytes, const int S) {
-  constexpr int Nh = 64;
+// tap pairs [qa, qa + np) and Cout half hf of MMA warpgroup w
+template <int NH, int NWG>
+__device__ __forceinline__ void wgrad_halo_wg_pairs(int w, int npairs, int cout, int& qa, int& np, int& hf) {
+  constexpr int P = WgradHaloCfg<NH>::kPairs;
+  const int nhalf = cout > 64 ? 2 : 1;
+  if (NWG == 2 && nhalf == 2) {
+    qa = blockIdx.z * P;
+    np = min(P, npairs - qa);
+    hf = w;
+    return;
+  }
+  const int q0 = (blockIdx.z / nhalf) * (NWG * P);
+  const int cnt = min(NWG * P, npairs - q0);
+  const int h = NWG == 2 ? (cnt + 1) / 2 : cnt;                       // two warpgroups: balanced halves of the CTA's pairs
+  qa = q0 + (w ? h : 0);
+  np = w ? cnt - h : h;
+  hf = blockIdx.z % nhalf;
+}
+
+template <int NH, int NWG>
+__global__ void __launch_bounds__(128 * (1 + NWG)) conv_wgrad_halo_kernel(const __grid_constant__ CisWgrad p, const __grid_constant__ WgradHaloMaps maps,
+                                                                          const int Wh, const int Hh, const int hoy, const int hox,
+                                                                          const int stage_bytes, const int S) {
+  using Cfg = WgradHaloCfg<NH>;
+  constexpr int P = Cfg::kPairs;
   extern __shared__ uint8_t smem_raw[];
   __shared__ uint64_t bars[2 * kWHMaxStages + 1];
   __shared__ int s_off[CIS_MAX_TAPS + 1];   // tap origin inside the halo, in pixel rows of 128 B
@@ -1434,7 +1465,9 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
   pdl_launch_dependents();
   if (tid < p.ntaps) s_off[tid] = (p.dh[tid] - hoy) * Wh + (p.dw[tid] - hox);
   if (tid == p.ntaps) s_off[tid] = 0;       // partner of an unpaired last tap (its accumulator rows are never stored)
-  const int halo_bytes = stage_bytes - 8192;                 // [halo (1024-rounded)] [gradient tile 8 KB]
+  const bool wg_halves = NWG == 2 && p.Cout > 64;              // warpgroup w multiplies by gradient half w
+  const int ng = wg_halves ? 2 : 1;                            // gradient tiles per stage
+  const int halo_bytes = stage_bytes - ng * (int)Cfg::kGTile;  // [halo (1024-rounded)] [gradient tile(s)]
   const int tiles_x = (p.OW + 7) / 8, tiles_y = (p.OH + 7) / 8;
   const int nkb_total = p.N * tiles_x * tiles_y;
   const int per = (nkb_total + (int)gridDim.y - 1) / (int)gridDim.y;
@@ -1444,17 +1477,15 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
   int m_chunks = 0;
   for (int i = 0; i < p.nsrc; ++i) m_chunks += p.src[i].chunks;
   const int nch64 = (m_chunks + 7) / 8;
-  const int nhalf = p.Cout > 64 ? 2 : 1;
-  const int c64 = blockIdx.x, half = blockIdx.z % nhalf;
-  const int q0 = (blockIdx.z / nhalf) * kWHPairs;                 // first tap pair of this CTA
-  const int npair = min(kWHPairs, (p.ntaps + 1) / 2 - q0);
+  const int npairs = (p.ntaps + 1) / 2;
+  const int c64 = blockIdx.x;
 
   if (tid == 128) {
     for (int s = 0; s < S; ++s) {
       mbar_init(bar_full + 8 * s, 1);
-      mbar_init(bar_empty + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, NWG);      // one release per MMA warpgroup
     }
-    mbar_init(bar_accum, 128);
+    mbar_init(bar_accum, 128 * NWG);
     fence_mbar_init();
   }
   pdl_wait();
@@ -1472,6 +1503,8 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
       if (si == 1) nm = p.src[1].n_mod;
       if (si == 2) nm = p.src[2].n_mod;
       if (si == 3) nm = p.src[3].n_mod;
+      int qa, np, hf0;
+      wgrad_halo_wg_pairs<NH, NWG>(0, npairs, p.Cout, qa, np, hf0);
       const int tpi = tiles_x * tiles_y;
       for (int it = 0; it < nkb; ++it) {
         const int s = it % S;
@@ -1480,9 +1513,10 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
         const int n = kb / tpi, r = kb - n * tpi;
         const int ty = r / tiles_x, tx = r - ty * tiles_x;
         const uint32_t st = tile_base + s * stage_bytes, bar = bar_full + 8 * s;
-        mbar_expect_tx(bar, (uint32_t)(Wh * Hh * 128 + 8192));
+        mbar_expect_tx(bar, (uint32_t)(Wh * Hh * 128 + ng * (int)Cfg::kGTile));
         tma_load_4d(st, &maps.x[si], bar, c * 8, tx * 8 + hox, ty * 8 + hoy, nm ? (n % nm) : n);     // out-of-image pixels / channels: zeros
-        tma_load_4d(st + halo_bytes, &maps.g, bar, half * 64, tx * 8, ty * 8, n);
+        for (int h = 0; h < ng; ++h)
+          tma_load_4d(st + halo_bytes + h * Cfg::kGTile, &maps.g, bar, (hf0 + h) * 64, tx * 8, ty * 8, n);
       }
     }
     __syncwarp();
@@ -1491,51 +1525,67 @@ __global__ void __launch_bounds__(kThreads) conv_wgrad_halo_kernel(const __grid_
     const int r = warp * 32 + lane;
     const int cch = r & 63;
     const uint32_t t_row = tile_base + (uint32_t)r * 16;
-    for (int q = 0; q < npair; ++q) {
-      const int t = 2 * (q0 + q) + (r >> 6);
-      const bool tv = t < p.ntaps;
-      const size_t kcol = ((size_t)t * nch64 + c64) * 64 + cch;
+    for (int w = 0; w < NWG; ++w) {
+      int qa, np, hf;
+      wgrad_halo_wg_pairs<NH, NWG>(w, npairs, p.Cout, qa, np, hf);
+      for (int q = 0; q < np; ++q) {
+        const int t = 2 * (qa + q) + (r >> 6);
+        if (t >= p.ntaps) continue;
+        const size_t kcol = ((size_t)t * nch64 + c64) * 64 + cch;
 #pragma unroll 1
-      for (int c0 = 0; c0 < Nh; c0 += 16) {
-        if (!tv) continue;
-        float v[16];
-        acc_ld16(t_row + (uint32_t)(q * Nh + c0) * kAccColBytes, v);
-        for (int e = 0; e < 16; ++e) {
-          const int co = half * 64 + c0 + e;
-          if (co < p.Cout) p.dwp[((size_t)blockIdx.y * p.Cout + co) * p.K_pad + kcol] = v[e];   // private slice; lanes = consecutive kcol: coalesced
+        for (int c0 = 0; c0 < NH && hf * 64 + c0 < p.Cout; c0 += 16) {
+          float v[16];
+          acc_ld16(t_row + (uint32_t)((w * P + q) * NH + c0) * kAccColBytes, v);
+          for (int e = 0; e < 16; ++e) {
+            const int co = hf * 64 + c0 + e;
+            if (co < p.Cout) p.dwp[((size_t)blockIdx.y * p.Cout + co) * p.K_pad + kcol] = v[e];   // private slice; lanes = consecutive kcol: coalesced
+          }
         }
       }
     }
   } else {
-    // ------------------------------------------------------------------ MMA warpgroup (warps 4-7)
-    const int wtid = tid - 128;
-    float acc[kWHPairs][Nh];
-    const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
+    // ------------------------------------------------------------------ MMA warpgroup(s) (warps 4-7, 8-11)
+    const int wg = NWG > 1 ? (warp - 4) >> 2 : 0;
+    const int wtid = tid - 128 * (1 + wg);
+    int qa, np, hf;
+    wgrad_halo_wg_pairs<NH, NWG>(wg, npairs, p.Cout, qa, np, hf);
+    // the pair count depends on the warpgroup: read it through a shuffle so that ptxas knows it is warp-uniform (a wgmma guard it
+    // takes for divergent makes it serialise the wgmma, C7520)
+    np = __shfl_sync(0xffffffffu, np, 0);
+    float acc[P][NH];
+    const uint32_t ahi = desc_hi((uint32_t)(Wh * 128));
+    const uint32_t bhi = (((8 * Cfg::kGRow) >> 4) & 0x3FFF) | (Cfg::kLayout << 30);   // SBO = 8 gradient pixels
     const uint32_t kstep = (uint32_t)(2 * Wh * 128) >> 4;                    // 16 pixels = two tile rows of the halo
+    const uint32_t g_off = (uint32_t)halo_bytes + (wg_halves ? (uint32_t)wg * Cfg::kGTile : 0u);
     for (int it = 0; it < nkb; ++it) {
       const int s = it % S;
       mbar_wait(bar_full + 8 * s, (uint32_t)((it / S) & 1));
       const uint32_t st = tile_base + s * stage_bytes;
-      const uint32_t blo0 = desc_lo(st + halo_bytes, 8192);
+      const uint32_t blo0 = desc_lo(st + g_off, Cfg::kGTile);       // LBO unused: the tile is one swizzle atom wide
       wg_fence();
 #pragma unroll
-      for (int q = 0; q < kWHPairs; ++q) {
-        if (q < npair) {
-          const int o0 = s_off[2 * (q0 + q)], o1 = s_off[2 * (q0 + q) + 1];
+      for (int q = 0; q < P; ++q) {
+        if (q < np) {
+          const int o0 = s_off[2 * (qa + q)], o1 = s_off[2 * (qa + q) + 1];
           const uint32_t lbo = (uint32_t)((o1 > o0 ? o1 - o0 : 1) * 128);      // distance between the two tap origins
           const uint32_t alo0 = desc_lo(st + (uint32_t)(o0 * 128), lbo);
 #pragma unroll
           for (int k = 0; k < 4; ++k)
-            mma128<Nh, 1, 1>(acc[q], alo0 + k * kstep, ahi, blo0 + 128 * k, bhi, lbo >> 4, (uint32_t)((it | k) != 0));
+            mma128<NH, 1, 1>(acc[q], alo0 + k * kstep, ahi, blo0 + Cfg::kGRow * k, bhi, lbo >> 4, (uint32_t)((it | k) != 0));
         }
       }
       wg_commit();
+      // release the stage once its wgmma are done (keeping one commit group in flight and releasing the stage behind the next one
+      // measured slower on the H100)
       wg_wait<0>();
       if (wtid == 0) mbar_arrive(bar_empty + 8 * s);
     }
+    // every operand stage has been consumed: the accumulators overlay the ring.  Two warpgroups: the other one may still be reading
+    // the last stage, so both finish their wgmma before either overwrites it.
+    if constexpr (NWG > 1) asm volatile("bar.sync 1, %0;" ::"n"(128 * NWG) : "memory");
 #pragma unroll
-    for (int q = 0; q < kWHPairs; ++q)
-      if (q < npair) acc_store<Nh>(acc[q], tile_base + (uint32_t)(q * Nh) * kAccColBytes, wtid);
+    for (int q = 0; q < P; ++q)
+      if (q < np) acc_store<NH>(acc[q], tile_base + (uint32_t)((wg * P + q) * NH) * kAccColBytes, wtid);
     mbar_arrive(bar_accum);
   }
 }
@@ -1643,8 +1693,9 @@ static EncodeTiledFn get_encode_tiled() {
 // space-to-depth phase (py, px) of the image: pixel (y, x) of the map is input pixel (2y + py, 2x + px).
 // step/py/px: a stride-2 phase view (coarser grid through the global strides, phase offset in the base address).
 // estride: dilated layers -- ONE map per source, every estride-th pixel of a box that starts at any (phase-carrying) coordinate.
+// bc / swz: box width in channels and its swizzle (the halo wgrad kernel's narrow gradient tiles: 16 channels = 32 B, 32 = 64 B).
 static bool encode_src_map(CUtensorMap* m, const CisSrc& s, int N, int H, int W, int bw, int bh, int step = 1, int py = 0, int px = 0,
-                           int estride = 1) {
+                           int estride = 1, int bc = 64, CUtensorMapSwizzle swz = CU_TENSOR_MAP_SWIZZLE_128B) {
   EncodeTiledFn enc = get_encode_tiled();
   if (!enc) return false;
   const int nb = s.n_mod > 0 ? s.n_mod : N;
@@ -1652,10 +1703,10 @@ static bool encode_src_map(CUtensorMap* m, const CisSrc& s, int N, int H, int W,
   if (Hq < 1 || Wq < 1) return false;
   cuuint64_t dims[4] = {(cuuint64_t)s.chunks * 8, (cuuint64_t)Wq, (cuuint64_t)Hq, (cuuint64_t)nb};
   cuuint64_t strides[3] = {(cuuint64_t)step * s.pitch * 2, (cuuint64_t)step * W * s.pitch * 2, (cuuint64_t)H * W * s.pitch * 2};
-  cuuint32_t box[4] = {64, (cuuint32_t)(bw * estride), (cuuint32_t)(bh * estride), 1};   // extent in the un-strided pixel space
+  cuuint32_t box[4] = {(cuuint32_t)bc, (cuuint32_t)(bw * estride), (cuuint32_t)(bh * estride), 1};   // extent in the un-strided pixel space
   cuuint32_t es[4] = {1, (cuuint32_t)estride, (cuuint32_t)estride, 1};
   void* base = (void*)((const char*)s.ptr + ((size_t)(py * W + px) * s.pitch + (size_t)s.c_off) * 2);
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, base, dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
              CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
@@ -1851,7 +1902,40 @@ extern "C" int cis_conv_igemm(const CisConv* d, cis_stream_t stream) {
   }
 }
 
-// Halo-resident swapped wgrad (CisWgrad.tma == 2, experimental).  Eligibility is re-checked here; the engine falls back to tma = 1.
+template <int NH, int NWG>
+static int launch_wgrad_halo_t(const CisWgrad* d, cudaStream_t st, int nch64, int Wh, int Hh, int hoy, int hox, int halo_bytes) {
+  using Cfg = WgradHaloCfg<NH>;
+  const bool wg_halves = NWG == 2 && d->Cout > 64;
+  const int stage = halo_bytes + (wg_halves ? 2 : 1) * (int)Cfg::kGTile;
+  const int npairs = (d->ntaps + 1) / 2, nhalf = d->Cout > 64 ? 2 : 1;
+  const int gz = wg_halves ? (npairs + Cfg::kPairs - 1) / Cfg::kPairs : nhalf * ((npairs + NWG * Cfg::kPairs - 1) / (NWG * Cfg::kPairs));
+  int S = (200 * 1024) / stage;
+  if (S > kWHMaxStages) S = kWHMaxStages;
+  if (S < 2) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_wgrad(halo): halo does not fit shared memory");
+  int smem = S * stage + 1024;
+  const int acc_smem = NWG * kMaxAccCols * (int)kAccColBytes + 1024;    // the accumulators overlay the stages
+  if (smem < acc_smem) smem = acc_smem;
+  static int attr_smem = 0;    // per instantiation
+  if (smem > attr_smem) {
+    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_halo_kernel<NH, NWG>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(conv_wgrad_halo)");
+    attr_smem = smem;
+  }
+  WgradHaloMaps maps;
+  memset(&maps, 0, sizeof(maps));
+  CisSrc gs;
+  gs.ptr = d->g; gs.pitch = d->g_pitch; gs.c_off = d->g_coff; gs.chunks = d->g_chunks; gs.n_mod = 0;
+  const CUtensorMapSwizzle gswz = NH == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : NH == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B;
+  bool ok = encode_src_map(&maps.g, gs, d->N, d->OH, d->OW, 8, 8, 1, 0, 0, 1, NH, gswz);
+  for (int i = 0; ok && i < d->nsrc; ++i) ok = encode_src_map(&maps.x[i], d->src[i], d->N, d->H, d->W, Wh, Hh);
+  if (!ok) return cis_set_error(CIS_ERR_CUDA, "cis_conv_wgrad(halo): cuTensorMapEncodeTiled failed / unavailable");
+  dim3 grid(nch64, d->splits, gz);
+  cudaError_t le = launch_pdl(conv_wgrad_halo_kernel<NH, NWG>, grid, dim3(128 * (1 + NWG)), (size_t)smem, st, *d, maps, Wh, Hh, hoy, hox, stage, S);
+  if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_wgrad_halo)");
+  return cis_check_launch("conv_wgrad_halo");
+}
+
+// Halo-resident swapped wgrad (CisWgrad.tma == 2).  Eligibility is re-checked here; the engine falls back to tma = 1.
 static int launch_wgrad_halo(const CisWgrad* d, cudaStream_t st) {
   if (d->sh != 1 || d->sw != 1) return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_wgrad(halo): needs a stride-1 layer");
   int chunks = 0;
@@ -1871,33 +1955,19 @@ static int launch_wgrad_halo(const CisWgrad* d, cudaStream_t st) {
       return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_wgrad(halo): taps must be listed in increasing row-major order");
   const int Wh = 8 + (mx - hox), Hh = 8 + (my - hoy);
   if (Wh > 256 || Hh > 256) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_wgrad(halo): tap extent too large");
-  const int halo_bytes = (Wh * Hh * 128 + 1023) & ~1023;
-  const int stage = halo_bytes + 8192;
-  const int nhalf = d->Cout > 64 ? 2 : 1;
-  const int npg = ((d->ntaps + 1) / 2 + kWHPairs - 1) / kWHPairs;      // groups of kWHPairs tap pairs
-  int S = (200 * 1024) / stage;
-  if (S > kWHMaxStages) S = kWHMaxStages;
-  if (S < 2) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_wgrad(halo): halo does not fit shared memory");
-  int smem = S * stage + 1024;
-  if (smem < kWHPairs * 64 * (int)kAccColBytes + 1024) smem = kWHPairs * 64 * (int)kAccColBytes + 1024;   // accumulators overlay the stages
-  static int attr_smem = 0;
-  if (smem > attr_smem) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_halo_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(conv_wgrad_halo)");
-    attr_smem = smem;
-  }
   if (d->K_pad < d->ntaps * nch64 * 64) return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_wgrad(halo): K_pad smaller than taps * 64-channel groups");
-  WgradHaloMaps maps;
-  memset(&maps, 0, sizeof(maps));
-  CisSrc gs;
-  gs.ptr = d->g; gs.pitch = d->g_pitch; gs.c_off = d->g_coff; gs.chunks = d->g_chunks; gs.n_mod = 0;
-  bool ok = encode_src_map(&maps.g, gs, d->N, d->OH, d->OW, 8, 8);
-  for (int i = 0; ok && i < d->nsrc; ++i) ok = encode_src_map(&maps.x[i], d->src[i], d->N, d->H, d->W, Wh, Hh);
-  if (!ok) return cis_set_error(CIS_ERR_CUDA, "cis_conv_wgrad(halo): cuTensorMapEncodeTiled failed / unavailable");
-  dim3 grid(nch64, d->splits, nhalf * npg);
-  cudaError_t le = launch_pdl(conv_wgrad_halo_kernel, grid, dim3(kThreads), (size_t)smem, st, *d, maps, Wh, Hh, hoy, hox, stage, S);
-  if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_wgrad_halo)");
-  return cis_check_launch("conv_wgrad_halo");
+  const int nh = d->nh ? d->nh : 64, nwg = d->nwg ? d->nwg : 1;
+  if ((nh != 16 && nh != 32 && nh != 64) || nh < (d->Cout > 64 ? 64 : (d->Cout + 15) / 16 * 16) || nwg < 1 || nwg > 2)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_wgrad(halo): nh must be 16/32/64 and cover Cout (64 above 64), nwg 1 or 2");
+  const int halo_bytes = (Wh * Hh * 128 + 1023) & ~1023;
+  switch (nh * 4 + nwg) {
+    case 16 * 4 + 1: return launch_wgrad_halo_t<16, 1>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+    case 16 * 4 + 2: return launch_wgrad_halo_t<16, 2>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+    case 32 * 4 + 1: return launch_wgrad_halo_t<32, 1>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+    case 32 * 4 + 2: return launch_wgrad_halo_t<32, 2>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+    case 64 * 4 + 1: return launch_wgrad_halo_t<64, 1>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+    default: return launch_wgrad_halo_t<64, 2>(d, st, nch64, Wh, Hh, hoy, hox, halo_bytes);
+  }
 }
 
 extern "C" int cis_conv_wgrad(const CisWgrad* d, cis_stream_t stream) {

@@ -292,8 +292,8 @@ WGRAD_HALO = os.environ.get('CIS_WGRAD_HALO', '1') == '1'   # halo-resident swap
 
 def wgrad_halo_fits(taps, cout, stride):
     """Eligibility of the halo-resident wgrad kernel (mirrors launch_wgrad_halo in csrc/conv_igemm.cu): stride 1, taps listed in
-    increasing row-major order, (taps/2) x min(Cout16, 64) accumulator columns <= 512 (a CTA owns two tap pairs and every CTA
-    re-reads the halo: larger tap sets are cheaper on the TMA kernel), >= 2 pipeline stages in shared memory."""
+    increasing row-major order, (taps/2) x min(Cout16, 64) accumulator columns <= 512 (every CTA along grid.z re-reads the halo:
+    larger tap sets are cheaper on the TMA kernel), >= 2 pipeline stages in shared memory.  The tiling is wgrad_halo_tiling's."""
     if stride != 1 or not taps:
         return False
     hoy, hox = min(a for a, _ in taps), min(b for _, b in taps)
@@ -306,6 +306,27 @@ def wgrad_halo_fits(taps, cout, stride):
         return False
     stage = ru(wh * hh * 128, 1024) + 8192
     return (200 * 1024) // stage >= 2
+
+
+# halo wgrad tiling (CisWgrad.nh / nwg).  CIS_WGRAD_HALO_NWG: 1 = N = 64 and one MMA warpgroup of two tap pairs per CTA, split count
+# from the input-chunk x Cout-half tiles only (the earlier plan, for A/B runs) | 2 (default) = wgrad_halo_tiling
+WGRAD_HALO_NWG = int(os.environ.get('CIS_WGRAD_HALO_NWG', '2'))
+
+
+def wgrad_halo_tiling(ntaps, cout):
+    """(nh, nwg, grid_z) of a tma = 2 launch (mirrors launch_wgrad_halo_t).  nh = min(64, Cout rounded to 16) is the MMA N, so no MMA
+    multiplies zero channels beyond the 16-channel granule; one MMA warpgroup holds 128 // nh tap pairs.  Cout > 64: two warpgroups take
+    the two 64-channel halves of Cout over the same pairs (one halo and one gradient stage feed both).  Cout <= 64: a second warpgroup
+    when the pairs do not fit one, splitting the CTA's pairs between the two.  grid_z counts the CTAs of one (input chunk, split)."""
+    npairs = (ntaps + 1) // 2
+    if WGRAD_HALO_NWG < 2:
+        return 64, 1, (2 if cout > 64 else 1) * (-(-npairs // 2))
+    nh = 64 if cout > 64 else ru(cout, 16)
+    p = MAX_ACC_COLS // nh
+    if cout > 64:
+        return 64, 2, -(-npairs // p)
+    nwg = 2 if npairs > p else 1
+    return nh, nwg, -(-npairs // (nwg * p))
 
 
 
@@ -947,8 +968,11 @@ class Builder(object):
             w.tma = 2 if layer.wg_halo else (1 if layer.wg_tma else 0)
             nkb = (nb * (-(-out.H // 8)) * (-(-out.W // 8))) if w.tma else -(-npix // 64)
             ntile = -(-layer.wg_K_pad // 128)
-            if w.tma == 2:      # grid.x = 64-channel chunks of the input, grid.z = 64-channel halves of Cout
-                ntile = (-(-len(layer.in_chanmap) // 64)) * (2 if layer.cout > 64 else 1)
+            if w.tma == 2:      # grid.x = 64-channel chunks of the input, grid.z = tap-pair groups (x 64-channel halves of Cout)
+                w.nh, w.nwg, gz = wgrad_halo_tiling(len(taps), layer.cout)
+                if WGRAD_HALO_NWG < 2:
+                    gz = 2 if layer.cout > 64 else 1
+                ntile = (-(-len(layer.in_chanmap) // 64)) * gz
             splits = max(1, min(nkb // 8 if nkb >= 8 else 1, max(1, (WGRAD_CTAS_PER_SM * NUM_SMS) // ntile)))
             if WGRAD_MAX_SLICE_MB > 0:      # the private slices are written once and read once more by the un-pack job: bound their volume
                 splits = max(1, min(splits, int(WGRAD_MAX_SLICE_MB * 1e6 / (layer.cout * layer.wg_K_pad * 4.0))))
