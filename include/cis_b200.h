@@ -285,7 +285,8 @@ int cis_cis_loss_bwd(const float* flow, const float* mask, const float* flow1, c
 int cis_resize_f32_bwd_to_bf16(const float* ddst, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, void* dsrc,
                                int32_t s_pitch, cis_stream_t stream);
 /* mask backward: dmask += chain through the recover inputs (d_in bf16 [>=2B,H,W,8], gradient of cis_mask_apply's output);
- * then through softmax(x/10)[0] -> bf16 gradient of the 2 logits [B,H,W,8]. */
+ * then through softmax(x/10)[0] -> bf16 gradient of the 2 logits [B,H,W,8].  d_in = NULL skips the recover-input chain (flow may then
+ * be NULL too): dlogits from dmask_direct alone, the stand-alone mask head of the function-level generator_net. */
 int cis_mask_bwd(const float* flow, const float* mask, const float* dmask_direct, const void* d_in, int32_t B, int64_t hw,
                  void* dlogits, cis_stream_t stream);
 
@@ -300,6 +301,29 @@ int cis_clip_adam(float* param, float* m, float* v, const float* grad, int64_t n
                   cis_stream_t stream);
 int cis_cast_f32_to_bf16(const float* src, int64_t n, void* dst, cis_stream_t stream);
 int cis_cast_bf16_to_f32(const void* src, int64_t npix, int32_t pitch, int32_t coff, int32_t C, float* dst, cis_stream_t stream);
+/* dst[p][c] = scale * src[p][coff + c] (the sign of an input gradient read out of a bf16 gradient slice) */
+int cis_cast_bf16_to_f32_scaled(const void* src, int64_t npix, int32_t pitch, int32_t coff, int32_t C, float scale, float* dst,
+                                cis_stream_t stream);
+
+/* ---- gradients of the stand-alone ops of the function-level API (models/functional.py; not used by the step graph) ---- */
+/* charbonnier_loss backward (loss_utils.py:34-51): dsum = fp32 [B] upstream gradient of cis_charbonnier_sum's per-sample sums;
+ * dpred = dsum * mask * d/dpred ((gt-pred)^2 + 1e-6)^cbn, dgt = -dpred, dmask = dsum * ((gt-pred)^2 + 1e-6)^cbn, summed over the
+ * C channels of a pixel when mask_c = 1.  Any of dpred / dgt / dmask may be NULL.  No atomics. */
+int cis_charbonnier_bwd(const float* gt, const float* pred, const float* mask, int32_t B, int64_t hw, int32_t C, int32_t mask_c, float cbn,
+                        const float* dsum, float* dpred, float* dgt, float* dmask, cis_stream_t stream);
+/* dense_image_warp backward (core_warp.py:42-202, clamping of SURVEY App. A.8) for the forward of cis_dense_image_warp; dout fp32
+ * [B,h,w,C].  dflow (fp32 [B,h,w,2], or NULL) is per pixel: the floor carries no gradient, alpha = clip(q - floor, 0, 1) passes it
+ * where 0 <= q - floor <= 1, q = grid - flow_scale * flow.  dimage (fp32 [B,h,w,C], or NULL) is a scatter: accumulated with fp64
+ * atomics into `scratch` (double [B,h,w,C], zeroed by this call) and rounded to fp32 once -- order-dependent below 1e-15 relative. */
+int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const float* flow, float flow_scale, int32_t B, int32_t h,
+                             int32_t w, int32_t C, const float* dout, float* dimage, double* scratch, float* dflow, cis_stream_t stream);
+/* cost_volume backward (core_costvol.py:20-40 as cis_warp_costvol evaluates it with flow = NULL): dout fp32 [B,h,w,81];
+ * g'[p,d] = dout[p,d] * leaky0.1'(recomputed pre-activation) goes to gscratch (fp32 [B,h,w,81]), then
+ * dc1[p] = sum_d g'[p,d] warp[p+d] / C and dwarp[q] = sum_d g'[q-d,d] c1[q-d] / C (fp32 [B,h,w,C]), displacements that leave the map
+ * contributing nothing.  Both are gathers over shared-memory halo tiles: no atomics, bit-reproducible. */
+int cis_cost_volume_bwd(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* warp, int32_t warp_pitch, int32_t warp_coff,
+                        const float* dout, int32_t B, int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp,
+                        cis_stream_t stream);
 
 #ifdef __cplusplus
 }

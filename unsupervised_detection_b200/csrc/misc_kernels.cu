@@ -1086,13 +1086,16 @@ __global__ void mask_bwd_kernel(const float* __restrict__ flow, const float* __r
   pdl_wait();
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= npix) return;
-  const float m = mask[p], f0 = flow[p * 2], f1 = flow[p * 2 + 1];
-  float d0[8], d1[8];
-  unpack8(*reinterpret_cast<const uint4*>(din + p * 8), d0);            // call 0 inputs [f(1-m), 1, 1-m]
-  unpack8(*reinterpret_cast<const uint4*>(din + (npix + p) * 8), d1);   // call 1 inputs [f m, 1, m]
+  const float m = mask[p];
   float dm = dmd[p];
-  dm += -(f0 * d0[0] + f1 * d0[1]) - d0[3];
-  dm += (f0 * d1[0] + f1 * d1[1]) + d1[3];
+  if (din) {      // NULL: the stand-alone mask head of the function-level generator_net (dmask -> dlogits only)
+    const float f0 = flow[p * 2], f1 = flow[p * 2 + 1];
+    float d0[8], d1[8];
+    unpack8(*reinterpret_cast<const uint4*>(din + p * 8), d0);            // call 0 inputs [f(1-m), 1, 1-m]
+    unpack8(*reinterpret_cast<const uint4*>(din + (npix + p) * 8), d1);   // call 1 inputs [f m, 1, m]
+    dm += -(f0 * d0[0] + f1 * d0[1]) - d0[3];
+    dm += (f0 * d1[0] + f1 * d1[1]) + d1[3];
+  }
   const float dl = dm * m * (1.f - m) * 0.1f;  // m = sigmoid((l0-l1)/10)   nets.py:38-41
   const float v[8] = {dl, -dl, 0, 0, 0, 0, 0, 0};
   *reinterpret_cast<uint4*>(dlogits + p * 8) = pack8(v);
@@ -1171,6 +1174,261 @@ __global__ void cast_bf16_f32_kernel(const bf16* __restrict__ s, size_t npix, in
   const size_t p = i / C;
   const int c = (int)(i % C);
   d[i] = __bfloat162float(s[p * pitch + coff + c]);
+}
+__global__ void cast_bf16_f32_scaled_kernel(const bf16* __restrict__ s, size_t npix, int pitch, int coff, int C, float scale,
+                                            float* __restrict__ d) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= npix * C) return;
+  const size_t p = i / C;
+  const int c = (int)(i % C);
+  d[i] = __bfloat162float(s[p * pitch + coff + c]) * scale;
+}
+
+// ------------------------------------------------------------------------------------------------ function-level backward
+// Gradients of the stand-alone ops of models/functional.py.  The step graph never launches these.
+
+// charbonnier_loss (loss_utils.py:34-51) backward, one thread per pixel: with g = dsum[b],
+// dpred = g * m * d/dpred ((gt-pred)^2 + 1e-6)^cbn, dgt = -dpred, dmask = g * ((gt-pred)^2 + 1e-6)^cbn (mask_c = 1: summed over the
+// C channels of the pixel in the thread).
+__global__ void charbonnier_bwd_kernel(const float* __restrict__ gt, const float* __restrict__ pred, const float* __restrict__ mask, size_t hw,
+                                       size_t npix, int C, int mask_c, float cbn, const float* __restrict__ dsum, float* __restrict__ dpred,
+                                       float* __restrict__ dgt, float* __restrict__ dmask) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= npix) return;
+  const float g = dsum[p / hw];
+  float dm = 0.f;
+  for (int c = 0; c < C; ++c) {
+    const size_t e = p * C + c;
+    const float d = gt[e] - pred[e];
+    const float m = mask[mask_c == 1 ? p : e];
+    const float dp = g * m * dcharb_dpred(d, cbn);
+    if (dpred) dpred[e] = dp;
+    if (dgt) dgt[e] = -dp;
+    const float v = g * charb(d, cbn);
+    if (mask_c == 1) dm += v;
+    else if (dmask) dmask[e] = v;
+  }
+  if (mask_c == 1 && dmask) dmask[p] = dm;
+}
+
+// dense_image_warp (core_warp.py:42-202) backward, one thread per pixel.  dflow is local: the floor carries no gradient, alpha =
+// clip(q - floor, 0, 1) passes it where 0 <= q - floor <= 1 (inclusive, as the gradient of tf.clip_by_value), and q = grid - fs * flow.
+// dimage is a scatter (the flow is unbounded): fp64 atomics into dimg, rounded to fp32 by the next kernel.
+__global__ void dense_image_warp_bwd_kernel(const bf16* __restrict__ img, int pitch, int coff, const float* __restrict__ flow, float fs, int B,
+                                            int h, int w, int C, const float* __restrict__ dout, double* __restrict__ dimg,
+                                            float* __restrict__ dflow) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= (size_t)B * h * w) return;
+  const int x = (int)(pix % w), y = (int)((pix / w) % h), b = (int)(pix / ((size_t)w * h));
+  const float qy = (float)y - flow[pix * 2] * fs, qx = (float)x - flow[pix * 2 + 1] * fs;
+  int y0, x0;
+  float ay, ax;
+  warp_coords(qy, h, y0, ay);
+  warp_coords(qx, w, x0, ax);
+  const float ry = qy - (float)y0, rx = qx - (float)x0;
+  const bool pass_y = ry >= 0.f && ry <= 1.f, pass_x = rx >= 0.f && rx <= 1.f;
+  const size_t q00 = (size_t)(b * h + y0) * w + x0;
+  const bf16* base = img + coff + q00 * pitch;
+  const float* go = dout + pix * C;
+  const double w00 = (1.0 - ax) * (1.0 - ay), w01 = (double)ax * (1.0 - ay), w10 = (1.0 - ax) * (double)ay, w11 = (double)ax * ay;
+  float sy = 0.f, sx = 0.f;
+  for (int c0 = 0; c0 < C; c0 += 8) {
+    float tl[8], tr[8], bl[8], br[8];
+    unpack8(__ldg(reinterpret_cast<const uint4*>(base + c0)), tl);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(base + pitch + c0)), tr);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(base + (size_t)w * pitch + c0)), bl);
+    unpack8(__ldg(reinterpret_cast<const uint4*>(base + (size_t)w * pitch + pitch + c0)), br);
+    const int n = min(8, C - c0);
+    for (int e = 0; e < n; ++e) {
+      const float g = go[c0 + e];
+      const float t = ax * (tr[e] - tl[e]) + tl[e];
+      const float bo = ax * (br[e] - bl[e]) + bl[e];
+      sy += g * (bo - t);
+      sx += g * (ay * (br[e] - bl[e]) + (1.f - ay) * (tr[e] - tl[e]));
+      if (dimg) {
+        const double gd = (double)g;
+        atomicAdd(dimg + q00 * C + c0 + e, gd * w00);
+        atomicAdd(dimg + (q00 + 1) * C + c0 + e, gd * w01);
+        atomicAdd(dimg + (q00 + w) * C + c0 + e, gd * w10);
+        atomicAdd(dimg + (q00 + w + 1) * C + c0 + e, gd * w11);
+      }
+    }
+  }
+  if (dflow) {
+    dflow[pix * 2] = pass_y ? -fs * sy : 0.f;
+    dflow[pix * 2 + 1] = pass_x ? -fs * sx : 0.f;
+  }
+}
+__global__ void round_f64_f32_kernel(const double* __restrict__ s, size_t n, float* __restrict__ d) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) d[i] = (float)s[i];
+}
+
+// cost_volume (core_costvol.py:20-40, cis_warp_costvol with flow = NULL) backward.
+// Pass 1: gs[p][d] = dout[p][d] * leaky0.1'(pre[p][d]) / C, the pre-activation recomputed from the bf16 c1 / warp slices through the
+// forward's 8x16 tile + 16x24 zero-padded halo staging.
+__global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
+                                                               int c2o, const float* __restrict__ dout, int B, int h, int w, int C,
+                                                               float* __restrict__ gs) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float cvs[];
+  float* s1 = cvs;                                 // [128][36]
+  float* s2 = cvs + kCvTH * kCvTW * kCvPitch;      // [384][36]
+  const int tid = threadIdx.x;
+  const int b = blockIdx.z, y0 = blockIdx.y * kCvTH, x0 = blockIdx.x * kCvTW;
+  const int pix = tid & 127, py = pix >> 4, px = pix & 15;
+  const int dyb = tid >> 7;  // this thread handles dy = dyb + 2k
+  float acc[5][9];
+#pragma unroll
+  for (int k = 0; k < 5; ++k)
+#pragma unroll
+    for (int d = 0; d < 9; ++d) acc[k][d] = 0.f;
+  const int Cp = (C + 7) & ~7;
+  for (int cc = 0; cc < Cp; cc += 32) {
+    const int nck = min(4, (Cp - cc) / 8);
+    for (int it = tid; it < 128 * 4; it += 256) {
+      const int p = it >> 2, ck = it & 3;
+      const int y = y0 + (p >> 4), x = x0 + (p & 15);
+      float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (ck < nck && y < h && x < w) unpack8(__ldg(reinterpret_cast<const uint4*>(c1 + ((size_t)(b * h + y) * w + x) * c1p + c1o + cc + ck * 8)), v);
+      float4* d = reinterpret_cast<float4*>(s1 + p * kCvPitch + ck * 8);
+      d[0] = make_float4(v[0], v[1], v[2], v[3]);
+      d[1] = make_float4(v[4], v[5], v[6], v[7]);
+    }
+    for (int it = tid; it < kCvHH * kCvHW * 4; it += 256) {
+      const int p = it >> 2, ck = it & 3;
+      const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
+      float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (ck < nck && y >= 0 && y < h && x >= 0 && x < w)
+        unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + ((size_t)(b * h + y) * w + x) * c2p + c2o + cc + ck * 8)), v);
+      float4* d = reinterpret_cast<float4*>(s2 + p * kCvPitch + ck * 8);
+      d[0] = make_float4(v[0], v[1], v[2], v[3]);
+      d[1] = make_float4(v[4], v[5], v[6], v[7]);
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+      const int dy = dyb + 2 * k;
+      if (dy < 9) {
+        const float* r2 = s2 + ((py + dy) * kCvHW + px) * kCvPitch;
+        const float* r1 = s1 + pix * kCvPitch;
+        for (int c4 = 0; c4 < nck * 2; ++c4) {
+          const float4 a = *reinterpret_cast<const float4*>(r1 + c4 * 4);
+#pragma unroll
+          for (int dx = 0; dx < 9; ++dx) {
+            const float4 q = *reinterpret_cast<const float4*>(r2 + dx * kCvPitch + c4 * 4);
+            acc[k][dx] += a.x * q.x + a.y * q.y + a.z * q.z + a.w * q.w;
+          }
+        }
+      }
+    }
+    __syncthreads();
+  }
+  const int y = y0 + py, x = x0 + px;
+  if (y >= h || x >= w) return;
+  const size_t o = ((size_t)(b * h + y) * w + x) * 81;
+  const float inv = 1.f / (float)C;
+#pragma unroll
+  for (int k = 0; k < 5; ++k) {
+    const int dy = dyb + 2 * k;
+    if (dy < 9) {
+#pragma unroll
+      for (int dx = 0; dx < 9; ++dx) gs[o + dy * 9 + dx] = dout[o + dy * 9 + dx] * (acc[k][dx] * inv > 0.f ? inv : 0.1f * inv);
+    }
+  }
+}
+// Pass 2, both sums as gathers over the 81 displacements (fixed order, no atomics):
+//   dc1[p]   = sum_d gs[p][d]     * warp[p + d]
+//   dwarp[q] = sum_d gs[q - d][d] * c1[q - d]
+// A CTA owns an 8x16 pixel tile.  It stages gs of its own pixels ([128][81]) and the shifted planes gs[q - d][d] ([81][128], zero where
+// q - d leaves the map: those displacements read the zero padding in the forward) once, then c1 and warp 16x24 halos per 32-channel pass.
+static constexpr int kCvBwdSmem = (2 * kCvTH * kCvTW * 81 + 2 * kCvHH * kCvHW * kCvPitch) * 4;
+__global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
+                                                          int c2o, const float* __restrict__ gs, int B, int h, int w, int C,
+                                                          float* __restrict__ dc1, float* __restrict__ dwarp) {
+  pdl_launch_dependents();
+  pdl_wait();
+  extern __shared__ float cvs[];
+  float* gself = cvs;                              // [128][81]
+  float* gsh = gself + kCvTH * kCvTW * 81;         // [81][128]
+  float* h1 = gsh + kCvTH * kCvTW * 81;            // c1 halo   [384][36]
+  float* h2 = h1 + kCvHH * kCvHW * kCvPitch;       // warp halo [384][36]
+  const int tid = threadIdx.x;
+  const int b = blockIdx.z, y0 = blockIdx.y * kCvTH, x0 = blockIdx.x * kCvTW;
+  for (int it = tid; it < kCvTH * kCvTW * 81; it += 256) {
+    const int p = it / 81, d = it % 81;
+    const int y = y0 + (p >> 4), x = x0 + (p & 15);
+    gself[it] = (y < h && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * 81 + d) : 0.f;
+  }
+  for (int it = tid; it < kCvTH * kCvTW * 81; it += 256) {
+    const int d = it >> 7, q = it & 127;
+    const int y = y0 + (q >> 4) - (d / 9 - kCvR), x = x0 + (q & 15) - (d % 9 - kCvR);
+    gsh[it] = (y >= 0 && y < h && x >= 0 && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * 81 + d) : 0.f;
+  }
+  const int pix = tid & 127, py = pix >> 4, px = pix & 15;
+  const int ck0 = (tid >> 7) * 2;   // this thread's two 8-channel chunks of the pass
+  const int oy = y0 + py, ox = x0 + px;
+  const bool own = oy < h && ox < w;
+  const size_t op = ((size_t)(b * h + oy) * w + ox) * C;
+  const int Cp = (C + 7) & ~7;
+  for (int cc = 0; cc < Cp; cc += 32) {
+    const int nck = min(4, (Cp - cc) / 8);
+    for (int it = tid; it < kCvHH * kCvHW * 4; it += 256) {
+      const int p = it >> 2, ck = it & 3;
+      const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
+      float v1[8] = {0, 0, 0, 0, 0, 0, 0, 0}, v2[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
+        const size_t q = (size_t)(b * h + y) * w + x;
+        unpack8(__ldg(reinterpret_cast<const uint4*>(c1 + q * c1p + c1o + cc + ck * 8)), v1);
+        unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + q * c2p + c2o + cc + ck * 8)), v2);
+      }
+      float4* d1 = reinterpret_cast<float4*>(h1 + p * kCvPitch + ck * 8);
+      float4* d2 = reinterpret_cast<float4*>(h2 + p * kCvPitch + ck * 8);
+      d1[0] = make_float4(v1[0], v1[1], v1[2], v1[3]);
+      d1[1] = make_float4(v1[4], v1[5], v1[6], v1[7]);
+      d2[0] = make_float4(v2[0], v2[1], v2[2], v2[3]);
+      d2[1] = make_float4(v2[4], v2[5], v2[6], v2[7]);
+    }
+    __syncthreads();
+    if (ck0 < nck) {
+      float a1[16], a2[16];
+#pragma unroll
+      for (int e = 0; e < 16; ++e) a1[e] = a2[e] = 0.f;
+      for (int dy = 0; dy < 9; ++dy) {
+        for (int dx = 0; dx < 9; ++dx) {
+          const int d = dy * 9 + dx;
+          const float g1 = gself[pix * 81 + d], g2 = gsh[d * 128 + pix];
+          const float* r2 = h2 + ((py + dy) * kCvHW + px + dx) * kCvPitch + ck0 * 8;               // warp[p + d]
+          const float* r1 = h1 + ((py + 2 * kCvR - dy) * kCvHW + px + 2 * kCvR - dx) * kCvPitch + ck0 * 8;   // c1[q - d]
+#pragma unroll
+          for (int e4 = 0; e4 < 4; ++e4) {
+            const float4 u = *reinterpret_cast<const float4*>(r2 + e4 * 4);
+            const float4 v = *reinterpret_cast<const float4*>(r1 + e4 * 4);
+            a1[e4 * 4 + 0] += g1 * u.x; a1[e4 * 4 + 1] += g1 * u.y; a1[e4 * 4 + 2] += g1 * u.z; a1[e4 * 4 + 3] += g1 * u.w;
+            a2[e4 * 4 + 0] += g2 * v.x; a2[e4 * 4 + 1] += g2 * v.y; a2[e4 * 4 + 2] += g2 * v.z; a2[e4 * 4 + 3] += g2 * v.w;
+          }
+        }
+      }
+      if (own) {
+        const int cbase = cc + ck0 * 8;
+        const int n = min(16, C - cbase);
+        for (int e = 0; e < n; ++e) {
+          dc1[op + cbase + e] = a1[e];
+          dwarp[op + cbase + e] = a2[e];
+        }
+      }
+    }
+    __syncthreads();
+  }
 }
 
 }  // namespace cis
@@ -1432,6 +1690,7 @@ int cis_resize_f32_bwd_to_bf16(const float* dd, int32_t N, int32_t OH, int32_t O
   return cis_check_launch("resize_f32_bwd_to_bf16");
 }
 int cis_mask_bwd(const float* flow, const float* mask, const float* dmd, const void* din, int32_t B, int64_t hw, void* dlogits, cis_stream_t stream) {
+  if (din && !flow) return cis_set_error(CIS_ERR_BAD_ARG, "cis_mask_bwd: the recover-input chain (d_in) needs the flow");
   CIS_LAUNCH(mask_bwd_kernel, nblk((size_t)B * hw), 256, 0, ST, flow, mask, dmd, (cbf)din, (size_t)B * hw, (mbf)dlogits);
   return cis_check_launch("mask_bwd");
 }
@@ -1458,6 +1717,50 @@ int cis_cast_f32_to_bf16(const float* src, int64_t n, void* dst, cis_stream_t st
 int cis_cast_bf16_to_f32(const void* src, int64_t npix, int32_t pitch, int32_t coff, int32_t C, float* dst, cis_stream_t stream) {
   CIS_LAUNCH(cast_bf16_f32_kernel, nblk((size_t)npix * C), 256, 0, ST, (cbf)src, (size_t)npix, pitch, coff, C, dst);
   return cis_check_launch("cast_bf16_to_f32");
+}
+int cis_cast_bf16_to_f32_scaled(const void* src, int64_t npix, int32_t pitch, int32_t coff, int32_t C, float scale, float* dst,
+                                cis_stream_t stream) {
+  CIS_LAUNCH(cast_bf16_f32_scaled_kernel, nblk((size_t)npix * C), 256, 0, ST, (cbf)src, (size_t)npix, pitch, coff, C, scale, dst);
+  return cis_check_launch("cast_bf16_to_f32_scaled");
+}
+int cis_charbonnier_bwd(const float* gt, const float* pred, const float* mask, int32_t B, int64_t hw, int32_t C, int32_t mask_c, float cbn,
+                        const float* dsum, float* dpred, float* dgt, float* dmask, cis_stream_t stream) {
+  if (C < 1 || (mask_c != 1 && mask_c != C)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_charbonnier_bwd: mask must have 1 or C channels");
+  if (!dsum) return cis_set_error(CIS_ERR_BAD_ARG, "cis_charbonnier_bwd: no upstream gradient");
+  CIS_LAUNCH(charbonnier_bwd_kernel, nblk((size_t)B * hw), 256, 0, ST, gt, pred, mask, (size_t)hw, (size_t)B * hw, C, mask_c, cbn, dsum, dpred, dgt,
+             dmask);
+  return cis_check_launch("charbonnier_bwd");
+}
+int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const float* flow, float fs, int32_t B, int32_t h, int32_t w,
+                             int32_t C, const float* dout, float* dimage, double* scratch, float* dflow, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_dense_image_warp_bwd: needs h,w >= 2 (core_warp.py:188)");
+  if ((pitch | coff) & 7 || coff + ((C + 7) & ~7) > pitch) return cis_set_error(CIS_ERR_BAD_ARG, "cis_dense_image_warp_bwd: bad image slice");
+  if (dimage && !scratch) return cis_set_error(CIS_ERR_BAD_ARG, "cis_dense_image_warp_bwd: dimage needs the fp64 scratch");
+  const size_t npix = (size_t)B * h * w;
+  if (dimage) {
+    cudaError_t e = cudaMemsetAsync(scratch, 0, npix * C * sizeof(double), ST);
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaMemsetAsync");
+  }
+  CIS_LAUNCH(dense_image_warp_bwd_kernel, nblk(npix), 256, 0, ST, (cbf)img, pitch, coff, flow, fs, B, h, w, C, dout, dimage ? scratch : nullptr,
+             dflow);
+  if (dimage) CIS_LAUNCH(round_f64_f32_kernel, nblk(npix * C), 256, 0, ST, (const double*)scratch, npix * C, dimage);
+  return cis_check_launch("dense_image_warp_bwd");
+}
+int cis_cost_volume_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* warp, int32_t wp, int32_t wo, const float* dout, int32_t B, int32_t h,
+                        int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: needs h,w >= 2 (core_warp.py:188)");
+  if (!gscratch || !dc1 || !dwarp) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: NULL output or scratch");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(costvol_bwd)");
+    attr = true;
+  }
+  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
+  CIS_LAUNCH(costvol_bwd_gate_kernel, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, dout, B, h, w, C, gscratch);
+  CIS_LAUNCH(costvol_bwd_kernel, grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)gscratch, B, h, w, C, dc1, dwarp);
+  return cis_check_launch("cost_volume_bwd");
 }
 
 }  // extern "C"

@@ -8,11 +8,18 @@ from the registry filled by `set_parameters()` (dict name -> tensor, names as in
 PyTorch is used for memory and the small amount of buffer plumbing only; there is no CPU fallback: without the CUDA library (or on CPU
 tensors) the calls raise.
 
-STATUS: the sub-graphs reuse the builders that the step graph is made of; the GPU tests of these wrappers
-(tests/test_functional_api_gpu.py) are gated behind CIS_TEST_EXPERIMENTAL=1; tests/test_functional_api_cpu.py checks the plumbing
-with a recording stub.
+Gradients: generator_net, recover_net, charbonnier_loss, cost_volume and dense_image_warp are torch.autograd Functions (first order
+only) when an input or one of the parameter tensors the call reads requires grad; the parameters then receive gradients under their
+variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain rule, resize transposes) and the
+backward kernels of the three stand-alone ops.  A call that needs no gradient runs exactly the forward-only path.  predict_from_img_pairs
+and train_op are not differentiable.
+
+The sub-graphs reuse the builders that the step graph is made of; tests/test_functional_api_gpu.py and
+tests/test_functional_grad_gpu.py check them against the oracle on the GPU, tests/test_functional_api_cpu.py and
+tests/test_functional_grad_cpu.py check the plumbing and the plans without one.
 """
 import torch
+from torch.autograd.function import once_differentiable
 
 from .. import _lib
 from ..engine import Act, Builder, ParamStore, Plan
@@ -20,6 +27,7 @@ from .nets import GeneratorNet, RecoverNet
 
 _PARAMS = {}
 _RUNNERS = {}
+_POOLS = {}      # runner key -> free runner instances of gradient-carrying calls
 
 
 def set_parameters(params):
@@ -44,7 +52,10 @@ def _scope_name(scope, default):
 
 
 class _NetRunner(object):
-    """One cached static plan: parameter store + packed operands + input/output buffers for a fixed shape."""
+    """One cached static plan: parameter store + packed operands + input/output buffers for a fixed shape.  `bwd` is the backward plan
+    (built by ensure_backward for the runners of gradient-carrying calls only); `runs` counts forward runs."""
+
+    MODE = None
 
     def __init__(self, device):
         self.device = device
@@ -53,8 +64,11 @@ class _NetRunner(object):
         self.pack = Plan('pack')
         self.dirty = True
         self._loaded = None
+        self.bwd = None
+        self.runs = 0
 
     def finish(self, layers):
+        self.layers = layers
         for L in layers:
             L.plan_pack(self.pack)
 
@@ -65,31 +79,95 @@ class _NetRunner(object):
             self.pack.run()
             self.dirty, self._loaded = False, src
 
+    def reload(self, params):
+        """Unconditional load + pack (a gradient-carrying call: the parameter tensors may have been updated in place since)."""
+        self.store.load(params)
+        self.pack.run()
+        self.dirty, self._loaded = False, None
+
+    def param_names(self):
+        return [e[0] for e in self.store.entries]
+
+    def ensure_backward(self):
+        """Backward plan: seed (`_plan_seed`) -> the builder's reverse tape -> fixed-order weight-gradient reduction + BN chain rule
+        (one cis_param_multi launch per kind) -> input gradients out of the bf16 input Acts (`_plan_inputs`).  The pack plan is rebuilt
+        with the data-gradient operands the tape needs."""
+        if self.bwd is not None:
+            return
+        self.store.grad = torch.zeros_like(self.store.flat)
+        seed, seeds = self._plan_seed()
+        body = self.bld.build_backward(self.MODE, seeds)
+        fin = Plan('fin')
+        for L in self.layers:
+            L.plan_finalize(fin, self.MODE)
+        full = Plan('bwd_' + self.MODE)
+        full.extend(seed)
+        full.extend(body)
+        full.join()            # weight-gradient lane -> main lane before the packed gradients are unpacked
+        full.extend(fin.batch_param_ops(self.device))
+        full.extend(self._plan_inputs())
+        self.bwd = full
+        self.pack = Plan('pack')
+        for L in self.layers:
+            L.plan_pack(self.pack, dgrad=True)
+        self.dirty = True
+
+    def param_grads(self):
+        return [self.store.view(n, 'grad').clone() for n in self.param_names()]
+
 
 class _GeneratorRunner(_NetRunner):
+    MODE = 'G'
+
     def __init__(self, B, H, W, device, scope):
         _NetRunner.__init__(self, device)
         self.net = GeneratorNet(self.store, scope)
         self.store.finalize(False)
         f32 = self.bld.f32
+        self.B, self.H, self.W = B, H, W
         self.image, self.flow, self.mask = f32(B, H, W, 3), f32(B, H, W, 2), f32(B, H, W, 1)
         # generator_net receives the ALREADY normalised flow (adversarial_learner.py:100-105); cis_pack_generator_input normalises with
         # the statistics it is given, so feed it mean 0 / variance 1: {sum, sum, sum of squares, sum of squares} = {0, 0, hw, hw}
         self.stats = torch.tensor([[0.0, 0.0, float(H * W), float(H * W)]] * B, dtype=torch.float64, device=device)
-        self.gen_in = self.bld.new_act(B, H, W, 5, name='gen_in')
+        # dependency 'G': a backward plan emits conv1's data gradient into gen_in.grad (image and flow gradients)
+        self.gen_in = self.bld.new_act(B, H, W, 5, name='gen_in', dep={'G'})
         self.bld.fwd.add('cis_pack_generator_input', self.image.data_ptr(), self.flow.data_ptr(), self.stats.data_ptr(), B, H * W, self.gen_in.ptr)
         self.net.build(self.bld, self.gen_in, self.mask)
         self.finish(self.net.all_layers())
 
-    def __call__(self, images, flows, params):
-        self.load(params)
+    def run(self, images, flows):
         self.image.copy_(images)
         self.flow.copy_(flows)
         self.bld.fwd.run()
+        self.runs += 1
         return self.mask.clone()
+
+    def __call__(self, images, flows, params):
+        self.load(params)
+        return self.run(images, flows)
+
+    def _plan_seed(self):
+        f32 = self.bld.f32
+        B, H, W = self.B, self.H, self.W
+        self.dmask, self.dimage, self.dflow = f32(B, H, W, 1), f32(B, H, W, 3), f32(B, H, W, 2)
+        lg = self.net.logits.get_grad()
+        seed = Plan('seed_G')
+        # mask = sigmoid((l0 - l1) / 10) fused into conv17's epilogue: dmask -> dlogits (no recover-input chain)
+        seed.add('cis_mask_bwd', None, self.mask.data_ptr(), self.dmask.data_ptr(), None, B, H * W, lg.ptr)
+        return seed, [self.net.logits]
+
+    def _plan_inputs(self):
+        assert self.gen_in.grad_written.get('G'), "generator backward did not reach conv1's data gradient"
+        g, npix = self.gen_in.get_grad(), self.B * self.H * self.W
+        P = Plan('inputs_G')
+        P.add('cis_cast_bf16_to_f32', g.ptr, npix, g.pitch, 0, 3, self.dimage.data_ptr())    # image: channels 0-2
+        P.add('cis_cast_bf16_to_f32', g.ptr, npix, g.pitch, 3, 2, self.dflow.data_ptr())     # normalised flow: channels 3-4
+        return P
 
 
 class _RecoverRunner(_NetRunner):
+    MODE = 'R'
+
     def __init__(self, B, H, W, device, scope, f):
         _NetRunner.__init__(self, device)
         self.net = RecoverNet(self.store, scope, f)
@@ -99,8 +177,9 @@ class _RecoverRunner(_NetRunner):
         self.h1, self.w1 = -(-H // 2), -(-W // 2)
         self.image, self.aug = f32(B, H, W, 3), f32(B, H, W, 4)
         self.flow1, self.pred = f32(B, self.h1, self.w1, 2), f32(B, H, W, 2)
-        self.img8 = self.bld.new_act(B, H, W, 3, name='img8')
-        self.flow_in = self.bld.new_act(B, H, W, 4, name='rec_in')
+        # dependency 'R': a backward plan emits aconv1's / bconv1's data gradients into the two input Acts
+        self.img8 = self.bld.new_act(B, H, W, 3, name='img8', dep={'R'})
+        self.flow_in = self.bld.new_act(B, H, W, 4, name='rec_in', dep={'R'})
         P = self.bld.fwd
         P.add('cis_pack_f32_to_bf16', self.image.data_ptr(), B * H * W, 3, 0.0, self.img8.ptr, 8, 0)
         P.add('cis_pack_f32_to_bf16', self.aug.data_ptr(), B * H * W, 4, 0.0, self.flow_in.ptr, 8, 0)
@@ -109,15 +188,38 @@ class _RecoverRunner(_NetRunner):
         P.add('cis_resize_bilinear_f32', self.flow1.data_ptr(), B, self.h1, self.w1, 2, self.pred.data_ptr(), H, W, 1.0)   # nets.py:108
         self.finish(self.net.all_layers())
 
-    def __call__(self, img1, flow_masked, mask, params):
-        self.load(params)
+    def run(self, img1, flow_masked, mask):
         self.image.copy_(img1)
         # input augmentation of nets.py:50-53: [flow_masked, ones, 1 - mask]
         self.aug[..., 0:2].copy_(flow_masked)
         self.aug[..., 2:3].fill_(1.0)
         self.aug[..., 3:4].copy_(1.0 - mask)
         self.bld.fwd.run()
+        self.runs += 1
         return self.pred.clone()
+
+    def __call__(self, img1, flow_masked, mask, params):
+        self.load(params)
+        return self.run(img1, flow_masked, mask)
+
+    def _plan_seed(self):
+        f32 = self.bld.f32
+        B, H, W = self.B, self.H, self.W
+        self.dpred, self.dimage, self.dflow, self.dmask = f32(B, H, W, 2), f32(B, H, W, 3), f32(B, H, W, 2), f32(B, H, W, 1)
+        fg = self.net.flow1.get_grad()
+        seed = Plan('seed_R')
+        # transpose of the final legacy-bilinear x2 (nets.py:108), as in the step graph's loss head
+        seed.add('cis_resize_f32_bwd_to_bf16', self.dpred.data_ptr(), B, H, W, 2, self.h1, self.w1, fg.ptr, fg.pitch)
+        return seed, [self.net.flow1]
+
+    def _plan_inputs(self):
+        assert self.img8.grad_written.get('R') and self.flow_in.grad_written.get('R'), 'recover backward did not reach its inputs'
+        gi, gf, npix = self.img8.get_grad(), self.flow_in.get_grad(), self.B * self.H * self.W
+        P = Plan('inputs_R')
+        P.add('cis_cast_bf16_to_f32', gi.ptr, npix, gi.pitch, 0, 3, self.dimage.data_ptr())
+        P.add('cis_cast_bf16_to_f32', gf.ptr, npix, gf.pitch, 0, 2, self.dflow.data_ptr())                  # flow_masked: channels 0-1
+        P.add('cis_cast_bf16_to_f32_scaled', gf.ptr, npix, gf.pitch, 3, 1, -1.0, self.dmask.data_ptr())     # channel 3 = 1 - mask
+        return P
 
 
 class _PWCRunner(_NetRunner):
@@ -152,28 +254,132 @@ def _runner(kind, key, make):
     return r
 
 
+class _Lease(object):
+    """A runner instance taken from the per-shape free list by one gradient-carrying call.  Runners hold static activation buffers, so
+    every call that is still waiting for its backward needs its own instance; the lease puts it back when the backward has run or when
+    the call's autograd context is released (no backward will come)."""
+
+    def __init__(self, free, runner):
+        self.free, self.runner = free, runner
+        self.run_id = None
+
+    def take(self):
+        r = self.runner
+        if r is None:
+            raise RuntimeError('this call has already run its backward (the functional API is first-order: no retain_graph / double backward)')
+        if r.runs != self.run_id:
+            raise RuntimeError('the runner of this call was re-run after its forward; its activations are gone')
+        return r
+
+    def release(self):
+        r, self.runner = self.runner, None
+        if r is not None:
+            self.free.append(r)
+
+    def __del__(self):
+        self.release()
+
+
+def _lease(kind, key, make):
+    free = _POOLS.setdefault((kind,) + key, [])
+    if free:
+        r = free.pop()
+    else:
+        _lib.load()
+        r = make()
+        r.ensure_backward()
+    return _Lease(free, r)
+
+
+def _param_inputs(runner, params):
+    """(names, tensors) of the parameters a call reads, in the runner's store order."""
+    src = params if params is not None else _PARAMS
+    names = runner.param_names()
+    missing = [n for n in names if n not in src]
+    if missing:
+        raise KeyError('missing parameter ' + missing[0])
+    return names, [src[n] for n in names]
+
+
+def _needs_grad(tensors):
+    return torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in tensors)
+
+
+class _NetFn(torch.autograd.Function):
+    """generator_net / recover_net with their parameters as explicit inputs: apply(lease, names, n_in, *inputs, *parameters)."""
+
+    @staticmethod
+    def forward(ctx, lease, names, n_in, *args):
+        r = lease.runner
+        r.reload(dict(zip(names, args[n_in:])))
+        out = r.run(*args[:n_in])
+        lease.run_id = r.runs
+        ctx.lease = lease
+        ctx.like = [(t.device, t.dtype, t.shape) for t in args]
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, gout):
+        r = ctx.lease.take()
+        seed = r.dmask if r.MODE == 'G' else r.dpred
+        seed.copy_(gout)
+        r.bwd.run()
+        ins = [r.dimage, r.dflow] if r.MODE == 'G' else [r.dimage, r.dflow, r.dmask]
+        grads = [g.clone() for g in ins] + r.param_grads()
+        ctx.lease.release()
+        out = []
+        for need, g, (dev, dt, shape) in zip(ctx.needs_input_grad[3:], grads, ctx.like):
+            out.append(g.to(device=dev, dtype=dt).reshape(shape) if need else None)
+        return (None, None, None) + tuple(out)
+
+
 # ------------------------------------------------------------------------------------------------------------------ networks
 def generator_net(images, flows, scope='MaskNet', reuse=None, training=True, params=None):
-    """models/nets.py:4-42 -> generated mask [B,H,W,1] in (0,1).  images [B,H,W,3] in [-0.5,0.5], flows [B,H,W,2] normalised."""
+    """models/nets.py:4-42 -> generated mask [B,H,W,1] in (0,1).  images [B,H,W,3] in [-0.5,0.5], flows [B,H,W,2] normalised.
+    Differentiable w.r.t. images, flows and every '<scope>/...' parameter (bf16 activations, fp32 gradients)."""
     _check_cuda(images, flows)
     B, H, W, _ = images.shape
     sc = _scope_name(scope, 'MaskNet')
-    r = _runner('gen', (B, H, W, str(images.device), sc), lambda: _GeneratorRunner(B, H, W, images.device, sc))
-    return r(images, flows, params)
+    key = (B, H, W, str(images.device), sc)
+    make = lambda: _GeneratorRunner(B, H, W, images.device, sc)
+    r = _runner('gen', key, make)
+    names, pvals = _param_inputs(r, params)
+    if not _needs_grad([images, flows] + pvals):
+        return r(images, flows, params)
+    lease = _lease('gen', key, make)
+    try:
+        return _NetFn.apply(lease, names, 2, images, flows, *pvals)
+    except BaseException:
+        lease.release()
+        raise
 
 
 def recover_net(img1, flow_masked, mask, scope='FlownetS', reuse=None, f=0.25, training=True, params=None):
-    """models/nets.py:45-110 -> recovered flow [B,H,W,2] at the input resolution."""
+    """models/nets.py:45-110 -> recovered flow [B,H,W,2] at the input resolution.  Differentiable w.r.t. img1, flow_masked, mask and
+    every '<scope>/...' parameter.  Every call that still waits for its backward holds its own runner instance, so a loss may call it
+    several times (three times in adversarial_learner.py:112-131) before one backward."""
     _check_cuda(img1, flow_masked, mask)
     B, H, W, _ = img1.shape
     sc = _scope_name(scope, 'FlownetS')
-    r = _runner('rec', (B, H, W, str(img1.device), sc, f), lambda: _RecoverRunner(B, H, W, img1.device, sc, f))
-    return r(img1, flow_masked, mask, params)
+    key = (B, H, W, str(img1.device), sc, f)
+    make = lambda: _RecoverRunner(B, H, W, img1.device, sc, f)
+    r = _runner('rec', key, make)
+    names, pvals = _param_inputs(r, params)
+    if not _needs_grad([img1, flow_masked, mask] + pvals):
+        return r(img1, flow_masked, mask, params)
+    lease = _lease('rec', key, make)
+    try:
+        return _NetFn.apply(lease, names, 3, img1, flow_masked, mask, *pvals)
+    except BaseException:
+        lease.release()
+        raise
 
 
 def predict_from_img_pairs(img1, img2, name='pwcnet', params=None):
     """ModelPWCNet.predict_from_img_pairs (model_pwcnet.py:39-76): forward flow img1 -> img2, [B,H,W,2] in pixels of the input size
-    (H, W multiples of 64, 384x640 in the reference's pipeline)."""
+    (H, W multiples of 64, 384x640 in the reference's pipeline).  Forward only: PWC-Net is frozen in the reference
+    (adversarial_learner.py:211-234), so the result carries no gradient."""
     _check_cuda(img1, img2)
     B, H, W, _ = img1.shape
     if H % 64 or W % 64:
@@ -190,10 +396,44 @@ def charbonnier_loss(gt_flows, pred_flows, masks, cbn=0.5):
     mc = masks.shape[-1]
     if tuple(masks.shape[:3]) != (B, H, W) or mc not in (1, C) or tuple(pred_flows.shape) != (B, H, W, C):
         raise ValueError('charbonnier_loss: shapes %s / %s / %s' % (tuple(gt_flows.shape), tuple(pred_flows.shape), tuple(masks.shape)))
+    if _needs_grad([gt_flows, pred_flows, masks]):
+        return _CharbonnierFn.apply(gt_flows, pred_flows, masks, float(cbn))
+    return _charbonnier_fwd(gt_flows, pred_flows, masks, cbn)[0]
+
+
+def _charbonnier_fwd(gt_flows, pred_flows, masks, cbn):
+    B, H, W, C = gt_flows.shape
     g, p, m = (t.contiguous().float() for t in (gt_flows, pred_flows, masks))
     sums = torch.zeros(B, dtype=torch.float64, device=g.device)
-    _lib.call('cis_charbonnier_sum', g.data_ptr(), p.data_ptr(), m.data_ptr(), B, H * W, C, mc, float(cbn), sums.data_ptr(), _stream())
-    return sums.float()
+    _lib.call('cis_charbonnier_sum', g.data_ptr(), p.data_ptr(), m.data_ptr(), B, H * W, C, m.shape[-1], float(cbn), sums.data_ptr(), _stream())
+    return sums.float(), (g, p, m)
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+class _CharbonnierFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, gt_flows, pred_flows, masks, cbn):
+        out, gpm = _charbonnier_fwd(gt_flows, pred_flows, masks, cbn)
+        ctx.save_for_backward(*gpm)
+        ctx.cbn = cbn
+        ctx.dtypes = (gt_flows.dtype, pred_flows.dtype, masks.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dsum):
+        g, p, m = ctx.saved_tensors
+        B, H, W, C = g.shape
+        need = ctx.needs_input_grad
+        dgt, dpred, dmask = (torch.empty_like(t) if n else None for t, n in zip((g, p, m), need[:3]))
+        ds = dsum.contiguous().float()
+        _lib.call('cis_charbonnier_bwd', g.data_ptr(), p.data_ptr(), m.data_ptr(), B, H * W, C, m.shape[-1], ctx.cbn, ds.data_ptr(),
+                  _ptr(dpred), _ptr(dgt), _ptr(dmask), _stream())
+        out = tuple(d.to(dt) if d is not None else None for d, dt in zip((dgt, dpred, dmask), ctx.dtypes))
+        return out + (None,)
 
 
 def train_op(params, grads, m, v, step_state, gradient_clip_value=0.1, can_change=False, learning_rate=1e-4, beta1=0.9, beta2=0.999,
@@ -228,23 +468,82 @@ def _to_act(x):
 def cost_volume(c1, warp, search_range=4, name=None):
     """models/PWCNet/core_costvol.py:20-40 -> [B,h,w,(2r+1)^2]: leaky_relu(mean_c c1 * shifted warp, 0.1), zero padded, dy outer.
     The kernel is built for the reference's search_range = 4 (81 displacements); features and result are bf16-rounded like in the
-    pipeline."""
+    pipeline.  Differentiable w.r.t. c1 and warp (gradients of the bf16-rounded features, fp32)."""
     _check_cuda(c1, warp)
     if search_range != 4:
         raise NotImplementedError('cost_volume: the fused kernel implements search_range=4 (model_pwcnet.py options)')
+    if _needs_grad([c1, warp]):
+        return _CostVolumeFn.apply(c1, warp)
+    return _cost_volume_fwd(c1, warp)[0]
+
+
+def _cost_volume_fwd(c1, warp):
     B, h, w, C = c1.shape
     a1, a2 = _to_act(c1), _to_act(warp)
     out = torch.zeros(B, h, w, 88, dtype=torch.bfloat16, device=c1.device)
     _lib.call('cis_warp_costvol', a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, None, 1.0, B, h, w, C, out.data_ptr(), 88, 0, _stream())
-    return out[..., :81].float()
+    return out[..., :81].float(), a1, a2
+
+
+class _CostVolumeFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, c1, warp):
+        out, a1, a2 = _cost_volume_fwd(c1, warp)
+        ctx.acts = (a1, a2)
+        ctx.dtypes = (c1.dtype, warp.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        a1, a2 = ctx.acts
+        B, h, w, C = a1.N, a1.H, a1.W, a1.C
+        d = dout.contiguous().float()
+        gs = torch.empty(B, h, w, 81, dtype=torch.float32, device=d.device)
+        dc1, dwarp = (torch.empty(B, h, w, C, dtype=torch.float32, device=d.device) for _ in range(2))
+        _lib.call('cis_cost_volume_bwd', a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, d.data_ptr(), B, h, w, C, gs.data_ptr(),
+                  dc1.data_ptr(), dwarp.data_ptr(), _stream())
+        ctx.acts = None
+        return tuple(g.to(dt) if n else None for g, dt, n in zip((dc1, dwarp), ctx.dtypes, ctx.needs_input_grad))
 
 
 def dense_image_warp(image, flow, name=None):
-    """models/PWCNet/core_warp.py:153-202 -> image sampled at (y - flow[...,0], x - flow[...,1]), bilinear, edge-clamped."""
+    """models/PWCNet/core_warp.py:153-202 -> image sampled at (y - flow[...,0], x - flow[...,1]), bilinear, edge-clamped.
+    Differentiable w.r.t. image (fp64-atomic scatter, rounded to fp32 once) and flow (the clamping rules of core_warp.py)."""
     _check_cuda(image, flow)
+    if _needs_grad([image, flow]):
+        return _DenseImageWarpFn.apply(image, flow)
+    return _dense_image_warp_fwd(image, flow)[0]
+
+
+def _dense_image_warp_fwd(image, flow):
     B, h, w, C = image.shape
     a = _to_act(image)
     fl = flow.contiguous().float()
     out = torch.zeros(B, h, w, a.pitch, dtype=torch.bfloat16, device=image.device)
     _lib.call('cis_dense_image_warp', a.ptr, a.pitch, a.c_off, fl.data_ptr(), 1.0, B, h, w, C, out.data_ptr(), a.pitch, _stream())
-    return out[..., :C].float()
+    return out[..., :C].float(), a, fl
+
+
+class _DenseImageWarpFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, image, flow):
+        out, a, fl = _dense_image_warp_fwd(image, flow)
+        ctx.act, ctx.flow = a, fl
+        ctx.dtypes = (image.dtype, flow.dtype)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        a, fl = ctx.act, ctx.flow
+        B, h, w, C = a.N, a.H, a.W, a.C
+        d = dout.contiguous().float()
+        need_img, need_flow = ctx.needs_input_grad[:2]
+        dimage = torch.empty(B, h, w, C, dtype=torch.float32, device=d.device) if need_img else None
+        scratch = torch.empty(B, h, w, C, dtype=torch.float64, device=d.device) if need_img else None
+        dflow = torch.empty(B, h, w, 2, dtype=torch.float32, device=d.device) if need_flow else None
+        _lib.call('cis_dense_image_warp_bwd', a.ptr, a.pitch, a.c_off, fl.data_ptr(), 1.0, B, h, w, C, d.data_ptr(), _ptr(dimage),
+                  _ptr(scratch), _ptr(dflow), _stream())
+        ctx.act = ctx.flow = None
+        return tuple(g.to(dt) if g is not None else None for g, dt in zip((dimage, dflow), ctx.dtypes))
