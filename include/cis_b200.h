@@ -162,9 +162,11 @@ int cis_pack_weights(const float* w, const int32_t* kmap, int32_t K_pad, int32_t
  * same tap-major map (k = tap*cin8 + channel). */
 int cis_pack_weights_tiled(const float* w, const int32_t* kmap, int32_t cin8, int32_t ntaps, int32_t n_tiles, int32_t BN, int32_t cout,
                            int32_t sn, const int32_t* nmap, void* out, cis_stream_t stream);
-/* dw[kmap[k] + n] = sum_{s < nsplit} dwp[s](n, k) for kmap[k] >= 0, n < cout (fixed summation order; forward orientation, sn = 1);
+/* dw[kmap[k] + n*sn] = sum_{s < nsplit} dwp[s](n, k) for kmap[k] >= 0, n < cout (fixed summation order);
  * and, when colpart != NULL, the bias gradient db[c] = sum_{b < nblocks} colpart[b][c], c < nch (the partials of cis_colsum).
- * layout = how cis_conv_wgrad stored a slice: 0 = [cout][K_pad] (CisWgrad.tma == 2), 1 = float4 columns [K_pad/4][cout][4] (tma 0 / 1). */
+ * layout bits 0-7 = how cis_conv_wgrad stored a slice: 0 = [cout][K_pad] (CisWgrad.tma == 2), 1 = float4 columns [K_pad/4][cout][4]
+ * (tma 0 / 1); bits 8+ = sn, the stride of n in dw (0 means 1: the HWIO slot of a conv; Cin: the [kh,kw,Cout,Cin] slot of a transposed
+ * conv, model_pwcnet.py:286). */
 int cis_unpack_wgrad(const float* dwp, const int32_t* kmap, int32_t K_pad, int32_t cout, int32_t nsplit, float* dw, const float* colpart,
                      int32_t nblocks, int32_t nch, float* db, int32_t layout, cis_stream_t stream);
 /* tf.layers.batch_normalization in inference mode folded into the conv (convolution_utils.py:46-51):
@@ -284,6 +286,9 @@ int cis_cis_loss_bwd(const float* flow, const float* mask, const float* flow1, c
 /* transpose of the final x2 resize: dflow1 [3B,h1,w1,2] -> bf16 [3B,h1,w1,8] gradient for the flow1 conv */
 int cis_resize_f32_bwd_to_bf16(const float* ddst, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, void* dsrc,
                                int32_t s_pitch, cis_stream_t stream);
+/* the same times `scale` (the final x4 of PWC-Net's flow, model_pwcnet.py:646) */
+int cis_resize_f32_bwd_to_bf16_scaled(const float* ddst, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, void* dsrc,
+                                      int32_t s_pitch, float scale, cis_stream_t stream);
 /* mask backward: dmask += chain through the recover inputs (d_in bf16 [>=2B,H,W,8], gradient of cis_mask_apply's output);
  * then through softmax(x/10)[0] -> bf16 gradient of the 2 logits [B,H,W,8].  d_in = NULL skips the recover-input chain (flow may then
  * be NULL too): dlogits from dmask_direct alone, the stand-alone mask head of the function-level generator_net. */
@@ -324,6 +329,23 @@ int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const
 int cis_cost_volume_bwd(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* warp, int32_t warp_pitch, int32_t warp_coff,
                         const float* dout, int32_t B, int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp,
                         cis_stream_t stream);
+
+/* ---- PWC-Net backward (function-level predict_from_img_pairs; the step graph keeps PWC-Net frozen) ---- */
+/* Transpose of cis_warp_costvol, same feature operands (c1, c2, flow, flow_scale; flow = NULL at level 6).  dcorr = bf16 gradient of the 81
+ * correlation channels (dcorr[p * dc_pitch + dc_coff + d]).  Results, bf16 slices, each overwritten or accumulated into (accumulate bit 0:
+ * dc1, bit 1: dc2, bit 2: dflow): dc1 and dwarp are the gathers of cis_cost_volume_bwd, with the warped c2 recomputed in the shared-memory
+ * halo tiles as the forward does; with a flow, dc2 is the scatter of cis_dense_image_warp_bwd (fp64 atomics into dscratch, rounded
+ * once) and dflow = d(flow) (the flow_scale factor included, inclusive clip rule of core_warp.py) goes to channels 0-1 of its slice.
+ * Scratch: gscratch fp32 [B,h,w,81]; with a flow, wscratch fp32 [B,h,w,C] (dwarp) and dscratch double [B,h,w,C] (zeroed here). */
+int cis_warp_costvol_bwd(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* c2, int32_t c2_pitch, int32_t c2_coff, const float* flow,
+                         float flow_scale, int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr, int32_t dc_pitch, int32_t dc_coff,
+                         void* dc1, int32_t dc1_pitch, int32_t dc1_coff, void* dc2, int32_t dc2_pitch, int32_t dc2_coff, void* dflow,
+                         int32_t dflow_pitch, int32_t dflow_coff, int32_t accumulate, float* gscratch, float* wscratch, double* dscratch,
+                         cis_stream_t stream);
+/* dst plane a*2+b [N,H,W,d_pitch] (one zero-padded 8-channel chunk per pixel) = src(n, 2y+a, 2x+b, s_coff .. s_coff+C), C <= 8, s_coff any:
+ * the output-parity gradient operands of the weight gradient of conv2d_transpose(k4, s2) */
+int cis_parity_split_bf16(const void* src, int32_t s_pitch, int32_t s_coff, int32_t N, int32_t H, int32_t W, int32_t C, void* dst,
+                          int32_t d_pitch, cis_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -107,6 +107,10 @@ _PROTOS = {
     'cis_charbonnier_bwd': [_p, _p, _p, _i32, _i64, _i32, _i32, _f32, _p, _p, _p, _p],
     'cis_dense_image_warp_bwd': [_p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _p, _p, _p],
     'cis_cost_volume_bwd': [_p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _p, _p],
+    'cis_resize_f32_bwd_to_bf16_scaled': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _f32],
+    'cis_warp_costvol_bwd': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32,
+                             _p, _i32, _i32, _i32, _p, _p, _p],
+    'cis_parity_split_bf16': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32],
 }
 EXPORTS = sorted(list(_PROTOS) + ['cis_last_error', 'cis_version', 'cis_set_persist_mode', 'cis_crc32c', 'cis_host_resize_bilinear_legacy',
                                   'cis_host_bgr8_to_rgb_resized'])

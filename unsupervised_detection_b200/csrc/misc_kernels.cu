@@ -103,9 +103,11 @@ __device__ __forceinline__ void unpack_wgrad_body(size_t i, const float* __restr
   const size_t nw = (size_t)cout * K_pad;
   if (i < nw) {
     // slice element i -> (output channel n, packed column k): layout 0 = [cout][K_pad] (halo-resident wgrad), layout 1 = float4 columns
-    // [K_pad / 4][cout][4] (gather / TMA-tile wgrad kernels)
+    // [K_pad / 4][cout][4] (gather / TMA-tile wgrad kernels).  Bits 8+ of layout: stride of n in dw (0 = 1, the HWIO slot; Cin for the
+    // [kh,kw,Cout,Cin] slot of a transposed conv)
+    const size_t sn = (layout >> 8) ? (size_t)(layout >> 8) : 1;
     int n, k;
-    if (layout == 0) {
+    if ((layout & 0xff) == 0) {
       n = (int)(i / K_pad);
       k = (int)(i % K_pad);
     } else {
@@ -128,7 +130,7 @@ __device__ __forceinline__ void unpack_wgrad_body(size_t i, const float* __restr
       for (int u = 0; u < 8; ++u) a[u] += t[u];
     }
     for (; s < nsplit; ++s) a[0] += __ldcg(q + (size_t)s * nw);
-    dw[(size_t)km + n] = ((a[0] + a[1]) + (a[2] + a[3])) + ((a[4] + a[5]) + (a[6] + a[7]));
+    dw[(size_t)km + n * sn] = ((a[0] + a[1]) + (a[2] + a[3])) + ((a[4] + a[5]) + (a[6] + a[7]));
   } else if (colpart != nullptr && i - nw < (size_t)nch) {
     const int c = (int)(i - nw);
     float a = 0.f;
@@ -663,9 +665,10 @@ __global__ void crop_resize_f32_kernel(const float* __restrict__ src, int Ws, in
     dst[(size_t)pix * C + c] = t + (bo - t) * ly.f;
   }
 }
-// transpose of the fp32 legacy resize, result stored as a bf16 8-channel chunk (C <= 8 real channels)
+// transpose of the fp32 legacy resize (times `scale`, the factor of cis_resize_bilinear_f32), result stored as a bf16 8-channel chunk
+// (C <= 8 real channels)
 __global__ void resize_f32_bwd_to_bf16_kernel(const float* __restrict__ dd, int N, int OH, int OW, int C, int H, int W, bf16* __restrict__ ds,
-                                              int sp) {
+                                              int sp, float scale) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -688,6 +691,8 @@ __global__ void resize_f32_bwd_to_bf16_kernel(const float* __restrict__ dd, int 
       for (int c = 0; c < C; ++c) a[c] += wt * q[c];
     }
   }
+#pragma unroll
+  for (int c = 0; c < 8; ++c) a[c] *= scale;
   *reinterpret_cast<uint4*>(ds + pix * sp) = pack8(a);
 }
 // tf.image.resize_nearest_neighbor(align_corners=True), out = 2*in: src = min(roundf(d*(in-1)/(out-1)), in-1)   App. A.5
@@ -1215,12 +1220,30 @@ __global__ void charbonnier_bwd_kernel(const float* __restrict__ gt, const float
   if (mask_c == 1 && dmask) dmask[p] = dm;
 }
 
+// Gradient destinations of the backward kernels below, element (pixel, channel) at p[pix * pitch + off + c]: plain fp32 stores (the
+// stand-alone ops) or bf16 slices of the engine's gradient buffers, overwritten or accumulated into (acc != 0; PWC-Net backward).
+struct F32Out {
+  float* p;
+  int pitch, off;
+  __device__ __forceinline__ void put(size_t pix, int c, float v) const { p[pix * pitch + off + c] = v; }
+};
+struct Bf16Out {
+  bf16* p;
+  int pitch, off, acc;
+  __device__ __forceinline__ void put(size_t pix, int c, float v) const {
+    bf16* q = p + pix * pitch + off + c;
+    *q = __float2bfloat16(acc ? __bfloat162float(*q) + v : v);
+  }
+};
+__device__ __forceinline__ float ldf(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ldf(const bf16* p) { return __bfloat162float(*p); }
+
 // dense_image_warp (core_warp.py:42-202) backward, one thread per pixel.  dflow is local: the floor carries no gradient, alpha =
 // clip(q - floor, 0, 1) passes it where 0 <= q - floor <= 1 (inclusive, as the gradient of tf.clip_by_value), and q = grid - fs * flow.
-// dimage is a scatter (the flow is unbounded): fp64 atomics into dimg, rounded to fp32 by the next kernel.
+// dimage is a scatter (the flow is unbounded): fp64 atomics into dimg, rounded once by round_f64_kernel.  dflow.p == NULL: no dflow.
+template <class OF>
 __global__ void dense_image_warp_bwd_kernel(const bf16* __restrict__ img, int pitch, int coff, const float* __restrict__ flow, float fs, int B,
-                                            int h, int w, int C, const float* __restrict__ dout, double* __restrict__ dimg,
-                                            float* __restrict__ dflow) {
+                                            int h, int w, int C, const float* __restrict__ dout, double* __restrict__ dimg, const OF dflow) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -1260,24 +1283,45 @@ __global__ void dense_image_warp_bwd_kernel(const bf16* __restrict__ img, int pi
       }
     }
   }
-  if (dflow) {
-    dflow[pix * 2] = pass_y ? -fs * sy : 0.f;
-    dflow[pix * 2 + 1] = pass_x ? -fs * sx : 0.f;
+  if (dflow.p) {
+    dflow.put(pix, 0, pass_y ? -fs * sy : 0.f);
+    dflow.put(pix, 1, pass_x ? -fs * sx : 0.f);
   }
 }
-__global__ void round_f64_f32_kernel(const double* __restrict__ s, size_t n, float* __restrict__ d) {
+// The four output-parity planes of a 2H x 2W gradient slice (C <= 8 channels from channel sc, any alignment): plane a*2+b, pixel (n,y,x) =
+// src(n, 2y + a, 2x + b) as one zero-padded 8-channel chunk -- the gradient operands of a k4 s2 transposed conv's weight gradient.
+__global__ void parity_split_bf16_kernel(const bf16* __restrict__ src, int sp, int sc, int N, int H, int W, int C, bf16* __restrict__ dst, int dp) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t npix = (size_t)N * H * W;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 4 * npix) return;
+  const int q = (int)(i / npix);
+  const size_t pix = i - (size_t)q * npix;
+  const int x = (int)(pix % W), y = (int)((pix / W) % H), n = (int)(pix / ((size_t)W * H));
+  const bf16* s = src + ((size_t)(n * 2 * H + 2 * y + (q >> 1)) * 2 * W + 2 * x + (q & 1)) * sp + sc;
+  float v[8];
+#pragma unroll
+  for (int c = 0; c < 8; ++c) v[c] = c < C ? __bfloat162float(s[c]) : 0.f;
+  *reinterpret_cast<uint4*>(dst + i * dp) = pack8(v);
+}
+// the fp64 scatter sums [npix][C], rounded once into their destination
+template <class O>
+__global__ void round_f64_kernel(const double* __restrict__ s, size_t npix, int C, const O d) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) d[i] = (float)s[i];
+  if (i < npix * C) d.put(i / C, (int)(i % C), (float)s[i]);
 }
 
-// cost_volume (core_costvol.py:20-40, cis_warp_costvol with flow = NULL) backward.
-// Pass 1: gs[p][d] = dout[p][d] * leaky0.1'(pre[p][d]) / C, the pre-activation recomputed from the bf16 c1 / warp slices through the
-// forward's 8x16 tile + 16x24 zero-padded halo staging.
+// cost_volume (core_costvol.py:20-40) backward, and with flow != NULL the backward of cis_warp_costvol's fused warp.
+// Pass 1: gs[p][d] = dout[p][d] * leaky0.1'(pre[p][d]) / C, the pre-activation recomputed from the bf16 c1 / c2 slices through the
+// forward's 8x16 tile + 16x24 zero-padded halo staging (c2 warped by fs * flow in the halo, as the forward does).  dout: fp32 or a bf16
+// slice, element d of pixel p at dout[p * dp + doff + d].
+template <typename TD>
 __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
-                                                               int c2o, const float* __restrict__ dout, int B, int h, int w, int C,
-                                                               float* __restrict__ gs) {
+                                                               int c2o, const float* __restrict__ flow, float fs, const TD* __restrict__ dout,
+                                                               int dp, int doff, int B, int h, int w, int C, float* __restrict__ gs) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float cvs[];
@@ -1308,8 +1352,14 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
       const int p = it >> 2, ck = it & 3;
       const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
       float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      if (ck < nck && y >= 0 && y < h && x >= 0 && x < w)
-        unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + ((size_t)(b * h + y) * w + x) * c2p + c2o + cc + ck * 8)), v);
+      if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
+        if (flow) {
+          const size_t fp = ((size_t)(b * h + y) * w + x) * 2;
+          warp_chunk(c2 + c2o + cc + ck * 8, c2p, h, w, b, (float)y - __ldg(flow + fp) * fs, (float)x - __ldg(flow + fp + 1) * fs, v);
+        } else {
+          unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + ((size_t)(b * h + y) * w + x) * c2p + c2o + cc + ck * 8)), v);
+        }
+      }
       float4* d = reinterpret_cast<float4*>(s2 + p * kCvPitch + ck * 8);
       d[0] = make_float4(v[0], v[1], v[2], v[3]);
       d[1] = make_float4(v[4], v[5], v[6], v[7]);
@@ -1335,14 +1385,15 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
   }
   const int y = y0 + py, x = x0 + px;
   if (y >= h || x >= w) return;
-  const size_t o = ((size_t)(b * h + y) * w + x) * 81;
+  const size_t q = (size_t)(b * h + y) * w + x, o = q * 81;
+  const TD* dq = dout + q * dp + doff;
   const float inv = 1.f / (float)C;
 #pragma unroll
   for (int k = 0; k < 5; ++k) {
     const int dy = dyb + 2 * k;
     if (dy < 9) {
 #pragma unroll
-      for (int dx = 0; dx < 9; ++dx) gs[o + dy * 9 + dx] = dout[o + dy * 9 + dx] * (acc[k][dx] * inv > 0.f ? inv : 0.1f * inv);
+      for (int dx = 0; dx < 9; ++dx) gs[o + dy * 9 + dx] = ldf(dq + dy * 9 + dx) * (acc[k][dx] * inv > 0.f ? inv : 0.1f * inv);
     }
   }
 }
@@ -1350,11 +1401,13 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
 //   dc1[p]   = sum_d gs[p][d]     * warp[p + d]
 //   dwarp[q] = sum_d gs[q - d][d] * c1[q - d]
 // A CTA owns an 8x16 pixel tile.  It stages gs of its own pixels ([128][81]) and the shifted planes gs[q - d][d] ([81][128], zero where
-// q - d leaves the map: those displacements read the zero padding in the forward) once, then c1 and warp 16x24 halos per 32-channel pass.
+// q - d leaves the map: those displacements read the zero padding in the forward) once, then c1 and warp 16x24 halos per 32-channel pass
+// (flow != NULL: the warp halo recomputed from c2 and fs * flow, never stored in HBM).
 static constexpr int kCvBwdSmem = (2 * kCvTH * kCvTW * 81 + 2 * kCvHH * kCvHW * kCvPitch) * 4;
+template <class O1, class O2>
 __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
-                                                          int c2o, const float* __restrict__ gs, int B, int h, int w, int C,
-                                                          float* __restrict__ dc1, float* __restrict__ dwarp) {
+                                                          int c2o, const float* __restrict__ flow, float fs, const float* __restrict__ gs, int B,
+                                                          int h, int w, int C, const O1 dc1, const O2 dwarp) {
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float cvs[];
@@ -1378,7 +1431,7 @@ __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict
   const int ck0 = (tid >> 7) * 2;   // this thread's two 8-channel chunks of the pass
   const int oy = y0 + py, ox = x0 + px;
   const bool own = oy < h && ox < w;
-  const size_t op = ((size_t)(b * h + oy) * w + ox) * C;
+  const size_t op = (size_t)(b * h + oy) * w + ox;
   const int Cp = (C + 7) & ~7;
   for (int cc = 0; cc < Cp; cc += 32) {
     const int nck = min(4, (Cp - cc) / 8);
@@ -1389,7 +1442,10 @@ __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict
       if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
         const size_t q = (size_t)(b * h + y) * w + x;
         unpack8(__ldg(reinterpret_cast<const uint4*>(c1 + q * c1p + c1o + cc + ck * 8)), v1);
-        unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + q * c2p + c2o + cc + ck * 8)), v2);
+        if (flow)
+          warp_chunk(c2 + c2o + cc + ck * 8, c2p, h, w, b, (float)y - __ldg(flow + 2 * q) * fs, (float)x - __ldg(flow + 2 * q + 1) * fs, v2);
+        else
+          unpack8(__ldg(reinterpret_cast<const uint4*>(c2 + q * c2p + c2o + cc + ck * 8)), v2);
       }
       float4* d1 = reinterpret_cast<float4*>(h1 + p * kCvPitch + ck * 8);
       float4* d2 = reinterpret_cast<float4*>(h2 + p * kCvPitch + ck * 8);
@@ -1422,8 +1478,8 @@ __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict
         const int cbase = cc + ck0 * 8;
         const int n = min(16, C - cbase);
         for (int e = 0; e < n; ++e) {
-          dc1[op + cbase + e] = a1[e];
-          dwarp[op + cbase + e] = a2[e];
+          dc1.put(op, cbase + e, a1[e]);
+          dwarp.put(op, cbase + e, a2[e]);
         }
       }
     }
@@ -1481,7 +1537,7 @@ int cis_pack_weights_tiled(const float* w, const int32_t* kmap, int32_t cin8, in
 }
 int cis_unpack_wgrad(const float* dwp, const int32_t* kmap, int32_t K_pad, int32_t cout, int32_t nsplit, float* dw, const float* colpart,
                      int32_t nblocks, int32_t nch, float* db, int32_t layout, cis_stream_t stream) {
-  if (nsplit < 1 || (colpart && (nblocks < 1 || !db)) || (layout != 0 && layout != 1) || K_pad % 4)
+  if (nsplit < 1 || (colpart && (nblocks < 1 || !db)) || ((layout & 0xff) != 0 && (layout & 0xff) != 1) || layout < 0 || K_pad % 4)
     return cis_set_error(CIS_ERR_BAD_ARG, "cis_unpack_wgrad: bad split / column-sum / layout arguments");
   CIS_LAUNCH(unpack_wgrad_kernel, nblk((size_t)cout * K_pad + (colpart ? nch : 0)), 256, 0, ST, dwp, kmap, K_pad, cout, nsplit, dw, colpart, nblocks,
              nch, db, layout);
@@ -1686,8 +1742,14 @@ int cis_cis_loss_bwd(const float* flow, const float* mask, const float* flow1, c
 int cis_resize_f32_bwd_to_bf16(const float* dd, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, void* ds, int32_t sp,
                                cis_stream_t stream) {
   if (C > 8) return cis_set_error(CIS_ERR_BAD_ARG, "cis_resize_f32_bwd_to_bf16: C > 8");
-  CIS_LAUNCH(resize_f32_bwd_to_bf16_kernel, nblk((size_t)N * H * W), 256, 0, ST, dd, N, OH, OW, C, H, W, (mbf)ds, sp);
+  CIS_LAUNCH(resize_f32_bwd_to_bf16_kernel, nblk((size_t)N * H * W), 256, 0, ST, dd, N, OH, OW, C, H, W, (mbf)ds, sp, 1.f);
   return cis_check_launch("resize_f32_bwd_to_bf16");
+}
+int cis_resize_f32_bwd_to_bf16_scaled(const float* dd, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, void* ds, int32_t sp,
+                                      float scale, cis_stream_t stream) {
+  if (C > 8) return cis_set_error(CIS_ERR_BAD_ARG, "cis_resize_f32_bwd_to_bf16_scaled: C > 8");
+  CIS_LAUNCH(resize_f32_bwd_to_bf16_kernel, nblk((size_t)N * H * W), 256, 0, ST, dd, N, OH, OW, C, H, W, (mbf)ds, sp, scale);
+  return cis_check_launch("resize_f32_bwd_to_bf16_scaled");
 }
 int cis_mask_bwd(const float* flow, const float* mask, const float* dmd, const void* din, int32_t B, int64_t hw, void* dlogits, cis_stream_t stream) {
   if (din && !flow) return cis_set_error(CIS_ERR_BAD_ARG, "cis_mask_bwd: the recover-input chain (d_in) needs the flow");
@@ -1741,9 +1803,9 @@ int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const
     cudaError_t e = cudaMemsetAsync(scratch, 0, npix * C * sizeof(double), ST);
     if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaMemsetAsync");
   }
-  CIS_LAUNCH(dense_image_warp_bwd_kernel, nblk(npix), 256, 0, ST, (cbf)img, pitch, coff, flow, fs, B, h, w, C, dout, dimage ? scratch : nullptr,
-             dflow);
-  if (dimage) CIS_LAUNCH(round_f64_f32_kernel, nblk(npix * C), 256, 0, ST, (const double*)scratch, npix * C, dimage);
+  CIS_LAUNCH(dense_image_warp_bwd_kernel<F32Out>, nblk(npix), 256, 0, ST, (cbf)img, pitch, coff, flow, fs, B, h, w, C, dout,
+             dimage ? scratch : nullptr, F32Out{dflow, 2, 0});
+  if (dimage) CIS_LAUNCH(round_f64_kernel<F32Out>, nblk(npix * C), 256, 0, ST, (const double*)scratch, npix, C, F32Out{dimage, C, 0});
   return cis_check_launch("dense_image_warp_bwd");
 }
 int cis_cost_volume_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* warp, int32_t wp, int32_t wo, const float* dout, int32_t B, int32_t h,
@@ -1752,15 +1814,58 @@ int cis_cost_volume_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* wa
   if (!gscratch || !dc1 || !dwarp) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: NULL output or scratch");
   static bool attr = false;
   if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
+    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<F32Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
     if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(costvol_bwd)");
     attr = true;
   }
   dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
-  CIS_LAUNCH(costvol_bwd_gate_kernel, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, dout, B, h, w, C, gscratch);
-  CIS_LAUNCH(costvol_bwd_kernel, grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)gscratch, B, h, w, C, dc1, dwarp);
+  CIS_LAUNCH(costvol_bwd_gate_kernel<float>, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr, 1.f, dout, 81, 0,
+             B, h, w, C, gscratch);
+  CIS_LAUNCH((costvol_bwd_kernel<F32Out, F32Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr, 1.f,
+             (const float*)gscratch, B, h, w, C, F32Out{dc1, C, 0}, F32Out{dwarp, C, 0});
   return cis_check_launch("cost_volume_bwd");
+}
+int cis_warp_costvol_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs,
+                         int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr, int32_t dcp, int32_t dco, void* dc1, int32_t dc1p,
+                         int32_t dc1o, void* dc2, int32_t dc2p, int32_t dc2o, void* dflow, int32_t dfp, int32_t dfo, int32_t accumulate,
+                         float* gscratch, float* wscratch, double* dscratch, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: needs h,w >= 2 (core_warp.py:188)");
+  if (!dcorr || !dc1 || !dc2 || !gscratch) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: NULL gradient or scratch");
+  if (flow && (!dflow || !wscratch || !dscratch)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: the warp needs dflow and scratch");
+  if ((c1p | c1o | c2p | c2o) & 7) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: feature slices must be 8-channel aligned");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<Bf16Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<Bf16Out, Bf16Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(warp_costvol_bwd)");
+    attr = true;
+  }
+  const Bf16Out o1{(mbf)dc1, dc1p, dc1o, accumulate & 1}, o2{(mbf)dc2, dc2p, dc2o, (accumulate >> 1) & 1};
+  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
+  CIS_LAUNCH(costvol_bwd_gate_kernel<bf16>, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (cbf)dcorr, dcp, dco, B, h, w, C,
+             gscratch);
+  if (!flow) {       // level 6: no warp, dwarp is dc2
+    CIS_LAUNCH((costvol_bwd_kernel<Bf16Out, Bf16Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (const float*)gscratch,
+               B, h, w, C, o1, o2);
+    return cis_check_launch("warp_costvol_bwd");
+  }
+  CIS_LAUNCH((costvol_bwd_kernel<Bf16Out, F32Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (const float*)gscratch,
+             B, h, w, C, o1, F32Out{wscratch, C, 0});
+  const size_t npix = (size_t)B * h * w;
+  cudaError_t e = cudaMemsetAsync(dscratch, 0, npix * C * sizeof(double), ST);
+  if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaMemsetAsync");
+  CIS_LAUNCH(dense_image_warp_bwd_kernel<Bf16Out>, nblk(npix), 256, 0, ST, (cbf)c2, c2p, c2o, flow, fs, B, h, w, C, (const float*)wscratch, dscratch,
+             Bf16Out{(mbf)dflow, dfp, dfo, (accumulate >> 2) & 1});
+  CIS_LAUNCH(round_f64_kernel<Bf16Out>, nblk(npix * C), 256, 0, ST, (const double*)dscratch, npix, C, o2);
+  return cis_check_launch("warp_costvol_bwd");
+}
+int cis_parity_split_bf16(const void* src, int32_t sp, int32_t sc, int32_t N, int32_t H, int32_t W, int32_t C, void* dst, int32_t dp,
+                          cis_stream_t stream) {
+  if (C < 1 || C > 8 || dp < 8 || (dp & 7)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_parity_split_bf16: 1..8 channels into 8-aligned planes");
+  CIS_LAUNCH(parity_split_bf16_kernel, nblk((size_t)4 * N * H * W), 256, 0, ST, (cbf)src, sp, sc, N, H, W, C, (mbf)dst, dp);
+  return cis_check_launch("parity_split_bf16");
 }
 
 }  // extern "C"

@@ -206,6 +206,7 @@ class Act(object):
         self.grad_written = {}   # mode -> bool
         self.device = device
         self.gen_rows = None     # batch rows processed by the generator-step backward (2B of 3B)
+        self.grad_buf = None     # set: the gradient is the same channel slice of this buffer (views of one zeroed, accumulated buffer)
 
     @property
     def ptr(self):
@@ -229,7 +230,8 @@ class Act(object):
         if getattr(self, '_owner', None) is not None:
             return self._owner.get_grad()
         if self.grad is None:
-            self.grad = Act(self.N, self.H, self.W, self.C, self.device, chanmap=self.chanmap, name=self.name + '.grad')
+            self.grad = Act(self.N, self.H, self.W, self.C, self.device, buf=self.grad_buf, c_off=self.c_off if self.grad_buf is not None else 0,
+                            chanmap=self.chanmap, name=self.name + '.grad')
         return self.grad
 
     def float(self):
@@ -311,6 +313,14 @@ def wgrad_halo_fits(taps, cout, stride):
 # halo wgrad tiling (CisWgrad.nh / nwg).  CIS_WGRAD_HALO_NWG: 1 = N = 64 and one MMA warpgroup of two tap pairs per CTA, split count
 # from the input-chunk x Cout-half tiles only (the earlier plan, for A/B runs) | 2 (default) = wgrad_halo_tiling
 WGRAD_HALO_NWG = int(os.environ.get('CIS_WGRAD_HALO_NWG', '2'))
+
+
+def wgrad_splits(nkb, ntile, cout, K_pad):
+    """Split-K factor of a weight-gradient launch of nkb reduction blocks and ntile column tiles (grid.x x grid.z)."""
+    splits = max(1, min(nkb // 8 if nkb >= 8 else 1, max(1, (WGRAD_CTAS_PER_SM * NUM_SMS) // ntile)))
+    if WGRAD_MAX_SLICE_MB > 0:      # the private slices are written once and read once more by the un-pack job: bound their volume
+        splits = max(1, min(splits, int(WGRAD_MAX_SLICE_MB * 1e6 / (cout * K_pad * 4.0))))
+    return -(-nkb // (-(-nkb // splits)))        # every split owns >= 1 reduction block (its slice is written, not accumulated)
 
 
 def wgrad_halo_tiling(ntaps, cout):
@@ -730,6 +740,10 @@ class ConvLayer(object):
                 if getattr(self, 'fwd_rows_used', True):
                     plan.add('cis_pack_weights', self.w_src_ptr(), self.fwd_kmap.data_ptr(), self.K_pad, self.npad, self.cout, 1,
                              None, self.fwd_pack.data_ptr())
+        if dgrad and getattr(self, 'tr_dgrad', None) is not None:
+            pk = self.tr_dgrad       # transposed conv: W[kh,kw,Cout,Cin] read as the HWIO weights of a stride-2 conv Cout -> Cin
+            plan.add('cis_pack_weights', self.w_src_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], pk['rows'], len(self.in_chanmap), 1,
+                     pk['nmap'].data_ptr(), pk['w'].data_ptr())
         if dgrad and self.dgrad_packs:
             cout8 = ru(self.cout, 8)
             for pk in self.dgrad_packs:
@@ -743,12 +757,24 @@ class ConvLayer(object):
     def plan_finalize(self, bp, mode):
         """Fixed-order sum of the private split-K slices of the packed fp32 weight gradient -> HWIO slot of the flat gradient
         buffer, same for the per-block bias-gradient partials (+ BN chain rule for the generator).  No atomics, nothing to zero."""
+        s = self.store
+        if self.transposed:
+            # four output-parity weight gradients, each into its own taps of the [kh,kw,Cout,Cin] slot (n stride Cin: layout bits 8+); the
+            # first also sums the bias partials of the whole output gradient
+            for q, pk in enumerate(p for p in getattr(self, 'tr_packs', []) if mode in p.get('wg_splits', {})):
+                bp.add('cis_unpack_wgrad', pk['dwp'].data_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], self.cout, pk['wg_splits'][mode],
+                       s.ptr(self.wkey, 'grad'), self.colpart.data_ptr() if q == 0 else None, self.col_blocks[mode] if q == 0 else 0,
+                       self.cout if q == 0 else 0, s.ptr(self.bkey, 'grad') if q == 0 else None, 1 | (self.cin << 8))
+            return
         if not hasattr(self, 'dwp') or mode not in getattr(self, 'wg_splits', {}):
             return
-        s = self.store
-        bp.add('cis_unpack_wgrad', self.dwp.data_ptr(), self.wg_kmap.data_ptr(), self.wg_K_pad, self.cout, self.wg_splits[mode],
+        bp.add('cis_unpack_wgrad', self.dwp.data_ptr(), self.wg_kmap.data_ptr(), self.wg_K_pad, min(128, self.cout), self.wg_splits[mode],
                s.ptr(self.wkey, 'grad'), self.colpart.data_ptr(), self.col_blocks[mode], self.cout,
                (self.db_eff.data_ptr() if self.bn else s.ptr(self.bkey, 'grad')), 0 if self.wg_halo else 1)
+        for g0, buf in sorted(getattr(self, 'dwp_hi', {}).items()):     # output channels >= 128: dw shifted by g0 (n stride 1)
+            if (mode, g0) in self.wg_splits_hi:
+                bp.add('cis_unpack_wgrad', buf.data_ptr(), self.wg_kmap.data_ptr(), self.wg_K_pad, min(128, self.cout - g0),
+                       self.wg_splits_hi[(mode, g0)], s.ptr(self.wkey, 'grad') + 4 * g0, None, 0, 0, None, 0 if self.wg_halo else 1)
         if self.bn:
             bp.add('cis_bn_chain', s.ptr(self.wkey), s.ptr(self.bkey), s.ptr(self.name + '/gamma'), s.ptr(self.wkey, 'grad'),
                    self.db_eff.data_ptr(), self.k * self.k * self.cin * self.cout, self.cout, s.ptr(self.bkey, 'grad'),
@@ -813,6 +839,23 @@ class ConvLayer(object):
         self.tr_packs = packs
         self.fwd_pack = True
 
+    def setup_transposed_dgrad(self, g_pos):
+        """Data gradient of the transposed conv: dx[y, x, ci] = sum dy[2y + ky - 1, 2x + kx - 1, co] * W[ky, kx, co, ci], a 4x4 stride-2
+        forward conv of the output gradient.  g_pos: position of output channel co inside the gradient's 8-channel chunk."""
+        if getattr(self, 'tr_dgrad', None) is not None:
+            return
+        g_chan = [-1] * 8
+        for co in range(self.cout):
+            g_chan[g_pos + co] = co
+        cin8 = len(self.in_chanmap)
+        bn_, nt = pick_bn(cin8)
+        rows = bn_ * nt
+        # K position (tap, gradient channel co) -> flat ((t*Cout + co)*Cin), row n -> + ci
+        kmap, Kp = self._kmap(range(16), g_chan, self.cout * self.cin, self.cin)
+        nmap = torch.tensor(list(self.in_chanmap) + [-1] * (rows - cin8), dtype=torch.int32, device=self.device)
+        self.tr_dgrad = dict(kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap,
+                             w=torch.zeros(rows, Kp, dtype=torch.bfloat16, device=self.device))
+
 
 # ================================================================================================ graph builder
 class Builder(object):
@@ -840,8 +883,9 @@ class Builder(object):
         return self.hold(torch.zeros(*shape, dtype=torch.float32, device=self.device))
 
     def conv(self, layer, srcs, out=None, post_add=None, addf=None, outf=None, outf_ch=0, mode=0, want_bf16=True, name=None,
-             plan=None, out_rows=None):
-        """y = act(conv(concat(srcs)) + bias [+ addf]) [+ post_add]; returns the output Act."""
+             plan=None, out_rows=None, grad_out=None):
+        """y = act(conv(concat(srcs)) + bias [+ addf]) [+ post_add]; returns the output Act.  grad_out: the Act whose gradient is this
+        layer's output gradient (an fp32-only output, want_bf16=False, that feeds the same value as that Act: PWC-Net's flow heads)."""
         plan = plan or self.fwd
         if MATERIALIZE_MISALIGNED_CONCAT and len(srcs) > 1 and layer.tag and layer.stride == 1 and \
                 any(s.C8 % 64 for s in srcs[:-1]):
@@ -904,13 +948,21 @@ class Builder(object):
         plan.keep += [srcs, out, outf, addf, post_add, layer]
         plan.add('cis_conv_igemm', C.byref(d), flops=2.0 * N * OH * OW * layer.k * layer.k * layer.cin * layer.cout, lane=self.lane)
         if layer.tag:
-            self.tape.append(lambda bp, m, L=layer, S=list(srcs), O=out, P=post_add: self._conv_bwd(bp, m, L, S, O, P))
+            # call index: a layer run more than once in one graph (the siamese PWC-Net feature pyramid) gets one range of weight-gradient
+            # slices per call, summed by the one un-pack of plan_finalize
+            call = layer.ncalls = getattr(layer, 'ncalls', 0) + 1
+            self.tape.append(lambda bp, m, L=layer, S=list(srcs), O=out, P=post_add, K=call - 1, GO=grad_out:
+                             self._conv_bwd(bp, m, L, S, O, P, K, GO))
         return out
 
-    def _conv_bwd(self, bp, mode, layer, srcs, out, post_add):
-        if out is None or mode not in out.dep or not out.grad_written.get(mode):
+    def _conv_bwd(self, bp, mode, layer, srcs, out, post_add, call=0, grad_out=None):
+        gout = grad_out if grad_out is not None else out
+        if gout is None or mode not in gout.dep or not gout.grad_written.get(mode):
             return
-        G = out.get_grad()
+        G = gout.get_grad()
+        if out is None:
+            out = gout            # fp32-only output: no activation (asserted below), the gradient Act gives the row grid
+            assert layer.act == ACT_NONE and post_add is None, layer.name
         nb = out.rows(mode)
         npix = nb * out.H * out.W
         if post_add is not None and mode in post_add.dep:
@@ -918,19 +970,22 @@ class Builder(object):
             bp.add('cis_add_slice', pg.ptr, pg.pitch, pg.c_off, G.ptr, G.pitch, G.c_off, npix, G.C8 // 8, 1,
                    1 if post_add.grad_written.get(mode) else 0)
             post_add.grad_written[mode] = True
+        ncalls = getattr(layer, 'ncalls', 1)
         if layer.tag == mode:
             chunks = -(-layer.cout // 8)
             ppb = (256 // chunks) * COLSUM_PIX                      # pixels per colsum block (P pixel lanes x COLSUM_PIX pixels each)
             if not hasattr(layer, 'col_blocks'):
                 layer.col_blocks = {}
-            layer.col_blocks[mode] = max(1, min(592, -(-npix // ppb)))
+            nblk = max(1, min(592, -(-npix // ppb)))
+            layer.col_blocks[mode] = nblk * ncalls                 # call k owns the partial blocks [k * nblk, (k + 1) * nblk)
             if getattr(layer, 'colpart', None) is None:
-                layer.colpart = torch.empty(592 * layer.cout, dtype=torch.float32, device=self.device)
+                layer.colpart = torch.empty(592 * ncalls * layer.cout, dtype=torch.float32, device=self.device)
+            colpart = layer.colpart.data_ptr() + 4 * call * nblk * layer.cout
         res = (post_add.ptr, post_add.pitch, post_add.c_off) if post_add is not None else (None, 0, 0)
         fused_colsum = bool(DACT_COLSUM and layer.act != ACT_NONE and layer.tag == mode)
         if fused_colsum:      # activation derivative + bias-gradient partials in one pass over the gradient
             bp.add('cis_dact_colsum', G.ptr, G.pitch, G.c_off, out.ptr, out.pitch, out.c_off, res[0], res[1], res[2], npix, layer.cout,
-                   layer.act, layer.alpha, layer.colpart.data_ptr(), layer.col_blocks[mode])
+                   layer.act, layer.alpha, colpart, nblk)
         elif layer.act != ACT_NONE:
             bp.add('cis_dact_mul', G.ptr, G.pitch, G.c_off, out.ptr, out.pitch, out.c_off, res[0], res[1], res[2], npix, G.C8 // 8,
                    layer.act, layer.alpha)
@@ -959,35 +1014,46 @@ class Builder(object):
                 else:
                     layer.wg_K_pad, layer.wg_kmap = layer.K_pad, layer.fwd_kmap
                 layer.dwp, layer.wg_splits = None, {}
-            w = CisWgrad()
-            w.N, w.H, w.W, w.OH, w.OW, w.sh, w.sw = nb, H, W, out.H, out.W, layer.stride, layer.stride
-            _fill_taps(w, taps)
-            _fill_srcs(w, srcs)
-            w.g, w.g_pitch, w.g_coff, w.g_chunks = G.ptr, G.pitch, G.c_off, G.C8 // 8
-            w.Cout, w.K_pad = layer.cout, layer.wg_K_pad
-            w.tma = 2 if layer.wg_halo else (1 if layer.wg_tma else 0)
-            nkb = (nb * (-(-out.H // 8)) * (-(-out.W // 8))) if w.tma else -(-npix // 64)
-            ntile = -(-layer.wg_K_pad // 128)
-            if w.tma == 2:      # grid.x = 64-channel chunks of the input, grid.z = tap-pair groups (x 64-channel halves of Cout)
-                w.nh, w.nwg, gz = wgrad_halo_tiling(len(taps), layer.cout)
-                if WGRAD_HALO_NWG < 2:
-                    gz = 2 if layer.cout > 64 else 1
-                ntile = (-(-len(layer.in_chanmap) // 64)) * gz
-            splits = max(1, min(nkb // 8 if nkb >= 8 else 1, max(1, (WGRAD_CTAS_PER_SM * NUM_SMS) // ntile)))
-            if WGRAD_MAX_SLICE_MB > 0:      # the private slices are written once and read once more by the un-pack job: bound their volume
-                splits = max(1, min(splits, int(WGRAD_MAX_SLICE_MB * 1e6 / (layer.cout * layer.wg_K_pad * 4.0))))
-            splits = -(-nkb // (-(-nkb // splits)))        # every split owns >= 1 reduction block (its slice is written, not accumulated)
-            w.splits = splits
-            layer.wg_splits[mode] = splits
-            if layer.dwp is None or layer.dwp.numel() < splits * layer.cout * layer.wg_K_pad:
-                assert not getattr(layer, 'wgrad_modes', None), 'slice buffer must be sized by the first (largest) mode'
-                layer.dwp = torch.empty(max(layer.wg_splits.values()) * layer.cout * layer.wg_K_pad, dtype=torch.float32, device=self.device)
-            w.dwp = layer.dwp.data_ptr()
-            bp.keep.append(w)
-            bp.add('cis_conv_wgrad', C.byref(w), flops=2.0 * npix * layer.k * layer.k * layer.cin * layer.cout, lane=1)
+                layer.dwp_hi, layer.wg_splits_hi = {}, {}   # Cout > 128: output channels [g0, g0 + 128), g0 >= 128, in launches of their own
+            for g0 in range(0, layer.cout, 128):             # cis_conv_wgrad takes at most 128 output channels
+                gc = min(128, layer.cout - g0)
+                w = CisWgrad()
+                w.N, w.H, w.W, w.OH, w.OW, w.sh, w.sw = nb, H, W, out.H, out.W, layer.stride, layer.stride
+                _fill_taps(w, taps)
+                _fill_srcs(w, srcs)
+                w.g, w.g_pitch, w.g_coff, w.g_chunks = G.ptr, G.pitch, G.c_off + g0, G.C8 // 8 - g0 // 8
+                w.Cout, w.K_pad = gc, layer.wg_K_pad
+                w.tma = 2 if layer.wg_halo else (1 if layer.wg_tma else 0)
+                nkb = (nb * (-(-out.H // 8)) * (-(-out.W // 8))) if w.tma else -(-npix // 64)
+                ntile = -(-layer.wg_K_pad // 128)
+                if w.tma == 2:      # grid.x = 64-channel chunks of the input, grid.z = tap-pair groups (x 64-channel halves of Cout)
+                    w.nh, w.nwg, gz = wgrad_halo_tiling(len(taps), gc)
+                    if WGRAD_HALO_NWG < 2:
+                        gz = 2 if gc > 64 else 1
+                    ntile = (-(-len(layer.in_chanmap) // 64)) * gz
+                splits = wgrad_splits(nkb, ntile, gc, layer.wg_K_pad)
+                w.splits = splits
+                # call k of the layer owns the slices [k * splits, (k + 1) * splits) (every call has the same shape, so the same splits)
+                size = splits * ncalls * gc * layer.wg_K_pad
+                if g0 == 0:
+                    assert ncalls == 1 or layer.wg_splits.get(mode) in (None, splits * ncalls), layer.name
+                    layer.wg_splits[mode] = splits * ncalls
+                    if layer.dwp is None or layer.dwp.numel() < size:
+                        assert not getattr(layer, 'wgrad_modes', None), 'slice buffer must be sized by the first (largest) mode'
+                        layer.dwp = torch.empty(max(layer.wg_splits.values()) * gc * layer.wg_K_pad, dtype=torch.float32, device=self.device)
+                    buf = layer.dwp
+                else:
+                    layer.wg_splits_hi[(mode, g0)] = splits * ncalls
+                    if g0 not in layer.dwp_hi or layer.dwp_hi[g0].numel() < size:
+                        assert not getattr(layer, 'wgrad_modes', None), 'slice buffer must be sized by the first (largest) mode'
+                        layer.dwp_hi[g0] = torch.empty(size, dtype=torch.float32, device=self.device)
+                    buf = layer.dwp_hi[g0]
+                w.dwp = buf.data_ptr() + 4 * call * splits * gc * layer.wg_K_pad
+                bp.keep.append(w)
+                bp.add('cis_conv_wgrad', C.byref(w), flops=2.0 * npix * layer.k * layer.k * layer.cin * gc, lane=1)
             layer.wgrad_modes = getattr(layer, 'wgrad_modes', set()) | {mode}
             if not fused_colsum:
-                bp.add('cis_colsum', G.ptr, G.pitch, G.c_off, npix, layer.cout, layer.colpart.data_ptr(), layer.col_blocks[mode], lane=1)
+                bp.add('cis_colsum', G.ptr, G.pitch, G.c_off, npix, layer.cout, colpart, nblk, lane=1)
         need = [s for s in srcs if mode in s.dep]
         if not need:
             return
@@ -1111,7 +1177,7 @@ class Builder(object):
         """Materialised concat (only where the virtual concat is not 64-channel aligned, so the TMA operand paths apply)."""
         return self.resize_concat(srcs, name=name)
 
-    # ---- transposed conv (PWC-Net up_flow / up_feat), forward only
+    # ---- transposed conv (PWC-Net up_flow / up_feat)
     def conv_transpose(self, layer, src, out=None, outf=None, plan=None, name=None):
         plan = plan or self.fwd
         if layer.fwd_pack is None:
@@ -1119,6 +1185,9 @@ class Builder(object):
         N, H, W = src.N, src.H, src.W
         if out is None:
             out = self.new_act(N, 2 * H, 2 * W, layer.cout, name=name or layer.name, dep=src.dep)
+        if layer.tag:
+            out.dep = out.dep | src.dep | {layer.tag}
+            self.tape.append(lambda bp, m, L=layer, S=src, O=out: self._conv_transpose_bwd(bp, m, L, S, O))
         emitted = []
         for pk in layer.tr_packs:
             d = CisConv()
@@ -1150,6 +1219,61 @@ class Builder(object):
                 plan.keep.append(d)
                 plan.add('cis_conv_igemm', C.byref(d), flops=fl)
         return out
+
+    def _conv_transpose_bwd(self, bp, mode, layer, src, out):
+        """Backward of conv_transpose.  Weights: the output gradient is split into its four output-parity planes, and parity (a, b) is a
+        stride-1 weight gradient over the taps setup_transposed gives it (gather kernel, private slices per parity, one un-pack job each);
+        bias: column sums over the four planes.  Data: a 4x4 stride-2 forward conv of the output gradient (setup_transposed_dgrad)."""
+        if mode not in out.dep or not out.grad_written.get(mode):
+            return
+        G = out.get_grad()
+        N, h, w = src.N, src.H, src.W
+        npix = N * h * w
+        if layer.tag == mode:
+            if getattr(layer, 'tr_planes', None) is None:
+                layer.tr_planes = torch.zeros(4, N, h, w, 8, dtype=torch.bfloat16, device=self.device)
+                layer.colpart = torch.empty(592 * layer.cout, dtype=torch.float32, device=self.device)
+                layer.col_blocks = {}
+            planes = layer.tr_planes
+            bp.add('cis_parity_split_bf16', G.ptr, G.pitch, G.c_off, N, h, w, layer.cout, planes.data_ptr(), 8)
+            layer.col_blocks[mode] = max(1, min(592, -(-4 * npix // (256 * COLSUM_PIX))))
+            bp.add('cis_colsum', planes.data_ptr(), 8, 0, 4 * npix, layer.cout, layer.colpart.data_ptr(), layer.col_blocks[mode], lane=1)
+            for q, pk in enumerate(layer.tr_packs):
+                wg = CisWgrad()
+                wg.N, wg.H, wg.W, wg.OH, wg.OW, wg.sh, wg.sw = N, h, w, h, w, 1, 1
+                _fill_taps(wg, pk['taps'])
+                _fill_srcs(wg, [src])
+                wg.g, wg.g_pitch, wg.g_coff, wg.g_chunks = planes[q].data_ptr(), 8, 0, 1
+                wg.Cout, wg.K_pad, wg.tma = layer.cout, pk['K_pad'], 0
+                nkb = -(-npix // 64)
+                wg.splits = wgrad_splits(nkb, -(-pk['K_pad'] // 128), layer.cout, pk['K_pad'])
+                pk.setdefault('wg_splits', {})[mode] = wg.splits
+                if pk.get('dwp') is None or pk['dwp'].numel() < wg.splits * layer.cout * pk['K_pad']:
+                    pk['dwp'] = torch.empty(wg.splits * layer.cout * pk['K_pad'], dtype=torch.float32, device=self.device)
+                wg.dwp = pk['dwp'].data_ptr()
+                bp.keep.append(wg)
+                bp.add('cis_conv_wgrad', C.byref(wg), flops=2.0 * npix * len(pk['taps']) * layer.cin * layer.cout, lane=1)
+        if mode not in src.dep:
+            return
+        g_pos = G.c_off % 8                  # the gradient's channels inside its 8-channel chunk (up_feat sits behind up_flow)
+        layer.setup_transposed_dgrad(g_pos)
+        dg = layer.tr_dgrad
+        tgt = src.get_grad()
+        d = CisConv()
+        d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = N, 2 * h, 2 * w, h, w, 2, 2
+        _fill_taps(d, [(r - 1, c - 1) for r in range(4) for c in range(4)])      # TF 'SAME' k4 s2: one row / column of padding in front
+        d.nsrc = 1
+        d.src[0] = CisSrc(G.ptr, G.pitch, G.c_off - g_pos, 1, 0)
+        d.wpack, d.K_pad, d.BN, d.n_tiles = dg['w'].data_ptr(), dg['K_pad'], dg['BN'], dg['n_tiles']
+        d.bias, d.act = None, ACT_NONE
+        d.DH, d.DW, d.osh, d.osw, d.oa, d.ob = h, w, 1, 1, 0, 0
+        d.out, d.out_pitch, d.out_coff, d.out_ch = tgt.ptr, tgt.pitch, tgt.c_off, tgt.C8
+        if src.grad_written.get(mode):
+            d.add_pre, d.add_pre_pitch, d.add_pre_coff = tgt.ptr, tgt.pitch, tgt.c_off
+        setup_splitk(d, self.device, bp.keep)
+        bp.keep.append(d)
+        bp.add('cis_conv_igemm', C.byref(d), flops=2.0 * npix * 16 * layer.cin * layer.cout)
+        src.grad_written[mode] = True
 
     # ---- resampling ops
     def resize_bilinear(self, src, OH, OW, name=''):

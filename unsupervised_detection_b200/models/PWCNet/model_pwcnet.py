@@ -1,13 +1,21 @@
-"""Frozen PWC-Net 'lg-6-2' (dense + residual/context) forward on the sm_90a kernels.
+"""PWC-Net 'lg-6-2' (dense + residual/context) on the sm_90a kernels.
 
 Mirrors models/PWCNet/model_pwcnet.py of the reference: extract_features :149-168, warp :173-245 (core_warp.py:153-202),
 corr :291-340 (core_costvol.py:20-40), predict_flow :476-506, refine_flow :559-576, deconv :283-286, nn :581-649,
-predict_from_img_pairs :61-76.  Forward only: the optimiser var_lists exclude 'pwcnet' (adversarial_learner.py:211-234).
+predict_from_img_pairs :61-76.  The training step keeps PWC-Net frozen, as the reference does (its optimiser var_lists exclude 'pwcnet',
+adversarial_learner.py:211-234): the step graph builds ModelPWCNet(trainable=False), forward only.  trainable=True tags every layer 'P'
+and records the backward on the builder's tape (the function-level predict_from_img_pairs, models/functional.py): gradients reach
+every pwcnet/* parameter and both images.
 
 Buffer layout: each pyramid level owns ONE NHWC bf16 buffer that holds the whole DenseNet concat
 [act4 32|act3 64|act2 96|act1 128|act0 128|corr 81(+7)|c1 C|up_flow 2,up_feat 2(+4)]; every conv writes its output straight
 into its channel slice (tf.concat never materialises), the fused warp+cost-volume kernel writes the 81 correlation
 channels, and the 4x4 stride-2 transposed convs of the level above write up_flow/up_feat into the tail.
+
+Backward (trainable): level buffer E[l] has a gradient buffer dE[l] of the same layout, zeroed once per backward.  Every view of E[l] has
+the same slice of dE[l] as its gradient and counts as written from the start, so every data gradient into it accumulates; in reverse tape
+order all consumers of an activation run before its producer's backward.  The two fp32 flow heads (predict_flow/flow{l} and the
+dc_conv{l}7 residual, flow = dc7(x) + flow_raw) both take the gradient of the level's bf16 flow as their output gradient.
 """
 import torch
 
@@ -24,12 +32,14 @@ C1_OFF = CORR_OFF + CORR_PAD
 
 
 class ModelPWCNet(object):
-    def __init__(self, store, name='pwcnet'):
+    def __init__(self, store, name='pwcnet', trainable=False):
         self.name = name
+        self.trainable = trainable
         self.L = {}
+        tag = 'P' if trainable else ''
         # lvl: pyramid level of the layer's OUTPUT map (selects the experimental narrow n-tiles on the coarse levels, engine.small_bn_cap)
         mk = lambda n, k, ci, co, s=1, d=1, act=ACT_LEAKY, tr=False, lvl=0: self.L.__setitem__(
-            n, ConvLayer(store, '%s/%s' % (name, n), k, ci, co, s, d, act, 0.1, tag='', transposed=tr, bn_cap=small_bn_cap(lvl)))
+            n, ConvLayer(store, '%s/%s' % (name, n), k, ci, co, s, d, act, 0.1, tag=tag, transposed=tr, bn_cap=small_bn_cap(lvl)))
         cin = 3
         for l in range(1, PYR_LVLS + 1):
             f = NUM_CHANN[l]
@@ -81,10 +91,19 @@ class ModelPWCNet(object):
         N, H, W = img1_8.N, img1_8.H, img1_8.W
         P = B.fwd
         hs = [None] + [(-(-H // 2 ** l), -(-W // 2 ** l)) for l in range(1, PYR_LVLS + 1)]
-        E = {}
+        E, dE, written = {}, {}, {}
         for l in range(FLOW_PRED_LVL, PYR_LVLS + 1):
             E[l] = torch.zeros(N, hs[l][0], hs[l][1], self.level_pitch(l), dtype=torch.bfloat16, device=dev)
-        self.level_buf = E
+            if self.trainable:
+                dE[l] = torch.zeros_like(E[l])
+                written[l] = {'P': True}          # shared by every view of E[l]: dE[l] is zeroed, every gradient into it accumulates
+        self.level_buf, self.level_grad = E, dE
+
+        def view(l, C, c_off, chanmap=None, name=''):
+            a = Act(N, hs[l][0], hs[l][1], C, dev, buf=E[l], c_off=c_off, chanmap=chanmap, name=name)
+            if self.trainable:      # written by tagged layers / the cost volume: their gradients flow back through every view
+                a.dep, a.grad_buf, a.grad_written = frozenset({'P'}), dE[l], written[l]
+            return a
         # ---- feature pyramids (shared weights; frame 1 features land inside the level buffers)
         c1, c2 = [None], [None]
         for pyr, x, first in ((c1, img1_8, True), (c2, img2_8, False)):
@@ -95,15 +114,15 @@ class ModelPWCNet(object):
                 x = B.conv(self.L['featpyr/conv%daa' % l], [x])
                 out = None
                 if first and FLOW_PRED_LVL <= l < PYR_LVLS:
-                    out = Act(N, hs[l][0], hs[l][1], f, dev, buf=E[l], c_off=C1_OFF, name='c1_%d' % l)
+                    out = view(l, f, C1_OFF, name='c1_%d' % l)
                 x = B.conv(self.L['featpyr/conv%db' % l], [x], out=out)
                 pyr.append(x)
         B.lane = 0
         P.join()
         self.c1, self.c2 = c1, c2
         B.hold((c1, c2, E))
-        up_flow_f32 = None
-        self.flows = {}
+        up_flow_f32 = up_flow = None
+        self.flows, self.flows_bf = {}, {}
         for l in range(PYR_LVLS, FLOW_PRED_LVL - 1, -1):
             h, w = hs[l]
             pitch = self.level_pitch(l)
@@ -112,29 +131,34 @@ class ModelPWCNet(object):
             scaler = 20.0 / 2 ** l                                              # :616
             P.add('cis_warp_costvol', c1[l].ptr, c1[l].pitch, c1[l].c_off, c2[l].ptr, c2[l].pitch, c2[l].c_off,
                   up_flow_f32.data_ptr() if up_flow_f32 is not None else None, scaler, N, h, w, C, E[l].data_ptr(), pitch, CORR_OFF)
+            if self.trainable:
+                B.tape.append(lambda bp, m, l=l, fl=up_flow_f32, uf=up_flow, s_=scaler: self._costvol_bwd(bp, m, l, fl, uf, s_))
             # ---- DenseNet flow estimator (:476-506)
             for i, co in enumerate(DENSE):
                 start = A_TOTAL if i == 0 else A_OFF[i - 1]
-                src = Act(N, h, w, 0, dev, buf=E[l], c_off=start, chanmap=self._chanmap(l, start), name='x%d_%d' % (l, i))
-                dst = Act(N, h, w, co, dev, buf=E[l], c_off=A_OFF[i], name='act%d_%d' % (l, i))
+                src = view(l, 0, start, chanmap=self._chanmap(l, start), name='x%d_%d' % (l, i))
+                dst = view(l, co, A_OFF[i], name='act%d_%d' % (l, i))
                 B.conv(self.L['predict_flow/conv%d_%d' % (l, i)], [src], out=dst)
-            upfeat = Act(N, h, w, 0, dev, buf=E[l], c_off=0, chanmap=self._chanmap(l, 0), name='upfeat%d' % l)
+            upfeat = view(l, 0, 0, chanmap=self._chanmap(l, 0), name='upfeat%d' % l)
             flow_raw = B.f32(N, h, w, 2)
-            B.conv(self.L['predict_flow/flow%d' % l], [upfeat], outf=flow_raw, want_bf16=False)
+            # bf16 copy of the refined flow (input of up_flow); its gradient is also the gradient of flow_raw
+            flow_bf = B.new_act(N, h, w, 2, name='ctxt/dc_conv%d7' % l)
+            B.conv(self.L['predict_flow/flow%d' % l], [upfeat], outf=flow_raw, want_bf16=False, grad_out=flow_bf)
             # ---- context network (:559-576): flow += ctx(upfeat)
             x = upfeat
             for i in range(1, 7):
                 x = B.conv(self.L['ctxt/dc_conv%d%d' % (l, i)], [x])
             flow = B.f32(N, h, w, 2)
-            flow_bf = B.conv(self.L['ctxt/dc_conv%d7' % l], [x], addf=flow_raw, outf=flow)
-            self.flows[l] = flow
+            B.conv(self.L['ctxt/dc_conv%d7' % l], [x], addf=flow_raw, outf=flow, out=flow_bf)
+            self.flows[l], self.flows_bf[l] = flow, flow_bf
             if l != FLOW_PRED_LVL:
                 # ---- 4x4 stride-2 transposed convs into the next level's buffer tail (:634-635)
                 nh, nw = hs[l - 1]
                 tail = C1_OFF + NUM_CHANN[l - 1]
                 up_flow_f32 = B.f32(N, nh, nw, 2)
-                o1 = Act(N, nh, nw, 2, dev, buf=E[l - 1], c_off=tail, chanmap=[0, 1], name='up_flow%d' % l)
-                o2 = Act(N, nh, nw, 2, dev, buf=E[l - 1], c_off=tail + 2, chanmap=[0, 1], name='up_feat%d' % l)
+                o1 = view(l - 1, 2, tail, chanmap=[0, 1], name='up_flow%d' % l)
+                o2 = view(l - 1, 2, tail + 2, chanmap=[0, 1], name='up_feat%d' % l)
+                up_flow = o1
                 assert (nh, nw) == (2 * h, 2 * w), 'PWC-Net needs H, W divisible by 64'
                 B.conv_transpose(self.L['upsample/up_flow%d' % l], flow_bf, out=o1, outf=up_flow_f32)
                 B.conv_transpose(self.L['upsample/up_feat%d' % l], upfeat, out=o2)
@@ -142,4 +166,32 @@ class ModelPWCNet(object):
                 s = 2 ** FLOW_PRED_LVL
                 assert (h * s, w * s) == (H, W)
                 P.add('cis_resize_bilinear_f32', flow.data_ptr(), N, h, w, 2, flow_out.data_ptr(), H, W, float(s))   # :646
+        if self.trainable:
+            # scratch of the warp + cost-volume backward (levels run one after another on one stream): gated correlation gradient,
+            # gradient of the warped features, fp64 scatter sums
+            npix = max(N * hs[l][0] * hs[l][1] for l in range(FLOW_PRED_LVL, PYR_LVLS + 1))
+            npc = max(N * hs[l][0] * hs[l][1] * NUM_CHANN[l] for l in range(FLOW_PRED_LVL, PYR_LVLS))
+            self.cv_scratch = (B.f32(npix * 81), B.f32(npc), B.hold(torch.zeros(npc, dtype=torch.float64, device=dev)))
         return flow_out
+
+    def _costvol_bwd(self, bp, mode, l, up_flow_f32, up_flow, scaler):
+        """Transpose of the level-l warp + cost volume: dc1 and dc2 into the pyramid gradients, d(up_flow) into the up_flow gradient slice
+        of dE[l] (its second consumer after the DenseNet convs), the correlation gradient read from the corr slice of dE[l]."""
+        if mode != 'P':
+            return
+        c1, c2, N = self.c1[l], self.c2[l], self.c1[l].N
+        h, w = c1.H, c1.W
+        g1, g2 = c1.get_grad(), c2.get_grad()
+        acc = (1 if c1.grad_written.get(mode) else 0) | (2 if c2.grad_written.get(mode) else 0)
+        gf = (None, 0, 0)
+        if up_flow_f32 is not None:
+            g = up_flow.get_grad()
+            gf = (g.ptr, g.pitch, g.c_off)
+            acc |= 4 if up_flow.grad_written.get(mode) else 0
+        gs, ws, ds = self.cv_scratch
+        bp.add('cis_warp_costvol_bwd', c1.ptr, c1.pitch, c1.c_off, c2.ptr, c2.pitch, c2.c_off,
+               up_flow_f32.data_ptr() if up_flow_f32 is not None else None, scaler, N, h, w, NUM_CHANN[l],
+               self.level_grad[l].data_ptr(), self.level_pitch(l), CORR_OFF, g1.ptr, g1.pitch, g1.c_off, g2.ptr, g2.pitch, g2.c_off,
+               gf[0], gf[1], gf[2], acc, gs.data_ptr(), ws.data_ptr() if up_flow_f32 is not None else None,
+               ds.data_ptr() if up_flow_f32 is not None else None)
+        c1.grad_written[mode] = c2.grad_written[mode] = True

@@ -8,11 +8,12 @@ from the registry filled by `set_parameters()` (dict name -> tensor, names as in
 PyTorch is used for memory and the small amount of buffer plumbing only; there is no CPU fallback: without the CUDA library (or on CPU
 tensors) the calls raise.
 
-Gradients: generator_net, recover_net, charbonnier_loss, cost_volume and dense_image_warp are torch.autograd Functions (first order
-only) when an input or one of the parameter tensors the call reads requires grad; the parameters then receive gradients under their
-variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain rule, resize transposes) and the
-backward kernels of the three stand-alone ops.  A call that needs no gradient runs exactly the forward-only path.  predict_from_img_pairs
-and train_op are not differentiable.
+Gradients: generator_net, recover_net, ModelPWCNet.predict_from_img_pairs, charbonnier_loss, cost_volume and dense_image_warp are
+torch.autograd Functions (first order only) when an input or one of the parameter tensors the call reads requires grad; the parameters
+then receive gradients under their variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain
+rule, resize transposes, the PWC-Net warp + cost-volume and transposed-conv backward) and the backward kernels of the three stand-alone
+ops.  A call that needs no gradient runs exactly the forward-only path.  train_op is an optimiser update and has nothing to differentiate.
+The training step (step_graph.py) still treats PWC-Net as frozen, as the reference does.
 
 The sub-graphs reuse the builders that the step graph is made of; tests/test_functional_api_gpu.py and
 tests/test_functional_grad_gpu.py check them against the oracle on the GPU, tests/test_functional_api_cpu.py and
@@ -53,9 +54,12 @@ def _scope_name(scope, default):
 
 class _NetRunner(object):
     """One cached static plan: parameter store + packed operands + input/output buffers for a fixed shape.  `bwd` is the backward plan
-    (built by ensure_backward for the runners of gradient-carrying calls only); `runs` counts forward runs."""
+    (built by ensure_backward for the runners of gradient-carrying calls only); `runs` counts forward runs.  SEED names the fp32 buffer the
+    backward plan reads the output gradient from, INPUT_GRADS the fp32 buffers it leaves the input gradients in (in argument order)."""
 
     MODE = None
+    SEED = None
+    INPUT_GRADS = ()
 
     def __init__(self, device):
         self.device = device
@@ -117,7 +121,7 @@ class _NetRunner(object):
 
 
 class _GeneratorRunner(_NetRunner):
-    MODE = 'G'
+    MODE, SEED, INPUT_GRADS = 'G', 'dmask', ('dimage', 'dflow')
 
     def __init__(self, B, H, W, device, scope):
         _NetRunner.__init__(self, device)
@@ -166,7 +170,7 @@ class _GeneratorRunner(_NetRunner):
 
 
 class _RecoverRunner(_NetRunner):
-    MODE = 'R'
+    MODE, SEED, INPUT_GRADS = 'R', 'dpred', ('dimage', 'dflow', 'dmask')
 
     def __init__(self, B, H, W, device, scope, f):
         _NetRunner.__init__(self, device)
@@ -223,26 +227,59 @@ class _RecoverRunner(_NetRunner):
 
 
 class _PWCRunner(_NetRunner):
-    def __init__(self, B, H, W, device, name):
+    """trainable=False: the forward-only plan of calls without gradients.  trainable=True: layers tagged 'P', backward recorded."""
+    MODE, SEED, INPUT_GRADS = 'P', 'dflow_out', ('dimg1', 'dimg2')
+
+    def __init__(self, B, H, W, device, name, trainable=False):
         from .PWCNet.model_pwcnet import ModelPWCNet
         _NetRunner.__init__(self, device)
-        self.net = ModelPWCNet(self.store, name)
+        self.net = ModelPWCNet(self.store, name, trainable=trainable)
         self.store.finalize(False)
         f32 = self.bld.f32
+        self.B, self.H, self.W = B, H, W
         self.img1, self.img2, self.flow = f32(B, H, W, 3), f32(B, H, W, 3), f32(B, H, W, 2)
-        i1, i2 = self.bld.new_act(B, H, W, 3, name='img1_8'), self.bld.new_act(B, H, W, 3, name='img2_8')
+        # dependency 'P': a backward plan emits conv1a's data gradients (both frames) into the two image Acts
+        dep = {'P'} if trainable else frozenset()
+        self.i1, self.i2 = self.bld.new_act(B, H, W, 3, name='img1_8', dep=dep), self.bld.new_act(B, H, W, 3, name='img2_8', dep=dep)
         P = self.bld.fwd
-        P.add('cis_pack_f32_to_bf16', self.img1.data_ptr(), B * H * W, 3, 0.5, i1.ptr, 8, 0)      # adapt_x: images arrive in [-0.5, 0.5]
-        P.add('cis_pack_f32_to_bf16', self.img2.data_ptr(), B * H * W, 3, 0.5, i2.ptr, 8, 0)
-        self.net.build(self.bld, i1, i2, self.flow)
+        P.add('cis_pack_f32_to_bf16', self.img1.data_ptr(), B * H * W, 3, 0.5, self.i1.ptr, 8, 0)      # adapt_x: images arrive in [-0.5, 0.5]
+        P.add('cis_pack_f32_to_bf16', self.img2.data_ptr(), B * H * W, 3, 0.5, self.i2.ptr, 8, 0)
+        self.net.build(self.bld, self.i1, self.i2, self.flow)
         self.finish(self.net.all_layers())
 
-    def __call__(self, img1, img2, params):
-        self.load(params)
+    def run(self, img1, img2):
         self.img1.copy_(img1)
         self.img2.copy_(img2)
         self.bld.fwd.run()
+        self.runs += 1
         return self.flow.clone()
+
+    def __call__(self, img1, img2, params):
+        self.load(params)
+        return self.run(img1, img2)
+
+    def _plan_seed(self):
+        from .PWCNet.model_pwcnet import FLOW_PRED_LVL
+        f32 = self.bld.f32
+        B, H, W = self.B, self.H, self.W
+        self.dflow_out, self.dimg1, self.dimg2 = f32(B, H, W, 2), f32(B, H, W, 3), f32(B, H, W, 3)
+        seed = Plan('seed_P')
+        for g in self.net.level_grad.values():      # the DenseNet level gradients accumulate from zero
+            seed.zero(g)
+        fb = self.net.flows_bf[FLOW_PRED_LVL]
+        fg, s = fb.get_grad(), 2 ** FLOW_PRED_LVL
+        # transpose of the final legacy-bilinear x4 and its x4 scale (model_pwcnet.py:642-647) into the level-2 flow gradient
+        seed.add('cis_resize_f32_bwd_to_bf16_scaled', self.dflow_out.data_ptr(), B, H, W, 2, H // s, W // s, fg.ptr, fg.pitch, float(s))
+        return seed, [fb]
+
+    def _plan_inputs(self):
+        assert self.i1.grad_written.get('P') and self.i2.grad_written.get('P'), 'PWC-Net backward did not reach its inputs'
+        npix = self.B * self.H * self.W
+        P = Plan('inputs_P')
+        for a, d in ((self.i1, self.dimg1), (self.i2, self.dimg2)):      # image + 0.5 (adapt_x): unit derivative
+            g = a.get_grad()
+            P.add('cis_cast_bf16_to_f32', g.ptr, npix, g.pitch, 0, 3, d.data_ptr())
+        return P
 
 
 def _runner(kind, key, make):
@@ -306,7 +343,8 @@ def _needs_grad(tensors):
 
 
 class _NetFn(torch.autograd.Function):
-    """generator_net / recover_net with their parameters as explicit inputs: apply(lease, names, n_in, *inputs, *parameters)."""
+    """generator_net / recover_net / predict_from_img_pairs with their parameters as explicit inputs:
+    apply(lease, names, n_in, *inputs, *parameters)."""
 
     @staticmethod
     def forward(ctx, lease, names, n_in, *args):
@@ -322,11 +360,9 @@ class _NetFn(torch.autograd.Function):
     @once_differentiable
     def backward(ctx, gout):
         r = ctx.lease.take()
-        seed = r.dmask if r.MODE == 'G' else r.dpred
-        seed.copy_(gout)
+        getattr(r, r.SEED).copy_(gout)
         r.bwd.run()
-        ins = [r.dimage, r.dflow] if r.MODE == 'G' else [r.dimage, r.dflow, r.dmask]
-        grads = [g.clone() for g in ins] + r.param_grads()
+        grads = [getattr(r, n).clone() for n in r.INPUT_GRADS] + r.param_grads()
         ctx.lease.release()
         out = []
         for need, g, (dev, dt, shape) in zip(ctx.needs_input_grad[3:], grads, ctx.like):
@@ -378,14 +414,24 @@ def recover_net(img1, flow_masked, mask, scope='FlownetS', reuse=None, f=0.25, t
 
 def predict_from_img_pairs(img1, img2, name='pwcnet', params=None):
     """ModelPWCNet.predict_from_img_pairs (model_pwcnet.py:39-76): forward flow img1 -> img2, [B,H,W,2] in pixels of the input size
-    (H, W multiples of 64, 384x640 in the reference's pipeline).  Forward only: PWC-Net is frozen in the reference
-    (adversarial_learner.py:211-234), so the result carries no gradient."""
+    (H, W multiples of 64, 384x640 in the reference's pipeline).  Differentiable w.r.t. img1, img2 and every '<name>/...' parameter
+    (kernels HWIO, transposed-conv kernels [kh,kw,Cout,Cin]; bf16 activations, fp32 gradients), for fine-tuning the flow network or
+    gradients with respect to the frames.  The training step keeps PWC-Net frozen, as the reference does (adversarial_learner.py:211-234)."""
     _check_cuda(img1, img2)
     B, H, W, _ = img1.shape
     if H % 64 or W % 64:
         raise ValueError('PWC-Net needs input sizes that are multiples of 64 (6 pyramid levels); got %dx%d' % (H, W))
-    r = _runner('pwc', (B, H, W, str(img1.device), name), lambda: _PWCRunner(B, H, W, img1.device, name))
-    return r(img1, img2, params)
+    key = (B, H, W, str(img1.device), name)
+    r = _runner('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name))
+    names, pvals = _param_inputs(r, params)
+    if not _needs_grad([img1, img2] + pvals):
+        return r(img1, img2, params)
+    lease = _lease('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name, trainable=True))
+    try:
+        return _NetFn.apply(lease, names, 2, img1, img2, *pvals)
+    except BaseException:
+        lease.release()
+        raise
 
 
 # -------------------------------------------------------------------------------------------------------------------- losses
