@@ -249,6 +249,11 @@ int cis_resize_nn_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t
 int cis_warp_costvol(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* c2, int32_t c2_pitch, int32_t c2_coff,
                      const float* flow, float flow_scale, int32_t B, int32_t h, int32_t w, int32_t C, void* out, int32_t out_pitch,
                      int32_t out_coff, cis_stream_t stream);
+/* the same for search range 1 <= search_range <= 4 (model_pwcnet.py option 'search_range'; cis_warp_costvol is search_range = 4):
+ * (2r+1)^2 channels out[b,y,x,(2r+1)*dy+dx], displacement (dy-r, dx-r).  CIS_ERR_BAD_ARG outside 1..4. */
+int cis_warp_costvol_r(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* c2, int32_t c2_pitch, int32_t c2_coff,
+                       const float* flow, float flow_scale, int32_t B, int32_t h, int32_t w, int32_t C, void* out, int32_t out_pitch,
+                       int32_t out_coff, int32_t search_range, cis_stream_t stream);
 /* standalone dense_image_warp (core_warp.py:153) on a bf16 slice -> bf16, for parity tests of the gather */
 int cis_dense_image_warp(const void* img, int32_t pitch, int32_t coff, const float* flow, float flow_scale, int32_t B, int32_t h,
                          int32_t w, int32_t C, void* out, int32_t out_pitch, cis_stream_t stream);
@@ -329,6 +334,10 @@ int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const
 int cis_cost_volume_bwd(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* warp, int32_t warp_pitch, int32_t warp_coff,
                         const float* dout, int32_t B, int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp,
                         cis_stream_t stream);
+/* the same for search range 1..4: dout and gscratch are fp32 [B,h,w,(2r+1)^2] (CIS_ERR_BAD_ARG outside 1..4) */
+int cis_cost_volume_bwd_r(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* warp, int32_t warp_pitch, int32_t warp_coff,
+                          const float* dout, int32_t B, int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp,
+                          int32_t search_range, cis_stream_t stream);
 
 /* ---- PWC-Net backward (function-level predict_from_img_pairs; the step graph keeps PWC-Net frozen) ---- */
 /* Transpose of cis_warp_costvol, same feature operands (c1, c2, flow, flow_scale; flow = NULL at level 6).  dcorr = bf16 gradient of the 81
@@ -342,6 +351,12 @@ int cis_warp_costvol_bwd(const void* c1, int32_t c1_pitch, int32_t c1_coff, cons
                          void* dc1, int32_t dc1_pitch, int32_t dc1_coff, void* dc2, int32_t dc2_pitch, int32_t dc2_coff, void* dflow,
                          int32_t dflow_pitch, int32_t dflow_coff, int32_t accumulate, float* gscratch, float* wscratch, double* dscratch,
                          cis_stream_t stream);
+/* the same for search range 1..4: dcorr holds (2r+1)^2 channels and gscratch is fp32 [B,h,w,(2r+1)^2] (CIS_ERR_BAD_ARG outside 1..4) */
+int cis_warp_costvol_bwd_r(const void* c1, int32_t c1_pitch, int32_t c1_coff, const void* c2, int32_t c2_pitch, int32_t c2_coff,
+                           const float* flow, float flow_scale, int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr,
+                           int32_t dc_pitch, int32_t dc_coff, void* dc1, int32_t dc1_pitch, int32_t dc1_coff, void* dc2, int32_t dc2_pitch,
+                           int32_t dc2_coff, void* dflow, int32_t dflow_pitch, int32_t dflow_coff, int32_t accumulate, float* gscratch,
+                           float* wscratch, double* dscratch, int32_t search_range, cis_stream_t stream);
 /* dst plane a*2+b [N,H,W,d_pitch] (one zero-padded 8-channel chunk per pixel) = src(n, 2y+a, 2x+b, s_coff .. s_coff+C), C <= 8, s_coff any:
  * the output-parity gradient operands of the weight gradient of conv2d_transpose(k4, s2) */
 int cis_parity_split_bf16(const void* src, int32_t s_pitch, int32_t s_coff, int32_t N, int32_t H, int32_t W, int32_t C, void* dst,

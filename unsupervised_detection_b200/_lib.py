@@ -111,6 +111,11 @@ _PROTOS = {
     'cis_warp_costvol_bwd': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32,
                              _p, _i32, _i32, _i32, _p, _p, _p],
     'cis_parity_split_bf16': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32],
+    # search-range variants: the arguments of the three entry points above plus search_range (1..4)
+    'cis_warp_costvol_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32],
+    'cis_cost_volume_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _i32],
+    'cis_warp_costvol_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32,
+                               _p, _i32, _i32, _i32, _p, _p, _p, _i32],
 }
 EXPORTS = sorted(list(_PROTOS) + ['cis_last_error', 'cis_version', 'cis_set_persist_mode', 'cis_crc32c', 'cis_host_resize_bilinear_legacy',
                                   'cis_host_bgr8_to_rgb_resized'])

@@ -792,28 +792,41 @@ __global__ void dense_image_warp_kernel(const bf16* __restrict__ img, int pitch,
   *reinterpret_cast<uint4*>(out + pix * op + c) = pack8(o);
 }
 
-static constexpr int kCvTH = 8, kCvTW = 16, kCvR = 4;
-static constexpr int kCvHH = kCvTH + 2 * kCvR, kCvHW = kCvTW + 2 * kCvR;  // 16 x 24 halo
+// Search range R (core_costvol.py:20-40, model_pwcnet.py options 'search_range'), 1 <= R <= 4: (2R+1)^2 displacements over an 8x16 pixel
+// tile and its (8+2R)x(16+2R) halo.  R = 4 is the upper bound: the backward's staging takes cv_bwd_smem(4) = 193,536 B, R = 5 would need
+// 258,688 B, more than a block's 227 KB.
+static constexpr int kCvTH = 8, kCvTW = 16, kCvRMax = 4;
 static constexpr int kCvPitch = 36;                                        // floats per smem pixel row (32 ch + pad)
-static constexpr int kCvSmem = (kCvTH * kCvTW + kCvHH * kCvHW) * kCvPitch * 4;
+__host__ __device__ constexpr int cv_span(int R) { return 2 * R + 1; }
+__host__ __device__ constexpr int cv_ndisp(int R) { return cv_span(R) * cv_span(R); }
+__host__ __device__ constexpr int cv_hh(int R) { return kCvTH + 2 * R; }   // halo rows
+__host__ __device__ constexpr int cv_hw(int R) { return kCvTW + 2 * R; }   // halo columns
+constexpr int cv_smem(int R) { return (kCvTH * kCvTW + cv_hh(R) * cv_hw(R)) * kCvPitch * 4; }
+static_assert(cv_smem(kCvRMax) == (128 + 16 * 24) * 36 * 4, "R = 4 keeps the 16 x 24 halo");
+// R < 4: without a minimum-blocks hint ptxas caps the smaller instances at 48-64 registers and spills; two CTAs per SM (128 registers)
+// removes the spills.  R = 4 keeps the plain __launch_bounds__(256) code (0 = no minimum).
+constexpr int cv_min_blocks(int R) { return R == kCvRMax ? 0 : 2; }
 
-__global__ void __launch_bounds__(256) warp_costvol_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
+template <int R>
+__global__ void __launch_bounds__(256, cv_min_blocks(R)) warp_costvol_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
                                                            int c2o, const float* __restrict__ flow, float fs, int B, int h, int w, int C,
                                                            bf16* __restrict__ out, int op, int oo) {
+  constexpr int S = cv_span(R), ND = cv_ndisp(R), HH = cv_hh(R), HW = cv_hw(R);
+  static_assert(kCvTH * kCvTW * ND * 2 <= HH * HW * kCvPitch * 4, "the bf16 result staging fits the halo buffer");
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float cvs[];
   float* s1 = cvs;                                 // [128][36]
-  float* s2 = cvs + kCvTH * kCvTW * kCvPitch;      // [384][36]
+  float* s2 = cvs + kCvTH * kCvTW * kCvPitch;      // [HH * HW][36]
   const int tid = threadIdx.x;
   const int b = blockIdx.z, y0 = blockIdx.y * kCvTH, x0 = blockIdx.x * kCvTW;
   const int pix = tid & 127, py = pix >> 4, px = pix & 15;
   const int dyb = tid >> 7;  // this thread handles dy = dyb + 2k
-  float acc[5][9];
+  float acc[R + 1][S];
 #pragma unroll
-  for (int k = 0; k < 5; ++k)
+  for (int k = 0; k < R + 1; ++k)
 #pragma unroll
-    for (int d = 0; d < 9; ++d) acc[k][d] = 0.f;
+    for (int d = 0; d < S; ++d) acc[k][d] = 0.f;
   const int Cp = (C + 7) & ~7;
   for (int cc = 0; cc < Cp; cc += 32) {
     const int nck = min(4, (Cp - cc) / 8);  // 8-channel chunks in this pass
@@ -828,9 +841,9 @@ __global__ void __launch_bounds__(256) warp_costvol_kernel(const bf16* __restric
       d[1] = make_float4(v[4], v[5], v[6], v[7]);
     }
     // warped c2 halo (zero outside the image: tf.pad of the warped map, core_costvol.py:27)
-    for (int it = tid; it < kCvHH * kCvHW * 4; it += 256) {
+    for (int it = tid; it < HH * HW * 4; it += 256) {
       const int p = it >> 2, ck = it & 3;
-      const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
+      const int y = y0 - R + p / HW, x = x0 - R + p % HW;
       float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
       if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
         if (flow) {
@@ -846,15 +859,15 @@ __global__ void __launch_bounds__(256) warp_costvol_kernel(const bf16* __restric
     }
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < 5; ++k) {
+    for (int k = 0; k < R + 1; ++k) {
       const int dy = dyb + 2 * k;
-      if (dy < 9) {
-        const float* r2 = s2 + ((py + dy) * kCvHW + px) * kCvPitch;
+      if (dy < S) {
+        const float* r2 = s2 + ((py + dy) * HW + px) * kCvPitch;
         const float* r1 = s1 + pix * kCvPitch;
         for (int c4 = 0; c4 < nck * 2; ++c4) {
           const float4 a = *reinterpret_cast<const float4*>(r1 + c4 * 4);
 #pragma unroll
-          for (int dx = 0; dx < 9; ++dx) {
+          for (int dx = 0; dx < S; ++dx) {
             const float4 q = *reinterpret_cast<const float4*>(r2 + dx * kCvPitch + c4 * 4);
             acc[k][dx] += a.x * q.x + a.y * q.y + a.z * q.z + a.w * q.w;
           }
@@ -863,24 +876,24 @@ __global__ void __launch_bounds__(256) warp_costvol_kernel(const bf16* __restric
     }
     __syncthreads();
   }
-  // mean over the REAL channel count, leaky 0.1, stage [128][81] bf16 in smem, coalesced store
+  // mean over the REAL channel count, leaky 0.1, stage [128][ND] bf16 in smem, coalesced store
   bf16* so = reinterpret_cast<bf16*>(s2);
   const float inv = 1.f / (float)C;
 #pragma unroll
-  for (int k = 0; k < 5; ++k) {
+  for (int k = 0; k < R + 1; ++k) {
     const int dy = dyb + 2 * k;
-    if (dy < 9) {
+    if (dy < S) {
 #pragma unroll
-      for (int dx = 0; dx < 9; ++dx) {
+      for (int dx = 0; dx < S; ++dx) {
         float v = acc[k][dx] * inv;
         v = v > 0.f ? v : 0.1f * v;
-        so[pix * 81 + dy * 9 + dx] = __float2bfloat16(v);
+        so[pix * ND + dy * S + dx] = __float2bfloat16(v);
       }
     }
   }
   __syncthreads();
-  for (int it = tid; it < 128 * 81; it += 256) {
-    const int p = it / 81, ch = it % 81;
+  for (int it = tid; it < 128 * ND; it += 256) {
+    const int p = it / ND, ch = it % ND;
     const int y = y0 + (p >> 4), x = x0 + (p & 15);
     if (y < h && x < w) out[((size_t)(b * h + y) * w + x) * op + oo + ch] = so[it];
   }
@@ -1314,28 +1327,29 @@ __global__ void round_f64_kernel(const double* __restrict__ s, size_t npix, int 
   if (i < npix * C) d.put(i / C, (int)(i % C), (float)s[i]);
 }
 
-// cost_volume (core_costvol.py:20-40) backward, and with flow != NULL the backward of cis_warp_costvol's fused warp.
+// cost_volume (core_costvol.py:20-40) backward, and with flow != NULL the backward of cis_warp_costvol's fused warp, search range R.
 // Pass 1: gs[p][d] = dout[p][d] * leaky0.1'(pre[p][d]) / C, the pre-activation recomputed from the bf16 c1 / c2 slices through the
-// forward's 8x16 tile + 16x24 zero-padded halo staging (c2 warped by fs * flow in the halo, as the forward does).  dout: fp32 or a bf16
-// slice, element d of pixel p at dout[p * dp + doff + d].
-template <typename TD>
-__global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
+// forward's 8x16 tile + (8+2R)x(16+2R) zero-padded halo staging (c2 warped by fs * flow in the halo, as the forward does).  dout: fp32 or
+// a bf16 slice, element d of pixel p at dout[p * dp + doff + d]; gs is [npix][(2R+1)^2].
+template <int R, typename TD>
+__global__ void __launch_bounds__(256, cv_min_blocks(R)) costvol_bwd_gate_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
                                                                int c2o, const float* __restrict__ flow, float fs, const TD* __restrict__ dout,
                                                                int dp, int doff, int B, int h, int w, int C, float* __restrict__ gs) {
+  constexpr int S = cv_span(R), ND = cv_ndisp(R), HH = cv_hh(R), HW = cv_hw(R);
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float cvs[];
   float* s1 = cvs;                                 // [128][36]
-  float* s2 = cvs + kCvTH * kCvTW * kCvPitch;      // [384][36]
+  float* s2 = cvs + kCvTH * kCvTW * kCvPitch;      // [HH * HW][36]
   const int tid = threadIdx.x;
   const int b = blockIdx.z, y0 = blockIdx.y * kCvTH, x0 = blockIdx.x * kCvTW;
   const int pix = tid & 127, py = pix >> 4, px = pix & 15;
   const int dyb = tid >> 7;  // this thread handles dy = dyb + 2k
-  float acc[5][9];
+  float acc[R + 1][S];
 #pragma unroll
-  for (int k = 0; k < 5; ++k)
+  for (int k = 0; k < R + 1; ++k)
 #pragma unroll
-    for (int d = 0; d < 9; ++d) acc[k][d] = 0.f;
+    for (int d = 0; d < S; ++d) acc[k][d] = 0.f;
   const int Cp = (C + 7) & ~7;
   for (int cc = 0; cc < Cp; cc += 32) {
     const int nck = min(4, (Cp - cc) / 8);
@@ -1348,9 +1362,9 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
       d[0] = make_float4(v[0], v[1], v[2], v[3]);
       d[1] = make_float4(v[4], v[5], v[6], v[7]);
     }
-    for (int it = tid; it < kCvHH * kCvHW * 4; it += 256) {
+    for (int it = tid; it < HH * HW * 4; it += 256) {
       const int p = it >> 2, ck = it & 3;
-      const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
+      const int y = y0 - R + p / HW, x = x0 - R + p % HW;
       float v[8] = {0, 0, 0, 0, 0, 0, 0, 0};
       if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
         if (flow) {
@@ -1366,15 +1380,15 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
     }
     __syncthreads();
 #pragma unroll
-    for (int k = 0; k < 5; ++k) {
+    for (int k = 0; k < R + 1; ++k) {
       const int dy = dyb + 2 * k;
-      if (dy < 9) {
-        const float* r2 = s2 + ((py + dy) * kCvHW + px) * kCvPitch;
+      if (dy < S) {
+        const float* r2 = s2 + ((py + dy) * HW + px) * kCvPitch;
         const float* r1 = s1 + pix * kCvPitch;
         for (int c4 = 0; c4 < nck * 2; ++c4) {
           const float4 a = *reinterpret_cast<const float4*>(r1 + c4 * 4);
 #pragma unroll
-          for (int dx = 0; dx < 9; ++dx) {
+          for (int dx = 0; dx < S; ++dx) {
             const float4 q = *reinterpret_cast<const float4*>(r2 + dx * kCvPitch + c4 * 4);
             acc[k][dx] += a.x * q.x + a.y * q.y + a.z * q.z + a.w * q.w;
           }
@@ -1385,47 +1399,49 @@ __global__ void __launch_bounds__(256) costvol_bwd_gate_kernel(const bf16* __res
   }
   const int y = y0 + py, x = x0 + px;
   if (y >= h || x >= w) return;
-  const size_t q = (size_t)(b * h + y) * w + x, o = q * 81;
+  const size_t q = (size_t)(b * h + y) * w + x, o = q * ND;
   const TD* dq = dout + q * dp + doff;
   const float inv = 1.f / (float)C;
 #pragma unroll
-  for (int k = 0; k < 5; ++k) {
+  for (int k = 0; k < R + 1; ++k) {
     const int dy = dyb + 2 * k;
-    if (dy < 9) {
+    if (dy < S) {
 #pragma unroll
-      for (int dx = 0; dx < 9; ++dx) gs[o + dy * 9 + dx] = ldf(dq + dy * 9 + dx) * (acc[k][dx] * inv > 0.f ? inv : 0.1f * inv);
+      for (int dx = 0; dx < S; ++dx) gs[o + dy * S + dx] = ldf(dq + dy * S + dx) * (acc[k][dx] * inv > 0.f ? inv : 0.1f * inv);
     }
   }
 }
-// Pass 2, both sums as gathers over the 81 displacements (fixed order, no atomics):
+// Pass 2, both sums as gathers over the (2R+1)^2 displacements (fixed order, no atomics):
 //   dc1[p]   = sum_d gs[p][d]     * warp[p + d]
 //   dwarp[q] = sum_d gs[q - d][d] * c1[q - d]
-// A CTA owns an 8x16 pixel tile.  It stages gs of its own pixels ([128][81]) and the shifted planes gs[q - d][d] ([81][128], zero where
-// q - d leaves the map: those displacements read the zero padding in the forward) once, then c1 and warp 16x24 halos per 32-channel pass
-// (flow != NULL: the warp halo recomputed from c2 and fs * flow, never stored in HBM).
-static constexpr int kCvBwdSmem = (2 * kCvTH * kCvTW * 81 + 2 * kCvHH * kCvHW * kCvPitch) * 4;
-template <class O1, class O2>
-__global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
+// A CTA owns an 8x16 pixel tile.  It stages gs of its own pixels ([128][ND]) and the shifted planes gs[q - d][d] ([ND][128], zero where
+// q - d leaves the map: those displacements read the zero padding in the forward) once, then c1 and warp (8+2R)x(16+2R) halos per
+// 32-channel pass (flow != NULL: the warp halo recomputed from c2 and fs * flow, never stored in HBM).
+constexpr int cv_bwd_smem(int R) { return (2 * kCvTH * kCvTW * cv_ndisp(R) + 2 * cv_hh(R) * cv_hw(R) * kCvPitch) * 4; }
+static_assert(cv_bwd_smem(kCvRMax) == 193536 && cv_bwd_smem(kCvRMax + 1) > 227 * 1024, "R = 4 is the largest range that fits a block");
+template <int R, class O1, class O2>
+__global__ void __launch_bounds__(256, cv_min_blocks(R)) costvol_bwd_kernel(const bf16* __restrict__ c1, int c1p, int c1o, const bf16* __restrict__ c2, int c2p,
                                                           int c2o, const float* __restrict__ flow, float fs, const float* __restrict__ gs, int B,
                                                           int h, int w, int C, const O1 dc1, const O2 dwarp) {
+  constexpr int S = cv_span(R), ND = cv_ndisp(R), HH = cv_hh(R), HW = cv_hw(R);
   pdl_launch_dependents();
   pdl_wait();
   extern __shared__ float cvs[];
-  float* gself = cvs;                              // [128][81]
-  float* gsh = gself + kCvTH * kCvTW * 81;         // [81][128]
-  float* h1 = gsh + kCvTH * kCvTW * 81;            // c1 halo   [384][36]
-  float* h2 = h1 + kCvHH * kCvHW * kCvPitch;       // warp halo [384][36]
+  float* gself = cvs;                              // [128][ND]
+  float* gsh = gself + kCvTH * kCvTW * ND;         // [ND][128]
+  float* h1 = gsh + kCvTH * kCvTW * ND;            // c1 halo   [HH * HW][36]
+  float* h2 = h1 + HH * HW * kCvPitch;             // warp halo [HH * HW][36]
   const int tid = threadIdx.x;
   const int b = blockIdx.z, y0 = blockIdx.y * kCvTH, x0 = blockIdx.x * kCvTW;
-  for (int it = tid; it < kCvTH * kCvTW * 81; it += 256) {
-    const int p = it / 81, d = it % 81;
+  for (int it = tid; it < kCvTH * kCvTW * ND; it += 256) {
+    const int p = it / ND, d = it % ND;
     const int y = y0 + (p >> 4), x = x0 + (p & 15);
-    gself[it] = (y < h && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * 81 + d) : 0.f;
+    gself[it] = (y < h && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * ND + d) : 0.f;
   }
-  for (int it = tid; it < kCvTH * kCvTW * 81; it += 256) {
+  for (int it = tid; it < kCvTH * kCvTW * ND; it += 256) {
     const int d = it >> 7, q = it & 127;
-    const int y = y0 + (q >> 4) - (d / 9 - kCvR), x = x0 + (q & 15) - (d % 9 - kCvR);
-    gsh[it] = (y >= 0 && y < h && x >= 0 && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * 81 + d) : 0.f;
+    const int y = y0 + (q >> 4) - (d / S - R), x = x0 + (q & 15) - (d % S - R);
+    gsh[it] = (y >= 0 && y < h && x >= 0 && x < w) ? __ldg(gs + ((size_t)(b * h + y) * w + x) * ND + d) : 0.f;
   }
   const int pix = tid & 127, py = pix >> 4, px = pix & 15;
   const int ck0 = (tid >> 7) * 2;   // this thread's two 8-channel chunks of the pass
@@ -1435,9 +1451,9 @@ __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict
   const int Cp = (C + 7) & ~7;
   for (int cc = 0; cc < Cp; cc += 32) {
     const int nck = min(4, (Cp - cc) / 8);
-    for (int it = tid; it < kCvHH * kCvHW * 4; it += 256) {
+    for (int it = tid; it < HH * HW * 4; it += 256) {
       const int p = it >> 2, ck = it & 3;
-      const int y = y0 - kCvR + p / kCvHW, x = x0 - kCvR + p % kCvHW;
+      const int y = y0 - R + p / HW, x = x0 - R + p % HW;
       float v1[8] = {0, 0, 0, 0, 0, 0, 0, 0}, v2[8] = {0, 0, 0, 0, 0, 0, 0, 0};
       if (ck < nck && y >= 0 && y < h && x >= 0 && x < w) {
         const size_t q = (size_t)(b * h + y) * w + x;
@@ -1459,12 +1475,12 @@ __global__ void __launch_bounds__(256) costvol_bwd_kernel(const bf16* __restrict
       float a1[16], a2[16];
 #pragma unroll
       for (int e = 0; e < 16; ++e) a1[e] = a2[e] = 0.f;
-      for (int dy = 0; dy < 9; ++dy) {
-        for (int dx = 0; dx < 9; ++dx) {
-          const int d = dy * 9 + dx;
-          const float g1 = gself[pix * 81 + d], g2 = gsh[d * 128 + pix];
-          const float* r2 = h2 + ((py + dy) * kCvHW + px + dx) * kCvPitch + ck0 * 8;               // warp[p + d]
-          const float* r1 = h1 + ((py + 2 * kCvR - dy) * kCvHW + px + 2 * kCvR - dx) * kCvPitch + ck0 * 8;   // c1[q - d]
+      for (int dy = 0; dy < S; ++dy) {
+        for (int dx = 0; dx < S; ++dx) {
+          const int d = dy * S + dx;
+          const float g1 = gself[pix * ND + d], g2 = gsh[d * 128 + pix];
+          const float* r2 = h2 + ((py + dy) * HW + px + dx) * kCvPitch + ck0 * 8;                    // warp[p + d]
+          const float* r1 = h1 + ((py + 2 * R - dy) * HW + px + 2 * R - dx) * kCvPitch + ck0 * 8;    // c1[q - d]
 #pragma unroll
           for (int e4 = 0; e4 < 4; ++e4) {
             const float4 u = *reinterpret_cast<const float4*>(r2 + e4 * 4);
@@ -1519,6 +1535,87 @@ static void cis_launch(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
 static inline unsigned nblk(size_t n, int t = 256) { return (unsigned)((n + t - 1) / t); }
 typedef const __nv_bfloat16* cbf;
 typedef __nv_bfloat16* mbf;
+
+// ---- warp + cost volume, forward and backward, for search range R (the three entry points without a range argument are R = 4)
+template <int R>
+static int warp_costvol_fwd(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs,
+                            int32_t B, int32_t h, int32_t w, int32_t C, void* out, int32_t op, int32_t oo, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol: needs h,w >= 2 (core_warp.py:188)");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(warp_costvol_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_smem(R));
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(warp_costvol)");
+    attr = true;
+  }
+  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
+  CIS_LAUNCH(warp_costvol_kernel<R>, grid, 256, cv_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, B, h, w, C, (mbf)out, op, oo);
+  return cis_check_launch("warp_costvol");
+}
+template <int R>
+static int cost_volume_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* warp, int32_t wp, int32_t wo, const float* dout, int32_t B,
+                           int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: needs h,w >= 2 (core_warp.py:188)");
+  if (!gscratch || !dc1 || !dwarp) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: NULL output or scratch");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<R, float>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_smem(R));
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<R, F32Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_bwd_smem(R));
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(costvol_bwd)");
+    attr = true;
+  }
+  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
+  CIS_LAUNCH((costvol_bwd_gate_kernel<R, float>), grid, 256, cv_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr, 1.f, dout,
+             cv_ndisp(R), 0, B, h, w, C, gscratch);
+  CIS_LAUNCH((costvol_bwd_kernel<R, F32Out, F32Out>), grid, 256, cv_bwd_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr,
+             1.f, (const float*)gscratch, B, h, w, C, F32Out{dc1, C, 0}, F32Out{dwarp, C, 0});
+  return cis_check_launch("cost_volume_bwd");
+}
+template <int R>
+static int warp_costvol_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs,
+                            int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr, int32_t dcp, int32_t dco, void* dc1, int32_t dc1p,
+                            int32_t dc1o, void* dc2, int32_t dc2p, int32_t dc2o, void* dflow, int32_t dfp, int32_t dfo, int32_t accumulate,
+                            float* gscratch, float* wscratch, double* dscratch, cis_stream_t stream) {
+  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: needs h,w >= 2 (core_warp.py:188)");
+  if (!dcorr || !dc1 || !dc2 || !gscratch) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: NULL gradient or scratch");
+  if (flow && (!dflow || !wscratch || !dscratch)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: the warp needs dflow and scratch");
+  if ((c1p | c1o | c2p | c2o) & 7) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: feature slices must be 8-channel aligned");
+  static bool attr = false;
+  if (!attr) {
+    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<R, bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_smem(R));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(costvol_bwd_kernel<R, Bf16Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_bwd_smem(R));
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(costvol_bwd_kernel<R, Bf16Out, Bf16Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, cv_bwd_smem(R));
+    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(warp_costvol_bwd)");
+    attr = true;
+  }
+  const Bf16Out o1{(mbf)dc1, dc1p, dc1o, accumulate & 1}, o2{(mbf)dc2, dc2p, dc2o, (accumulate >> 1) & 1};
+  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
+  CIS_LAUNCH((costvol_bwd_gate_kernel<R, bf16>), grid, 256, cv_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (cbf)dcorr, dcp, dco, B,
+             h, w, C, gscratch);
+  if (!flow) {       // level 6: no warp, dwarp is dc2
+    CIS_LAUNCH((costvol_bwd_kernel<R, Bf16Out, Bf16Out>), grid, 256, cv_bwd_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs,
+               (const float*)gscratch, B, h, w, C, o1, o2);
+    return cis_check_launch("warp_costvol_bwd");
+  }
+  CIS_LAUNCH((costvol_bwd_kernel<R, Bf16Out, F32Out>), grid, 256, cv_bwd_smem(R), ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs,
+             (const float*)gscratch, B, h, w, C, o1, F32Out{wscratch, C, 0});
+  const size_t npix = (size_t)B * h * w;
+  cudaError_t e = cudaMemsetAsync(dscratch, 0, npix * C * sizeof(double), ST);
+  if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaMemsetAsync");
+  CIS_LAUNCH(dense_image_warp_bwd_kernel<Bf16Out>, nblk(npix), 256, 0, ST, (cbf)c2, c2p, c2o, flow, fs, B, h, w, C, (const float*)wscratch, dscratch,
+             Bf16Out{(mbf)dflow, dfp, dfo, (accumulate >> 2) & 1});
+  CIS_LAUNCH(round_f64_kernel<Bf16Out>, nblk(npix * C), 256, 0, ST, (const double*)dscratch, npix, C, o2);
+  return cis_check_launch("warp_costvol_bwd");
+}
+#define CIS_CV_DISPATCH(fn, what, ...)                                                                                  \
+  switch (search_range) {                                                                                              \
+    case 1: return fn<1>(__VA_ARGS__);                                                                                 \
+    case 2: return fn<2>(__VA_ARGS__);                                                                                 \
+    case 3: return fn<3>(__VA_ARGS__);                                                                                 \
+    case 4: return fn<4>(__VA_ARGS__);                                                                                 \
+    default: return cis_set_error(CIS_ERR_BAD_ARG, what ": search_range must be 1, 2, 3 or 4");                       \
+  }
 
 extern "C" {
 
@@ -1679,16 +1776,11 @@ int cis_resize_nn_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t
 }
 int cis_warp_costvol(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs, int32_t B,
                      int32_t h, int32_t w, int32_t C, void* out, int32_t op, int32_t oo, cis_stream_t stream) {
-  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol: needs h,w >= 2 (core_warp.py:188)");
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(warp_costvol_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
-    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(warp_costvol)");
-    attr = true;
-  }
-  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
-  CIS_LAUNCH(warp_costvol_kernel, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, B, h, w, C, (mbf)out, op, oo);
-  return cis_check_launch("warp_costvol");
+  return warp_costvol_fwd<4>(c1, c1p, c1o, c2, c2p, c2o, flow, fs, B, h, w, C, out, op, oo, stream);
+}
+int cis_warp_costvol_r(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs, int32_t B,
+                       int32_t h, int32_t w, int32_t C, void* out, int32_t op, int32_t oo, int32_t search_range, cis_stream_t stream) {
+  CIS_CV_DISPATCH(warp_costvol_fwd, "cis_warp_costvol_r", c1, c1p, c1o, c2, c2p, c2o, flow, fs, B, h, w, C, out, op, oo, stream)
 }
 int cis_dense_image_warp(const void* img, int32_t pitch, int32_t coff, const float* flow, float fs, int32_t B, int32_t h, int32_t w, int32_t C,
                          void* out, int32_t op, cis_stream_t stream) {
@@ -1810,56 +1902,25 @@ int cis_dense_image_warp_bwd(const void* img, int32_t pitch, int32_t coff, const
 }
 int cis_cost_volume_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* warp, int32_t wp, int32_t wo, const float* dout, int32_t B, int32_t h,
                         int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp, cis_stream_t stream) {
-  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: needs h,w >= 2 (core_warp.py:188)");
-  if (!gscratch || !dc1 || !dwarp) return cis_set_error(CIS_ERR_BAD_ARG, "cis_cost_volume_bwd: NULL output or scratch");
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<F32Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
-    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(costvol_bwd)");
-    attr = true;
-  }
-  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
-  CIS_LAUNCH(costvol_bwd_gate_kernel<float>, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr, 1.f, dout, 81, 0,
-             B, h, w, C, gscratch);
-  CIS_LAUNCH((costvol_bwd_kernel<F32Out, F32Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)warp, wp, wo, (const float*)nullptr, 1.f,
-             (const float*)gscratch, B, h, w, C, F32Out{dc1, C, 0}, F32Out{dwarp, C, 0});
-  return cis_check_launch("cost_volume_bwd");
+  return cost_volume_bwd<4>(c1, c1p, c1o, warp, wp, wo, dout, B, h, w, C, gscratch, dc1, dwarp, stream);
+}
+int cis_cost_volume_bwd_r(const void* c1, int32_t c1p, int32_t c1o, const void* warp, int32_t wp, int32_t wo, const float* dout, int32_t B,
+                          int32_t h, int32_t w, int32_t C, float* gscratch, float* dc1, float* dwarp, int32_t search_range, cis_stream_t stream) {
+  CIS_CV_DISPATCH(cost_volume_bwd, "cis_cost_volume_bwd_r", c1, c1p, c1o, warp, wp, wo, dout, B, h, w, C, gscratch, dc1, dwarp, stream)
 }
 int cis_warp_costvol_bwd(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs,
                          int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr, int32_t dcp, int32_t dco, void* dc1, int32_t dc1p,
                          int32_t dc1o, void* dc2, int32_t dc2p, int32_t dc2o, void* dflow, int32_t dfp, int32_t dfo, int32_t accumulate,
                          float* gscratch, float* wscratch, double* dscratch, cis_stream_t stream) {
-  if (h < 2 || w < 2) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: needs h,w >= 2 (core_warp.py:188)");
-  if (!dcorr || !dc1 || !dc2 || !gscratch) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: NULL gradient or scratch");
-  if (flow && (!dflow || !wscratch || !dscratch)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: the warp needs dflow and scratch");
-  if ((c1p | c1o | c2p | c2o) & 7) return cis_set_error(CIS_ERR_BAD_ARG, "cis_warp_costvol_bwd: feature slices must be 8-channel aligned");
-  static bool attr = false;
-  if (!attr) {
-    cudaError_t e = cudaFuncSetAttribute(costvol_bwd_gate_kernel<bf16>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<Bf16Out, F32Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(costvol_bwd_kernel<Bf16Out, Bf16Out>, cudaFuncAttributeMaxDynamicSharedMemorySize, kCvBwdSmem);
-    if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(warp_costvol_bwd)");
-    attr = true;
-  }
-  const Bf16Out o1{(mbf)dc1, dc1p, dc1o, accumulate & 1}, o2{(mbf)dc2, dc2p, dc2o, (accumulate >> 1) & 1};
-  dim3 grid((w + kCvTW - 1) / kCvTW, (h + kCvTH - 1) / kCvTH, B);
-  CIS_LAUNCH(costvol_bwd_gate_kernel<bf16>, grid, 256, kCvSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (cbf)dcorr, dcp, dco, B, h, w, C,
-             gscratch);
-  if (!flow) {       // level 6: no warp, dwarp is dc2
-    CIS_LAUNCH((costvol_bwd_kernel<Bf16Out, Bf16Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (const float*)gscratch,
-               B, h, w, C, o1, o2);
-    return cis_check_launch("warp_costvol_bwd");
-  }
-  CIS_LAUNCH((costvol_bwd_kernel<Bf16Out, F32Out>), grid, 256, kCvBwdSmem, ST, (cbf)c1, c1p, c1o, (cbf)c2, c2p, c2o, flow, fs, (const float*)gscratch,
-             B, h, w, C, o1, F32Out{wscratch, C, 0});
-  const size_t npix = (size_t)B * h * w;
-  cudaError_t e = cudaMemsetAsync(dscratch, 0, npix * C * sizeof(double), ST);
-  if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaMemsetAsync");
-  CIS_LAUNCH(dense_image_warp_bwd_kernel<Bf16Out>, nblk(npix), 256, 0, ST, (cbf)c2, c2p, c2o, flow, fs, B, h, w, C, (const float*)wscratch, dscratch,
-             Bf16Out{(mbf)dflow, dfp, dfo, (accumulate >> 2) & 1});
-  CIS_LAUNCH(round_f64_kernel<Bf16Out>, nblk(npix * C), 256, 0, ST, (const double*)dscratch, npix, C, o2);
-  return cis_check_launch("warp_costvol_bwd");
+  return warp_costvol_bwd<4>(c1, c1p, c1o, c2, c2p, c2o, flow, fs, B, h, w, C, dcorr, dcp, dco, dc1, dc1p, dc1o, dc2, dc2p, dc2o, dflow, dfp, dfo,
+                             accumulate, gscratch, wscratch, dscratch, stream);
+}
+int cis_warp_costvol_bwd_r(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs,
+                           int32_t B, int32_t h, int32_t w, int32_t C, const void* dcorr, int32_t dcp, int32_t dco, void* dc1, int32_t dc1p,
+                           int32_t dc1o, void* dc2, int32_t dc2p, int32_t dc2o, void* dflow, int32_t dfp, int32_t dfo, int32_t accumulate,
+                           float* gscratch, float* wscratch, double* dscratch, int32_t search_range, cis_stream_t stream) {
+  CIS_CV_DISPATCH(warp_costvol_bwd, "cis_warp_costvol_bwd_r", c1, c1p, c1o, c2, c2p, c2o, flow, fs, B, h, w, C, dcorr, dcp, dco, dc1, dc1p, dc1o,
+                  dc2, dc2p, dc2o, dflow, dfp, dfo, accumulate, gscratch, wscratch, dscratch, stream)
 }
 int cis_parity_split_bf16(const void* src, int32_t sp, int32_t sc, int32_t N, int32_t H, int32_t W, int32_t C, void* dst, int32_t dp,
                           cis_stream_t stream) {

@@ -15,6 +15,7 @@ import numpy as np
 import torch
 
 from ..step_graph import CISGraph, PWC_H, PWC_W
+from .PWCNet import model_pwcnet
 from ..data.synthetic import SyntheticReader
 from .. import params_init
 from .. import checkpoint as ckpt_io
@@ -100,7 +101,8 @@ class AdversarialLearner(object):
         self.local_batch = cfg.batch_size // self.world
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
-                              flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True)
+                              flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
+                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self.val_steps_per_epoch = int(np.ceil(float(self.num_samples_val) / cfg.batch_size))
         self._init_params()
@@ -426,7 +428,8 @@ class AdversarialLearner(object):
         self._inference = True
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
-                              cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False)
+                              cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False,
+                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 
@@ -440,7 +443,7 @@ class AdversarialLearner(object):
         self._inference = True
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
-                              with_pwc=True, train=False)
+                              with_pwc=True, train=False, pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 

@@ -8,7 +8,7 @@ from the registry filled by `set_parameters()` (dict name -> tensor, names as in
 PyTorch is used for memory and the small amount of buffer plumbing only; there is no CPU fallback: without the CUDA library (or on CPU
 tensors) the calls raise.
 
-Gradients: generator_net, recover_net, ModelPWCNet.predict_from_img_pairs, charbonnier_loss, cost_volume and dense_image_warp are
+Gradients: generator_net, recover_net, ModelPWCNet.predict_from_img_pairs, charbonnier_loss, cost_volume(_r) and dense_image_warp are
 torch.autograd Functions (first order only) when an input or one of the parameter tensors the call reads requires grad; the parameters
 then receive gradients under their variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain
 rule, resize transposes, the PWC-Net warp + cost-volume and transposed-conv backward) and the backward kernels of the three stand-alone
@@ -227,13 +227,14 @@ class _RecoverRunner(_NetRunner):
 
 
 class _PWCRunner(_NetRunner):
-    """trainable=False: the forward-only plan of calls without gradients.  trainable=True: layers tagged 'P', backward recorded."""
+    """trainable=False: the forward-only plan of calls without gradients.  trainable=True: layers tagged 'P', backward recorded.
+    options: the PWC-Net options (None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)."""
     MODE, SEED, INPUT_GRADS = 'P', 'dflow_out', ('dimg1', 'dimg2')
 
-    def __init__(self, B, H, W, device, name, trainable=False):
-        from .PWCNet.model_pwcnet import ModelPWCNet
+    def __init__(self, B, H, W, device, name, trainable=False, options=None):
+        from .PWCNet.model_pwcnet import PWCNetBuilder
         _NetRunner.__init__(self, device)
-        self.net = ModelPWCNet(self.store, name, trainable=trainable)
+        self.net = PWCNetBuilder(self.store, name, trainable=trainable, options=options)
         self.store.finalize(False)
         f32 = self.bld.f32
         self.B, self.H, self.W = B, H, W
@@ -412,21 +413,24 @@ def recover_net(img1, flow_masked, mask, scope='FlownetS', reuse=None, f=0.25, t
         raise
 
 
-def predict_from_img_pairs(img1, img2, name='pwcnet', params=None):
+def predict_from_img_pairs(img1, img2, name='pwcnet', params=None, options=None):
     """ModelPWCNet.predict_from_img_pairs (model_pwcnet.py:39-76): forward flow img1 -> img2, [B,H,W,2] in pixels of the input size
     (H, W multiples of 64, 384x640 in the reference's pipeline).  Differentiable w.r.t. img1, img2 and every '<name>/...' parameter
     (kernels HWIO, transposed-conv kernels [kh,kw,Cout,Cin]; bf16 activations, fp32 gradients), for fine-tuning the flow network or
-    gradients with respect to the frames.  The training step keeps PWC-Net frozen, as the reference does (adversarial_learner.py:211-234)."""
+    gradients with respect to the frames.  The training step keeps PWC-Net frozen, as the reference does (adversarial_learner.py:211-234).
+    options: the PWC-Net options (dense connections, context network, search range; None = the module default), part of the plan key."""
+    from .PWCNet.model_pwcnet import normalize_options
     _check_cuda(img1, img2)
     B, H, W, _ = img1.shape
     if H % 64 or W % 64:
         raise ValueError('PWC-Net needs input sizes that are multiples of 64 (6 pyramid levels); got %dx%d' % (H, W))
-    key = (B, H, W, str(img1.device), name)
-    r = _runner('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name))
+    opts = normalize_options(options)
+    key = (B, H, W, str(img1.device), name, opts)
+    r = _runner('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name, options=opts))
     names, pvals = _param_inputs(r, params)
     if not _needs_grad([img1, img2] + pvals):
         return r(img1, img2, params)
-    lease = _lease('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name, trainable=True))
+    lease = _lease('pwc', key, lambda: _PWCRunner(B, H, W, img1.device, name, trainable=True, options=opts))
     try:
         return _NetFn.apply(lease, names, 2, img1, img2, *pvals)
     except BaseException:
@@ -512,30 +516,48 @@ def _to_act(x):
 
 
 def cost_volume(c1, warp, search_range=4, name=None):
-    """models/PWCNet/core_costvol.py:20-40 -> [B,h,w,(2r+1)^2]: leaky_relu(mean_c c1 * shifted warp, 0.1), zero padded, dy outer.
-    The kernel is built for the reference's search_range = 4 (81 displacements); features and result are bf16-rounded like in the
-    pipeline.  Differentiable w.r.t. c1 and warp (gradients of the bf16-rounded features, fp32)."""
-    _check_cuda(c1, warp)
+    """models/PWCNet/core_costvol.py:20-40 -> [B,h,w,81]: leaky_relu(mean_c c1 * shifted warp, 0.1), zero padded, dy outer, for the
+    reference's default search_range = 4; features and result are bf16-rounded like in the pipeline.  Differentiable w.r.t. c1 and warp
+    (gradients of the bf16-rounded features, fp32).  Other ranges raise NotImplementedError here; cost_volume_r takes ranges 1..4."""
     if search_range != 4:
-        raise NotImplementedError('cost_volume: the fused kernel implements search_range=4 (model_pwcnet.py options)')
+        raise NotImplementedError('cost_volume: implements search_range=4 (model_pwcnet.py options); cost_volume_r(c1, warp, search_range) '
+                                  'takes 1, 2, 3 and 4')
+    return cost_volume_r(c1, warp, 4)
+
+
+def cost_volume_r(c1, warp, search_range, name=None):
+    """cost_volume for search_range 1..4 -> [B,h,w,(2r+1)^2] (model_pwcnet.py option 'search_range'): the same op, forward and gradient,
+    on the fused kernels' range variants; range 4 runs exactly cost_volume."""
+    _check_cuda(c1, warp)
+    if isinstance(search_range, bool) or search_range not in (1, 2, 3, 4):
+        raise NotImplementedError('cost_volume_r: the fused kernels implement search_range 1, 2, 3 and 4; got %r' % (search_range,))
+    r = int(search_range)
     if _needs_grad([c1, warp]):
-        return _CostVolumeFn.apply(c1, warp)
-    return _cost_volume_fwd(c1, warp)[0]
+        return _CostVolumeFn.apply(c1, warp, r)
+    return _cost_volume_fwd(c1, warp, r)[0]
 
 
-def _cost_volume_fwd(c1, warp):
+def _costvol_entry(name, r):
+    """Entry point and trailing arguments for range r: the range-free (R = 4) entry point for the default range."""
+    return (name, ()) if r == 4 else (name + '_r', (r,))
+
+
+def _cost_volume_fwd(c1, warp, r=4):
     B, h, w, C = c1.shape
+    nd = (2 * r + 1) ** 2
+    pitch = (nd + 7) // 8 * 8
     a1, a2 = _to_act(c1), _to_act(warp)
-    out = torch.zeros(B, h, w, 88, dtype=torch.bfloat16, device=c1.device)
-    _lib.call('cis_warp_costvol', a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, None, 1.0, B, h, w, C, out.data_ptr(), 88, 0, _stream())
-    return out[..., :81].float(), a1, a2
+    out = torch.zeros(B, h, w, pitch, dtype=torch.bfloat16, device=c1.device)
+    op, rng = _costvol_entry('cis_warp_costvol', r)
+    _lib.call(op, a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, None, 1.0, B, h, w, C, out.data_ptr(), pitch, 0, *rng, _stream())
+    return out[..., :nd].float(), a1, a2
 
 
 class _CostVolumeFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, c1, warp):
-        out, a1, a2 = _cost_volume_fwd(c1, warp)
-        ctx.acts = (a1, a2)
+    def forward(ctx, c1, warp, r):
+        out, a1, a2 = _cost_volume_fwd(c1, warp, r)
+        ctx.acts, ctx.r = (a1, a2), r
         ctx.dtypes = (c1.dtype, warp.dtype)
         return out
 
@@ -545,12 +567,13 @@ class _CostVolumeFn(torch.autograd.Function):
         a1, a2 = ctx.acts
         B, h, w, C = a1.N, a1.H, a1.W, a1.C
         d = dout.contiguous().float()
-        gs = torch.empty(B, h, w, 81, dtype=torch.float32, device=d.device)
+        gs = torch.empty(B, h, w, (2 * ctx.r + 1) ** 2, dtype=torch.float32, device=d.device)
         dc1, dwarp = (torch.empty(B, h, w, C, dtype=torch.float32, device=d.device) for _ in range(2))
-        _lib.call('cis_cost_volume_bwd', a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, d.data_ptr(), B, h, w, C, gs.data_ptr(),
-                  dc1.data_ptr(), dwarp.data_ptr(), _stream())
+        op, rng = _costvol_entry('cis_cost_volume_bwd', ctx.r)
+        _lib.call(op, a1.ptr, a1.pitch, a1.c_off, a2.ptr, a2.pitch, a2.c_off, d.data_ptr(), B, h, w, C, gs.data_ptr(),
+                  dc1.data_ptr(), dwarp.data_ptr(), *rng, _stream())
         ctx.acts = None
-        return tuple(g.to(dt) if n else None for g, dt, n in zip((dc1, dwarp), ctx.dtypes, ctx.needs_input_grad))
+        return tuple(g.to(dt) if n else None for g, dt, n in zip((dc1, dwarp), ctx.dtypes, ctx.needs_input_grad)) + (None,)
 
 
 def dense_image_warp(image, flow, name=None):

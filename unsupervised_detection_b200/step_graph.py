@@ -9,14 +9,15 @@ import torch
 from . import _lib
 from .engine import Builder, ParamStore, Plan, Act
 from .models.nets import GeneratorNet, RecoverNet
-from .models.PWCNet.model_pwcnet import ModelPWCNet
+from .models.PWCNet.model_pwcnet import PWCNetBuilder
 
 PWC_H, PWC_W = 384, 640   # data/davis2016_data_utils.py:87-88: frames are resized to 384x640 before PWC-Net
 
 
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
-                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964):
+                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None):
+        """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)."""
         _lib.load()
         self.H, self.W, self.B = img_height, img_width, batch
         self.GB = global_batch or batch
@@ -33,7 +34,7 @@ class CISGraph(object):
         self.gen_store.finalize(True)
         self.rec_store.finalize(True)
         if with_pwc:
-            self.pwc = ModelPWCNet(self.pwc_store)
+            self.pwc = PWCNetBuilder(self.pwc_store, options=pwc_options)
             self.pwc_store.finalize(False)
         self.step_state = torch.zeros(1, dtype=torch.int64, device=device)   # shared Adam beta-power step (App. A.14)
         self.avg_abs = f32(1)
