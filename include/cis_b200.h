@@ -242,6 +242,18 @@ int cis_crop_resize_bilinear_f32(const float* src, int32_t Hs, int32_t Ws, int32
 /* tf.image.resize_images(NEAREST_NEIGHBOR) for GT masks (adversarial_learner.py:92-94) */
 int cis_resize_nn_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW,
                       cis_stream_t stream);
+/* tf.image.resize_bilinear / resize_nearest_neighbor with TF 1.13 semantics (no half-pixel centres) on fp32 NHWC [N,H,W,C] -> [N,OH,OW,C],
+ * any sizes up or down (the `func` of convolution_utils.py:4-24).  Step = (in-1)/(out-1) when align_corners and out > 1, else in/out (fp32);
+ * bilinear: lo = floor(d*step), hi = min(lo+1, in-1); nearest: roundf(d*step) with align_corners, floor without, clamped to in-1.
+ * method = CIS_RESIZE_*, align_corners = 0 / 1 (CIS_ERR_BAD_ARG otherwise, and for sizes < 1).  method = BILINEAR, align_corners = 0
+ * computes cis_resize_bilinear_f32 with scale 1; NEAREST, 0 computes cis_resize_nn_f32. */
+enum { CIS_RESIZE_BILINEAR = 0, CIS_RESIZE_NEAREST = 1 };
+int cis_resize_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW, int32_t method,
+                   int32_t align_corners, cis_stream_t stream);
+/* its transpose: dsrc [N,H,W,C] = R^T ddst [N,OH,OW,C] (overwritten).  A gather with no atomics: every dsrc element sums its own
+ * contiguous rectangle of ddst in a fixed order, so the result is bit-identical run to run, for downsampling as well. */
+int cis_resize_f32_bwd(const float* ddst, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, float* dsrc, int32_t method,
+                       int32_t align_corners, cis_stream_t stream);
 
 /* ---- PWC-Net warp + cost volume (core_warp.py:153-202 fused into core_costvol.py:20-40) ----
  * out[b,y,x,9*dy+dx] = leaky0.1( mean_c c1[b,y,x,c] * warp(c2, flow)[b,y+dy-4,x+dx-4,c] ), zero outside; flow may be
@@ -266,6 +278,13 @@ int cis_pack_f32_to_bf16(const float* src, int64_t npix, int32_t C, float offset
 int cis_flow_stats(const float* flow, int32_t B, int64_t hw, double* stats, cis_stream_t stream);
 /* generator input = concat(image, (flow-mean)/sqrt(var)) -> bf16 [B,H,W,8]  (nets.py:14, flow_utils.py:5-12) */
 int cis_pack_generator_input(const float* image, const float* flow, const double* stats, int32_t B, int64_t hw, void* dst,
+                             cis_stream_t stream);
+/* stand-alone preprocess_flow_batch (flow_utils.py:5-12): out fp32 [B,hw,2] = (flow - mean) / sqrt(population variance) per sample and
+ * channel, no epsilon, with the statistics of cis_flow_stats (the normalisation cis_pack_generator_input applies, in fp32) */
+int cis_flow_standardize(const float* flow, const double* stats, int32_t B, int64_t hw, float* out, cis_stream_t stream);
+/* its gradient: dx = (dy - mean(dy) - y * mean(dy * y)) / sigma per sample and channel, y = the forward output.  The two means are
+ * fixed-order reductions through `scratch` (double [B * 256], need not be initialised): bit-identical run to run. */
+int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stats, int32_t B, int64_t hw, double* scratch, float* dx,
                              cis_stream_t stream);
 
 /* ---- mask (x) flow + Charbonnier contextual-information loss (adversarial_learner.py:107-110,141-204) ---- */

@@ -11,6 +11,7 @@ LIB_PATH = os.path.join(_HERE, os.environ.get('CIS_LIB_NAME', 'libcis_b200.so'))
 
 MAX_TAPS, MAX_SRC = 49, 4
 ACT_NONE, ACT_ELU, ACT_LEAKY = 0, 1, 2
+RESIZE_BILINEAR, RESIZE_NEAREST = 0, 1
 
 
 class CisSrc(C.Structure):
@@ -86,6 +87,10 @@ _PROTOS = {
     'cis_upsample_nn2x_bwd': [_p, _i32, _i32, _i32, _i32, _p, _i32],
     'cis_crop_resize_bilinear_f32': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
     'cis_resize_nn_f32': [_p, _i32, _i32, _i32, _i32, _p, _i32, _i32],
+    'cis_resize_f32': [_p, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32, _i32],
+    'cis_resize_f32_bwd': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
+    'cis_flow_standardize': [_p, _p, _i32, _i64, _p],
+    'cis_flow_standardize_bwd': [_p, _p, _p, _i32, _i64, _p, _p],
     'cis_warp_costvol': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
     'cis_dense_image_warp': [_p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32],
     'cis_pack_f32_to_bf16': [_p, _i64, _i32, _f32, _p, _i32, _i32],

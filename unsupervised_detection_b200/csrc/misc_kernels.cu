@@ -628,6 +628,13 @@ __global__ void resize_concat_bf16_bwd_kernel(const bf16* __restrict__ dd, int d
   }
   *o = pack8(acc);
 }
+// source step of tf.image.resize_* in TF 1.13 (no half-pixel centres): (in-1)/(out-1) with align_corners and out > 1, else in/out
+template <bool AC>
+__device__ __forceinline__ float resize_step(int n_in, int n_out) {
+  return (AC && n_out > 1) ? (float)(n_in - 1) / (float)(n_out - 1) : (float)n_in / (float)n_out;
+}
+// AC = align_corners; AC = false is the legacy resize of the step graph (cis_resize_bilinear_f32)
+template <bool AC>
 __global__ void resize_bilinear_f32_kernel(const float* __restrict__ src, int N, int H, int W, int C, float* __restrict__ dst, int OH, int OW,
                                            float scale) {
   pdl_launch_dependents();
@@ -637,7 +644,7 @@ __global__ void resize_bilinear_f32_kernel(const float* __restrict__ src, int N,
   const int ox = (int)(pix % OW);
   const int oy = (int)((pix / OW) % OH);
   const int n = (int)(pix / ((size_t)OW * OH));
-  const Lerp ly = legacy_lerp(oy, H, (float)H / (float)OH), lx = legacy_lerp(ox, W, (float)W / (float)OW);
+  const Lerp ly = legacy_lerp(oy, H, resize_step<AC>(H, OH)), lx = legacy_lerp(ox, W, resize_step<AC>(W, OW));
   const float* b = src + (size_t)n * H * W * C;
   for (int c = 0; c < C; ++c) {
     const float tl = b[((size_t)ly.lo * W + lx.lo) * C + c], tr = b[((size_t)ly.lo * W + lx.hi) * C + c];
@@ -741,6 +748,12 @@ __global__ void upsample_nn2x_bwd_kernel(const bf16* __restrict__ dd, int N, int
   }
   *o = pack8(a);
 }
+// nearest source index: roundf with align_corners (App. A.5), floor without, clamped to in-1
+template <bool AC>
+__device__ __forceinline__ int nn_index(int d, int n_in, float step) {
+  return min((int)(AC ? roundf(d * step) : floorf(d * step)), n_in - 1);
+}
+template <bool AC>
 __global__ void resize_nn_f32_kernel(const float* __restrict__ src, int N, int H, int W, int C, float* __restrict__ dst, int OH, int OW) {
   pdl_launch_dependents();
   pdl_wait();
@@ -749,8 +762,59 @@ __global__ void resize_nn_f32_kernel(const float* __restrict__ src, int N, int H
   const int ox = (int)(pix % OW);
   const int oy = (int)((pix / OW) % OH);
   const int n = (int)(pix / ((size_t)OW * OH));
-  const int sy = min((int)floorf(oy * ((float)H / (float)OH)), H - 1), sx = min((int)floorf(ox * ((float)W / (float)OW)), W - 1);
+  const int sy = nn_index<AC>(oy, H, resize_step<AC>(H, OH)), sx = nn_index<AC>(ox, W, resize_step<AC>(W, OW));
   for (int c = 0; c < C; ++c) dst[pix * C + c] = src[((size_t)(n * H + sy) * W + sx) * C + c];
+}
+// Transpose of the four fp32 resizes as a gather: thread = one element (n, y, x, c) of dsrc.  Along each axis the source map d -> lo(d)
+// (bilinear) or d -> index(d) (nearest) is monotone, so the outputs that read input index i form one contiguous range, found by binary
+// search; each element sums its own rectangle of ddst in a fixed order -- no atomics, bit-identical run to run, for any scale.
+template <bool NEAREST, bool AC>
+__device__ __forceinline__ int resize_src_key(int d, int n_in, float step) {
+  return NEAREST ? nn_index<AC>(d, n_in, step) : (int)floorf(d * step);
+}
+// first d in [0, n_out) whose key is >= v (n_out when none)
+template <bool NEAREST, bool AC>
+__device__ __forceinline__ int resize_lower_bound(int v, int n_in, int n_out, float step) {
+  int lo = 0, hi = n_out;
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (resize_src_key<NEAREST, AC>(mid, n_in, step) < v) lo = mid + 1; else hi = mid;
+  }
+  return lo;
+}
+// weight of input index i in output index d
+template <bool NEAREST, bool AC>
+__device__ __forceinline__ float resize_w(int d, int i, int n_in, float step) {
+  if (NEAREST) return nn_index<AC>(d, n_in, step) == i ? 1.f : 0.f;
+  return legacy_w(d, i, n_in, step);
+}
+template <bool NEAREST, bool AC>
+__global__ void resize_f32_bwd_kernel(const float* __restrict__ dd, int N, int OH, int OW, int C, int H, int W, float* __restrict__ ds) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (size_t)N * H * W * C) return;
+  const int c = (int)(i % C);
+  const size_t pix = i / C;
+  const int x = (int)(pix % W);
+  const int y = (int)((pix / W) % H);
+  const int n = (int)(pix / ((size_t)W * H));
+  const float sy = resize_step<AC>(H, OH), sx = resize_step<AC>(W, OW);
+  // bilinear: outputs with lo in {i-1, i} read i (as hi or lo); nearest: outputs with index == i
+  const int kd = NEAREST ? 0 : 1;
+  const int y0 = resize_lower_bound<NEAREST, AC>(y - kd, H, OH, sy), y1 = resize_lower_bound<NEAREST, AC>(y + 1, H, OH, sy);
+  const int x0 = resize_lower_bound<NEAREST, AC>(x - kd, W, OW, sx), x1 = resize_lower_bound<NEAREST, AC>(x + 1, W, OW, sx);
+  float a = 0.f;
+  for (int dy = y0; dy < y1; ++dy) {
+    const float wy = resize_w<NEAREST, AC>(dy, y, H, sy);
+    if (wy == 0.f) continue;
+    const float* row = dd + ((size_t)(n * OH + dy) * OW) * C + c;
+    for (int dx = x0; dx < x1; ++dx) {
+      const float wt = wy * resize_w<NEAREST, AC>(dx, x, W, sx);
+      if (wt != 0.f) a += wt * row[(size_t)dx * C];
+    }
+  }
+  ds[i] = a;
 }
 
 // ------------------------------------------------------------------------------------------------ warp + cost volume
@@ -938,6 +1002,77 @@ __global__ void pack_generator_input_kernel(const float* __restrict__ image, con
   float v[8] = {image[pix * 3], image[pix * 3 + 1], image[pix * 3 + 2], (flow[pix * 2] - (float)m0) * r0, (flow[pix * 2 + 1] - (float)m1) * r1,
                 0, 0, 0};
   *reinterpret_cast<uint4*>(dst + pix * 8) = pack8(v);
+}
+// ---- stand-alone preprocess_flow_batch (flow_utils.py:5-12) and its gradient, fp32 [B,hw,2]
+// mean and 1/sqrt(population variance) of channel k of sample b, from cis_flow_stats' sums; the same arithmetic as
+// pack_generator_input_kernel, so the stand-alone call and the generator's fused input agree bit for bit
+__device__ __forceinline__ void flow_moments(const double* __restrict__ stats, int b, double n, float* m, float* r) {
+#pragma unroll
+  for (int k = 0; k < 2; ++k) {
+    const double mk = stats[b * 4 + k] / n;
+    m[k] = (float)mk;
+    r[k] = (float)(1.0 / sqrt(stats[b * 4 + 2 + k] / n - mk * mk));
+  }
+}
+__global__ void flow_standardize_kernel(const float* __restrict__ flow, const double* __restrict__ stats, size_t hw, float* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.y;
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= hw) return;
+  float m[2], r[2];
+  flow_moments(stats, b, (double)hw, m, r);
+  const size_t i = ((size_t)b * hw + p) * 2;
+  const float2 f = *reinterpret_cast<const float2*>(flow + i);
+  *reinterpret_cast<float2*>(out + i) = make_float2((f.x - m[0]) * r[0], (f.y - m[1]) * r[1]);
+}
+// backward, pass 1: block x of sample b sums {g0, g1, g0*y0, g1*y1} over a fixed pixel subset (grid-stride), in double, reduced in a
+// fixed order (warp butterfly, then the 8 warps in index order) into part[(b * kFlowStdBlocks + x) * 4 + k]
+constexpr int kFlowStdBlocks = 64;
+__global__ void flow_standardize_bwd_sums_kernel(const float* __restrict__ y, const float* __restrict__ g, size_t hw, double* __restrict__ part) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ double sm[8][4];
+  const int b = blockIdx.y;
+  double s[4] = {0, 0, 0, 0};
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (size_t)gridDim.x * blockDim.x) {
+    const size_t i = ((size_t)b * hw + p) * 2;
+    const float2 gv = *reinterpret_cast<const float2*>(g + i), yv = *reinterpret_cast<const float2*>(y + i);
+    s[0] += gv.x; s[1] += gv.y; s[2] += (double)gv.x * yv.x; s[3] += (double)gv.y * yv.y;
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) s[k] = warp_sum_d(s[k]);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sm[threadIdx.x >> 5][k] = s[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < 4) {
+    double t = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += sm[w][threadIdx.x];
+    part[((size_t)b * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = t;
+  }
+}
+// pass 2: dx = (g - mean(g) - y * mean(g * y)) / sigma per (sample, channel); every block re-adds the kFlowStdBlocks partials in order
+__global__ void flow_standardize_bwd_kernel(const float* __restrict__ y, const float* __restrict__ g, const double* __restrict__ stats,
+                                            const double* __restrict__ part, size_t hw, float* __restrict__ dx) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float mean[4];
+  const int b = blockIdx.y;
+  if (threadIdx.x < 4) {
+    double t = 0;
+    for (int q = 0; q < kFlowStdBlocks; ++q) t += part[((size_t)b * kFlowStdBlocks + q) * 4 + threadIdx.x];
+    mean[threadIdx.x] = (float)(t / (double)hw);
+  }
+  __syncthreads();
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= hw) return;
+  float m[2], r[2];
+  flow_moments(stats, b, (double)hw, m, r);
+  const size_t i = ((size_t)b * hw + p) * 2;
+  const float2 gv = *reinterpret_cast<const float2*>(g + i), yv = *reinterpret_cast<const float2*>(y + i);
+  *reinterpret_cast<float2*>(dx + i) = make_float2((gv.x - mean[0] - yv.x * mean[2]) * r[0], (gv.y - mean[1] - yv.y * mean[3]) * r[1]);
 }
 
 // ------------------------------------------------------------------------------------------------ mask (x) flow + loss
@@ -1748,7 +1883,7 @@ int cis_resize_concat_bf16_bwd(const void* ddst, int32_t dp, int32_t dc, int32_t
 }
 int cis_resize_bilinear_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW, float scale,
                             cis_stream_t stream) {
-  CIS_LAUNCH(resize_bilinear_f32_kernel, nblk((size_t)N * OH * OW), 256, 0, ST, src, N, H, W, C, dst, OH, OW, scale);
+  CIS_LAUNCH(resize_bilinear_f32_kernel<false>, nblk((size_t)N * OH * OW), 256, 0, ST, src, N, H, W, C, dst, OH, OW, scale);
   return cis_check_launch("resize_bilinear_f32");
 }
 int cis_crop_resize_bilinear_f32(const float* src, int32_t Hs, int32_t Ws, int32_t C, int32_t y0, int32_t x0, int32_t ch, int32_t cw, float* dst,
@@ -1771,8 +1906,45 @@ int cis_upsample_nn2x_bwd(const void* dd, int32_t N, int32_t H, int32_t W, int32
   return cis_check_launch("upsample_nn2x_bwd");
 }
 int cis_resize_nn_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW, cis_stream_t stream) {
-  CIS_LAUNCH(resize_nn_f32_kernel, nblk((size_t)N * OH * OW), 256, 0, ST, src, N, H, W, C, dst, OH, OW);
+  CIS_LAUNCH(resize_nn_f32_kernel<false>, nblk((size_t)N * OH * OW), 256, 0, ST, src, N, H, W, C, dst, OH, OW);
   return cis_check_launch("resize_nn_f32");
+}
+static int resize_f32_args(const char* what, const void* src, const void* dst, int32_t N, int32_t H, int32_t W, int32_t C, int32_t OH,
+                           int32_t OW, int32_t method, int32_t align_corners) {
+  if (method != CIS_RESIZE_BILINEAR && method != CIS_RESIZE_NEAREST) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  if (align_corners != 0 && align_corners != 1) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  if (!src || !dst || N < 1 || H < 1 || W < 1 || C < 1 || OH < 1 || OW < 1) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  return CIS_OK;
+}
+int cis_resize_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW, int32_t method,
+                   int32_t align_corners, cis_stream_t stream) {
+  const int rc = resize_f32_args("cis_resize_f32: bad method, align_corners, pointer or size", src, dst, N, H, W, C, OH, OW, method,
+                                 align_corners);
+  if (rc) return rc;
+  const unsigned g = nblk((size_t)N * OH * OW);
+  if (method == CIS_RESIZE_BILINEAR) {
+    if (align_corners) CIS_LAUNCH(resize_bilinear_f32_kernel<true>, g, 256, 0, ST, src, N, H, W, C, dst, OH, OW, 1.f);
+    else CIS_LAUNCH(resize_bilinear_f32_kernel<false>, g, 256, 0, ST, src, N, H, W, C, dst, OH, OW, 1.f);
+  } else {
+    if (align_corners) CIS_LAUNCH(resize_nn_f32_kernel<true>, g, 256, 0, ST, src, N, H, W, C, dst, OH, OW);
+    else CIS_LAUNCH(resize_nn_f32_kernel<false>, g, 256, 0, ST, src, N, H, W, C, dst, OH, OW);
+  }
+  return cis_check_launch("resize_f32");
+}
+int cis_resize_f32_bwd(const float* ddst, int32_t N, int32_t OH, int32_t OW, int32_t C, int32_t H, int32_t W, float* dsrc, int32_t method,
+                       int32_t align_corners, cis_stream_t stream) {
+  const int rc = resize_f32_args("cis_resize_f32_bwd: bad method, align_corners, pointer or size", ddst, dsrc, N, H, W, C, OH, OW, method,
+                                 align_corners);
+  if (rc) return rc;
+  const unsigned g = nblk((size_t)N * H * W * C);
+  if (method == CIS_RESIZE_BILINEAR) {
+    if (align_corners) CIS_LAUNCH((resize_f32_bwd_kernel<false, true>), g, 256, 0, ST, ddst, N, OH, OW, C, H, W, dsrc);
+    else CIS_LAUNCH((resize_f32_bwd_kernel<false, false>), g, 256, 0, ST, ddst, N, OH, OW, C, H, W, dsrc);
+  } else {
+    if (align_corners) CIS_LAUNCH((resize_f32_bwd_kernel<true, true>), g, 256, 0, ST, ddst, N, OH, OW, C, H, W, dsrc);
+    else CIS_LAUNCH((resize_f32_bwd_kernel<true, false>), g, 256, 0, ST, ddst, N, OH, OW, C, H, W, dsrc);
+  }
+  return cis_check_launch("resize_f32_bwd");
 }
 int cis_warp_costvol(const void* c1, int32_t c1p, int32_t c1o, const void* c2, int32_t c2p, int32_t c2o, const float* flow, float fs, int32_t B,
                      int32_t h, int32_t w, int32_t C, void* out, int32_t op, int32_t oo, cis_stream_t stream) {
@@ -1802,6 +1974,19 @@ int cis_pack_generator_input(const float* image, const float* flow, const double
   dim3 grid(nblk((size_t)hw), B);
   CIS_LAUNCH(pack_generator_input_kernel, grid, 256, 0, ST, image, flow, stats, (size_t)hw, (mbf)dst);
   return cis_check_launch("pack_generator_input");
+}
+int cis_flow_standardize(const float* flow, const double* stats, int32_t B, int64_t hw, float* out, cis_stream_t stream) {
+  if (!flow || !stats || !out || B < 1 || hw < 1) return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_standardize: bad pointer or size");
+  CIS_LAUNCH(flow_standardize_kernel, dim3(nblk((size_t)hw), B), 256, 0, ST, flow, stats, (size_t)hw, out);
+  return cis_check_launch("flow_standardize");
+}
+int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stats, int32_t B, int64_t hw, double* scratch, float* dx,
+                             cis_stream_t stream) {
+  if (!y || !dy || !stats || !scratch || !dx || B < 1 || hw < 1)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_standardize_bwd: bad pointer or size");
+  CIS_LAUNCH(flow_standardize_bwd_sums_kernel, dim3(kFlowStdBlocks, B), 256, 0, ST, y, dy, (size_t)hw, scratch);
+  CIS_LAUNCH(flow_standardize_bwd_kernel, dim3(nblk((size_t)hw), B), 256, 0, ST, y, dy, stats, (const double*)scratch, (size_t)hw, dx);
+  return cis_check_launch("flow_standardize_bwd");
 }
 int cis_mask_apply(const float* flow, const float* mask, int32_t B, int64_t hw, void* dst, cis_stream_t stream) {
   CIS_LAUNCH(mask_apply_kernel, nblk((size_t)B * hw), 256, 0, ST, flow, mask, (size_t)B * hw, (mbf)dst);

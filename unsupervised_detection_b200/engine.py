@@ -306,7 +306,8 @@ def wgrad_halo_fits(taps, cout, stride):
     nh = 64 if cout > 64 else ru(cout, 16)
     if ((len(taps) + 1) // 2) * nh > 512 or wh > 256 or hh > 256:
         return False
-    stage = ru(wh * hh * 128, 1024) + 8192
+    # a stage holds the halo and one 8x8-pixel gradient tile per MMA warpgroup when two warpgroups take the two halves of Cout
+    stage = ru(wh * hh * 128, 1024) + 8192 * (2 if WGRAD_HALO_NWG >= 2 and cout > 64 else 1)
     return (200 * 1024) // stage >= 2
 
 
@@ -810,6 +811,9 @@ class ConvLayer(object):
                             continue
                         tl.append(r * k + c)
                         offs.append(((a + pt - r * d) // s, (b + pl - c * d) // s))
+                if not tl:        # k = 1, stride 2: no tap lands on this parity, its input-gradient pixels are zero (see _conv_bwd)
+                    packs.append(dict(a=a, b=b, taps=[], rows_used=False))
+                    continue
                 # value = W[t, ci, co] -> flat (t*cin + ci)*cout + co ; K position (ti, co), row n = ci
                 kmap, Kp = self._kmap(tl, g_chan, self.cin * self.cout, 1)
                 packs.append(dict(a=a, b=b, taps=offs, kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap,
@@ -1068,12 +1072,16 @@ class Builder(object):
             if not hasattr(layer, 'dcat'):
                 layer.dcat = Act(max(s.N for s in srcs), H, W, cin8, self.device, chanmap=layer.in_chanmap, name=layer.name + '.dcat')
             tgt, acc = layer.dcat, False
+        if not acc and any(not pk['taps'] for pk in layer.dgrad_packs):
+            # a parity no tap reaches (k = 1, stride 2) contributes nothing: when accumulating its pixels keep what they hold, on the
+            # first write they are zero -- zero the whole slice (add_slice of 0 sources), the parities with taps then overwrite theirs
+            bp.add('cis_add_slice', tgt.ptr, tgt.pitch, tgt.c_off, tgt.ptr, tgt.pitch, tgt.c_off, nb * H * W, tgt.C8 // 8, 0, 0)
         emitted = []
         for pk in layer.dgrad_packs:
             s = layer.stride
             oh = -(-(H - pk['a']) // s)
             ow = -(-(W - pk['b']) // s)
-            if oh <= 0 or ow <= 0:
+            if oh <= 0 or ow <= 0 or not pk['taps']:
                 continue
             d = CisConv()
             d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = nb, out.H, out.W, oh, ow, 1, 1

@@ -8,9 +8,13 @@ from the registry filled by `set_parameters()` (dict name -> tensor, names as in
 PyTorch is used for memory and the small amount of buffer plumbing only; there is no CPU fallback: without the CUDA library (or on CPU
 tensors) the calls raise.
 
-Gradients: generator_net, recover_net, ModelPWCNet.predict_from_img_pairs, charbonnier_loss, cost_volume(_r) and dense_image_warp are
-torch.autograd Functions (first order only) when an input or one of the parameter tensors the call reads requires grad; the parameters
-then receive gradients under their variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain
+The layer primitives of models/utils/convolution_utils.py (resize, resize_bilinear, resize_nearest_neighbor, gen_conv, gen_deconv, conv,
+deconv) and flow_utils.preprocess_flow_batch are here too, for building variants of the two networks: each conv call is one ConvLayer
+of the engine in a runner of its own (_LayerRunner), the resizes and the flow standardisation are stand-alone fp32 kernels.
+
+Gradients: generator_net, recover_net, ModelPWCNet.predict_from_img_pairs, charbonnier_loss, cost_volume(_r), dense_image_warp and the
+layer primitives are torch.autograd Functions (first order only) when an input or one of the parameter tensors the call reads requires
+grad; the parameters then receive gradients under their variable names.  The backward runs the engine's backward kernels (data / weight gradients, BN chain
 rule, resize transposes, the PWC-Net warp + cost-volume and transposed-conv backward) and the backward kernels of the three stand-alone
 ops.  A call that needs no gradient runs exactly the forward-only path.  train_op is an optimiser update and has nothing to differentiate.
 The training step (step_graph.py) still treats PWC-Net as frozen, as the reference does.
@@ -23,7 +27,7 @@ import torch
 from torch.autograd.function import once_differentiable
 
 from .. import _lib
-from ..engine import Act, Builder, ParamStore, Plan
+from ..engine import Act, Builder, ConvLayer, ParamStore, Plan, ru
 from .nets import GeneratorNet, RecoverNet
 
 _PARAMS = {}
@@ -280,6 +284,67 @@ class _PWCRunner(_NetRunner):
         for a, d in ((self.i1, self.dimg1), (self.i2, self.dimg2)):      # image + 0.5 (adapt_x): unit derivative
             g = a.get_grad()
             P.add('cis_cast_bf16_to_f32', g.ptr, npix, g.pitch, 0, 3, d.data_ptr())
+        return P
+
+
+class _LayerRunner(_NetRunner):
+    """One layer primitive of convolution_utils.py on a fixed input shape: f32 -> bf16 pack of the input, an optional pre-op ('nn2x':
+    NN x2 with align_corners, gen_deconv; 'bilinear': the legacy resize to `size`, deconv), then one ConvLayer -- bias, inference BN
+    folded into the weights (gen_conv), fused activation -- that writes the bf16 Act its activation derivative reads and the fp32 output
+    the call returns.  spec = (kind, k, cout, stride, rate, act, pre, size, name); kind 'gen' = gen_conv parameters
+    <name>/kernel|bias|gamma|beta, 'conv' = <name>/weights|biases."""
+    MODE, SEED, INPUT_GRADS = 'L', 'dout', ('dx',)
+
+    def __init__(self, B, H, W, cin, spec, device):
+        _NetRunner.__init__(self, device)
+        kind, k, cout, stride, rate, act, pre, size, name = spec
+        gen = kind == 'gen'
+        self.layer = ConvLayer(self.store, name, k, cin, cout, stride, rate, act, 0.2, tag='L', bn=gen,
+                               wname='kernel' if gen else 'weights', bname='bias' if gen else 'biases')
+        self.store.finalize(False)
+        f32 = self.bld.f32
+        self.B, self.H, self.W, self.cin = B, H, W, cin
+        # the input is staged in a buffer padded to the bf16 Act's 8-channel pitch, so one cast kernel packs it; padding stays zero
+        self.x_pad = f32(B, H, W, ru(cin, 8))
+        self.x = self.x_pad[..., :cin]
+        # dependency 'L': the backward plan emits the conv's data gradient (through the pre-op) into x8.grad
+        self.x8 = self.bld.new_act(B, H, W, cin, name='x8', dep={'L'})
+        self.bld.fwd.add('cis_cast_f32_to_bf16', self.x_pad.data_ptr(), self.x_pad.numel(), self.x8.ptr)
+        src = self.x8
+        if pre == 'nn2x':
+            src = self.bld.upsample_nn2x(src)
+        elif pre == 'bilinear':
+            src = self.bld.resize_bilinear(src, size[0], size[1])
+        self.outf = f32(B, -(-src.H // stride), -(-src.W // stride), cout)
+        self.out = self.bld.conv(self.layer, [src], outf=self.outf)
+        self.finish([self.layer])
+
+    def run(self, x):
+        self.x.copy_(x)
+        self.bld.fwd.run()
+        self.runs += 1
+        return self.outf.clone()
+
+    def __call__(self, x, params):
+        self.load(params)
+        return self.run(x)
+
+    def _plan_seed(self):
+        f32 = self.bld.f32
+        B, OH, OW, cout = self.outf.shape
+        self.dout_pad = f32(B, OH, OW, ru(cout, 8))
+        self.dout = self.dout_pad[..., :cout]
+        self.dx = f32(self.B, self.H, self.W, self.cin)
+        g = self.out.get_grad()
+        seed = Plan('seed_L')
+        seed.add('cis_cast_f32_to_bf16', self.dout_pad.data_ptr(), self.dout_pad.numel(), g.ptr)
+        return seed, [self.out]
+
+    def _plan_inputs(self):
+        assert self.x8.grad_written.get('L'), "layer backward did not reach the input's data gradient"
+        g = self.x8.get_grad()
+        P = Plan('inputs_L')
+        P.add('cis_cast_bf16_to_f32', g.ptr, self.B * self.H * self.W, g.pitch, 0, self.cin, self.dx.data_ptr())
         return P
 
 
@@ -616,3 +681,228 @@ class _DenseImageWarpFn(torch.autograd.Function):
                   _ptr(scratch), _ptr(dflow), _stream())
         ctx.act = ctx.flow = None
         return tuple(g.to(dt) if g is not None else None for g, dt in zip((dimage, dflow), ctx.dtypes))
+
+
+# ------------------------------------------------------------------------------------------- convolution_utils.py layer primitives
+def elu(x):
+    """tf.nn.elu.  Passed as the `activation` of gen_conv / conv it is fused into the conv epilogue (ACT_ELU)."""
+    return torch.nn.functional.elu(x)
+
+
+def leaky_relu(x, alpha=0.2):
+    """tf.nn.leaky_relu (alpha = 0.2, TF's default).  Passed as an `activation` it is fused into the conv epilogue (ACT_LEAKY, 0.2)."""
+    return torch.nn.functional.leaky_relu(x, alpha)
+
+
+def identity(x):
+    """tf.identity.  Passed as an `activation` the conv has no activation (ACT_NONE)."""
+    return x
+
+
+_FUSED_ACTS = ((elu, _lib.ACT_ELU), (leaky_relu, _lib.ACT_LEAKY), (identity, _lib.ACT_NONE))
+LAYER_SUPPORTED = ("square kernels k = 1..7, stride 1 or 2, rate 1..16 with stride 1, padding 'SAME', any Cin >= 1 and Cout >= 1 "
+                   "(Cout <= 256 when a gradient is needed)")
+
+
+def _unsupported(fn, what):
+    raise NotImplementedError('%s: %s is not supported; the supported set is %s' % (fn, what, LAYER_SUPPORTED))
+
+
+def _square(fn, v, what):
+    """int or a pair of equal ints (tf.layers accepts both) -> int."""
+    if isinstance(v, (list, tuple)):
+        if len(v) != 2 or v[0] != v[1]:
+            _unsupported(fn, 'non-square %s %r' % (what, tuple(v)))
+        v = v[0]
+    if isinstance(v, bool) or int(v) != v:
+        raise ValueError('%s: %s must be an integer; got %r' % (fn, what, v))
+    return int(v)
+
+
+def _size(fn, size):
+    if size is None or len(size) != 2 or any(isinstance(v, bool) or int(v) != v or int(v) < 1 for v in size):
+        raise ValueError('%s: size must be two integers >= 1; got %r' % (fn, size))
+    return int(size[0]), int(size[1])
+
+
+def _layer(fn, x, kind, k, cout, stride, rate, padding, activation, name, pre=None, size=None, params=None):
+    """Validate one layer call, run it on its _LayerRunner (forward-only plan, or _NetFn when a gradient is needed), apply a non-fused
+    activation with torch."""
+    if x.dim() != 4:
+        raise ValueError('%s: expects an NHWC tensor; got shape %s' % (fn, tuple(x.shape)))
+    B, H, W, cin = (int(v) for v in x.shape)
+    k, stride, rate = _square(fn, k, 'kernel size'), _square(fn, stride, 'stride'), _square(fn, rate, 'rate')
+    if not 1 <= k <= 7:
+        _unsupported(fn, 'kernel size %d' % k)
+    if stride not in (1, 2):
+        _unsupported(fn, 'stride %d' % stride)
+    if not 1 <= rate <= 16 or (rate > 1 and stride != 1):
+        _unsupported(fn, 'rate %d with stride %d' % (rate, stride))
+    if str(padding).upper() != 'SAME':
+        _unsupported(fn, 'padding %r' % (padding,))
+    if cout < 1 or cin < 1:
+        raise ValueError('%s: %d input and %d output channels' % (fn, cin, cout))
+    act = next((a for f, a in _FUSED_ACTS if activation is f), None)
+    _check_cuda(x)
+    sc = str(name).rstrip('/')
+    spec = (kind, k, int(cout), stride, rate, _lib.ACT_NONE if act is None else act, pre, size, sc)
+    key = (B, H, W, cin) + spec + (str(x.device),)
+    make = lambda: _LayerRunner(B, H, W, cin, spec, x.device)
+    r = _runner('layer', key, make)
+    names, pvals = _param_inputs(r, params)
+    for (n, shape, _, _, _), t in zip(r.store.entries, pvals):
+        if tuple(t.shape) != shape:
+            raise ValueError('%s: parameter %s has shape %s, the call needs %s' % (fn, n, tuple(t.shape), shape))
+    if not _needs_grad([x] + pvals):
+        y = r(x, params)
+    else:
+        if cout > 256:
+            _unsupported(fn, 'a gradient with Cout %d' % cout)
+        lease = _lease('layer', key, make)
+        try:
+            y = _NetFn.apply(lease, names, 1, x, *pvals)
+        except BaseException:
+            lease.release()
+            raise
+    return y if act is not None else activation(y)
+
+
+def gen_conv(x, cnum, ksize, stride=1, rate=1, name='conv', padding='SAME', activation=elu, training=True, kernel_initializer=None,
+             params=None):
+    """convolution_utils.py:26-53: conv2d SAME + bias -> inference BN (gamma * x / sqrt(1 + 1e-3) + beta, folded into the weights) ->
+    activation.  Parameters <name>/kernel [k,k,Cin,cnum], <name>/bias, <name>/gamma, <name>/beta (name='MaskNet/conv1' reads the
+    generator's conv1).  x: fp32 NHWC cuda tensor -> fp32 [B, ceil(H/stride), ceil(W/stride), cnum]; bf16 activations inside, fp32
+    gradients w.r.t. x and the four parameters.  elu / leaky_relu / identity are fused; any other callable is applied to the output."""
+    return _layer('gen_conv', x, 'gen', ksize, cnum, stride, rate, padding, activation, name, params=params)
+
+
+def gen_deconv(x, cnum, name='upsample', padding='SAME', training=True, params=None):
+    """convolution_utils.py:55-75: nearest-neighbour x2 (align_corners=True), then a 3x3 gen_conv with ELU.  Parameters
+    <name>/kernel|bias|gamma|beta (the internal names of MaskNet/conv13_upsample; checkpoint/tf_names.py maps them to TF's
+    <name>/<name>_conv/...).  -> fp32 [B, 2H, 2W, cnum]."""
+    return _layer('gen_deconv', x, 'gen', 3, cnum, 1, 1, padding, elu, name, pre='nn2x', params=params)
+
+
+def conv(inputs, name, shape, stride, reuse=None, training=True, activation=leaky_relu, init_w=None, init_b=None, params=None):
+    """convolution_utils.py:77-85: tf.nn.conv2d SAME + bias + activation.  shape = [k, k, Cin, Cout]; parameters <name>/weights
+    (`shape`) and <name>/biases [Cout]."""
+    shape = [int(v) for v in shape]
+    if len(shape) != 4:
+        raise ValueError('conv: shape must be [k, k, Cin, Cout]; got %r' % (shape,))
+    if shape[0] != shape[1]:
+        _unsupported('conv', 'non-square kernel %dx%d' % (shape[0], shape[1]))
+    if inputs.dim() == 4 and shape[2] != inputs.shape[-1]:
+        raise ValueError('conv: shape[2] = %d but the input has %d channels' % (shape[2], inputs.shape[-1]))
+    return _layer('conv', inputs, 'conv', shape[0], shape[3], stride, 1, 'SAME', activation, name, params=params)
+
+
+def deconv(inputs, size, name, shape, reuse=None, training=True, activation=leaky_relu, params=None):
+    """convolution_utils.py:87-90: legacy bilinear resize (tf.image.resize_images, align_corners=False) to `size` = [h, w], then conv
+    with stride 1.  Parameters <name>/weights (`shape`) and <name>/biases."""
+    shape = [int(v) for v in shape]
+    if len(shape) != 4:
+        raise ValueError('deconv: shape must be [k, k, Cin, Cout]; got %r' % (shape,))
+    if shape[0] != shape[1]:
+        _unsupported('deconv', 'non-square kernel %dx%d' % (shape[0], shape[1]))
+    if inputs.dim() == 4 and shape[2] != inputs.shape[-1]:
+        raise ValueError('deconv: shape[2] = %d but the input has %d channels' % (shape[2], inputs.shape[-1]))
+    return _layer('deconv', inputs, 'conv', shape[0], shape[3], 1, 1, 'SAME', activation, name, pre='bilinear',
+                  size=_size('deconv', size), params=params)
+
+
+def resize_bilinear(x, size, align_corners=False, name=None):
+    """tf.image.resize_bilinear (TF 1.13, no half-pixel centres) on fp32 NHWC: step (in-1)/(out-1) with align_corners and out > 1, else
+    in/out; lo = floor(d * step), hi = min(lo + 1, in - 1).  Any sizes, up or down.  Differentiable w.r.t. x (a deterministic gather)."""
+    return _resize('resize_bilinear', x, size, _lib.RESIZE_BILINEAR, align_corners)
+
+
+def resize_nearest_neighbor(x, size, align_corners=False, name=None):
+    """tf.image.resize_nearest_neighbor (TF 1.13) on fp32 NHWC: source index roundf(d * step) with align_corners, floor(d * step)
+    without, clamped to in - 1.  Any sizes.  Differentiable w.r.t. x (a deterministic gather)."""
+    return _resize('resize_nearest_neighbor', x, size, _lib.RESIZE_NEAREST, align_corners)
+
+
+def resize(x, scale=2, to_shape=None, align_corners=True, dynamic=False, func=resize_bilinear, name='resize'):
+    """convolution_utils.py:4-24: func(x, [int(H * scale), int(W * scale)] or to_shape[:2], align_corners=align_corners); any callable
+    with that signature runs as it is."""
+    size = [int(x.shape[1] * scale), int(x.shape[2] * scale)] if to_shape is None else [to_shape[0], to_shape[1]]
+    return func(x, size, align_corners=align_corners)
+
+
+def _resize(fn, x, size, method, align_corners):
+    if x.dim() != 4:
+        raise ValueError('%s: expects an NHWC tensor; got shape %s' % (fn, tuple(x.shape)))
+    oh, ow = _size(fn, size)
+    _check_cuda(x)
+    ac = 1 if align_corners else 0
+    if _needs_grad([x]):
+        return _ResizeFn.apply(x, oh, ow, method, ac)
+    return _resize_fwd(x, oh, ow, method, ac)
+
+
+def _resize_fwd(x, oh, ow, method, ac):
+    N, H, W, C = x.shape
+    xs = x.contiguous().float()
+    out = torch.empty(N, oh, ow, C, dtype=torch.float32, device=x.device)
+    _lib.call('cis_resize_f32', xs.data_ptr(), N, H, W, C, out.data_ptr(), oh, ow, method, ac, _stream())
+    return out
+
+
+class _ResizeFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, oh, ow, method, ac):
+        ctx.meta = (tuple(x.shape), x.dtype, oh, ow, method, ac)
+        return _resize_fwd(x, oh, ow, method, ac)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        (N, H, W, C), dt, oh, ow, method, ac = ctx.meta
+        d = dout.contiguous().float()
+        dx = torch.empty(N, H, W, C, dtype=torch.float32, device=d.device)
+        _lib.call('cis_resize_f32_bwd', d.data_ptr(), N, oh, ow, C, H, W, dx.data_ptr(), method, ac, _stream())
+        return dx.to(dt), None, None, None, None
+
+
+# ---------------------------------------------------------------------------------------------------------- flow_utils.py
+def preprocess_flow_batch(flow):
+    """flow_utils.py:5-12: (flow - mean) / sqrt(variance) per sample and channel over H x W (population variance, no epsilon) for fp32
+    [B,H,W,2] flows -- the standardisation in front of generator_net.  Differentiable w.r.t. flow: dx = (g - mean(g) - y mean(g y)) / sigma
+    with fixed-order reductions (bit-identical run to run)."""
+    if flow.dim() != 4 or flow.shape[-1] != 2:
+        raise ValueError('preprocess_flow_batch: expects a [B,H,W,2] flow; got shape %s' % (tuple(flow.shape),))
+    _check_cuda(flow)
+    if _needs_grad([flow]):
+        return _FlowStdFn.apply(flow)
+    return _flow_std_fwd(flow)[0]
+
+
+def _flow_std_fwd(flow):
+    B, H, W, _ = flow.shape
+    f = flow.contiguous().float()
+    stats = torch.zeros(B, 4, dtype=torch.float64, device=f.device)
+    out = torch.empty_like(f)
+    _lib.call('cis_flow_stats', f.data_ptr(), B, H * W, stats.data_ptr(), _stream())
+    _lib.call('cis_flow_standardize', f.data_ptr(), stats.data_ptr(), B, H * W, out.data_ptr(), _stream())
+    return out, stats
+
+
+class _FlowStdFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, flow):
+        out, stats = _flow_std_fwd(flow)
+        ctx.y, ctx.stats, ctx.dtype = out, stats, flow.dtype
+        return out.clone()
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dout):
+        y, stats = ctx.y, ctx.stats
+        B, H, W, _ = y.shape
+        d = dout.contiguous().float()
+        scratch = torch.empty(B * 256, dtype=torch.float64, device=d.device)
+        dx = torch.empty_like(y)
+        _lib.call('cis_flow_standardize_bwd', y.data_ptr(), d.data_ptr(), stats.data_ptr(), B, H * W, scratch.data_ptr(), dx.data_ptr(),
+                  _stream())
+        ctx.y = ctx.stats = None
+        return dx.to(ctx.dtype)

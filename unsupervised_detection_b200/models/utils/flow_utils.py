@@ -1,7 +1,13 @@
 """Flow visualisation for the TensorBoard images (reference models/utils/flow_utils.py:14-109): the Middlebury colour code
 (Baker et al., "A Database and Evaluation Methodology for Optical Flow") as used by `flow_to_image_tf`.  Host side, numpy;
-the device path never calls this."""
+the device path never calls this.  `preprocess_flow_batch` (flow_utils.py:5-12) is the device call of ..functional."""
 import numpy as np
+
+
+def preprocess_flow_batch(flow):
+    """Function-level API of the reference (flow_utils.py:5-12); see models/functional.py."""
+    from .. import functional
+    return functional.preprocess_flow_batch(flow)
 
 # (segment length, channel that ramps, ramp direction, channel held at 255): R->Y->G->C->B->M->R
 _SEGMENTS = ((15, 1, +1, 0), (6, 0, -1, 1), (4, 2, +1, 1), (11, 1, -1, 2), (13, 0, +1, 2), (6, 2, -1, 0))
