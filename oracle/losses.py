@@ -31,8 +31,6 @@ def resize_inputs(image_384, flow_384, h, w, flow_normalizer=80.0):
 def adversarial_losses(image, flow, p, cbn=0.5, epsilon=75.0, global_batch=None):
     """adversarial_learner.py:99-204 given the resized image [B,H,W,3] and normalised flow [B,H,W,2].
     `global_batch` = config.batch_size used in num_pixels (defaults to the local batch)."""
-    b, h, w, _ = image.shape
-    gb = global_batch or b
     m = generator_net(image, preprocess_flow_batch(flow), p)          # :101-105
     mc = 1.0 - m                                                      # :107
     flow_masked = flow * (1.0 - m)                                    # :109
@@ -40,17 +38,32 @@ def adversarial_losses(image, flow, p, cbn=0.5, epsilon=75.0, global_batch=None)
     pred = recover_net(image, flow_masked, m, p)                      # :114
     pred_c = recover_net(image, flow_compl, mc, p)                    # :120
     pred_i = recover_net(image, torch.zeros_like(flow), torch.ones_like(m), p)  # :127
+    out = dict(masks=m, pred=pred, pred_c=pred_c, pred_i=pred_i)
+    out.update(loss_head(flow, m, pred, pred_c, pred_i, cbn, epsilon, global_batch))
+    return out
+
+
+def loss_head(flow, mask, pred, pred_c, pred_i, cbn=0.5, epsilon=75.0, global_batch=None):
+    """adversarial_learner.py:141-204 from the networks' outputs on: flow [B,H,W,2], mask [B,H,W,1] and the three recovered
+    flows [B,H,W,2] -> the loss scalars, the per-sample terms, and `sums` [B,5] = the per-sample Charbonnier sums in the order
+    the step graph accumulates them: {rec, rec_c, prior, den - epsilon, den_c - epsilon}.  Runs in the dtype of its inputs."""
+    b, h, w, _ = flow.shape
+    gb = global_batch or b
+    m = mask
+    mc = 1.0 - m                                                      # :107
     rec = charbonnier_loss(flow, pred, m, cbn)                        # :144
     rec_c = charbonnier_loss(flow, pred_c, mc, cbn)                   # :149
-    prior = charbonnier_loss(flow, pred_i, torch.ones_like(flow), cbn).sum()   # :161-165
+    prior_b = charbonnier_loss(flow, pred_i, torch.ones_like(flow), cbn)
+    prior = prior_b.sum()                                             # :161-165
     recover_loss = (rec.sum() + rec_c.sum() + prior) / float(w * h * gb)        # :167-172
-    den = charbonnier_loss(flow, pred_i, m, cbn) + epsilon            # :179-182
+    den_s = charbonnier_loss(flow, pred_i, m, cbn)
+    den = den_s + epsilon                                             # :179-182
     rr = (1.0 - rec / den).sum() / gb                                 # :183-184 (mean over the global batch)
-    den_c = charbonnier_loss(flow, pred_i, mc, cbn) + epsilon         # :186-189
+    den_cs = charbonnier_loss(flow, pred_i, mc, cbn)
+    den_c = den_cs + epsilon                                          # :186-189
     rr_c = (1.0 - rec_c / den_c).sum() / gb                           # :190-191
-    out = dict(generator=rr + rr_c, recover=recover_loss, red_rate=rr, red_rate_compl=rr_c,
-               masks=m, pred=pred, pred_c=pred_c, pred_i=pred_i, rec=rec, rec_c=rec_c, den=den, den_c=den_c)
-    return out
+    return dict(generator=rr + rr_c, recover=recover_loss, red_rate=rr, red_rate_compl=rr_c, rec=rec, rec_c=rec_c, den=den,
+                den_c=den_c, sums=torch.stack([rec, rec_c, prior_b, den_s, den_cs], dim=1))
 
 
 def clip_or_noise(grads, clip=0.2, can_change=False, gen=None):
