@@ -115,14 +115,11 @@ WGH_CASES = [CASES[0], CASES[1], CASES[2], CASES[4], CASES[6], CASES[7], CASES[1
 
 
 @pytest.mark.parametrize('case', WGH_CASES, ids=lambda c: 'k%d_d%d_c%s_o%d' % (c['k'], c.get('dil', 1), '+'.join(map(str, c['cins'])), c['cout']))
-def test_conv_engine_halo_wgrad(case):
+def test_conv_engine_halo_wgrad(case, monkeypatch):
     """CisWgrad.tma = 2 (engine.WGRAD_HALO): swapped, halo-resident weight gradient; same tolerance as the default kernels."""
     from unsupervised_detection_b200 import engine
-    engine.WGRAD_HALO = True
-    try:
-        r = run_conv_case(**case)
-    finally:
-        engine.WGRAD_HALO = False
+    monkeypatch.setattr(engine, 'WGRAD_HALO', True)     # restored afterwards: later tests plan with the configured default
+    r = run_conv_case(**case)
     assert r['dw_err'] <= 2 ** -7 * r['dw_ref'] + 1e-3, r
     assert r['db_err'] <= 2 ** -7 * r['db_ref'] + 1e-3, r
     if 'dgamma_err' in r:

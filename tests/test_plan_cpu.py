@@ -5,6 +5,7 @@ import collections
 
 import pytest
 
+import plan_digest
 from unsupervised_detection_b200 import engine
 from unsupervised_detection_b200.step_graph import CISGraph
 
@@ -156,3 +157,19 @@ def test_param_job_tables_follow_the_device_side_block_mapping(graph):
                 seen.add(j.kind)
             assert first == total
     assert seen == {JOB_PACK, JOB_PACK_TILED, JOB_UNPACK, JOB_BN_FOLD, JOB_BN_CHAIN}
+
+
+def test_plan_digest_is_stable_across_builds():
+    """Two builds of the same graph and of the same layer runner give the same canonical plans (tests/plan_digest.py): the check
+    that a change to the plan builders leaves every launch, pointer target and packed table as it was relies on it."""
+    from unsupervised_detection_b200.models import functional as F
+    spec = ('gen', 1, 16, 2, 1, engine.ACT_ELU, None, None, 'Net/l')       # stride-2 1x1: tapless output parities
+    digests = []
+    for _ in range(2):
+        with plan_digest.filled_uninitialized():
+            g = CISGraph(64, 96, 1, device='cpu', pwc_hw=(128, 192))
+            r = F._LayerRunner(2, 37, 53, 20, spec, 'cpu')
+            r.ensure_backward()
+        digests.append((plan_digest.digest(plan_digest.graph_plans(g)), plan_digest.digest(plan_digest.runner_plans(r))))
+    assert digests[0] == digests[1]
+    assert any(line.startswith('cis_conv_wgrad') for line in digests[0][0])

@@ -50,7 +50,7 @@ def test_every_pwcnet_layer_has_a_weight_gradient(runner):
     dws = collections.Counter(p for p, _, _ in jobs)
     for L in r.layers:
         base = s.ptr(L.wkey, 'grad')
-        assert getattr(L, 'dgrad_used', False) or getattr(L, 'tr_dgrad', None) is not None, L.name   # data gradient emitted
+        assert L.dgrad_used or L.tr_dgrad is not None, L.name                       # data gradient emitted
         if L.transposed:
             assert dws[base] == 4, L.name                                             # one job per output parity
             assert all(lay == 1 | (L.cin << 8) for p, _, lay in jobs if p == base)  # [kh,kw,Cout,Cin] slot: n stride Cin
@@ -122,13 +122,11 @@ def test_step_graph_keeps_pwcnet_frozen():
     g = CISGraph(128, 192, 1, device='cpu', with_pwc=True)
     assert not g.pwc.trainable and all(L.tag == '' for L in g.pwc.all_layers())
     for L in g.pwc.all_layers():
-        assert not hasattr(L, 'dwp') and getattr(L, 'tr_dgrad', None) is None and L.dgrad_packs is None and not hasattr(L, 'ncalls')
+        assert L.wg_kmap is None and L.dwp is None and L.tr_dgrad is None and L.dgrad_packs is None and L.ncalls == 0
     # no backward launch of the recover / generator steps reads a PWC-Net operand or level buffer
     pwc = {t.data_ptr() for t in g.pwc.level_buf.values()}
     for L in g.pwc.all_layers():
-        pwc |= {t.data_ptr() for t in (getattr(L, 'fwd_tiles', None), L.fwd_pack if isinstance(L.fwd_pack, torch.Tensor) else None)
-                if t is not None}
-        pwc |= {pk[k].data_ptr() for pk in getattr(L, 'tr_packs', []) for k in ('w', 'wt') if pk.get(k) is not None}
+        pwc |= {t.data_ptr() for pk in [L.fwd_pack] + (L.tr_packs or []) if pk is not None for t in (pk.w, pk.wt) if t is not None}
     assert set(g.bwd) == {'R', 'G'}
     for plan in g.bwd.values():
         for op in plan.ops:

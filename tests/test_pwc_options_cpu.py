@@ -2,11 +2,11 @@
 layout, launch plans, the public ModelPWCNet(name, options) class and the option checks.  The numerical checks live in
 test_pwc_options_gpu.py."""
 import collections
-import ctypes
 
 import pytest
 import torch
 
+import plan_digest
 import pwc_options_ref as REF
 from oracle import params as OP
 from unsupervised_detection_b200 import engine
@@ -145,40 +145,18 @@ def test_default_range_keeps_the_range_free_entry_points():
     assert not any(n.endswith('_r') for n in _names(r.bld.fwd) + _names(r.bwd))
 
 
-def _plain(v):
-    """A launch argument without its addresses: ctypes structures field by field, pointer fields dropped."""
-    if isinstance(v, ctypes._Pointer) or type(v).__name__ == 'CArgObject':
-        v = v._obj
-    if isinstance(v, ctypes.Structure):
-        return tuple((f, _plain(getattr(v, f))) for f, t in v._fields_ if t is not ctypes.c_void_p)
-    if isinstance(v, ctypes.Array):
-        return tuple(_plain(x) for x in v)
-    return v
-
-
-def _plan_args(plan):
-    """(entry point, arguments) of every launch, the address arguments (void* in the C prototype) left out."""
-    from unsupervised_detection_b200._lib import _PROTOS
-    out = []
-    for op in plan.ops:
-        if op[0] is None or op[2] not in _PROTOS:
-            continue
-        out.append((op[2], tuple(_plain(a) for a, t in zip(op[1], _PROTOS[op[2]]) if t is not ctypes.c_void_p)))
-    return out
-
-
 def test_none_and_an_explicit_copy_of_the_defaults_give_the_same_plans():
-    a = F._PWCRunner(1, 128, 192, 'cpu', 'pwcnet', trainable=True)
-    b = F._PWCRunner(1, 128, 192, 'cpu', 'pwcnet', trainable=True, options=dict(MP._DEFAULT_PWCNET_TEST_OPTIONS))
-    a.ensure_backward()
-    b.ensure_backward()
-    assert a.net.options == b.net.options == MP.normalize_options(None)
-    assert _plan_args(a.bld.fwd) == _plan_args(b.bld.fwd)
-    assert _plan_args(a.bwd) == _plan_args(b.bwd)
     from unsupervised_detection_b200.step_graph import CISGraph
-    g1 = CISGraph(128, 192, 1, device='cpu', with_pwc=True)
-    g2 = CISGraph(128, 192, 1, device='cpu', with_pwc=True, pwc_options=dict(MP._DEFAULT_PWCNET_TEST_OPTIONS))
-    assert _plan_args(g1.bld.fwd) == _plan_args(g2.bld.fwd)
+    with plan_digest.filled_uninitialized():
+        a = F._PWCRunner(1, 128, 192, 'cpu', 'pwcnet', trainable=True)
+        b = F._PWCRunner(1, 128, 192, 'cpu', 'pwcnet', trainable=True, options=dict(MP._DEFAULT_PWCNET_TEST_OPTIONS))
+        a.ensure_backward()
+        b.ensure_backward()
+        g1 = CISGraph(128, 192, 1, device='cpu', with_pwc=True)
+        g2 = CISGraph(128, 192, 1, device='cpu', with_pwc=True, pwc_options=dict(MP._DEFAULT_PWCNET_TEST_OPTIONS))
+    assert a.net.options == b.net.options == MP.normalize_options(None)
+    assert plan_digest.digest(plan_digest.runner_plans(a)) == plan_digest.digest(plan_digest.runner_plans(b))
+    assert plan_digest.digest([('fwd', g1.bld.fwd)]) == plan_digest.digest([('fwd', g2.bld.fwd)])
 
 
 def test_step_graph_takes_the_options():

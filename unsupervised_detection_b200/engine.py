@@ -5,6 +5,7 @@ step and backward for the generator step -- that are then replayed (optionally i
 PyTorch only owns device memory and streams here; there is no autograd and no torch compute on the hot path.
 """
 import ctypes as C
+import dataclasses
 import os
 
 import numpy as np
@@ -207,6 +208,7 @@ class Act(object):
         self.device = device
         self.gen_rows = None     # batch rows processed by the generator-step backward (2B of 3B)
         self.grad_buf = None     # set: the gradient is the same channel slice of this buffer (views of one zeroed, accumulated buffer)
+        self._owner = None       # alias(): the Act whose gradient this view shares
 
     @property
     def ptr(self):
@@ -227,7 +229,7 @@ class Act(object):
         return a
 
     def get_grad(self):
-        if getattr(self, '_owner', None) is not None:
+        if self._owner is not None:
             return self._owner.get_grad()
         if self.grad is None:
             self.grad = Act(self.N, self.H, self.W, self.C, self.device, buf=self.grad_buf, c_off=self.c_off if self.grad_buf is not None else 0,
@@ -251,6 +253,31 @@ def _fill_srcs(d, srcs):
     d.nsrc = len(srcs)
     for i, s in enumerate(srcs):
         d.src[i] = s.src()
+
+
+def conv_desc(N, H, W, OH, OW, stride, taps, srcs, pk, out, out_ch=None, bias=None, act=ACT_NONE, alpha=0.0, grid=None, add_pre=False,
+              outf=None, outf_ch=0):
+    """A gather-kernel CisConv (setup_halo / setup_halo_s2 may move it to the halo kernel): the N x H x W concat of `srcs` (CisSrc)
+    through `taps` at `stride` -> OH x OW, with the row pack of Pack `pk`, bias and activation, into the Act `out` (out_ch channels,
+    default its padded width; add_pre: added to what `out` holds) and the fp32 tensor `outf`.  grid = (DH, DW, step, oa, ob): output
+    pixel (oh, ow) is pixel (step * oh + oa, step * ow + ob) of a DH x DW map (an output-parity launch); default the OH x OW map."""
+    d = CisConv()
+    d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = N, H, W, OH, OW, stride, stride
+    _fill_taps(d, taps)
+    d.nsrc = len(srcs)
+    for i, s in enumerate(srcs):
+        d.src[i] = s
+    d.wpack, d.K_pad, d.BN, d.n_tiles = pk.w.data_ptr(), pk.K_pad, pk.BN, pk.n_tiles
+    d.bias, d.act, d.alpha = bias, act, alpha
+    d.DH, d.DW, step, d.oa, d.ob = grid or (OH, OW, 1, 0, 0)
+    d.osh = d.osw = step
+    if out is not None:
+        d.out, d.out_pitch, d.out_coff, d.out_ch = out.ptr, out.pitch, out.c_off, out.C8 if out_ch is None else out_ch
+        if add_pre:
+            d.add_pre, d.add_pre_pitch, d.add_pre_coff = out.ptr, out.pitch, out.c_off
+    if outf is not None:
+        d.outf, d.outf_pitch, d.outf_coff, d.outf_ch = outf.data_ptr(), outf.shape[-1], 0, outf_ch or outf.shape[-1]
+    return d
 
 
 def pick_bn(cout, cap=None):
@@ -644,6 +671,45 @@ class ParamStore(object):
         return sum(e[2] for e in self.entries)
 
 
+@dataclasses.dataclass(eq=False)
+class Pack:
+    """One packed bf16 weight operand of a conv layer.  a, b: output parity of a parity launch; taps: its (dy, dx) offsets (forward
+    operand: the tap indices, in its tiled copy's order); kmap: packed K position -> flat weight offset; w: row pack [rows][K_pad] of
+    the gather kernel; nmap: row -> output channel (None = identity); wt: tiled copy of the halo kernel, allocated when the first launch
+    goes there, wt_kmap its kmap if the tap order differs; rows_used: None until a launch is placed (rows packed), False while only halo
+    launches read the operand; wg_splits / dwp: per-mode split count and fp32 slices of the parity's weight gradient (transposed conv)."""
+    a: int = 0
+    b: int = 0
+    taps: list = dataclasses.field(default_factory=list)
+    kmap: torch.Tensor = None
+    K_pad: int = 0
+    rows: int = 0
+    BN: int = 0
+    n_tiles: int = 0
+    nmap: torch.Tensor = None
+    w: torch.Tensor = None
+    wt: torch.Tensor = None
+    wt_kmap: torch.Tensor = None
+    rows_used: bool = None
+    wg_splits: dict = dataclasses.field(default_factory=dict)
+    dwp: torch.Tensor = None
+
+    def __getitem__(self, field):       # read access by field name, as for the pack dicts this record replaced
+        return getattr(self, field)
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _parity_taps(k, s, d, pt, pl, a, b):
+    """Taps of a k x k conv (stride s, dilation d, pt / pl rows / columns of padding in front) that connect input pixels of parity
+    (a, b) to output pixels: input (s y + a, s x + b) meets output (y + dy, x + dx) through tap r * k + c.  -> (indices, offsets)."""
+    rows = [r for r in range(k) if (a + pt - r * d) % s == 0]
+    cols = [c for c in range(k) if (b + pl - c * d) % s == 0]
+    return [r * k + c for r in rows for c in cols], [((a + pt - r * d) // s, (b + pl - c * d) // s) for r in rows for c in cols]
+
+
 class ConvLayer(object):
     """One conv layer's static data: parameter views, packed bf16 operands (forward and data-gradient orientation),
     the fp32 packed weight-gradient buffer and the channel maps that tie packed K positions to HWIO indices."""
@@ -665,9 +731,26 @@ class ConvLayer(object):
         if bn:
             store.declare('%s/gamma' % name, (cout,))
             store.declare('%s/beta' % name, (cout,))
-        self.fwd_pack = None
-        self.dgrad_packs = None
         self.device = store.device
+        # set up by the first launch that needs them
+        self.in_chanmap = None          # packed input position -> input channel
+        self.fwd_kmap, self.K_pad = None, 0            # forward K layout: packed K position -> flat HWIO offset (setup_fwd)
+        self.fwd_pack = None            # Pack of the forward operand (setup_fwd)
+        self.tr_packs = None            # transposed conv: the four output-parity Packs of the forward (setup_transposed)
+        self.dgrad_packs = None         # data gradient: one Pack per input parity (setup_dgrad)
+        self.tr_dgrad = None            # transposed conv: the Pack of the data gradient (setup_transposed_dgrad)
+        self.dgrad_used = False         # a data-gradient launch was emitted
+        self.w_eff = self.b_eff = self.db_eff = None     # BN: folded weights and bias, gradient of the folded bias
+        self.ncalls = 0                 # forward calls with a backward (the siamese PWC-Net feature pyramid runs twice)
+        self.colpart, self.col_blocks = None, {}         # bias-gradient partials of every call, their block count per mode
+        self.tr_planes = None           # transposed conv: the output gradient split into its four output-parity planes
+        self.dcat = None                # gradient of a multi-source input (the virtual concat)
+        # weight gradient (setup_wgrad): kernel path and packed K layout; per mode the split count of the fp32 slice buffers
+        self.wg_tma = self.wg_halo = False
+        self.wg_kmap, self.wg_K_pad = None, 0
+        self.dwp, self.wg_splits = None, {}
+        self.dwp_hi, self.wg_splits_hi = {}, {}   # Cout > 128: output channels [g0, g0 + 128), g0 >= 128, in launches of their own
+        self.wgrad_modes = set()
 
     # ---- packed operands -------------------------------------------------------------------------------------
     def _kmap(self, taps_idx, chanmap, per_tap_stride, chan_stride):
@@ -682,6 +765,9 @@ class ConvLayer(object):
             km[ti * m:(ti + 1) * m] = v
         return torch.from_numpy(km).to(self.device), Kp
 
+    def _rows(self, rows, K_pad):
+        return torch.zeros(rows, K_pad, dtype=torch.bfloat16, device=self.device)
+
     def setup_fwd(self, chanmap):
         """chanmap: packed input position -> original input channel (or -1)."""
         assert max(chanmap) == self.cin - 1, (self.name, max(chanmap), self.cin)
@@ -689,9 +775,9 @@ class ConvLayer(object):
         kk = self.k * self.k
         if self.transposed:
             raise RuntimeError('use setup_transposed')
-        kmap, Kp = self._kmap(range(kk), chanmap, self.cin * self.cout, self.cout)
-        self.fwd_kmap, self.K_pad = kmap, Kp
-        self.fwd_pack = torch.zeros(self.npad, Kp, dtype=torch.bfloat16, device=self.device)
+        self.fwd_kmap, self.K_pad = self._kmap(range(kk), chanmap, self.cin * self.cout, self.cout)
+        self.fwd_pack = Pack(taps=list(range(kk)), kmap=self.fwd_kmap, K_pad=self.K_pad, rows=self.npad, BN=self.BN, n_tiles=self.n_tiles,
+                             w=self._rows(self.npad, self.K_pad))
         if self.bn:
             self.w_eff = torch.zeros(kk * self.cin * self.cout, dtype=torch.float32, device=self.device)
             self.b_eff = torch.zeros(self.npad, dtype=torch.float32, device=self.device)
@@ -701,17 +787,21 @@ class ConvLayer(object):
         nchunks = -(-cin8 // 64)
         return torch.zeros(n_tiles * nchunks * ntaps * BN * 64, dtype=torch.bfloat16, device=self.device)
 
-    def fwd_tiles_buf(self, tap_order=None):
-        """Pre-swizzled tile-major copy of the forward operand (halo kernel).  tap_order: the phase-major tap permutation of a
-        stride-2 layer (setup_halo_s2); the tiles then follow that order."""
-        if getattr(self, 'fwd_tiles', None) is None:
-            self.fwd_tiles = self._alloc_tiles(self.k * self.k, len(self.in_chanmap), self.BN, self.n_tiles)
-            self.fwd_tiles_kmap = self.fwd_kmap
-            if tap_order is not None:
-                self.fwd_tiles_kmap, _ = self._kmap(list(tap_order), self.in_chanmap, self.cin * self.cout, self.cout)
-            self.fwd_tap_order = tap_order
-        assert getattr(self, 'fwd_tap_order', None) == tap_order, self.name
-        return self.fwd_tiles
+    def place(self, d, pk, taps, dil, kch, order=None):
+        """Put launch `d` of operand `pk` (kch channels along K) on the halo kernel when setup_halo takes it -- or setup_halo_s2 already
+        did and gave the phase-major tap `order` -- reading the operand's pre-swizzled tiled copy, else leave it on the gather kernel."""
+        if order is None and not setup_halo(d, taps, dil, pk.n_tiles):
+            pk.rows_used = True
+            return
+        if pk.wt is None:
+            pk.wt = self._alloc_tiles(len(taps), kch, pk.BN, pk.n_tiles)
+            if order is not None:
+                pk.taps = list(order)
+                pk.wt_kmap, _ = self._kmap(pk.taps, self.in_chanmap, self.cin * self.cout, self.cout)
+        assert order is None or pk.taps == list(order), self.name
+        d.wpack = pk.wt.data_ptr()
+        if pk.rows_used is None:
+            pk.rows_used = False
 
     def w_src_ptr(self):
         return self.w_eff.data_ptr() if self.bn else self.store.ptr(self.wkey)
@@ -725,35 +815,20 @@ class ConvLayer(object):
         if self.bn:
             plan.add('cis_bn_fold', s.ptr(self.wkey), s.ptr(self.bkey), s.ptr(self.name + '/gamma'), s.ptr(self.name + '/beta'),
                      self.k * self.k * self.cin * self.cout, self.cout, self.w_eff.data_ptr(), self.b_eff.data_ptr())
-        if self.fwd_pack is not None:
-            if self.transposed:
-                for pk in self.tr_packs:
-                    if pk.get('wt') is not None:
-                        plan.add('cis_pack_weights_tiled', self.w_src_ptr(), pk['kmap'].data_ptr(), len(self.in_chanmap), len(pk['taps']),
-                                 self.n_tiles, self.BN, self.cout, self.cin, None, pk['wt'].data_ptr())
-                    if pk.get('rows_used', True):
-                        plan.add('cis_pack_weights', self.w_src_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], self.npad, self.cout, self.cin,
-                                 None, pk['w'].data_ptr())
-            else:
-                if getattr(self, 'fwd_tiles', None) is not None:
-                    plan.add('cis_pack_weights_tiled', self.w_src_ptr(), self.fwd_tiles_kmap.data_ptr(), len(self.in_chanmap), self.k * self.k,
-                             self.n_tiles, self.BN, self.cout, 1, None, self.fwd_tiles.data_ptr())
-                if getattr(self, 'fwd_rows_used', True):
-                    plan.add('cis_pack_weights', self.w_src_ptr(), self.fwd_kmap.data_ptr(), self.K_pad, self.npad, self.cout, 1,
-                             None, self.fwd_pack.data_ptr())
-        if dgrad and getattr(self, 'tr_dgrad', None) is not None:
-            pk = self.tr_dgrad       # transposed conv: W[kh,kw,Cout,Cin] read as the HWIO weights of a stride-2 conv Cout -> Cin
-            plan.add('cis_pack_weights', self.w_src_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], pk['rows'], len(self.in_chanmap), 1,
-                     pk['nmap'].data_ptr(), pk['w'].data_ptr())
-        if dgrad and self.dgrad_packs:
-            cout8 = ru(self.cout, 8)
-            for pk in self.dgrad_packs:
-                if pk.get('wt') is not None:
-                    plan.add('cis_pack_weights_tiled', self.w_src_ptr(), pk['kmap'].data_ptr(), cout8, len(pk['taps']), pk['n_tiles'], pk['BN'],
-                             len(self.in_chanmap), self.cout, pk['nmap'].data_ptr(), pk['wt'].data_ptr())
-                if pk.get('rows_used', True):
-                    plan.add('cis_pack_weights', self.w_src_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], pk['rows'], len(self.in_chanmap),
-                             self.cout, pk['nmap'].data_ptr(), pk['w'].data_ptr())
+        cin8 = len(self.in_chanmap or ())
+        # (pack, channels along K, output channels, n stride of the weights): a transposed conv's [kh,kw,Cout,Cin] weights have n stride
+        # Cin; its data gradient reads them as the HWIO weights of a stride-2 conv Cout -> Cin
+        packs = [(pk, cin8, self.cout, self.cin) for pk in self.tr_packs or ()]
+        packs += [(pk, cin8, self.cout, 1) for pk in (self.fwd_pack,) if pk is not None]
+        if dgrad:
+            packs += [(pk, cin8, cin8, 1) for pk in (self.tr_dgrad,) if pk is not None]
+            packs += [(pk, ru(self.cout, 8), cin8, self.cout) for pk in self.dgrad_packs or ()]
+        for pk, kch, nch, sn in packs:
+            if pk.wt is not None:
+                plan.add('cis_pack_weights_tiled', self.w_src_ptr(), (pk.kmap if pk.wt_kmap is None else pk.wt_kmap).data_ptr(), kch,
+                         len(pk.taps), pk.n_tiles, pk.BN, nch, sn, _ptr(pk.nmap), pk.wt.data_ptr())
+            if pk.rows_used is not False:
+                plan.add('cis_pack_weights', self.w_src_ptr(), pk.kmap.data_ptr(), pk.K_pad, pk.rows, nch, sn, _ptr(pk.nmap), pk.w.data_ptr())
 
     def plan_finalize(self, bp, mode):
         """Fixed-order sum of the private split-K slices of the packed fp32 weight gradient -> HWIO slot of the flat gradient
@@ -762,17 +837,17 @@ class ConvLayer(object):
         if self.transposed:
             # four output-parity weight gradients, each into its own taps of the [kh,kw,Cout,Cin] slot (n stride Cin: layout bits 8+); the
             # first also sums the bias partials of the whole output gradient
-            for q, pk in enumerate(p for p in getattr(self, 'tr_packs', []) if mode in p.get('wg_splits', {})):
-                bp.add('cis_unpack_wgrad', pk['dwp'].data_ptr(), pk['kmap'].data_ptr(), pk['K_pad'], self.cout, pk['wg_splits'][mode],
+            for q, pk in enumerate(p for p in self.tr_packs or () if mode in p.wg_splits):
+                bp.add('cis_unpack_wgrad', pk.dwp.data_ptr(), pk.kmap.data_ptr(), pk.K_pad, self.cout, pk.wg_splits[mode],
                        s.ptr(self.wkey, 'grad'), self.colpart.data_ptr() if q == 0 else None, self.col_blocks[mode] if q == 0 else 0,
                        self.cout if q == 0 else 0, s.ptr(self.bkey, 'grad') if q == 0 else None, 1 | (self.cin << 8))
             return
-        if not hasattr(self, 'dwp') or mode not in getattr(self, 'wg_splits', {}):
+        if mode not in self.wg_splits:
             return
         bp.add('cis_unpack_wgrad', self.dwp.data_ptr(), self.wg_kmap.data_ptr(), self.wg_K_pad, min(128, self.cout), self.wg_splits[mode],
                s.ptr(self.wkey, 'grad'), self.colpart.data_ptr(), self.col_blocks[mode], self.cout,
                (self.db_eff.data_ptr() if self.bn else s.ptr(self.bkey, 'grad')), 0 if self.wg_halo else 1)
-        for g0, buf in sorted(getattr(self, 'dwp_hi', {}).items()):     # output channels >= 128: dw shifted by g0 (n stride 1)
+        for g0, buf in sorted(self.dwp_hi.items()):     # output channels >= 128: dw shifted by g0 (n stride 1)
             if (mode, g0) in self.wg_splits_hi:
                 bp.add('cis_unpack_wgrad', buf.data_ptr(), self.wg_kmap.data_ptr(), self.wg_K_pad, min(128, self.cout - g0),
                        self.wg_splits_hi[(mode, g0)], s.ptr(self.wkey, 'grad') + 4 * g0, None, 0, 0, None, 0 if self.wg_halo else 1)
@@ -786,6 +861,28 @@ class ConvLayer(object):
         pt, _ = same_pad(H, self.k, self.stride, self.dil)
         pl, _ = same_pad(W, self.k, self.stride, self.dil)
         return [(r * self.dil - pt, c * self.dil - pl) for r in range(self.k) for c in range(self.k)], pt, pl
+
+    def setup_wgrad(self, taps, srcs):
+        """Weight-gradient kernel path and packed K layout, once: the TMA operand path (8x8 pixel tiles) for stride-1 layers whose concat
+        sources are 64-channel aligned, the halo-resident kernel where it fits; both lay the K columns out per tap in 64-channel groups
+        and exclude thin inputs (the per-tap 64-channel padding would waste the loads).  Else the gather kernel on the forward K layout."""
+        if self.wg_kmap is not None:
+            return
+        cin8 = len(self.in_chanmap)
+        aligned = all(s.C8 % 64 == 0 for s in srcs[:-1])
+        self.wg_tma = bool(WGRAD_TMA and self.stride == 1 and cin8 >= 32 and aligned)
+        self.wg_halo = bool(WGRAD_HALO and cin8 >= WGRAD_HALO_MIN_CH and wgrad_halo_fits(taps, self.cout, self.stride) and aligned)
+        if not (self.wg_tma or self.wg_halo):
+            self.wg_K_pad, self.wg_kmap = self.K_pad, self.fwd_kmap
+            return
+        nch64 = -(-cin8 // 64)
+        self.wg_K_pad = ru(self.k * self.k * nch64 * 64, 128)
+        km = np.full(self.wg_K_pad, -1, dtype=np.int32)
+        fk = self.fwd_kmap.cpu().numpy()
+        for t in range(self.k * self.k):
+            for pos in range(cin8):
+                km[(t * nch64 + pos // 64) * 64 + pos % 64] = fk[t * cin8 + pos]
+        self.wg_kmap = torch.from_numpy(km).to(self.device)
 
     def setup_dgrad(self, H, W):
         """Packed weights for the data gradient on an input of size HxW: one launch for stride 1, four output-parity
@@ -802,22 +899,13 @@ class ConvLayer(object):
         packs = []
         for a in range(s):
             for b in range(s):
-                tl, offs = [], []
-                for r in range(k):
-                    if (a + pt - r * d) % s:
-                        continue
-                    for c in range(k):
-                        if (b + pl - c * d) % s:
-                            continue
-                        tl.append(r * k + c)
-                        offs.append(((a + pt - r * d) // s, (b + pl - c * d) // s))
+                tl, offs = _parity_taps(k, s, d, pt, pl, a, b)
                 if not tl:        # k = 1, stride 2: no tap lands on this parity, its input-gradient pixels are zero (see _conv_bwd)
-                    packs.append(dict(a=a, b=b, taps=[], rows_used=False))
+                    packs.append(Pack(a=a, b=b, rows_used=False))
                     continue
                 # value = W[t, ci, co] -> flat (t*cin + ci)*cout + co ; K position (ti, co), row n = ci
                 kmap, Kp = self._kmap(tl, g_chan, self.cin * self.cout, 1)
-                packs.append(dict(a=a, b=b, taps=offs, kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap,
-                                  w=torch.zeros(rows, Kp, dtype=torch.bfloat16, device=self.device)))
+                packs.append(Pack(a=a, b=b, taps=offs, kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap, w=self._rows(rows, Kp)))
         self.dgrad_packs = packs
 
     def setup_transposed(self, chanmap):
@@ -827,26 +915,17 @@ class ConvLayer(object):
         packs = []
         for a in range(2):
             for b in range(2):
-                tl, offs = [], []
-                for ky in range(4):
-                    if (a + 1 - ky) % 2:
-                        continue
-                    for kx in range(4):
-                        if (b + 1 - kx) % 2:
-                            continue
-                        tl.append(ky * 4 + kx)
-                        offs.append(((a + 1 - ky) // 2, (b + 1 - kx) // 2))
+                tl, offs = _parity_taps(4, 2, 1, 1, 1, a, b)       # output pixel 2y + a reads input y + dy through tap ky = a + 1 - 2 dy
                 # kernel [kh,kw,Cout,Cin]: flat ((t*Cout + co)*Cin + ci) ; K position (ti, ci), row n = co (stride Cin)
                 kmap, Kp = self._kmap(tl, chanmap, self.cout * self.cin, 1)
-                packs.append(dict(a=a, b=b, taps=offs, kmap=kmap, K_pad=Kp,
-                                  w=torch.zeros(self.npad, Kp, dtype=torch.bfloat16, device=self.device)))
+                packs.append(Pack(a=a, b=b, taps=offs, kmap=kmap, K_pad=Kp, rows=self.npad, BN=self.BN, n_tiles=self.n_tiles,
+                                  w=self._rows(self.npad, Kp)))
         self.tr_packs = packs
-        self.fwd_pack = True
 
     def setup_transposed_dgrad(self, g_pos):
         """Data gradient of the transposed conv: dx[y, x, ci] = sum dy[2y + ky - 1, 2x + kx - 1, co] * W[ky, kx, co, ci], a 4x4 stride-2
         forward conv of the output gradient.  g_pos: position of output channel co inside the gradient's 8-channel chunk."""
-        if getattr(self, 'tr_dgrad', None) is not None:
+        if self.tr_dgrad is not None:
             return
         g_chan = [-1] * 8
         for co in range(self.cout):
@@ -857,8 +936,30 @@ class ConvLayer(object):
         # K position (tap, gradient channel co) -> flat ((t*Cout + co)*Cin), row n -> + ci
         kmap, Kp = self._kmap(range(16), g_chan, self.cout * self.cin, self.cin)
         nmap = torch.tensor(list(self.in_chanmap) + [-1] * (rows - cin8), dtype=torch.int32, device=self.device)
-        self.tr_dgrad = dict(kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap,
-                             w=torch.zeros(rows, Kp, dtype=torch.bfloat16, device=self.device))
+        taps = [(r - 1, c - 1) for r in range(4) for c in range(4)]      # TF 'SAME' k4 s2: one row / column of padding in front
+        self.tr_dgrad = Pack(taps=taps, kmap=kmap, K_pad=Kp, rows=rows, BN=bn_, n_tiles=nt, nmap=nmap, w=self._rows(rows, Kp))
+
+
+def _concat_bwd(bp, mode, srcs, g, nb, OH, OW):
+    """Gradient g (nb x OH x OW) of the concat of `srcs` brought to OH x OW -> the sources' gradient slices, ONE launch (the fused
+    resize-concat transpose: slices the channels, folds the replicas of batch-broadcast sources, accumulates where a gradient exists)."""
+    want = [1 if mode in s.dep else 0 for s in srcs]
+    if not any(want):
+        return
+    garr, acc = [], []
+    for s, w in zip(srcs, want):
+        if w:
+            sg = s.get_grad()
+            garr.append(CisSrc(sg.ptr, sg.pitch, sg.c_off, s.C8 // 8, s.n_mod))
+            acc.append(1 if s.grad_written.get(mode) else 0)
+            s.grad_written[mode] = True
+        else:
+            garr.append(CisSrc(None, 8, 0, s.C8 // 8, s.n_mod))
+            acc.append(0)
+    ga = (CisSrc * len(srcs))(*garr)
+    wa, aa = (C.c_int32 * len(srcs))(*want), (C.c_int32 * len(srcs))(*acc)
+    bp.keep += [ga, wa, aa]
+    bp.add('cis_resize_concat_bf16_bwd', g.ptr, g.pitch, g.c_off, nb, OH, OW, ga, wa, aa, len(srcs), srcs[0].H, srcs[0].W)
 
 
 # ================================================================================================ graph builder
@@ -886,6 +987,23 @@ class Builder(object):
     def f32(self, *shape):
         return self.hold(torch.zeros(*shape, dtype=torch.float32, device=self.device))
 
+    def _launch(self, plan, d, flops, lane=0):
+        """One conv launch, split-K where it pays."""
+        setup_splitk(d, self.device, plan.keep)
+        plan.keep.append(d)
+        plan.add('cis_conv_igemm', C.byref(d), flops=flops, lane=lane)
+
+    def _launch_parities(self, plan, emitted, lane):
+        """Output-parity launches [(CisConv, flops)]: ONE grouped launch on `lane` when merge_parity_launches takes them, else one
+        launch each on lane 0."""
+        grp = merge_parity_launches([d for d, _ in emitted])
+        if grp is None:
+            for d, fl in emitted:
+                self._launch(plan, d, fl)
+            return
+        plan.keep.append(grp)
+        plan.add('cis_conv_igemm', C.byref(grp), flops=sum(f for _, f in emitted), lane=lane)
+
     def conv(self, layer, srcs, out=None, post_add=None, addf=None, outf=None, outf_ch=0, mode=0, want_bf16=True, name=None,
              plan=None, out_rows=None, grad_out=None):
         """y = act(conv(concat(srcs)) + bias [+ addf]) [+ post_add]; returns the output Act.  grad_out: the Act whose gradient is this
@@ -893,7 +1011,8 @@ class Builder(object):
         plan = plan or self.fwd
         if MATERIALIZE_MISALIGNED_CONCAT and len(srcs) > 1 and layer.tag and layer.stride == 1 and \
                 any(s.C8 % 64 for s in srcs[:-1]):
-            srcs = [self.concat(srcs, name=layer.name + '.cat')]
+            # materialised concat: the virtual one is not 64-channel aligned, so the TMA operand paths would not apply
+            srcs = [self.resize_concat(srcs, name=layer.name + '.cat')]
         s0 = srcs[0]
         N = out_rows or max(s.N for s in srcs)
         H, W = s0.H, s0.W
@@ -920,17 +1039,8 @@ class Builder(object):
             if gr:
                 out.gen_rows = gr[0]
         taps, _, _ = layer.fwd_taps(H, W)
-        d = CisConv()
-        d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = N, H, W, OH, OW, layer.stride, layer.stride
-        _fill_taps(d, taps)
-        _fill_srcs(d, srcs)
-        d.wpack, d.K_pad, d.BN, d.n_tiles = layer.fwd_pack.data_ptr(), layer.K_pad, layer.BN, layer.n_tiles
-        d.bias, d.act, d.alpha = layer.bias_ptr(), layer.act, layer.alpha
-        d.DH, d.DW, d.osh, d.osw, d.oa, d.ob = OH, OW, 1, 1, 0, 0
-        if out is not None:
-            d.out, d.out_pitch, d.out_coff, d.out_ch = out.ptr, out.pitch, out.c_off, out.C8
-        if outf is not None:
-            d.outf, d.outf_pitch, d.outf_coff, d.outf_ch = outf.data_ptr(), outf.shape[-1], 0, outf_ch or outf.shape[-1]
+        d = conv_desc(N, H, W, OH, OW, layer.stride, taps, [s.src() for s in srcs], layer.fwd_pack, out, bias=layer.bias_ptr(),
+                      act=layer.act, alpha=layer.alpha, outf=outf, outf_ch=outf_ch)
         if addf is not None:
             d.addf_pre, d.addf_pitch, d.addf_coff = addf.data_ptr(), addf.shape[-1], 0
             if outf is None:
@@ -939,23 +1049,14 @@ class Builder(object):
             d.add_post, d.add_post_pitch, d.add_post_coff = post_add.ptr, post_add.pitch, post_add.c_off
         d.mode = mode
         order = setup_halo_s2(d, taps, layer.n_tiles) if (layer.stride == 2 and layer.dil == 1) else None
-        if order is not None:
-            d.wpack = layer.fwd_tiles_buf(order).data_ptr()
-            layer.fwd_rows_used = getattr(layer, 'fwd_rows_used', False)
-        elif layer.stride == 1 and setup_halo(d, taps, layer.dil, layer.n_tiles):
-            d.wpack = layer.fwd_tiles_buf().data_ptr()
-            layer.fwd_rows_used = getattr(layer, 'fwd_rows_used', False)
-        else:
-            layer.fwd_rows_used = True
-        setup_splitk(d, self.device, plan.keep)
-        plan.keep.append(d)
+        layer.place(d, layer.fwd_pack, taps, layer.dil, len(layer.in_chanmap), order)
         plan.keep += [srcs, out, outf, addf, post_add, layer]
-        plan.add('cis_conv_igemm', C.byref(d), flops=2.0 * N * OH * OW * layer.k * layer.k * layer.cin * layer.cout, lane=self.lane)
+        self._launch(plan, d, 2.0 * N * OH * OW * layer.k * layer.k * layer.cin * layer.cout, lane=self.lane)
         if layer.tag:
             # call index: a layer run more than once in one graph (the siamese PWC-Net feature pyramid) gets one range of weight-gradient
             # slices per call, summed by the one un-pack of plan_finalize
-            call = layer.ncalls = getattr(layer, 'ncalls', 0) + 1
-            self.tape.append(lambda bp, m, L=layer, S=list(srcs), O=out, P=post_add, K=call - 1, GO=grad_out:
+            layer.ncalls += 1
+            self.tape.append(lambda bp, m, L=layer, S=list(srcs), O=out, P=post_add, K=layer.ncalls - 1, GO=grad_out:
                              self._conv_bwd(bp, m, L, S, O, P, K, GO))
         return out
 
@@ -974,15 +1075,13 @@ class Builder(object):
             bp.add('cis_add_slice', pg.ptr, pg.pitch, pg.c_off, G.ptr, G.pitch, G.c_off, npix, G.C8 // 8, 1,
                    1 if post_add.grad_written.get(mode) else 0)
             post_add.grad_written[mode] = True
-        ncalls = getattr(layer, 'ncalls', 1)
+        ncalls = layer.ncalls
         if layer.tag == mode:
             chunks = -(-layer.cout // 8)
             ppb = (256 // chunks) * COLSUM_PIX                      # pixels per colsum block (P pixel lanes x COLSUM_PIX pixels each)
-            if not hasattr(layer, 'col_blocks'):
-                layer.col_blocks = {}
             nblk = max(1, min(592, -(-npix // ppb)))
             layer.col_blocks[mode] = nblk * ncalls                 # call k owns the partial blocks [k * nblk, (k + 1) * nblk)
-            if getattr(layer, 'colpart', None) is None:
+            if layer.colpart is None:
                 layer.colpart = torch.empty(592 * ncalls * layer.cout, dtype=torch.float32, device=self.device)
             colpart = layer.colpart.data_ptr() + 4 * call * nblk * layer.cout
         res = (post_add.ptr, post_add.pitch, post_add.c_off) if post_add is not None else (None, 0, 0)
@@ -997,28 +1096,7 @@ class Builder(object):
         H, W = s0.H, s0.W
         taps, _, _ = layer.fwd_taps(H, W)
         if layer.tag == mode:   # weight + bias gradients
-            if not hasattr(layer, 'dwp'):
-                # TMA operand path (8x8 pixel tiles) for stride-1 layers whose concat sources are 64-channel aligned
-                layer.wg_tma = bool(WGRAD_TMA and layer.stride == 1 and len(layer.in_chanmap) >= 32 and
-                                    all(s_.C8 % 64 == 0 for s_ in srcs[:-1]))   # thin inputs: per-tap 64-channel padding would waste the loads
-                # (thin inputs are excluded like for the TMA path: every tap is padded to a 64-channel column group there)
-                layer.wg_halo = bool(WGRAD_HALO and len(layer.in_chanmap) >= WGRAD_HALO_MIN_CH and wgrad_halo_fits(taps, layer.cout, layer.stride) and
-                                     all(s_.C8 % 64 == 0 for s_ in srcs[:-1]))
-                if layer.wg_tma or layer.wg_halo:
-                    cin8 = len(layer.in_chanmap)
-                    nch64 = -(-cin8 // 64)
-                    ncol = layer.k * layer.k * nch64 * 64
-                    layer.wg_K_pad = ru(ncol, 128)
-                    km = np.full(layer.wg_K_pad, -1, dtype=np.int32)
-                    fk = layer.fwd_kmap.cpu().numpy()
-                    for t in range(layer.k * layer.k):
-                        for pos in range(cin8):
-                            km[(t * nch64 + pos // 64) * 64 + pos % 64] = fk[t * cin8 + pos]
-                    layer.wg_kmap = torch.from_numpy(km).to(self.device)
-                else:
-                    layer.wg_K_pad, layer.wg_kmap = layer.K_pad, layer.fwd_kmap
-                layer.dwp, layer.wg_splits = None, {}
-                layer.dwp_hi, layer.wg_splits_hi = {}, {}   # Cout > 128: output channels [g0, g0 + 128), g0 >= 128, in launches of their own
+            layer.setup_wgrad(taps, srcs)
             for g0 in range(0, layer.cout, 128):             # cis_conv_wgrad takes at most 128 output channels
                 gc = min(128, layer.cout - g0)
                 w = CisWgrad()
@@ -1043,19 +1121,19 @@ class Builder(object):
                     assert ncalls == 1 or layer.wg_splits.get(mode) in (None, splits * ncalls), layer.name
                     layer.wg_splits[mode] = splits * ncalls
                     if layer.dwp is None or layer.dwp.numel() < size:
-                        assert not getattr(layer, 'wgrad_modes', None), 'slice buffer must be sized by the first (largest) mode'
+                        assert not layer.wgrad_modes, 'slice buffer must be sized by the first (largest) mode'
                         layer.dwp = torch.empty(max(layer.wg_splits.values()) * gc * layer.wg_K_pad, dtype=torch.float32, device=self.device)
                     buf = layer.dwp
                 else:
                     layer.wg_splits_hi[(mode, g0)] = splits * ncalls
                     if g0 not in layer.dwp_hi or layer.dwp_hi[g0].numel() < size:
-                        assert not getattr(layer, 'wgrad_modes', None), 'slice buffer must be sized by the first (largest) mode'
+                        assert not layer.wgrad_modes, 'slice buffer must be sized by the first (largest) mode'
                         layer.dwp_hi[g0] = torch.empty(size, dtype=torch.float32, device=self.device)
                     buf = layer.dwp_hi[g0]
                 w.dwp = buf.data_ptr() + 4 * call * splits * gc * layer.wg_K_pad
                 bp.keep.append(w)
                 bp.add('cis_conv_wgrad', C.byref(w), flops=2.0 * npix * layer.k * layer.k * layer.cin * gc, lane=1)
-            layer.wgrad_modes = getattr(layer, 'wgrad_modes', set()) | {mode}
+            layer.wgrad_modes.add(mode)
             if not fused_colsum:
                 bp.add('cis_colsum', G.ptr, G.pitch, G.c_off, npix, layer.cout, colpart, nblk, lane=1)
         need = [s for s in srcs if mode in s.dep]
@@ -1069,68 +1147,28 @@ class Builder(object):
             tgt = srcs[0].get_grad()
             acc = bool(srcs[0].grad_written.get(mode))
         else:
-            if not hasattr(layer, 'dcat'):
+            if layer.dcat is None:
                 layer.dcat = Act(max(s.N for s in srcs), H, W, cin8, self.device, chanmap=layer.in_chanmap, name=layer.name + '.dcat')
             tgt, acc = layer.dcat, False
-        if not acc and any(not pk['taps'] for pk in layer.dgrad_packs):
+        if not acc and any(not pk.taps for pk in layer.dgrad_packs):
             # a parity no tap reaches (k = 1, stride 2) contributes nothing: when accumulating its pixels keep what they hold, on the
             # first write they are zero -- zero the whole slice (add_slice of 0 sources), the parities with taps then overwrite theirs
             bp.add('cis_add_slice', tgt.ptr, tgt.pitch, tgt.c_off, tgt.ptr, tgt.pitch, tgt.c_off, nb * H * W, tgt.C8 // 8, 0, 0)
         emitted = []
+        s = layer.stride
         for pk in layer.dgrad_packs:
-            s = layer.stride
-            oh = -(-(H - pk['a']) // s)
-            ow = -(-(W - pk['b']) // s)
-            if oh <= 0 or ow <= 0 or not pk['taps']:
+            oh = -(-(H - pk.a) // s)
+            ow = -(-(W - pk.b) // s)
+            if oh <= 0 or ow <= 0 or not pk.taps:
                 continue
-            d = CisConv()
-            d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = nb, out.H, out.W, oh, ow, 1, 1
-            _fill_taps(d, pk['taps'])
-            d.nsrc = 1
-            d.src[0] = G.src()
-            d.wpack, d.K_pad, d.BN, d.n_tiles = pk['w'].data_ptr(), pk['K_pad'], pk['BN'], pk['n_tiles']
-            d.bias, d.act = None, ACT_NONE
-            d.DH, d.DW, d.osh, d.osw, d.oa, d.ob = H, W, s, s, pk['a'], pk['b']
-            d.out, d.out_pitch, d.out_coff, d.out_ch = tgt.ptr, tgt.pitch, tgt.c_off, tgt.C8
-            if acc:
-                d.add_pre, d.add_pre_pitch, d.add_pre_coff = tgt.ptr, tgt.pitch, tgt.c_off
-            if setup_halo(d, pk['taps'], layer.dil if s == 1 else 1, pk['n_tiles']):
-                if pk.get('wt') is None:
-                    pk['wt'] = layer._alloc_tiles(len(pk['taps']), ru(layer.cout, 8), pk['BN'], pk['n_tiles'])
-                d.wpack = pk['wt'].data_ptr()
-                pk['rows_used'] = pk.get('rows_used', False)
-            else:
-                pk['rows_used'] = True
-            emitted.append((d, 2.0 * nb * oh * ow * len(pk['taps']) * layer.cin * layer.cout))
-        grp = merge_parity_launches([d for d, _ in emitted]) if len(emitted) > 1 else None
-        if grp is not None:
-            bp.keep.append(grp)
-            bp.add('cis_conv_igemm', C.byref(grp), flops=sum(f for _, f in emitted))
-        else:
-            for d, fl in emitted:
-                setup_splitk(d, self.device, bp.keep)
-                bp.keep.append(d)
-                bp.add('cis_conv_igemm', C.byref(d), flops=fl)
+            d = conv_desc(nb, out.H, out.W, oh, ow, 1, pk.taps, [G.src()], pk, tgt, grid=(H, W, s, pk.a, pk.b), add_pre=acc)
+            layer.place(d, pk, pk.taps, layer.dil if s == 1 else 1, ru(layer.cout, 8))
+            emitted.append((d, 2.0 * nb * oh * ow * len(pk.taps) * layer.cin * layer.cout))
+        self._launch_parities(bp, emitted, lane=0)
         if single:
             srcs[0].grad_written[mode] = True
         else:
-            # gradient of the virtual concat -> the sources' gradient slices, ONE launch (same-size case of the fused resize-concat
-            # transpose: slices the channels, folds the replicas of batch-broadcast sources, accumulates where a gradient exists)
-            want = [1 if mode in s_.dep else 0 for s_ in srcs]
-            garr, acc = [], []
-            for s_, w_ in zip(srcs, want):
-                if w_:
-                    sg = s_.get_grad()
-                    garr.append(CisSrc(sg.ptr, sg.pitch, sg.c_off, s_.C8 // 8, s_.n_mod))
-                    acc.append(1 if s_.grad_written.get(mode) else 0)
-                    s_.grad_written[mode] = True
-                else:
-                    garr.append(CisSrc(None, 8, 0, s_.C8 // 8, s_.n_mod))
-                    acc.append(0)
-            ga = (CisSrc * len(srcs))(*garr)
-            wa, aa = (C.c_int32 * len(srcs))(*want), (C.c_int32 * len(srcs))(*acc)
-            bp.keep += [ga, wa, aa]
-            bp.add('cis_resize_concat_bf16_bwd', tgt.ptr, tgt.pitch, 0, nb, H, W, ga, wa, aa, len(srcs), H, W)
+            _concat_bwd(bp, mode, srcs, tgt, nb, H, W)     # the virtual concat's gradient -> the sources' gradient slices
 
     # ---- fused resize + concat: ONE launch brings up to 4 same-resolution sources (batch-broadcast ones included) to OH x OW and lays
     # them side by side in one buffer, ONE launch takes the gradient back (folding the broadcast replicas); replaces a resize launch
@@ -1159,36 +1197,14 @@ class Builder(object):
         def bwd(bp, mode):
             if mode not in cat.dep or not cat.grad_written.get(mode):
                 return
-            g = cat.get_grad()
-            nb = cat.rows(mode)
-            want = [1 if mode in s_.dep else 0 for s_ in srcs]
-            if not any(want):
-                return
-            garr, acc = [], []
-            for s_, w_ in zip(srcs, want):
-                if w_:
-                    sg = s_.get_grad()
-                    garr.append(CisSrc(sg.ptr, sg.pitch, sg.c_off, s_.C8 // 8, s_.n_mod))
-                    acc.append(1 if s_.grad_written.get(mode) else 0)
-                    s_.grad_written[mode] = True
-                else:
-                    garr.append(CisSrc(None, 8, 0, s_.C8 // 8, s_.n_mod))
-                    acc.append(0)
-            ga = (CisSrc * len(srcs))(*garr)
-            wa, aa = (C.c_int32 * len(srcs))(*want), (C.c_int32 * len(srcs))(*acc)
-            bp.keep += [ga, wa, aa]
-            bp.add('cis_resize_concat_bf16_bwd', g.ptr, g.pitch, g.c_off, nb, OH, OW, ga, wa, aa, len(srcs), H, W)
+            _concat_bwd(bp, mode, srcs, cat.get_grad(), cat.rows(mode), OH, OW)
         self.tape.append(bwd)
         return cat
-
-    def concat(self, srcs, name='cat'):
-        """Materialised concat (only where the virtual concat is not 64-channel aligned, so the TMA operand paths apply)."""
-        return self.resize_concat(srcs, name=name)
 
     # ---- transposed conv (PWC-Net up_flow / up_feat)
     def conv_transpose(self, layer, src, out=None, outf=None, plan=None, name=None):
         plan = plan or self.fwd
-        if layer.fwd_pack is None:
+        if layer.tr_packs is None:
             layer.setup_transposed(src.chanmap)
         N, H, W = src.N, src.H, src.W
         if out is None:
@@ -1198,34 +1214,12 @@ class Builder(object):
             self.tape.append(lambda bp, m, L=layer, S=src, O=out: self._conv_transpose_bwd(bp, m, L, S, O))
         emitted = []
         for pk in layer.tr_packs:
-            d = CisConv()
-            d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = N, H, W, H, W, 1, 1
-            _fill_taps(d, pk['taps'])
-            _fill_srcs(d, [src])
-            d.wpack, d.K_pad, d.BN, d.n_tiles = pk['w'].data_ptr(), pk['K_pad'], layer.BN, layer.n_tiles
-            d.bias, d.act = layer.bias_ptr(), ACT_NONE
-            d.DH, d.DW, d.osh, d.osw, d.oa, d.ob = 2 * H, 2 * W, 2, 2, pk['a'], pk['b']
-            d.out, d.out_pitch, d.out_coff, d.out_ch = out.ptr, out.pitch, out.c_off, layer.cout
-            if outf is not None:
-                d.outf, d.outf_pitch, d.outf_coff, d.outf_ch = outf.data_ptr(), outf.shape[-1], 0, layer.cout
-            if setup_halo(d, pk['taps'], 1, layer.n_tiles):
-                if pk.get('wt') is None:
-                    pk['wt'] = layer._alloc_tiles(len(pk['taps']), len(layer.in_chanmap), layer.BN, layer.n_tiles)
-                d.wpack = pk['wt'].data_ptr()
-                pk['rows_used'] = pk.get('rows_used', False)
-            else:
-                pk['rows_used'] = True
-            plan.keep += [src, out, outf, layer]
-            emitted.append((d, 2.0 * N * H * W * len(pk['taps']) * layer.cin * layer.cout))
-        grp = merge_parity_launches([d for d, _ in emitted])
-        if grp is not None:
-            plan.keep.append(grp)
-            plan.add('cis_conv_igemm', C.byref(grp), flops=sum(f for _, f in emitted), lane=self.lane)
-        else:
-            for d, fl in emitted:
-                setup_splitk(d, self.device, plan.keep)
-                plan.keep.append(d)
-                plan.add('cis_conv_igemm', C.byref(d), flops=fl)
+            d = conv_desc(N, H, W, H, W, 1, pk.taps, [src.src()], pk, out, out_ch=layer.cout, bias=layer.bias_ptr(),
+                          grid=(2 * H, 2 * W, 2, pk.a, pk.b), outf=outf, outf_ch=layer.cout)
+            layer.place(d, pk, pk.taps, 1, len(layer.in_chanmap))
+            emitted.append((d, 2.0 * N * H * W * len(pk.taps) * layer.cin * layer.cout))
+        plan.keep += [src, out, outf, layer]
+        self._launch_parities(plan, emitted, lane=self.lane)
         return out
 
     def _conv_transpose_bwd(self, bp, mode, layer, src, out):
@@ -1238,10 +1232,9 @@ class Builder(object):
         N, h, w = src.N, src.H, src.W
         npix = N * h * w
         if layer.tag == mode:
-            if getattr(layer, 'tr_planes', None) is None:
+            if layer.tr_planes is None:
                 layer.tr_planes = torch.zeros(4, N, h, w, 8, dtype=torch.bfloat16, device=self.device)
                 layer.colpart = torch.empty(592 * layer.cout, dtype=torch.float32, device=self.device)
-                layer.col_blocks = {}
             planes = layer.tr_planes
             bp.add('cis_parity_split_bf16', G.ptr, G.pitch, G.c_off, N, h, w, layer.cout, planes.data_ptr(), 8)
             layer.col_blocks[mode] = max(1, min(592, -(-4 * npix // (256 * COLSUM_PIX))))
@@ -1249,38 +1242,26 @@ class Builder(object):
             for q, pk in enumerate(layer.tr_packs):
                 wg = CisWgrad()
                 wg.N, wg.H, wg.W, wg.OH, wg.OW, wg.sh, wg.sw = N, h, w, h, w, 1, 1
-                _fill_taps(wg, pk['taps'])
+                _fill_taps(wg, pk.taps)
                 _fill_srcs(wg, [src])
                 wg.g, wg.g_pitch, wg.g_coff, wg.g_chunks = planes[q].data_ptr(), 8, 0, 1
-                wg.Cout, wg.K_pad, wg.tma = layer.cout, pk['K_pad'], 0
+                wg.Cout, wg.K_pad, wg.tma = layer.cout, pk.K_pad, 0
                 nkb = -(-npix // 64)
-                wg.splits = wgrad_splits(nkb, -(-pk['K_pad'] // 128), layer.cout, pk['K_pad'])
-                pk.setdefault('wg_splits', {})[mode] = wg.splits
-                if pk.get('dwp') is None or pk['dwp'].numel() < wg.splits * layer.cout * pk['K_pad']:
-                    pk['dwp'] = torch.empty(wg.splits * layer.cout * pk['K_pad'], dtype=torch.float32, device=self.device)
-                wg.dwp = pk['dwp'].data_ptr()
+                wg.splits = wgrad_splits(nkb, -(-pk.K_pad // 128), layer.cout, pk.K_pad)
+                pk.wg_splits[mode] = wg.splits
+                if pk.dwp is None or pk.dwp.numel() < wg.splits * layer.cout * pk.K_pad:
+                    pk.dwp = torch.empty(wg.splits * layer.cout * pk.K_pad, dtype=torch.float32, device=self.device)
+                wg.dwp = pk.dwp.data_ptr()
                 bp.keep.append(wg)
-                bp.add('cis_conv_wgrad', C.byref(wg), flops=2.0 * npix * len(pk['taps']) * layer.cin * layer.cout, lane=1)
+                bp.add('cis_conv_wgrad', C.byref(wg), flops=2.0 * npix * len(pk.taps) * layer.cin * layer.cout, lane=1)
         if mode not in src.dep:
             return
         g_pos = G.c_off % 8                  # the gradient's channels inside its 8-channel chunk (up_feat sits behind up_flow)
         layer.setup_transposed_dgrad(g_pos)
-        dg = layer.tr_dgrad
-        tgt = src.get_grad()
-        d = CisConv()
-        d.N, d.H, d.W, d.OH, d.OW, d.sh, d.sw = N, 2 * h, 2 * w, h, w, 2, 2
-        _fill_taps(d, [(r - 1, c - 1) for r in range(4) for c in range(4)])      # TF 'SAME' k4 s2: one row / column of padding in front
-        d.nsrc = 1
-        d.src[0] = CisSrc(G.ptr, G.pitch, G.c_off - g_pos, 1, 0)
-        d.wpack, d.K_pad, d.BN, d.n_tiles = dg['w'].data_ptr(), dg['K_pad'], dg['BN'], dg['n_tiles']
-        d.bias, d.act = None, ACT_NONE
-        d.DH, d.DW, d.osh, d.osw, d.oa, d.ob = h, w, 1, 1, 0, 0
-        d.out, d.out_pitch, d.out_coff, d.out_ch = tgt.ptr, tgt.pitch, tgt.c_off, tgt.C8
-        if src.grad_written.get(mode):
-            d.add_pre, d.add_pre_pitch, d.add_pre_coff = tgt.ptr, tgt.pitch, tgt.c_off
-        setup_splitk(d, self.device, bp.keep)
-        bp.keep.append(d)
-        bp.add('cis_conv_igemm', C.byref(d), flops=2.0 * npix * 16 * layer.cin * layer.cout)
+        dg, tgt = layer.tr_dgrad, src.get_grad()
+        d = conv_desc(N, 2 * h, 2 * w, h, w, 2, dg.taps, [CisSrc(G.ptr, G.pitch, G.c_off - g_pos, 1, 0)], dg, tgt,
+                      add_pre=bool(src.grad_written.get(mode)))
+        self._launch(bp, d, 2.0 * npix * 16 * layer.cin * layer.cout)
         src.grad_written[mode] = True
 
     # ---- resampling ops
@@ -1328,3 +1309,17 @@ class Builder(object):
         for fn in reversed(self.tape):
             fn(bp, mode)
         return bp
+
+    def backward_plan(self, mode, seed, seeds, layers):
+        """The backward Plan of `mode`: the Plan `seed` (the launches that write the gradients of the Acts `seeds`), the reverse tape, a
+        join of the weight-gradient lane, then the fixed-order reduction of the weight-gradient slices and the BN chain rule of `layers`
+        (one cis_param_multi launch per kind)."""
+        full = Plan('bwd_' + mode)
+        full.extend(seed)
+        full.extend(self.build_backward(mode, seeds))
+        full.join()
+        fin = Plan('fin_' + mode)
+        for L in layers:
+            L.plan_finalize(fin, mode)
+        full.extend(fin.batch_param_ops(self.device))
+        return full

@@ -98,23 +98,14 @@ class _NetRunner(object):
 
     def ensure_backward(self):
         """Backward plan: seed (`_plan_seed`) -> the builder's reverse tape -> fixed-order weight-gradient reduction + BN chain rule
-        (one cis_param_multi launch per kind) -> input gradients out of the bf16 input Acts (`_plan_inputs`).  The pack plan is rebuilt
-        with the data-gradient operands the tape needs."""
+        (Builder.backward_plan) -> input gradients out of the bf16 input Acts (`_plan_inputs`).  The pack plan is rebuilt with the
+        data-gradient operands the tape needs."""
         if self.bwd is not None:
             return
         self.store.grad = torch.zeros_like(self.store.flat)
         seed, seeds = self._plan_seed()
-        body = self.bld.build_backward(self.MODE, seeds)
-        fin = Plan('fin')
-        for L in self.layers:
-            L.plan_finalize(fin, self.MODE)
-        full = Plan('bwd_' + self.MODE)
-        full.extend(seed)
-        full.extend(body)
-        full.join()            # weight-gradient lane -> main lane before the packed gradients are unpacked
-        full.extend(fin.batch_param_ops(self.device))
-        full.extend(self._plan_inputs())
-        self.bwd = full
+        self.bwd = self.bld.backward_plan(self.MODE, seed, seeds, self.layers)
+        self.bwd.extend(self._plan_inputs())
         self.pack = Plan('pack')
         for L in self.layers:
             L.plan_pack(self.pack, dgrad=True)

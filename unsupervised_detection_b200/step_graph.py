@@ -128,21 +128,11 @@ class CISGraph(object):
                          self.scalars.data_ptr(), B, H, W, h1, w1, cbn, which, self.dpred.data_ptr(), self.dmask.data_ptr())
                 fg = self.rec.flow1.get_grad()
                 head.add('cis_resize_f32_bwd_to_bf16', self.dpred.data_ptr(), nb, H, W, 2, h1, w1, fg.ptr, fg.pitch)
-                body = bld.build_backward(mode, [self.rec.flow1])
                 store = self.rec_store if mode == 'R' else self.gen_store
                 layers = self.rec.all_layers() if mode == 'R' else self.gen.all_layers()
                 # nothing to zero: every real entry of the flat gradient buffer is overwritten by cis_unpack_wgrad / cis_bn_chain each
                 # step, and its padding slots are never written (they stay at their initial 0, also through the all-reduce)
-                pre = Plan('zero_' + mode)
-                fin = Plan('fin_' + mode)
-                for L in layers:
-                    L.plan_finalize(fin, mode)
-                full = Plan('bwd_' + mode)
-                for pl in (pre, head, body):
-                    full.extend(pl)
-                full.join()            # weight-gradient lane -> main lane before the packed gradients are unpacked
-                full.extend(fin.batch_param_ops(device))
-                self.bwd[mode] = full
+                self.bwd[mode] = bld.backward_plan(mode, head, [self.rec.flow1], layers)
                 ad = Plan('adam_' + mode)
                 if mode == 'G':
                     # can_change branch of train_op (loss_utils.py:18-26)
