@@ -290,6 +290,14 @@ int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stat
 /* ---- mask (x) flow + Charbonnier contextual-information loss (adversarial_learner.py:107-110,141-204) ---- */
 /* recover inputs, batch 3B: [flow*(1-m),1,1-m | flow*m,1,m | 0,0,1,0] -> bf16 [3B,H,W,8] (nets.py:50-53) */
 int cis_mask_apply(const float* flow, const float* mask, int32_t B, int64_t hw, void* dst, cis_stream_t stream);
+/* box occlusions of the recover-net pretraining: mask fp32 [B,H,W,1] = 1 inside one box per sample, 0 elsewhere.  Sample b's box is four
+ * counter-hash draws r_k = hash32(seed ^ D ^ t<<40 ^ g<<2 ^ k), k = 0..3, D = 0x426f784d61736b73, t = step[0] (device int64, read when the
+ * kernel runs: the Adam step counter, so graph replays draw new boxes), g = sample_offset + b (the global sample index under data
+ * parallelism), hash32 = the 64-bit MurmurHash3 finaliser truncated to 32 bits; all modulo operations unsigned 32-bit:
+ * bh = lo_h + r0 % (hi_h-lo_h+1), bw = lo_w + r1 % (hi_w-lo_w+1), y0 = r2 % (H-bh+1), x0 = r3 % (W-bw+1); rows [y0, y0+bh), columns
+ * [x0, x0+bw).  CIS_ERR_BAD_ARG unless 1 <= lo <= hi <= the image side (both axes), 1 <= B <= 65535, sample_offset >= 0. */
+int cis_box_masks(float* mask, int32_t B, int32_t H, int32_t W, int32_t lo_h, int32_t hi_h, int32_t lo_w, int32_t hi_w, int64_t sample_offset,
+                  const long long* step, uint64_t seed, cis_stream_t stream);
 /* stand-alone charbonnier_loss (loss_utils.py:34-51): sums[b] += sum over pixels and C channels of ((gt-pred)^2 + 1e-6)^cbn * mask;
  * mask_c = 1 (one value per pixel) or C (one per element); sums = double [B], zeroed by the caller */
 int cis_charbonnier_sum(const float* gt, const float* pred, const float* mask, int32_t B, int64_t hw, int32_t C, int32_t mask_c, float cbn,

@@ -97,6 +97,7 @@ _PROTOS = {
     'cis_flow_stats': [_p, _i32, _i64, _p],
     'cis_pack_generator_input': [_p, _p, _p, _i32, _i64, _p],
     'cis_mask_apply': [_p, _p, _i32, _i64, _p],
+    'cis_box_masks': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _i64, _p, _u64],
     'cis_charbonnier_sum': [_p, _p, _p, _i32, _i64, _i32, _i32, _f32, _p],
     'cis_cis_loss_fwd': [_p, _p, _p, _i32, _i32, _i32, _i32, _i32, _f32, _p, _p],
     'cis_cis_loss_reduce': [_p, _i32, _i32, _i64, _f32, _p, _p],

@@ -1305,6 +1305,27 @@ __global__ void clip_adam_kernel(float* __restrict__ param, float* __restrict__ 
 __global__ void step_inc_kernel(long long* step) {
   pdl_launch_dependents();
   pdl_wait(); step[0] += 1; }
+// Box occlusions of the recover-net pretraining.  Draw k of sample g at step t = hash32(seed ^ kBoxDomain ^ t<<40 ^ g<<2 ^ k): its own
+// domain constant keeps it apart from the noise branch above, and integer arithmetic only keeps it restatable bit for bit on the host.
+constexpr uint64_t kBoxDomain = 0x426f784d61736b73ULL;   // "BoxMasks"
+__device__ __forceinline__ uint32_t box_draw(unsigned long long seed, long long t, long long g, int k) {
+  return hash32((uint64_t)seed ^ kBoxDomain ^ ((uint64_t)t << 40) ^ ((uint64_t)g << 2) ^ (uint64_t)k);
+}
+__global__ void box_masks_kernel(float* __restrict__ mask, int H, int W, int lo_h, int hi_h, int lo_w, int hi_w, long long sample_offset,
+                                 const long long* __restrict__ step, unsigned long long seed) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t hw = (size_t)H * W;
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= hw) return;
+  const long long t = step[0], g = sample_offset + blockIdx.y;
+  const uint32_t bh = (uint32_t)lo_h + box_draw(seed, t, g, 0) % (uint32_t)(hi_h - lo_h + 1);
+  const uint32_t bw = (uint32_t)lo_w + box_draw(seed, t, g, 1) % (uint32_t)(hi_w - lo_w + 1);
+  const uint32_t y0 = box_draw(seed, t, g, 2) % ((uint32_t)H - bh + 1);
+  const uint32_t x0 = box_draw(seed, t, g, 3) % ((uint32_t)W - bw + 1);
+  const uint32_t y = (uint32_t)(i / W), x = (uint32_t)(i - (size_t)y * W);
+  mask[blockIdx.y * hw + i] = (y - y0 < bh && x - x0 < bw) ? 1.f : 0.f;   // unsigned: y < y0 wraps around and fails the test
+}
 __global__ void abs_sum_kernel(const float* __restrict__ g, size_t n, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
@@ -1991,6 +2012,15 @@ int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stat
 int cis_mask_apply(const float* flow, const float* mask, int32_t B, int64_t hw, void* dst, cis_stream_t stream) {
   CIS_LAUNCH(mask_apply_kernel, nblk((size_t)B * hw), 256, 0, ST, flow, mask, (size_t)B * hw, (mbf)dst);
   return cis_check_launch("mask_apply");
+}
+int cis_box_masks(float* mask, int32_t B, int32_t H, int32_t W, int32_t lo_h, int32_t hi_h, int32_t lo_w, int32_t hi_w, int64_t sample_offset,
+                  const long long* step, uint64_t seed, cis_stream_t stream) {
+  if (!mask || !step || B < 1 || B > 65535 || sample_offset < 0) return cis_set_error(CIS_ERR_BAD_ARG, "cis_box_masks: bad buffer, batch or sample offset");
+  if (lo_h < 1 || lo_w < 1 || hi_h < lo_h || hi_w < lo_w || hi_h > H || hi_w > W)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_box_masks: box sides need 1 <= lo <= hi <= image side");
+  CIS_LAUNCH(box_masks_kernel, dim3(nblk((size_t)H * W), B), 256, 0, ST, mask, H, W, lo_h, hi_h, lo_w, hi_w, (long long)sample_offset, step,
+             (unsigned long long)seed);
+  return cis_check_launch("box_masks");
 }
 int cis_charbonnier_sum(const float* gt, const float* pred, const float* mask, int32_t B, int64_t hw, int32_t C, int32_t mask_c, float cbn,
                         double* sums, cis_stream_t stream) {

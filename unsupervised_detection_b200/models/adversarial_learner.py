@@ -1,7 +1,8 @@
 """AdversarialLearner: the reference's learner surface (models/adversarial_learner.py:18-623) on the CUDA step graph.
 
 Kept API: AdversarialLearner().train(config) / .setup_inference(config, aug_test=False) / .inference(sess) with the same
-result keys (:617-619), plus .step() = one iteration of the loop body (:380-409).  `sess` arguments are accepted and
+result keys (:617-619), plus .step() = one iteration of the loop body (:380-409) and .pretrain_recover(config) = pretraining of the
+recover net on box-shaped occlusions (the pre-training behind --recover_ckpt that the reference's README describes).  `sess` arguments are accepted and
 ignored (there is no tf.Session).  Data parallelism (not in the reference): one process per GPU, the frame-pair batch is
 sharded over ranks and the active network's flat gradient buffer is summed with ONE NCCL all-reduce per step
 (SURVEY.md section 8e); clip / noise test / Adam then run identically on every rank.
@@ -14,7 +15,7 @@ from itertools import count
 import numpy as np
 import torch
 
-from ..step_graph import CISGraph, PWC_H, PWC_W
+from ..step_graph import CISGraph, PWC_H, PWC_W, box_sides
 from .PWCNet import model_pwcnet
 from ..data.synthetic import SyntheticReader
 from .. import params_init
@@ -190,10 +191,25 @@ class AdversarialLearner(object):
             return
         base = 'model.best' if step == 'best' else 'model-%s' % step
         print(" [*] Saving checkpoint to {}/model-{}".format(checkpoint_dir, step))
-        os.makedirs(checkpoint_dir, exist_ok=True)
         params = {k: v.cpu() for k, v in self.graph.export_params().items()}
+        self._write_checkpoint(checkpoint_dir, base, params, self.global_step)
+
+    def save_recover(self, checkpoint_dir, epoch):
+        """The recover net alone, as the reference's recover_saver covers it (adversarial_learner.py:329): `recover-<epoch>` as a TF V2
+        bundle of the FlownetS variables (no global_step, no Adam slots) plus the same tensors as a native `.pt`, and the `checkpoint`
+        state file.  train.py --recover_ckpt=<dir>/recover-<epoch> and a TF recover_saver.restore both read it."""
+        if self.rank != 0:
+            return
+        base = 'recover-%d' % epoch
+        print(" [*] Saving recover net to {}/{}".format(checkpoint_dir, base))
+        params = {k: v.cpu() for k, v in self.graph.rec_store.export().items()}
+        self._write_checkpoint(checkpoint_dir, base, params, None)
+
+    def _write_checkpoint(self, checkpoint_dir, base, params, bundle_step):
+        """<base>.pt + the <base> bundle (global_step in the bundle when bundle_step is not None); old entries beyond max_to_keep=40 go."""
+        os.makedirs(checkpoint_dir, exist_ok=True)
         torch.save({'params': params, 'global_step': self.global_step}, os.path.join(checkpoint_dir, base + '.pt'))
-        ckpt_io.write_bundle(os.path.join(checkpoint_dir, base), ckpt_io.export_params(params, self.global_step))
+        ckpt_io.write_bundle(os.path.join(checkpoint_dir, base), ckpt_io.export_params(params, bundle_step))
         for old in ckpt_io.update_checkpoint_state(checkpoint_dir, base, keep=40):
             for suf in ('.index', '.data-00000-of-00001', '.pt'):
                 fp = os.path.join(checkpoint_dir, old + suf)
@@ -258,6 +274,22 @@ class AdversarialLearner(object):
         if batch is None:
             batch = self.reader.batch(self.local_batch)
         summarize = summarize and step % cfg.summary_freq == 0                 # :391-394 (same decision on every rank)
+        other_grads = self._train_on(mode, batch, next_batch, use_graph, summarize)
+        res = {"global_step": self.global_step, "train_op": mode}
+        fetch = fetch_losses if fetch_losses is not None else (step % cfg.summary_freq == 0)
+        if fetch or summarize:
+            # device -> host read; under data parallelism every rank holds its share of the global-batch losses (each is already
+            # divided by the GLOBAL batch), so one SUM all-reduce of the four scalars gives every rank the true values -- all ranks
+            # take this branch on the same steps
+            L = self.graph.losses(full=summarize, reduce=self._allreduce())
+            res["loss_recover"], res["loss_generator"] = L['recover'], L['generator']
+        if summarize:
+            self._write_step_summary(self.global_step, mode, other_grads, L)   # add_summary(results["summary"], gs), :403
+        return res
+
+    def _train_on(self, mode, batch, next_batch, use_graph, summarize):
+        """Runs train op `mode` on `batch` (host tensors), overlapping the upload of `next_batch`; -> the other net's gradients
+        when `summarize` (the summary pre-pass), else None."""
         g = self.graph
         if use_graph and next_batch is not None and not summarize and PIPELINE:
             # Software pipeline over steps: PWC-Net (frozen, parameter-independent) runs for `next_batch` on a second stream while
@@ -284,17 +316,7 @@ class AdversarialLearner(object):
             g.train_step(mode, allreduce=self._allreduce(), use_graph=use_graph)
             if next_batch is not None:
                 self.prefetch(next_batch)          # overlaps this step's kernels; consumed by the next step() call
-        res = {"global_step": self.global_step, "train_op": mode}
-        fetch = fetch_losses if fetch_losses is not None else (step % cfg.summary_freq == 0)
-        if fetch or summarize:
-            # device -> host read; under data parallelism every rank holds its share of the global-batch losses (each is already
-            # divided by the GLOBAL batch), so one SUM all-reduce of the four scalars gives every rank the true values -- all ranks
-            # take this branch on the same steps
-            L = self.graph.losses(full=summarize, reduce=self._allreduce())
-            res["loss_recover"], res["loss_generator"] = L['recover'], L['generator']
-        if summarize:
-            self._write_step_summary(self.global_step, mode, other_grads, L)   # add_summary(results["summary"], gs), :403
-        return res
+        return other_grads
 
     # ------------------------------------------------------------------------------------------------ summaries
     def collect_summaries(self):
@@ -418,6 +440,82 @@ class AdversarialLearner(object):
             self.min_val_iou = validation_iou
         if epoch_num % self.config.save_freq == 0:
             self.save(sess, self.config.checkpoint_dir, epoch_num)
+
+    # ------------------------------------------------------------------------------------------------ recover-net pretraining
+    def build_pretrain_graph(self):
+        """The recover step of adversarial_learner.py:72-258 with one random box per sample as the mask: PWC-Net -> resize -> box masks ->
+        3x recover -> losses -> train_recover_op.  No generator runs.  config.box_min / box_max = box side range as fractions of the
+        image sides (defaults 0.1 / 0.5)."""
+        cfg = self.config
+        self._init_dist()
+        if cfg.batch_size % self.world:
+            raise ValueError('batch_size must be divisible by the number of ranks')
+        self.local_batch = cfg.batch_size // self.world
+        box = box_sides(getattr(cfg, 'box_min', 0.1), getattr(cfg, 'box_max', 0.5), cfg.img_height, cfg.img_width)
+        self.load_training_data()
+        # sample_offset: sample b of rank r is global sample r * local_batch + b, so a DP job draws the boxes of one GPU running the global batch
+        self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
+                              flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
+                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='boxes', box=box,
+                              sample_offset=self.rank * self.local_batch)
+        self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
+        self._init_params()
+
+    def pretrain_step(self, batch, next_batch=None, fetch_losses=False, use_graph=True):
+        """One pretraining iteration: train_recover_op on `batch` under box masks (one NCCL all-reduce of the recover gradient under
+        torchrun); -> {global_step, loss_recover?, reconstruction_loss?, reconstruction_compl_loss?}.  All ranks must pass the same
+        fetch_losses (the losses are all-reduced)."""
+        self.global_step += 1
+        self._train_on('R', batch, next_batch, use_graph, False)
+        res = {"global_step": self.global_step}
+        if fetch_losses:
+            L = self.graph.losses(full=True, reduce=self._allreduce())
+            res.update(loss_recover=L['recover'], reconstruction_loss=L['reconstruction_loss'],
+                       reconstruction_compl_loss=L['reconstruction_compl_loss'])
+        return res
+
+    def pretrain_recover(self, config):
+        """Pretrains the recover net (scope FlownetS) to inpaint optical flow under box-shaped occlusions, the pre-training the reference's
+        README describes for --recover_ckpt.  num_samples_train / batch_size steps per epoch for max_epochs epochs; every summary_freq
+        steps rank 0 prints the loss and writes the scalars recover / reconstruction_loss / reconstruction_compl_loss; every save_freq
+        epochs and after the last one it saves recover-<epoch> (save_recover).  --flow_ckpt is mandatory, --recover_ckpt gives the
+        starting weights (else the reference's initialisation)."""
+        self.config = config
+        self.build_pretrain_graph()
+        if self.rank == 0:
+            print("Number of recover params: {}".format(self.graph.rec_store.real_count()))
+            print("-------------------------------------")
+            print("Pretraining Recover on box masks, sides {} px (h lo, h hi, w lo, w hi)".format(self.graph.box))
+            print("-------------------------------------")
+        w = self.collect_summaries()
+        steps_per_epoch = self.train_steps_per_epoch
+        batch = self.reader.batch(self.local_batch)
+        for step in count(start=1):
+            start_time = time.time()
+            nxt = self.reader.batch(self.local_batch)
+            fetch = step % config.summary_freq == 0
+            results = self.pretrain_step(batch, next_batch=nxt, fetch_losses=fetch)
+            batch = nxt
+            if fetch and self.rank == 0:
+                epoch = math.ceil(step / steps_per_epoch)
+                print("Epoch: [%2d] [%5d/%5d] time: %4.4f/it loss_recover %4.4f"
+                      % (epoch, step - (epoch - 1) * steps_per_epoch, steps_per_epoch, time.time() - start_time, results["loss_recover"]))
+                if w is not None:
+                    w.add_scalar("recover", results["loss_recover"])
+                    w.add_scalar("reconstruction_loss", results["reconstruction_loss"])
+                    w.add_scalar("reconstruction_compl_loss", results["reconstruction_compl_loss"])
+                    w.flush_step(results["global_step"])
+            if step % steps_per_epoch == 0:
+                epoch = step // steps_per_epoch
+                last = epoch == config.max_epochs
+                if epoch % config.save_freq == 0 or last:
+                    self.save_recover(config.checkpoint_dir, epoch)
+                if last:
+                    if self.rank == 0:
+                        print("-------------------------------")
+                        print("Pretraining completed successfully")
+                        print("-------------------------------")
+                    break
 
     # ------------------------------------------------------------------------------------------------ inference
     def build_test_graph(self):

@@ -3,6 +3,7 @@
 One `CISGraph` owns the parameters (flat fp32 master copies per scope), all activation buffers for a fixed
 (batch, 384x640 -> HxW) geometry, and the launch lists: forward (PWC-Net -> resize -> generator -> mask (x) flow ->
 3x recover -> Charbonnier losses), backward for the recover step, backward for the generator step, and clip + TF-Adam.
+With masks='boxes' the same graph pretrains the recover net: random boxes (cis_box_masks) replace the generator, which is not built.
 """
 import torch
 
@@ -14,11 +15,37 @@ from .models.PWCNet.model_pwcnet import PWCNetBuilder
 PWC_H, PWC_W = 384, 640   # data/davis2016_data_utils.py:87-88: frames are resized to 384x640 before PWC-Net
 
 
+def box_sides(box_min, box_max, H, W):
+    """Box side range of the recover-net pretraining from fractions of the image sides -> (lo_h, hi_h, lo_w, hi_w) in pixels:
+    lo = max(1, floor(box_min * side)), hi = max(lo, floor(box_max * side)).  ValueError unless 0 < box_min <= box_max <= 1."""
+    if not 0.0 < box_min <= box_max <= 1.0:
+        raise ValueError('box fractions need 0 < box_min <= box_max <= 1, got box_min=%r box_max=%r' % (box_min, box_max))
+    out = []
+    for side in (H, W):
+        lo = max(1, int(box_min * side))
+        out += [lo, max(lo, int(box_max * side))]
+    return tuple(out)
+
+
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
-                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None):
-        """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)."""
+                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks='generator', box=None,
+                 sample_offset=0):
+        """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS).
+        masks: 'generator' (the adversarial graph) or 'boxes' (pretraining of the recover net): one random box per sample, drawn on the
+        device by cis_box_masks, replaces the generator's mask; the generator is neither run nor trained and only the recover step
+        exists.  box = (lo_h, hi_h, lo_w, hi_w) box sides in pixels (None = box_sides(0.1, 0.5, H, W)); sample_offset = global index of
+        this rank's first sample (rank * batch under data parallelism), so that every sample of the global batch gets its own box."""
         _lib.load()
+        if masks not in ('generator', 'boxes'):
+            raise ValueError("masks must be 'generator' or 'boxes', got %r" % (masks,))
+        self.masks = masks
+        boxes = masks == 'boxes'
+        self.box = tuple(box) if box is not None else box_sides(0.1, 0.5, img_height, img_width)
+        self.sample_offset = sample_offset
+        lo_h, hi_h, lo_w, hi_w = self.box
+        if boxes and not (1 <= lo_h <= hi_h <= img_height and 1 <= lo_w <= hi_w <= img_width and sample_offset >= 0):
+            raise ValueError('box sides %r need 1 <= lo <= hi <= the image side (%dx%d)' % (self.box, img_height, img_width))
         self.H, self.W, self.B = img_height, img_width, batch
         self.GB = global_batch or batch
         self.dev = device
@@ -65,28 +92,36 @@ class CISGraph(object):
             P.add('cis_resize_bilinear_f32', self.flow_full.data_ptr(), B, ph, pw, 2, self.flow_st.data_ptr(), H, W, 1.0 / flow_normalizer)
             self._pwc_ops = len(P.ops)                  # fwd.ops[:_pwc_ops] = everything that depends only on the frame pair
             P.add_py(self._take_stage, 'take_stage')
-        self.stats = torch.zeros(B, 4, dtype=torch.float64, device=device)
-        self.gen_in = Act(B, H, W, 5, device, name='gen_in')
+        if not boxes:
+            self.stats = torch.zeros(B, 4, dtype=torch.float64, device=device)
+            self.gen_in = Act(B, H, W, 5, device, name='gen_in')
         self.img8 = Act(B, H, W, 3, device, name='img8')
         hw = H * W
-        P.zero(self.stats)
-        P.add('cis_flow_stats', self.flow.data_ptr(), B, hw, self.stats.data_ptr())                       # flow_utils.py:10
-        P.add('cis_pack_generator_input', self.image.data_ptr(), self.flow.data_ptr(), self.stats.data_ptr(), B, hw, self.gen_in.ptr)
+        if not boxes:
+            P.zero(self.stats)
+            P.add('cis_flow_stats', self.flow.data_ptr(), B, hw, self.stats.data_ptr())                       # flow_utils.py:10
+            P.add('cis_pack_generator_input', self.image.data_ptr(), self.flow.data_ptr(), self.stats.data_ptr(), B, hw, self.gen_in.ptr)
         P.add('cis_pack_f32_to_bf16', self.image.data_ptr(), B * hw, 3, 0.0, self.img8.ptr, 8, 0)
         self.mask = f32(B, H, W, 1)
+        if boxes:
+            # The boxes depend on the Adam step counter, so this launch belongs to the main-lane part of the forward, after take_stage:
+            # fwd.ops[:_pwc_ops] runs on the side stream in the pipelined schedule, concurrently with the previous step's Adam update.
+            P.add('cis_box_masks', self.mask.data_ptr(), B, H, W, *self.box, sample_offset, self.step_state.data_ptr(), seed)
         bld.lane = 1
         i0 = len(P.ops)
         self.rec.build_a_encoder(bld, self.img8)        # side stream, overlaps the generator
         i1 = len(P.ops)
         bld.lane = 0
-        self.gen.build(bld, self.gen_in, self.mask)
+        if not boxes:
+            self.gen.build(bld, self.gen_in, self.mask)
         self._mask_ops = (i0, i1, len(P.ops))           # forward ops [0,i0) + [i1,end) produce the masks (no recover net, no losses)
         # mask (x) flow -> recover inputs for the 3 calls (adversarial_learner.py:107-131)
-        self.rec_in = Act(3 * B, H, W, 4, device, name='rec_in', dep={'G'})
-        self.rec_in.gen_rows = 2 * B
+        self.rec_in = Act(3 * B, H, W, 4, device, name='rec_in', dep=frozenset() if boxes else {'G'})
+        if not boxes:
+            self.rec_in.gen_rows = 2 * B
         P.add('cis_mask_apply', self.flow.data_ptr(), self.mask.data_ptr(), B, hw, self.rec_in.ptr)
         self.dmask = f32(B, H, W)
-        logits = self.gen.logits
+        logits = None if boxes else self.gen.logits
 
         def mask_bwd(bp, mode):
             if mode != 'G':
@@ -96,7 +131,8 @@ class CISGraph(object):
             lg = logits.get_grad()
             bp.add('cis_mask_bwd', self.flow.data_ptr(), self.mask.data_ptr(), self.dmask.data_ptr(), g.ptr, B, hw, lg.ptr)
             logits.grad_written['G'] = True
-        bld.tape.append(mask_bwd)
+        if not boxes:
+            bld.tape.append(mask_bwd)
         h1, w1 = -(-H // 2), -(-W // 2)
         self.h1, self.w1 = h1, w1
         self.flow1 = f32(3 * B, h1, w1, 2)
@@ -121,7 +157,7 @@ class CISGraph(object):
         self.adam = {}
         if train:
             self.dpred = f32(3 * B, H, W, 2)
-            for mode, which in (('R', 0), ('G', 1)):
+            for mode, which in (('R', 0),) if boxes else (('R', 0), ('G', 1)):
                 nb = 3 * B if mode == 'R' else 2 * B
                 head = Plan('loss_bwd_' + mode)
                 head.add('cis_cis_loss_bwd', self.flow.data_ptr(), self.mask.data_ptr(), self.flow1.data_ptr(), self.coef.data_ptr(),
@@ -144,7 +180,7 @@ class CISGraph(object):
                 self.adam[mode] = ad
         # packing of the trainable nets (forward + data-gradient orientation), after backward planning decided what is needed
         self.pack_gen, self.pack_rec = Plan('pack_gen'), Plan('pack_rec')
-        for L in self.gen.all_layers():
+        for L in self.gen.all_layers() if not boxes else ():    # box masks: the generator's parameters exist but nothing reads them
             L.plan_pack(self.pack_gen, dgrad=train)
         for L in self.rec.all_layers():
             L.plan_pack(self.pack_rec, dgrad=train)
@@ -242,6 +278,8 @@ class CISGraph(object):
         pair currently in self.img1 / self.img2 -- the NEXT batch -- for the next call.  `inputs_ready`: an event after which
         img1 / img2 hold that next batch (the host-to-device copy).  The first pipelined call primes the stage from img1 / img2.
         Results are identical to the sequential order; only the schedule changes."""
+        if self.masks == 'boxes' and mode != 'R':
+            raise ValueError("a masks='boxes' graph trains the recover net only (mode 'R'), got mode %r" % (mode,))
         self._ensure_packed()
         if use_graph and pipeline and self.with_pwc:
             return self._train_step_pipelined(mode, allreduce, inputs_ready)
