@@ -165,6 +165,7 @@ def _cases():
     yield 'graph pwc dense off', lambda: _graph(64, 96, 1, pwc_options={'use_dense_cx': False}, **small)
     yield 'graph pwc range 3', lambda: _graph(64, 96, 1, pwc_options={'search_range': 3}, **small)
     yield 'graph no pwc no train', lambda: _graph(64, 96, 1, with_pwc=False, train=False, **small)
+    yield 'graph boxes', lambda: _graph(64, 96, 2, masks='boxes', box=(6, 32, 9, 48), sample_offset=2, **small)
     yield 'generator', lambda: _runner('_GeneratorRunner', 2, 64, 96, 'cpu', 'MaskNet')
     yield 'recover', lambda: _runner('_RecoverRunner', 2, 64, 96, 'cpu', 'FlownetS', 0.25)
     for opts in (None, {'use_dense_cx': False}, {'use_res_cx': False}, {'search_range': 2}):

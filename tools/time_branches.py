@@ -39,7 +39,6 @@ for m in 'RG':
 
 # ---- where the train branch spends its time: forward, backward main lane (data gradients) and side lane (weight gradients) on their own
 from unsupervised_detection_b200.engine import Plan
-pp = g._pipe_state()
 
 
 def sub(plan, keep):
@@ -49,7 +48,7 @@ def sub(plan, keep):
     return q
 
 
-print('train branch forward only                          : %.3f ms' % t(g._capture_plans('tb_fwd', [pp['rest']]).replay))
+print('train branch forward only                          : %.3f ms' % t(g._capture_plans('tb_fwd', [g._pipe_rest]).replay))
 for m in 'RG':
     bw = g.bwd[m]
     both = g._capture_plans('tb_bwd_' + m, [bw])

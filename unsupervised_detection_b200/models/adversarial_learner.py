@@ -33,11 +33,17 @@ def _dist():
 
 
 class AdversarialLearner(object):
-    def __init__(self):
-        self.graph = None
-        self.global_step = 0
-        self._step = 0
-        self.aug_test = False
+    # Every attribute the methods read, with its initial value.  All are immutable, so they are declared on the class: a learner
+    # made without __init__ (object.__new__, as host-side stubs do) reads the same defaults; assignments make instance attributes.
+    config = graph = reader = val_reader = None
+    global_step = 0
+    _step = 0
+    aug_test = False
+    _inference = False                                  # test graphs: the dataset reader yields test inputs
+    world, rank, local_rank, device = 1, 0, 0, None
+    local_batch = num_samples_val = train_steps_per_epoch = val_steps_per_epoch = None
+    min_val_iou = summary_writer = test_crops = None
+    _gt_crops = _gt_small = None                        # device buffers of the multi-crop inference (_device_crops)
 
     # ------------------------------------------------------------------------------------------------ data
     def load_training_data(self):
@@ -54,24 +60,23 @@ class AdversarialLearner(object):
                 from ..data.davis2016_data_utils import Davis2016Reader as Reader
             elif ds == 'FBMS':
                 from ..data.fbms_data_utils import FBMS59Reader as Reader
-                if getattr(self, '_inference', False) and self.aug_test:
+                if self._inference and self.aug_test:
                     assert 'FBMS' in cfg.root_dir                              # adversarial_learner.py:542
             else:
                 from ..data.segtrackv2_data_utils import SegTrackV2Reader as Reader
             rd = Reader(cfg.root_dir, max_temporal_len=cfg.max_temporal_len, min_temporal_len=cfg.min_temporal_len,
                         num_threads=cfg.num_threads, seed=8964 + self.rank)
             self.dataset_reader = rd
-            if getattr(self, '_inference', False):
+            if self._inference:
                 self.reader = rd.test_inputs(batch_size=cfg.batch_size, t_len=cfg.test_temporal_shift, with_fname=True,
                                              test_crop=(1.0 if self.aug_test else cfg.test_crop), partition=cfg.test_partition)
                 self.reader.val_samples = rd.val_samples
-                world = getattr(self, 'world', 1)
-                if world > 1:      # batch-sharded evaluation (eval_dp.py): rank r reads its slice of every global batch
+                if self.world > 1:      # batch-sharded evaluation (eval_dp.py): rank r reads its slice of every global batch
                     per_rank = 1 if self.aug_test else cfg.batch_size
-                    self.reader.shard(self.rank, world, per_rank * world)
+                    self.reader.shard(self.rank, self.world, per_rank * self.world)
             else:
                 self.val_reader = rd.test_inputs(batch_size=cfg.batch_size, t_len=cfg.test_temporal_shift, test_crop=cfg.test_crop,
-                                                 partition='val').shard(self.rank, getattr(self, 'world', 1), cfg.batch_size)
+                                                 partition='val').shard(self.rank, self.world, cfg.batch_size)
                 self.num_samples_val = rd.val_samples
                 self.reader = rd.image_inputs(batch_size=cfg.batch_size, train_crop=cfg.train_crop, partition=cfg.train_partition)
                 self.reader.val_samples = self.num_samples_val
@@ -107,7 +112,6 @@ class AdversarialLearner(object):
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self.val_steps_per_epoch = int(np.ceil(float(self.num_samples_val) / cfg.batch_size))
         self._init_params()
-        self._pinned = None
 
     # ------------------------------------------------------------------------------------------------ checkpoints
     @staticmethod
@@ -137,7 +141,7 @@ class AdversarialLearner(object):
 
     def _names(self, *scopes):
         g = self.graph
-        stores = {'MaskNet': g.gen_store, 'FlownetS': g.rec_store, 'pwcnet': getattr(g, 'pwc_store', None)}
+        stores = {'MaskNet': g.gen_store, 'FlownetS': g.rec_store, 'pwcnet': g.pwc_store}
         return [e[0] for sc in scopes for e in stores[sc].entries]
 
     def _init_params(self):
@@ -224,42 +228,12 @@ class AdversarialLearner(object):
         return lambda t: d.all_reduce(t)     # sum: every rank's loss is already divided by the global batch
 
     def feed(self, img1, img2):
-        """Host -> device copy of one batch of frame pairs [B,384,640,3] fp32 (pinned host tensors copy asynchronously)."""
-        g = self.graph
-        g.pipeline_drain()          # a pipelined flow-network branch may still be reading img1 / img2
-        st = getattr(self, '_staged', None)
-        if st is not None and st[0] is img1:
-            # this batch was prefetched on the copy stream while the previous step was computing: device-to-device hand-over
-            cur = torch.cuda.current_stream()
-            cur.wait_event(st[3])
-            g.img1.copy_(st[1], non_blocking=True)
-            g.img2.copy_(st[2], non_blocking=True)
-            # the staging slot may be overwritten by a later prefetch only after these two reads have executed
-            self._slot_read[st[4]] = torch.cuda.Event()
-            self._slot_read[st[4]].record(cur)
-            self._staged = None
-            return
-        g.img1.copy_(img1, non_blocking=True)
-        g.img2.copy_(img2, non_blocking=True)
+        """Host -> device copy of one batch of frame pairs [B,384,640,3] fp32 (CISGraph.feed)."""
+        self.graph.feed(img1, img2)
 
     def prefetch(self, batch):
-        """Start the host -> device copy of the NEXT batch on a side stream so it overlaps the current step's kernels."""
-        g = self.graph
-        if getattr(self, '_copy_stream', None) is None:
-            self._copy_stream = torch.cuda.Stream()
-            self._stage_bufs = [(torch.empty_like(g.img1), torch.empty_like(g.img2)) for _ in range(2)]
-            self._stage_idx = 0
-            self._slot_read = [None, None]     # per slot: event recorded after the main stream's last read of it (feed)
-        self._stage_idx ^= 1
-        d1, d2 = self._stage_bufs[self._stage_idx]
-        if self._slot_read[self._stage_idx] is not None:
-            self._copy_stream.wait_event(self._slot_read[self._stage_idx])   # write-after-read: the host can run steps ahead of the GPU
-        with torch.cuda.stream(self._copy_stream):
-            d1.copy_(batch[0], non_blocking=True)
-            d2.copy_(batch[1], non_blocking=True)
-            ev = torch.cuda.Event()
-            ev.record(self._copy_stream)
-        self._staged = (batch[0], d1, d2, ev, self._stage_idx)
+        """Start the host -> device copy of the NEXT batch on the copy stream so it overlaps the current step's kernels."""
+        self.graph.prefetch(batch[0], batch[1])
 
     def step(self, batch=None, fetch_losses=None, use_graph=True, next_batch=None, summarize=False):
         """One iteration of the training loop body (adversarial_learner.py:380-409): picks train_recover_op or
@@ -294,28 +268,17 @@ class AdversarialLearner(object):
         if use_graph and next_batch is not None and not summarize and PIPELINE:
             # Software pipeline over steps: PWC-Net (frozen, parameter-independent) runs for `next_batch` on a second stream while
             # this step trains on `batch`, whose flow the previous call already left in the stage buffers.
-            if getattr(self, '_pipe_for', None) is not batch[0] or not getattr(g, '_stage_valid', False):
+            if g.stage_for is not batch[0]:
                 self.feed(batch[0], batch[1])
                 g.prime_pipeline()
-            if getattr(self, '_copy_stream', None) is None:
-                self._copy_stream = torch.cuda.Stream()
-            cs = self._copy_stream
-            cs.wait_event(g.pipeline_inputs_free())          # the flow network of `batch` has finished reading img1 / img2
-            with torch.cuda.stream(cs):
-                g.img1.copy_(next_batch[0], non_blocking=True)
-                g.img2.copy_(next_batch[1], non_blocking=True)
-                ready = torch.cuda.Event()
-                ready.record(cs)
+            ready = g.feed_next(next_batch[0], next_batch[1])
             g.train_step(mode, allreduce=self._allreduce(), use_graph=True, pipeline=True, inputs_ready=ready)
-            self._pipe_for, self._staged = next_batch[0], None
-            other_grads = None
-        else:
-            self._pipe_for = None
-            self.feed(batch[0], batch[1])
-            other_grads = self._summary_prepass(mode) if summarize else None
-            g.train_step(mode, allreduce=self._allreduce(), use_graph=use_graph)
-            if next_batch is not None:
-                self.prefetch(next_batch)          # overlaps this step's kernels; consumed by the next step() call
+            return None
+        self.feed(batch[0], batch[1])
+        other_grads = self._summary_prepass(mode) if summarize else None
+        g.train_step(mode, allreduce=self._allreduce(), use_graph=use_graph)
+        if next_batch is not None:
+            self.prefetch(next_batch)          # overlaps this step's kernels; consumed by the next step() call
         return other_grads
 
     # ------------------------------------------------------------------------------------------------ summaries
@@ -330,7 +293,7 @@ class AdversarialLearner(object):
 
     def _net_gradients(self, mode):
         """Host copy of one net's per-variable gradients as train_op returns them (loss_utils.py:28-32: clipped to +-0.2)."""
-        store = self.graph.rec_store if mode == 'R' else self.graph.gen_store
+        store = self.graph.rec_store if mode == 'R' else self.graph.gen_store     # also works for a graph stub with the two stores
         flat = store.grad.detach().clamp(-0.2, 0.2).cpu().numpy()
         return [(name, flat[off:off + n]) for name, _, n, off, _ in store.entries]
 
@@ -343,14 +306,14 @@ class AdversarialLearner(object):
         g.bwd[other].run()
         ar = self._allreduce()
         if ar is not None:
-            ar((g.rec_store if other == 'R' else g.gen_store).grad)
+            ar(g.store(other).grad)
         torch.cuda.synchronize()
         return self._net_gradients(other)
 
     def _write_step_summary(self, gs, mode, other_grads, losses=None):
         """`losses`: the (already all-reduced) dict of CISGraph.losses(full=True); its four first-sample diagnostics
         (reconstruction_loss, ..., adversarial_learner.py:201-204) are those of rank 0's first sample."""
-        w = getattr(self, 'summary_writer', None)
+        w = self.summary_writer
         if w is None:
             return
         from .utils.flow_utils import flow_to_image_pm
@@ -415,7 +378,7 @@ class AdversarialLearner(object):
     def epoch_end_callback(self, sess, sv, epoch_num):
         """adversarial_learner.py:422-448: validation IoU, save best / every save_freq epochs."""
         validation_iou = 0.0
-        vr = getattr(self, 'val_reader', None) or self.reader
+        vr = self.val_reader or self.reader
         for _ in range(self.val_steps_per_epoch):
             img1, img2, gt, _ = vr.batch(self.local_batch)
             self.feed(img1, img2)
@@ -430,7 +393,7 @@ class AdversarialLearner(object):
             validation_iou = float(t)
         validation_iou /= self.val_steps_per_epoch * self.config.batch_size
         if self.rank == 0:
-            w = getattr(self, 'summary_writer', None)
+            w = self.summary_writer
             if w is not None:
                 w.add_scalar("IoU on Validation", validation_iou)             # :296-298, :436-439
                 w.flush_step(epoch_num)
@@ -581,7 +544,7 @@ class AdversarialLearner(object):
         hs, ws = int(img1.shape[1]), int(img1.shape[2])
         d1, d2, dg = img1.to(dev, non_blocking=True), img2.to(dev, non_blocking=True), gt.to(dev, non_blocking=True)
         nc = len(self.test_crops)
-        if getattr(self, '_gt_crops', None) is None or self._gt_crops.shape[0] != nc:
+        if self._gt_crops is None or self._gt_crops.shape[0] != nc:
             self._gt_crops = torch.empty(nc, hs, ws, 1, dtype=torch.float32, device=dev)
             self._gt_small = torch.empty(nc, g.H, g.W, 1, dtype=torch.float32, device=dev)
         for i, c in enumerate(self.test_crops):

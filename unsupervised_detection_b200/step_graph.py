@@ -114,7 +114,7 @@ class CISGraph(object):
         bld.lane = 0
         if not boxes:
             self.gen.build(bld, self.gen_in, self.mask)
-        self._mask_ops = (i0, i1, len(P.ops))           # forward ops [0,i0) + [i1,end) produce the masks (no recover net, no losses)
+        mask_ops = P.ops[:i0] + P.ops[i1:]              # the forward ops that produce the masks (no recover net, no losses)
         # mask (x) flow -> recover inputs for the 3 calls (adversarial_learner.py:107-131)
         self.rec_in = Act(3 * B, H, W, 4, device, name='rec_in', dep=frozenset() if boxes else {'G'})
         if not boxes:
@@ -164,7 +164,7 @@ class CISGraph(object):
                          self.scalars.data_ptr(), B, H, W, h1, w1, cbn, which, self.dpred.data_ptr(), self.dmask.data_ptr())
                 fg = self.rec.flow1.get_grad()
                 head.add('cis_resize_f32_bwd_to_bf16', self.dpred.data_ptr(), nb, H, W, 2, h1, w1, fg.ptr, fg.pitch)
-                store = self.rec_store if mode == 'R' else self.gen_store
+                store = self.store(mode)
                 layers = self.rec.all_layers() if mode == 'R' else self.gen.all_layers()
                 # nothing to zero: every real entry of the flat gradient buffer is overwritten by cis_unpack_wgrad / cis_bn_chain each
                 # step, and its padding slots are never written (they stay at their initial 0, also through the all-reduce)
@@ -187,7 +187,23 @@ class CISGraph(object):
         self.pack_gen, self.pack_rec, self.pack_pwc = (pl.batch_param_ops(device) for pl in (self.pack_gen, self.pack_rec, self.pack_pwc))
         self._pwc_packed = False
         self._dirty = True      # packed bf16 operands out of date w.r.t. the fp32 master weights
-        self.graphs = {}
+        self._mask_plan = self._sub_plan('fwd_masks', mask_ops)
+        # the two parts of the forward in the pipelined step: the flow network (side stream) and everything after take_stage
+        self._pipe_pwc = self._sub_plan('fwd_pwc', self.fwd.ops[:self._pwc_ops])
+        self._pipe_rest = self._sub_plan('fwd_rest', self.fwd.ops[self._pwc_ops + 1:])
+        # ---- device-only state, made on first use (a CISGraph is also built with device='cpu' to inspect its plans)
+        self.graphs = {}                    # CUDA graphs by key (_capture_plans)
+        self._side = self._copy = None      # streams of the pipelined flow-network branch and of batch uploads (_streams)
+        self._slots = None                  # two device staging slots (img1, img2) of prefetch
+        self._slot = 0                      # the slot the last prefetch wrote
+        self._slot_read = [None, None]      # per slot: event after the main stream's last read of it (feed)
+        self._staged = None                 # (host img1, slot, copy-done event) of the last prefetched batch
+        self._pipe_done = None              # event: the last pipelined step's flow-network branch has filled the stage
+        self._pipe_free = None              # event: prime_pipeline has finished reading img1 / img2
+        # Which frame pair is where.  A frame pair is named by its host img1 tensor when feed_next uploaded it, and by the device
+        # buffer img1 when it was written there in any other way (feed, a direct copy).
+        self.inputs_for = self.img1 if with_pwc else None   # the frame pair in img1 / img2
+        self.stage_for = None               # the frame pair whose flow the stage holds for the next pipelined step; None: stale
 
     # ------------------------------------------------------------------------------------------------ parameters
     def load_params(self, params):
@@ -211,17 +227,18 @@ class CISGraph(object):
         return self.gen_store.real_count() + self.rec_store.real_count() + (self.pwc_store.real_count() if self.with_pwc else 0)
 
     # ------------------------------------------------------------------------------------------------ execution
-    def _ensure_pwc(self):
+    def _ensure_packed(self):
         if self.with_pwc and not self._pwc_packed:
             self.pack_pwc.run()
             self._pwc_packed = True
-
-    def _ensure_packed(self):
-        self._ensure_pwc()
         if self._dirty:
             self.pack_gen.run()
             self.pack_rec.run()
             self._dirty = False
+
+    def store(self, mode):
+        """The parameter store of the network that train step `mode` updates: 'R' the recover net, 'G' the generator."""
+        return self.rec_store if mode == 'R' else self.gen_store
 
     def _pack_of(self, mode):
         return self.pack_rec if mode == 'R' else self.pack_gen
@@ -229,7 +246,7 @@ class CISGraph(object):
     def forward(self):
         self._ensure_packed()
         self.pipeline_drain()
-        self._stage_valid = False
+        self.stage_for = None
         self.fwd.run()
 
     def forward_masks(self, use_graph=False):
@@ -238,30 +255,11 @@ class CISGraph(object):
         CUDA graph."""
         self._ensure_packed()
         self.pipeline_drain()
-        self._stage_valid = False
-        if getattr(self, '_mask_plan', None) is None:
-            i0, i1, i2 = self._mask_ops
-            mp = Plan('fwd_masks')
-            mp.ops = self.fwd.ops[:i0] + self.fwd.ops[i1:i2]
-            mp.keep = self.fwd.keep
-            self._mask_plan = mp
-        if not use_graph:
+        self.stage_for = None
+        if use_graph:
+            self._capture_plans('masks', [self._mask_plan]).replay()
+        else:
             self._mask_plan.run()
-            return
-        g = self.graphs.get('masks')
-        if g is None:
-            torch.cuda.synchronize()
-            s = torch.cuda.Stream()
-            s.wait_stream(torch.cuda.current_stream())
-            with torch.cuda.stream(s):
-                self._mask_plan.run()          # warm-up outside capture (function attributes, lazy allocations)
-            torch.cuda.current_stream().wait_stream(s)
-            torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                self._mask_plan.run()
-            self.graphs['masks'] = g
-        g.replay()
 
     def _take_stage(self):
         self.image.copy_(self.image_st, non_blocking=True)
@@ -286,32 +284,25 @@ class CISGraph(object):
         if inputs_ready is not None:
             torch.cuda.current_stream().wait_event(inputs_ready)
         self.pipeline_drain()
-        self._stage_valid = False
+        self.stage_for = None
         if use_graph:
-            g = self.graphs.get(mode)
-            if g is None:
-                g = self._capture(mode)
-            g[0].replay()
+            fwd_bwd = self._capture_plans('seq_fwd_bwd_' + mode, [self.fwd, self.bwd[mode]])
+            adam = self._capture_plans('seq_adam_' + mode, [self.adam[mode], self._pack_of(mode)], warm=False)
+            fwd_bwd.replay()
             if allreduce is not None:
-                allreduce((self.rec_store if mode == 'R' else self.gen_store).grad)
-            g[1].replay()
+                allreduce(self.store(mode).grad)
+            adam.replay()
             return
         self.fwd.run()
         self.bwd[mode].run()
         if allreduce is not None:
-            allreduce((self.rec_store if mode == 'R' else self.gen_store).grad)
+            allreduce(self.store(mode).grad)
         self.adam[mode].run()
         self._pack_of(mode).run()      # only the updated network's bf16 operands are re-packed
 
-    def _capture(self, mode):
-        g1 = self._capture_plans('seq_fwd_bwd_' + mode, [self.fwd, self.bwd[mode]])
-        g2 = self._capture_plans('seq_adam_' + mode, [self.adam[mode], self._pack_of(mode)], warm=False)
-        self.graphs[mode] = (g1, g2)
-        return self.graphs[mode]
-
-    def _sub_plan(self, lo, hi, name):
+    def _sub_plan(self, name, ops):
         sp = Plan(name)
-        sp.ops = self.fwd.ops[lo:hi]
+        sp.ops = ops
         sp.keep = self.fwd.keep
         return sp
 
@@ -336,43 +327,88 @@ class CISGraph(object):
             self.graphs[key] = g
         return g
 
-    def _pipe_state(self):
-        if getattr(self, '_pipe', None) is None:
-            k = self._pwc_ops
-            self._pipe = dict(stream=torch.cuda.Stream(), done=None, free=None, pwc=self._sub_plan(0, k, 'fwd_pwc'),
-                              rest=self._sub_plan(k + 1, len(self.fwd.ops), 'fwd_rest'))
-        return self._pipe
+    def _streams(self):
+        """(side, copy): the stream of the pipelined flow-network branch and the stream of the host-to-device batch uploads."""
+        if self._side is None:
+            self._side, self._copy = torch.cuda.Stream(), torch.cuda.Stream()
+        return self._side, self._copy
+
+    def feed(self, img1, img2):
+        """Host -> device copy of one batch of frame pairs [B,384,640,3] fp32 into img1 / img2 (pinned host tensors copy
+        asynchronously).  A batch that prefetch staged is handed over from its staging slot on the device."""
+        self.pipeline_drain()          # a pipelined flow-network branch may still be reading img1 / img2
+        self.inputs_for = self.img1
+        st = self._staged
+        if st is not None and st[0] is img1:
+            _, slot, ready = st
+            cur = torch.cuda.current_stream()
+            cur.wait_event(ready)
+            self.img1.copy_(self._slots[slot][0], non_blocking=True)
+            self.img2.copy_(self._slots[slot][1], non_blocking=True)
+            # the staging slot may be overwritten by a later prefetch only after these two reads have executed
+            self._slot_read[slot] = torch.cuda.Event()
+            self._slot_read[slot].record(cur)
+            self._staged = None
+            return
+        self.img1.copy_(img1, non_blocking=True)
+        self.img2.copy_(img2, non_blocking=True)
+
+    def _upload(self, after, dst, img1, img2):
+        """Host -> device copy of a frame pair into the device tensors dst = (d1, d2) on the copy stream, once event `after` (if any)
+        has completed -> the event after the copy."""
+        copy = self._streams()[1]
+        if after is not None:
+            copy.wait_event(after)
+        with torch.cuda.stream(copy):
+            dst[0].copy_(img1, non_blocking=True)
+            dst[1].copy_(img2, non_blocking=True)
+            ready = torch.cuda.Event()
+            ready.record(copy)
+        return ready
+
+    def prefetch(self, img1, img2):
+        """Starts the host -> device copy of an upcoming batch into a staging slot on the copy stream, so that it overlaps the kernels
+        queued now; feed(img1, img2) then hands it over on the device."""
+        if self._slots is None:
+            self._slots = [(torch.empty_like(self.img1), torch.empty_like(self.img2)) for _ in range(2)]
+        self._slot ^= 1
+        # write-after-read: the slot's last hand-over must have executed (the host can run steps ahead of the GPU)
+        self._staged = (img1, self._slot, self._upload(self._slot_read[self._slot], self._slots[self._slot], img1, img2))
+
+    def feed_next(self, img1, img2):
+        """Host -> device copy of the frame pair that the next pipelined train_step runs the flow network on, on the copy stream
+        once the flow network has finished reading img1 / img2 -> the event to pass as train_step(inputs_ready=)."""
+        ready = self._upload(self.pipeline_inputs_free(), (self.img1, self.img2), img1, img2)
+        self.inputs_for, self._staged = img1, None
+        return ready
 
     def prime_pipeline(self):
         """Run the frozen flow network (on the current stream) for the frame pair now in img1 / img2 so that the next
         train_step(pipeline=True) trains on it.  Needed before the first pipelined step and whenever the stream of batches restarts."""
         self._ensure_packed()
-        pp = self._pipe_state()
         self.pipeline_drain()
-        self._capture_plans('pipe_pwc', [pp['pwc']], lane_key=1).replay()
-        pp['done'] = None
-        pp['free'] = torch.cuda.Event()
-        pp['free'].record(torch.cuda.current_stream())
-        self._stage_valid = True
+        self._capture_plans('pipe_pwc', [self._pipe_pwc], lane_key=1).replay()
+        self._pipe_done = None
+        self._pipe_free = torch.cuda.Event()
+        self._pipe_free.record(torch.cuda.current_stream())
+        self.stage_for = self.inputs_for
 
     def pipeline_inputs_free(self):
         """Event after which img1 / img2 may be overwritten with the next frame pair (the flow network last reading them is done)."""
-        pp = self._pipe_state()
-        return pp['done'] if pp['done'] is not None else pp['free']
+        return self._pipe_done if self._pipe_done is not None else self._pipe_free
 
     def _train_step_pipelined(self, mode, allreduce, inputs_ready):
-        pp = self._pipe_state()
-        main, side = torch.cuda.current_stream(), pp['stream']
-        g_pwc = self._capture_plans('pipe_pwc', [pp['pwc']], lane_key=1)
-        g_rest = self._capture_plans('pipe_rest_' + mode, [pp['rest'], self.bwd[mode]])
+        main, side = torch.cuda.current_stream(), self._streams()[0]
+        g_pwc = self._capture_plans('pipe_pwc', [self._pipe_pwc], lane_key=1)
+        g_rest = self._capture_plans('pipe_rest_' + mode, [self._pipe_rest, self.bwd[mode]])
         g_adam = self._capture_plans('pipe_adam_' + mode, [self.adam[mode], self._pack_of(mode)], warm=False)
-        if not getattr(self, '_stage_valid', False):
+        if self.stage_for is None:
             # prime: the stage must hold the flow of the batch this call trains on (= what img1 / img2 hold right now)
             if inputs_ready is not None:
                 main.wait_event(inputs_ready)
             self.prime_pipeline()
-        if pp['done'] is not None:
-            main.wait_event(pp['done'])              # the previous call's side branch filled the stage
+        if self._pipe_done is not None:
+            main.wait_event(self._pipe_done)         # the previous call's side branch filled the stage
         self._take_stage()
         taken = torch.cuda.Event()
         taken.record(main)
@@ -381,18 +417,18 @@ class CISGraph(object):
             side.wait_event(inputs_ready)
         with torch.cuda.stream(side):
             g_pwc.replay()                           # PWC-Net on the NEXT batch, concurrent with everything below
-            pp['done'] = torch.cuda.Event()
-            pp['done'].record(side)
+            self._pipe_done = torch.cuda.Event()
+            self._pipe_done.record(side)
+        self.stage_for = self.inputs_for
         g_rest.replay()
         if allreduce is not None:
-            allreduce((self.rec_store if mode == 'R' else self.gen_store).grad)
+            allreduce(self.store(mode).grad)
         g_adam.replay()
 
     def pipeline_drain(self):
         """Join the side branch (call before reading PWC-Net outputs or re-feeding img1 / img2 outside train_step)."""
-        pp = getattr(self, '_pipe', None)
-        if pp is not None and pp['done'] is not None:
-            torch.cuda.current_stream().wait_event(pp['done'])
+        if self._pipe_done is not None:
+            torch.cuda.current_stream().wait_event(self._pipe_done)
 
     def losses(self, full=False, reduce=None):
         """The `losses` dict of adversarial_learner.py:196-204 (device -> host read).  full=True adds the four first-sample
