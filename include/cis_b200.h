@@ -286,6 +286,11 @@ int cis_flow_standardize(const float* flow, const double* stats, int32_t B, int6
  * fixed-order reductions through `scratch` (double [B * 256], need not be initialised): bit-identical run to run. */
 int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stats, int32_t B, int64_t hw, double* scratch, float* dx,
                              cis_stream_t stream);
+/* held-out end-point error of the recover net: for each sample b of pred, gt (fp32 [B,hw,2]) and mask (fp32 [B,hw]), with
+ * e = ||pred - gt||_2 per pixel, out[b*4 + 0..3] = {sum m*e, sum (1-m)*e, sum m, sum (1-m)} in double.  Fixed-order reductions
+ * through `scratch` (double [B * 256], need not be initialised), no atomics: bit-identical run to run.  out need not be zeroed. */
+int cis_masked_epe(const float* pred, const float* gt, const float* mask, int32_t B, int64_t hw, double* scratch, double* out,
+                   cis_stream_t stream);
 
 /* ---- mask (x) flow + Charbonnier contextual-information loss (adversarial_learner.py:107-110,141-204) ---- */
 /* recover inputs, batch 3B: [flow*(1-m),1,1-m | flow*m,1,m | 0,0,1,0] -> bf16 [3B,H,W,8] (nets.py:50-53) */

@@ -4,7 +4,9 @@ PWC-Net at 384x640, with the frozen flow network pipelined as pretrain_recover.p
 
 The two graphs are timed in alternation inside one process (--rounds rounds, CUDA events, warm-up first), so that clock and thermal drift hit
 both alike.  Prints the card's name and power limit, one JSON line per graph and round, then the medians in frame-pairs/s.
-Usage: python tools/time_recover_pretrain.py [--rounds 5] [--steps 30] [--warmup 5]"""
+--flow gt times the pretraining step on ground-truth flow (CISGraph(flow_source='input'): no PWC-Net, the flow is uploaded at 384x640)
+against the same step on PWC-Net's flow instead.
+Usage: python tools/time_recover_pretrain.py [--flow pwc|gt] [--rounds 5] [--steps 30] [--warmup 5]"""
 import argparse
 import json
 import os
@@ -21,9 +23,9 @@ B, H, W = 4, 256, 448
 
 
 class Case(object):
-    def __init__(self, name, masks, seed=0):
+    def __init__(self, name, masks, seed=0, flow_source='pwc'):
         self.name = name
-        self.graph = CISGraph(H, W, B, masks=masks)
+        self.graph = CISGraph(H, W, B, masks=masks, flow_source=flow_source)
         p = {}
         p.update(params_init.init_generator())
         p.update(params_init.init_recover())
@@ -32,7 +34,10 @@ class Case(object):
         g = torch.Generator().manual_seed(seed)
         a = (torch.rand(B, 384, 640, 3, generator=g) - 0.5).cuda()
         self.graph.img1.copy_(a)
-        self.graph.img2.copy_(torch.roll(a, shifts=(2, 3), dims=(1, 2)))
+        if flow_source == 'input':
+            self.graph.flow_full.copy_(torch.randn(B, 384, 640, 2, generator=g).cuda() * 3.0)
+        else:
+            self.graph.img2.copy_(torch.roll(a, shifts=(2, 3), dims=(1, 2)))
 
     def step(self, _):
         self.graph.train_step('R', use_graph=True, pipeline=True)
@@ -46,6 +51,7 @@ class Case(object):
 
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
+    ap.add_argument('--flow', choices=['pwc', 'gt'], default='pwc', help='gt: ground-truth flow pretraining vs PWC-Net flow pretraining')
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--steps', type=int, default=30)
     ap.add_argument('--warmup', type=int, default=5)
@@ -54,7 +60,11 @@ def main():
     print('card: %s' % card())
     print('recover step %dx%d batch %d, PWC-Net 384x640, pipelined; %d rounds x %d steps (warm-up %d)'
           % (H, W, B, args.rounds, args.steps, args.warmup))
-    cases = [Case('pretrain_boxes', 'boxes'), Case('adversarial_R', 'generator')]
+    if args.flow == 'gt':
+        cases = [Case('pretrain_gt_flow', 'boxes', flow_source='input'), Case('pretrain_boxes', 'boxes')]
+    else:
+        cases = [Case('pretrain_boxes', 'boxes'), Case('adversarial_R', 'generator')]
+    a, b = (c.name for c in cases)
     rows = {c.name: [] for c in cases}
     for r in range(args.rounds):
         for c in cases:
@@ -66,8 +76,27 @@ def main():
     print('medians over %d rounds:' % args.rounds)
     s = {n: {k: med([m[k] for m in rows[n]]) for k in rows[n][0]} for n in rows}
     for n in rows:
-        print('  %-15s %6.2f ms/step  %7.1f frame-pairs/s' % (n, s[n]['step_ms'], s[n]['pairs_per_s']))
-    print('  pretraining / adversarial recover step throughput: %.3f' % (s['pretrain_boxes']['pairs_per_s'] / s['adversarial_R']['pairs_per_s']))
+        print('  %-17s %6.2f ms/step  %7.1f frame-pairs/s' % (n, s[n]['step_ms'], s[n]['pairs_per_s']))
+    print('  %s / %s throughput: %.3f' % (a, b, s[a]['pairs_per_s'] / s[b]['pairs_per_s']))
+    if args.flow == 'gt':
+        validation_share(args.steps, args.warmup)
+
+
+def validation_share(steps, warmup):
+    """One batch of validate_recover on ground-truth flow (eager forward of a forward-only boxes graph + cis_masked_epe) against
+    cis_masked_epe alone: the EPE kernel's share of a validation pass."""
+    g = CISGraph(H, W, B, masks='boxes', flow_source='input', train=False)
+    g.load_params(dict(params_init.init_generator(), **params_init.init_recover()))
+    g.flow_full.normal_(0.0, 3.0)
+
+    def batch(_):
+        g.forward()
+        g.masked_epe()
+    timed_ms(batch, warmup)
+    full = timed_ms(batch, steps)
+    timed_ms(lambda _: g.masked_epe(), warmup)
+    epe = timed_ms(lambda _: g.masked_epe(), steps)
+    print(json.dumps(dict(graph='validate_gt_flow', batch_ms=round(full, 4), masked_epe_ms=round(epe, 4), epe_share=round(epe / full, 4))))
 
 
 if __name__ == '__main__':

@@ -91,6 +91,7 @@ _PROTOS = {
     'cis_resize_f32_bwd': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
     'cis_flow_standardize': [_p, _p, _i32, _i64, _p],
     'cis_flow_standardize_bwd': [_p, _p, _p, _i32, _i64, _p, _p],
+    'cis_masked_epe': [_p, _p, _p, _i32, _i64, _p, _p],
     'cis_warp_costvol': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
     'cis_dense_image_warp': [_p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32],
     'cis_pack_f32_to_bf16': [_p, _i64, _i32, _f32, _p, _i32, _i32],

@@ -28,7 +28,8 @@ _SPEC = [
     # ---- paths
     ('string', 'root_dir', '/your/path/to/DAVIS_2016', 'dataset root folder'),
     ('string', 'train_partition', 'trainval', 'partition used for training: train / val / trainval'),
-    ('string', 'dataset', 'DAVIS2016', 'DAVIS2016, FBMS, SEGTRACK, or SYNTHETIC (seeded synthetic frame pairs)'),
+    ('string', 'dataset', 'DAVIS2016', 'DAVIS2016, FBMS, SEGTRACK, or SYNTHETIC (seeded synthetic frame pairs); pretrain_recover.py '
+                                       'also reads FLYINGCHAIRS'),
     ('string', 'recover_ckpt', '', 'pre-trained recover net (TF checkpoint prefix or .pt); empty = train it from scratch'),
     ('string', 'flow_ckpt', '', 'pre-trained PWC-Net (mandatory; TF checkpoint prefix, its .index/.data file, or .pt)'),
     ('string', 'full_model_ckpt', '', 'checkpoint of all networks, used together with resume_train'),

@@ -1074,6 +1074,44 @@ __global__ void flow_standardize_bwd_kernel(const float* __restrict__ y, const f
   const float2 gv = *reinterpret_cast<const float2*>(g + i), yv = *reinterpret_cast<const float2*>(y + i);
   *reinterpret_cast<float2*>(dx + i) = make_float2((gv.x - mean[0] - yv.x * mean[2]) * r[0], (gv.y - mean[1] - yv.y * mean[3]) * r[1]);
 }
+// ---- masked end-point error of the recover net's held-out pass, same fixed-order rule as the standardisation gradient above.
+// pass 1: block x of sample b sums {m*e, (1-m)*e, m, 1-m}, e = |pred - gt|_2, all in double, over a fixed pixel subset (grid-stride),
+// reduced warp butterfly -> the 8 warps in index order into part[(b * kFlowStdBlocks + x) * 4 + k]
+__global__ void masked_epe_sums_kernel(const float* __restrict__ pred, const float* __restrict__ gt, const float* __restrict__ mask, size_t hw,
+                                       double* __restrict__ part) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ double sm[8][4];
+  const int b = blockIdx.y;
+  double s[4] = {0, 0, 0, 0};
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (size_t)gridDim.x * blockDim.x) {
+    const size_t pix = (size_t)b * hw + p;
+    const float2 pv = *reinterpret_cast<const float2*>(pred + pix * 2), gv = *reinterpret_cast<const float2*>(gt + pix * 2);
+    const double dx = (double)pv.x - gv.x, dy = (double)pv.y - gv.y, e = sqrt(dx * dx + dy * dy), m = mask[pix];
+    s[0] += m * e; s[1] += (1.0 - m) * e; s[2] += m; s[3] += 1.0 - m;
+  }
+#pragma unroll
+  for (int k = 0; k < 4; ++k) s[k] = warp_sum_d(s[k]);
+  if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) sm[threadIdx.x >> 5][k] = s[k];
+  }
+  __syncthreads();
+  if (threadIdx.x < 4) {
+    double t = 0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += sm[w][threadIdx.x];
+    part[((size_t)b * gridDim.x + blockIdx.x) * 4 + threadIdx.x] = t;
+  }
+}
+// pass 2: one block per sample, thread k adds the kFlowStdBlocks partials of sum k in block order
+__global__ void masked_epe_reduce_kernel(const double* __restrict__ part, double* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, k = threadIdx.x;
+  double t = 0;
+  for (int q = 0; q < kFlowStdBlocks; ++q) t += part[((size_t)b * kFlowStdBlocks + q) * 4 + k];
+  out[b * 4 + k] = t;
+}
 
 // ------------------------------------------------------------------------------------------------ mask (x) flow + loss
 __global__ void mask_apply_kernel(const float* __restrict__ flow, const float* __restrict__ mask, size_t npix, bf16* __restrict__ dst) {
@@ -2008,6 +2046,14 @@ int cis_flow_standardize_bwd(const float* y, const float* dy, const double* stat
   CIS_LAUNCH(flow_standardize_bwd_sums_kernel, dim3(kFlowStdBlocks, B), 256, 0, ST, y, dy, (size_t)hw, scratch);
   CIS_LAUNCH(flow_standardize_bwd_kernel, dim3(nblk((size_t)hw), B), 256, 0, ST, y, dy, stats, (const double*)scratch, (size_t)hw, dx);
   return cis_check_launch("flow_standardize_bwd");
+}
+int cis_masked_epe(const float* pred, const float* gt, const float* mask, int32_t B, int64_t hw, double* scratch, double* out,
+                   cis_stream_t stream) {
+  if (!pred || !gt || !mask || !scratch || !out || B < 1 || B > 65535 || hw < 1)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_masked_epe: bad pointer or size");
+  CIS_LAUNCH(masked_epe_sums_kernel, dim3(kFlowStdBlocks, B), 256, 0, ST, pred, gt, mask, (size_t)hw, scratch);
+  CIS_LAUNCH(masked_epe_reduce_kernel, B, 4, 0, ST, (const double*)scratch, out);
+  return cis_check_launch("masked_epe");
 }
 int cis_mask_apply(const float* flow, const float* mask, int32_t B, int64_t hw, void* dst, cis_stream_t stream) {
   CIS_LAUNCH(mask_apply_kernel, nblk((size_t)B * hw), 256, 0, ST, flow, mask, (size_t)B * hw, (mbf)dst);

@@ -103,6 +103,28 @@ def nn_resize(x, oh, ow):
     return x[yi][:, xi]
 
 
+def train_augmentation(r, train_crop, h, w):
+    """The random draws of one training sample's augmentation (augment_pair :136-148 + aug_flips.random_flip_images), in the reference's
+    order, from the random.Random r: the flip case (0 keep | 1 rotate 180 | 2 left-right | 3 top-down, 25 % each), then the crop
+    fraction pct in [train_crop, 1) and the crop's corner (random_crop_image_pair :101-128) -> (case, y0, x0, ch, cw)."""
+    case = r.randrange(4)
+    pct = train_crop + r.random() * (1 - train_crop)
+    ch, cw = int(h * pct), int(w * pct)
+    y0, x0 = r.randint(0, h - ch), r.randint(0, w - cw)
+    return case, y0, x0, ch, cw
+
+
+def flip(x, case):
+    """The flip of train_augmentation's case on an HWC array (a view)."""
+    return (x, x[::-1, ::-1], x[:, ::-1], x[::-1])[case]
+
+
+def crop_resized(x, y0, x0, ch, cw):
+    """The crop [y0:y0+ch, x0:x0+cw] of an HWC array, legacy-bilinear resized back to the array's size."""
+    h, w = x.shape[:2]
+    return legacy_resize(np.ascontiguousarray(x[y0:y0 + ch, x0:x0 + cw]), h, w)
+
+
 def central_crop_box(h, w, frac):
     """tf.image.central_crop geometry: offset = int((dim - dim*frac)/2), size = dim - 2*offset."""
     y0 = int((h - h * frac) / 2)
@@ -283,19 +305,10 @@ class Davis2016Reader(object):
         t_shift = r.randint(self.min_temporal_len, self.max_temporal_len)
         i2 = int(t_shift * direction + i1)
         a, b = self.preprocess_image(self.filenames[i1]), self.preprocess_image(self.filenames[i2])
-        case = r.randrange(4)                      # keep | rotate 180 | left-right | top-down, each 25 %
-        if case == 1:
-            a, b = a[::-1, ::-1], b[::-1, ::-1]
-        elif case == 2:
-            a, b = a[:, ::-1], b[:, ::-1]
-        elif case == 3:
-            a, b = a[::-1], b[::-1]
-        pct = self.train_crop + r.random() * (1 - self.train_crop)       # random_crop_image_pair :101-128
         h, w = a.shape[:2]
-        ch, cw = int(h * pct), int(w * pct)
-        y0, x0 = r.randint(0, h - ch), r.randint(0, w - cw)
-        a = legacy_resize(np.ascontiguousarray(a[y0:y0 + ch, x0:x0 + cw]), h, w)
-        b = legacy_resize(np.ascontiguousarray(b[y0:y0 + ch, x0:x0 + cw]), h, w)
+        case, y0, x0, ch, cw = train_augmentation(r, self.train_crop, h, w)
+        a = crop_resized(flip(a, case), y0, x0, ch, cw)
+        b = crop_resized(flip(b, case), y0, x0, ch, cw)
         return a.astype(np.float32), b.astype(np.float32), np.ones((h, w, 1), np.float32), self.filenames[i1]
 
     def _test_sample(self, pair, seed):

@@ -2,7 +2,8 @@
 
 Kept API: AdversarialLearner().train(config) / .setup_inference(config, aug_test=False) / .inference(sess) with the same
 result keys (:617-619), plus .step() = one iteration of the loop body (:380-409) and .pretrain_recover(config) = pretraining of the
-recover net on box-shaped occlusions (the pre-training behind --recover_ckpt that the reference's README describes).  `sess` arguments are accepted and
+recover net on box-shaped occlusions (the pre-training behind --recover_ckpt that the reference's README describes), on PWC-Net's flow or
+a dataset's ground-truth flow, with .validate_recover() = its held-out inpainting error.  `sess` arguments are accepted and
 ignored (there is no tf.Session).  Data parallelism (not in the reference): one process per GPU, the frame-pair batch is
 sharded over ranks and the active network's flat gradient buffer is summed with ONE NCCL all-reduce per step
 (SURVEY.md section 8e); clip / noise test / Adam then run identically on every rank.
@@ -25,6 +26,8 @@ from .utils.general_utils import compute_all_IoU
 
 # CIS_PIPELINE=0 disables the cross-step software pipeline of the frozen flow network (see CISGraph.train_step)
 PIPELINE = os.environ.get('CIS_PIPELINE', '1') != '0'
+# datasets whose batches carry ground-truth flow (img1, img2, flow, names): recover-net pretraining with pretrain_flow=gt
+FLOW_DATASETS = ('FLYINGCHAIRS',)
 
 
 def _dist():
@@ -44,6 +47,9 @@ class AdversarialLearner(object):
     local_batch = num_samples_val = train_steps_per_epoch = val_steps_per_epoch = None
     min_val_iou = summary_writer = test_crops = None
     _gt_crops = _gt_small = None                        # device buffers of the multi-crop inference (_device_crops)
+    _pretrain = False                                   # recover-net pretraining: datasets with flow (FLYINGCHAIRS) are accepted
+    val_graph = None                                    # forward-only boxes graph of validate_recover, built on first use
+    min_val_epe = math.inf
 
     # ------------------------------------------------------------------------------------------------ data
     def load_training_data(self):
@@ -53,6 +59,15 @@ class AdversarialLearner(object):
         if ds == 'SYNTHETIC':
             self.reader = SyntheticReader(PWC_H, PWC_W, seed=8964 + self.rank)
             self.num_samples_val = self.reader.val_samples
+            return
+        if ds == 'FLYINGCHAIRS' and self._pretrain:
+            # frame pairs with ground-truth flow and no masks: recover-net pretraining only (train.py validates IoU on masks).  Training
+            # reads the split's train pairs whatever --train_partition says, so that the val pairs stay held out.
+            from ..data.flyingchairs_data_utils import FlyingChairsReader
+            cfg = self.config
+            self.dataset_reader = FlyingChairsReader(cfg.root_dir, num_threads=cfg.num_threads, seed=8964 + self.rank)
+            self.reader = self.dataset_reader.image_inputs(batch_size=cfg.batch_size, train_crop=cfg.train_crop)
+            self.num_samples_val = self.dataset_reader.val_samples
             return
         if ds in ('DAVIS2016', 'FBMS', 'SEGTRACK'):
             cfg = self.config
@@ -151,7 +166,9 @@ class AdversarialLearner(object):
         p.update(params_init.init_recover())
         g = self.graph
         fc = getattr(cfg, 'flow_ckpt', '')
-        if fc.startswith('synthetic'):
+        if g.flow_source == 'input':
+            pass                                                                # ground-truth flow: the graph has no PWC-Net
+        elif fc.startswith('synthetic'):
             p.update(params_init.init_pwcnet(g.pwc_store.entries))
         elif self._is_ckpt(fc):
             p.update(self._read_ckpt(fc, self._names('pwcnet'))[0])               # flow_saver.restore, adversarial_learner.py:339-341
@@ -201,10 +218,11 @@ class AdversarialLearner(object):
     def save_recover(self, checkpoint_dir, epoch):
         """The recover net alone, as the reference's recover_saver covers it (adversarial_learner.py:329): `recover-<epoch>` as a TF V2
         bundle of the FlownetS variables (no global_step, no Adam slots) plus the same tensors as a native `.pt`, and the `checkpoint`
-        state file.  train.py --recover_ckpt=<dir>/recover-<epoch> and a TF recover_saver.restore both read it."""
+        state file.  train.py --recover_ckpt=<dir>/recover-<epoch> and a TF recover_saver.restore both read it.  epoch='best' writes
+        recover-best (the lowest validation EPE so far), which later saves never delete."""
         if self.rank != 0:
             return
-        base = 'recover-%d' % epoch
+        base = 'recover-%s' % epoch
         print(" [*] Saving recover net to {}/{}".format(checkpoint_dir, base))
         params = {k: v.cpu() for k, v in self.graph.rec_store.export().items()}
         self._write_checkpoint(checkpoint_dir, base, params, None)
@@ -217,7 +235,7 @@ class AdversarialLearner(object):
         for old in ckpt_io.update_checkpoint_state(checkpoint_dir, base, keep=40):
             for suf in ('.index', '.data-00000-of-00001', '.pt'):
                 fp = os.path.join(checkpoint_dir, old + suf)
-                if os.path.isfile(fp) and old != 'model.best':
+                if os.path.isfile(fp) and old not in ('model.best', 'recover-best'):
                     os.remove(fp)
 
     # ------------------------------------------------------------------------------------------------ stepping
@@ -408,28 +426,40 @@ class AdversarialLearner(object):
     def build_pretrain_graph(self):
         """The recover step of adversarial_learner.py:72-258 with one random box per sample as the mask: PWC-Net -> resize -> box masks ->
         3x recover -> losses -> train_recover_op.  No generator runs.  config.box_min / box_max = box side range as fractions of the
-        image sides (defaults 0.1 / 0.5)."""
+        image sides (defaults 0.1 / 0.5).  config.pretrain_flow = 'pwc' (default: PWC-Net's flow of the frame pair) or 'gt' (the
+        dataset's ground-truth flow, FLYINGCHAIRS: no PWC-Net is built and --flow_ckpt is not read)."""
         cfg = self.config
         self._init_dist()
         if cfg.batch_size % self.world:
             raise ValueError('batch_size must be divisible by the number of ranks')
         self.local_batch = cfg.batch_size // self.world
         box = box_sides(getattr(cfg, 'box_min', 0.1), getattr(cfg, 'box_max', 0.5), cfg.img_height, cfg.img_width)
+        gt = getattr(cfg, 'pretrain_flow', 'pwc') == 'gt'
+        if gt and cfg.dataset not in FLOW_DATASETS:
+            raise ValueError('pretrain_flow=gt needs a dataset with ground-truth flow (%s), got %s' % (', '.join(FLOW_DATASETS), cfg.dataset))
+        self._pretrain = True
         self.load_training_data()
         # sample_offset: sample b of rank r is global sample r * local_batch + b, so a DP job draws the boxes of one GPU running the global batch
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
                               flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
                               pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='boxes', box=box,
-                              sample_offset=self.rank * self.local_batch)
+                              sample_offset=self.rank * self.local_batch, flow_source='input' if gt else 'pwc')
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self._init_params()
+
+    def _uploads(self, batch):
+        """The two tensors of a reader batch (img1, img2, ... ) that the graph uploads: (frame 1, frame 2), or (frame 1, its flow) under
+        ground-truth flow (a flow reader's batch is (img1, img2, flow, names))."""
+        if batch is None:
+            return None
+        return (batch[0], batch[2]) if self.graph.flow_source == 'input' else (batch[0], batch[1])
 
     def pretrain_step(self, batch, next_batch=None, fetch_losses=False, use_graph=True):
         """One pretraining iteration: train_recover_op on `batch` under box masks (one NCCL all-reduce of the recover gradient under
         torchrun); -> {global_step, loss_recover?, reconstruction_loss?, reconstruction_compl_loss?}.  All ranks must pass the same
         fetch_losses (the losses are all-reduced)."""
         self.global_step += 1
-        self._train_on('R', batch, next_batch, use_graph, False)
+        self._train_on('R', self._uploads(batch), self._uploads(next_batch), use_graph, False)
         res = {"global_step": self.global_step}
         if fetch_losses:
             L = self.graph.losses(full=True, reduce=self._allreduce())
@@ -441,8 +471,10 @@ class AdversarialLearner(object):
         """Pretrains the recover net (scope FlownetS) to inpaint optical flow under box-shaped occlusions, the pre-training the reference's
         README describes for --recover_ckpt.  num_samples_train / batch_size steps per epoch for max_epochs epochs; every summary_freq
         steps rank 0 prints the loss and writes the scalars recover / reconstruction_loss / reconstruction_compl_loss; every save_freq
-        epochs and after the last one it saves recover-<epoch> (save_recover).  --flow_ckpt is mandatory, --recover_ckpt gives the
-        starting weights (else the reference's initialisation)."""
+        epochs and after the last one it saves recover-<epoch> (save_recover).  --flow_ckpt is mandatory unless pretrain_flow=gt,
+        --recover_ckpt gives the starting weights (else the reference's initialisation).  config.validate: at every epoch end,
+        validate_recover() on the val split; rank 0 prints and logs the EPE inside the boxes, and recover-best is saved whenever it
+        improves."""
         self.config = config
         self.build_pretrain_graph()
         if self.rank == 0:
@@ -473,12 +505,60 @@ class AdversarialLearner(object):
                 last = epoch == config.max_epochs
                 if epoch % config.save_freq == 0 or last:
                     self.save_recover(config.checkpoint_dir, epoch)
+                if getattr(config, 'validate', False):
+                    self._validation_epoch_end(epoch)
                 if last:
                     if self.rank == 0:
                         print("-------------------------------")
                         print("Pretraining completed successfully")
                         print("-------------------------------")
                     break
+
+    def _validation_epoch_end(self, epoch):
+        epe, epe_out = self.validate_recover()
+        if self.rank == 0:
+            print("Epoch [{}] Validation EPE (boxes): {:.4f} (outside the boxes: {:.4f})".format(epoch, epe, epe_out))
+            if self.summary_writer is not None:
+                self.summary_writer.add_scalar("Validation EPE", epe)
+                self.summary_writer.flush_step(epoch)
+        if epe < self.min_val_epe:                  # the same all-reduced value on every rank
+            self.min_val_epe = epe
+            self.save_recover(self.config.checkpoint_dir, 'best')
+
+    def validate_recover(self):
+        """Held-out inpainting error of the recover net -> (EPE inside the boxes, EPE outside them), means over the pixels of the val
+        split in pixels of the 384x640 grid.  A forward-only boxes graph with the training graph's weights runs the val pairs in order,
+        sharded over ranks like the evaluation; its step counter stays 0 and each batch's sample_offset is its global val index, so
+        every call scores the same boxes.  cis_masked_epe's per-sample sums are added over the batches on the device (pairs that only
+        pad the last global batch are left out) and merged by one all-reduce."""
+        cfg, g = self.config, self.graph
+        if self.val_graph is None:
+            self.val_graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
+                                      flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False,
+                                      pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='boxes', box=g.box,
+                                      flow_source=g.flow_source)
+        vg = self.val_graph
+        vg.load_params(g.export_params())
+        n, GB, lb = self.num_samples_val, cfg.batch_size, self.local_batch
+        tot = torch.zeros(4, dtype=torch.float64, device=self.device)
+        it = self.dataset_reader.test_inputs(batch_size=GB).shard(self.rank, self.world, GB)     # a fresh ordered pass every call
+        try:
+            for k in range(-(-n // GB)):
+                batch = it.batch(lb)
+                first = k * GB + self.rank * lb
+                vg.set_sample_offset(first)
+                vg.feed(*self._uploads(batch))
+                vg.forward()
+                valid = min(lb, n - first)
+                if valid > 0:
+                    tot += vg.masked_epe()[:valid].sum(0)
+        finally:
+            it.close()
+        d = _dist()
+        if d is not None and self.world > 1:
+            d.all_reduce(tot)
+        s = tot.tolist()
+        return tuple(e / m * cfg.flow_normalizer if m else math.nan for e, m in ((s[0], s[2]), (s[1], s[3])))
 
     # ------------------------------------------------------------------------------------------------ inference
     def build_test_graph(self):

@@ -30,17 +30,32 @@ def box_sides(box_min, box_max, H, W):
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
                  beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks='generator', box=None,
-                 sample_offset=0):
+                 sample_offset=0, flow_source='pwc'):
         """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS).
         masks: 'generator' (the adversarial graph) or 'boxes' (pretraining of the recover net): one random box per sample, drawn on the
         device by cis_box_masks, replaces the generator's mask; the generator is neither run nor trained and only the recover step
         exists.  box = (lo_h, hi_h, lo_w, hi_w) box sides in pixels (None = box_sides(0.1, 0.5, H, W)); sample_offset = global index of
-        this rank's first sample (rank * batch under data parallelism), so that every sample of the global batch gets its own box."""
+        this rank's first sample (rank * batch under data parallelism), so that every sample of the global batch gets its own box.
+        with_pwc=False: no 384x640 inputs at all; image and flow are written at HxW directly (no stage, no pipelined schedule).
+        flow_source: where the flow at 384x640 comes from.  'pwc' (the default): PWC-Net run on the frame pair img1 / img2.  'input'
+        (masks='boxes' only): a known flow field uploaded into flow_full next to img1, in PWC-Net's channel order and sign; no PWC-Net
+        is built.  The flow then reaches the recover net through the same resize and 1/flow_normalizer as PWC-Net's output, and the
+        stage, the pipelined schedule and the batch hand-over work on the pair (img1, flow_full) in place of (img1, img2)."""
         _lib.load()
         if masks not in ('generator', 'boxes'):
             raise ValueError("masks must be 'generator' or 'boxes', got %r" % (masks,))
-        self.masks = masks
+        if flow_source not in ('pwc', 'input'):
+            raise ValueError("flow_source must be 'pwc' or 'input', got %r" % (flow_source,))
+        if flow_source == 'input' and (masks != 'boxes' or not with_pwc):
+            raise ValueError("flow_source='input' needs masks='boxes' and the 384x640 inputs (with_pwc=True)")
+        self.masks, self.flow_source = masks, flow_source
         boxes = masks == 'boxes'
+        # Two attributes, two meanings: self.staged = the graph takes 384x640 uploads (self.inputs) that fwd.ops[:_pwc_ops] resizes into
+        # the stage (the pipelined schedule needs this); self.with_pwc = PWC-Net is built (pwc_store, pack_pwc).  flow_source='input'
+        # is staged without PWC-Net.
+        staged = with_pwc
+        with_pwc = with_pwc and flow_source == 'pwc'
+        self.staged = staged
         self.box = tuple(box) if box is not None else box_sides(0.1, 0.5, img_height, img_width)
         self.sample_offset = sample_offset
         lo_h, hi_h, lo_w, hi_w = self.box
@@ -69,6 +84,7 @@ class CISGraph(object):
         bld = Builder(device)
         self.bld = bld
         P = bld.fwd
+        self.img2 = None
         if with_pwc:
             ph, pw = pwc_hw
             self.img1, self.img2 = f32(B, ph, pw, 3), f32(B, ph, pw, 3)
@@ -79,14 +95,19 @@ class CISGraph(object):
             P.add('cis_pack_f32_to_bf16', self.img1.data_ptr(), npx, 3, 0.5, i1.ptr, 8, 0)     # adapt_x: img + 0.5
             P.add('cis_pack_f32_to_bf16', self.img2.data_ptr(), npx, 3, 0.5, i2.ptr, 8, 0)
             self.pwc.build(bld, i1, i2, self.flow_full)
+        elif staged:
+            ph, pw = pwc_hw
+            self.img1, self.flow_full = f32(B, ph, pw, 3), f32(B, ph, pw, 2)
+        # the two device buffers one batch upload writes (feed, prefetch, feed_next): the frame pair, or frame 1 and its flow
+        self.inputs = (self.img1, self.img2 if with_pwc else self.flow_full) if staged else None
         self.image = f32(B, H, W, 3)
         self.flow = f32(B, H, W, 2)
         self._pwc_ops = 0
-        if with_pwc:
+        if staged:
             # adversarial_learner.py:87-97: legacy bilinear to (H,W); flow / flow_normalizer.  The frozen flow network writes its
             # results to STAGE buffers; the two small device copies below hand them to the trainable part.  That split is what lets
             # train_step(pipeline=True) run PWC-Net for the NEXT batch on a second stream while this batch trains (the flow network
-            # has no dependency on the parameters being trained).
+            # has no dependency on the parameters being trained).  With flow_source='input' the prefix is these two resizes alone.
             self.image_st, self.flow_st = f32(B, H, W, 3), f32(B, H, W, 2)
             P.add('cis_resize_bilinear_f32', self.img1.data_ptr(), B, ph, pw, 3, self.image_st.data_ptr(), H, W, 1.0)
             P.add('cis_resize_bilinear_f32', self.flow_full.data_ptr(), B, ph, pw, 2, self.flow_st.data_ptr(), H, W, 1.0 / flow_normalizer)
@@ -103,6 +124,9 @@ class CISGraph(object):
             P.add('cis_pack_generator_input', self.image.data_ptr(), self.flow.data_ptr(), self.stats.data_ptr(), B, hw, self.gen_in.ptr)
         P.add('cis_pack_f32_to_bf16', self.image.data_ptr(), B * hw, 3, 0.0, self.img8.ptr, 8, 0)
         self.mask = f32(B, H, W, 1)
+        # held-out inpainting error of a boxes graph (masked_epe): per-sample sums and the kernel's block partials
+        self.epe_sums = torch.zeros(B, 4, dtype=torch.float64, device=device) if boxes else None
+        self._epe_scratch = torch.zeros(B * 256, dtype=torch.float64, device=device) if boxes else None
         if boxes:
             # The boxes depend on the Adam step counter, so this launch belongs to the main-lane part of the forward, after take_stage:
             # fwd.ops[:_pwc_ops] runs on the side stream in the pipelined schedule, concurrently with the previous step's Adam update.
@@ -202,7 +226,7 @@ class CISGraph(object):
         self._pipe_free = None              # event: prime_pipeline has finished reading img1 / img2
         # Which frame pair is where.  A frame pair is named by its host img1 tensor when feed_next uploaded it, and by the device
         # buffer img1 when it was written there in any other way (feed, a direct copy).
-        self.inputs_for = self.img1 if with_pwc else None   # the frame pair in img1 / img2
+        self.inputs_for = self.img1 if staged else None     # the frame pair in img1 / img2
         self.stage_for = None               # the frame pair whose flow the stage holds for the next pipelined step; None: stale
 
     # ------------------------------------------------------------------------------------------------ parameters
@@ -261,6 +285,24 @@ class CISGraph(object):
         else:
             self._mask_plan.run()
 
+    def set_sample_offset(self, sample_offset):
+        """Global index of the first sample for the box draws of the next eager forward() (a validation pass sets it per batch).  The
+        offset is a launch argument, so CUDA graphs captured earlier would keep the old one: refused once one exists."""
+        if self.masks != 'boxes' or self.graphs or sample_offset < 0:
+            raise ValueError('set_sample_offset needs a boxes graph that has captured no CUDA graph and an offset >= 0')
+        for plan in (self.fwd, self._mask_plan, self._pipe_rest):
+            plan.ops = [op[:1] + (op[1][:8] + (sample_offset,) + op[1][9:],) + op[2:] if op[2] == 'cis_box_masks' else op for op in plan.ops]
+        self.sample_offset = sample_offset
+
+    def masked_epe(self):
+        """Held-out inpainting error of the last forward of a boxes graph -> self.epe_sums, fp64 [B,4] on the device: per sample
+        {sum m*e, sum (1-m)*e, sum m, sum (1-m)} with e = |pred - flow|_2 per HxW pixel, pred = the masked recover call (the first B
+        rows of self.pred), m = the box mask.  e is in units of the normalised flow (times flow_normalizer: pixels of the 384x640
+        grid).  Fixed-order reductions: bit-identical run to run."""
+        _lib.call('cis_masked_epe', self.pred.data_ptr(), self.flow.data_ptr(), self.mask.data_ptr(), self.B, self.H * self.W,
+                  self._epe_scratch.data_ptr(), self.epe_sums.data_ptr(), torch.cuda.current_stream().cuda_stream)
+        return self.epe_sums
+
     def _take_stage(self):
         self.image.copy_(self.image_st, non_blocking=True)
         self.flow.copy_(self.flow_st, non_blocking=True)
@@ -279,7 +321,7 @@ class CISGraph(object):
         if self.masks == 'boxes' and mode != 'R':
             raise ValueError("a masks='boxes' graph trains the recover net only (mode 'R'), got mode %r" % (mode,))
         self._ensure_packed()
-        if use_graph and pipeline and self.with_pwc:
+        if use_graph and pipeline and self.staged:
             return self._train_step_pipelined(mode, allreduce, inputs_ready)
         if inputs_ready is not None:
             torch.cuda.current_stream().wait_event(inputs_ready)
@@ -335,7 +377,8 @@ class CISGraph(object):
 
     def feed(self, img1, img2):
         """Host -> device copy of one batch of frame pairs [B,384,640,3] fp32 into img1 / img2 (pinned host tensors copy
-        asynchronously).  A batch that prefetch staged is handed over from its staging slot on the device."""
+        asynchronously).  A batch that prefetch staged is handed over from its staging slot on the device.  With
+        flow_source='input' the second tensor is frame 1's flow [B,384,640,2] and goes to flow_full."""
         self.pipeline_drain()          # a pipelined flow-network branch may still be reading img1 / img2
         self.inputs_for = self.img1
         st = self._staged
@@ -343,15 +386,15 @@ class CISGraph(object):
             _, slot, ready = st
             cur = torch.cuda.current_stream()
             cur.wait_event(ready)
-            self.img1.copy_(self._slots[slot][0], non_blocking=True)
-            self.img2.copy_(self._slots[slot][1], non_blocking=True)
+            for dst, src in zip(self.inputs, self._slots[slot]):
+                dst.copy_(src, non_blocking=True)
             # the staging slot may be overwritten by a later prefetch only after these two reads have executed
             self._slot_read[slot] = torch.cuda.Event()
             self._slot_read[slot].record(cur)
             self._staged = None
             return
-        self.img1.copy_(img1, non_blocking=True)
-        self.img2.copy_(img2, non_blocking=True)
+        self.inputs[0].copy_(img1, non_blocking=True)
+        self.inputs[1].copy_(img2, non_blocking=True)
 
     def _upload(self, after, dst, img1, img2):
         """Host -> device copy of a frame pair into the device tensors dst = (d1, d2) on the copy stream, once event `after` (if any)
@@ -370,7 +413,7 @@ class CISGraph(object):
         """Starts the host -> device copy of an upcoming batch into a staging slot on the copy stream, so that it overlaps the kernels
         queued now; feed(img1, img2) then hands it over on the device."""
         if self._slots is None:
-            self._slots = [(torch.empty_like(self.img1), torch.empty_like(self.img2)) for _ in range(2)]
+            self._slots = [tuple(torch.empty_like(t) for t in self.inputs) for _ in range(2)]
         self._slot ^= 1
         # write-after-read: the slot's last hand-over must have executed (the host can run steps ahead of the GPU)
         self._staged = (img1, self._slot, self._upload(self._slot_read[self._slot], self._slots[self._slot], img1, img2))
@@ -378,7 +421,7 @@ class CISGraph(object):
     def feed_next(self, img1, img2):
         """Host -> device copy of the frame pair that the next pipelined train_step runs the flow network on, on the copy stream
         once the flow network has finished reading img1 / img2 -> the event to pass as train_step(inputs_ready=)."""
-        ready = self._upload(self.pipeline_inputs_free(), (self.img1, self.img2), img1, img2)
+        ready = self._upload(self.pipeline_inputs_free(), self.inputs, img1, img2)
         self.inputs_for, self._staged = img1, None
         return ready
 
