@@ -110,5 +110,5 @@ def run_conv_case(N, H, W, cins, cout, k, stride=1, dil=1, act=ACT_NONE, alpha=0
     r.update(db_err=float((db - grads[2]).abs().max()), db_ref=float(grads[2].abs().max()))
     if bn:
         r.update(dgamma_err=float((store.view('L/gamma', 'grad') - grads[3]).abs().max()), dgamma_ref=float(grads[3].abs().max()),
-                 dbeta_err=float((store.view('L/beta', 'grad') - grads[4]).abs().max()))
+                 dbeta_err=float((store.view('L/beta', 'grad') - grads[4]).abs().max()), dbeta_ref=float(grads[4].abs().max()))
     return r

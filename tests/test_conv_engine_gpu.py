@@ -48,6 +48,7 @@ def test_conv_engine(case):
         assert r['db_err'] <= 2 ** -7 * r['db_ref'] + 1e-3, r
     if 'dgamma_err' in r:
         assert r['dgamma_err'] <= 2 ** -6 * r['dgamma_ref'] + 1e-2, r
+        assert r['dbeta_err'] <= 2 ** -6 * r['dbeta_ref'] + 1e-2, r
 
 
 MODE_CASES = [CASES[0], CASES[1], CASES[4], CASES[6], CASES[11], CASES[12], CASES[14], CASES[17]]
@@ -124,6 +125,7 @@ def test_conv_engine_halo_wgrad(case, monkeypatch):
     assert r['db_err'] <= 2 ** -7 * r['db_ref'] + 1e-3, r
     if 'dgamma_err' in r:
         assert r['dgamma_err'] <= 2 ** -6 * r['dgamma_ref'] + 1e-2, r
+        assert r['dbeta_err'] <= 2 ** -6 * r['dbeta_ref'] + 1e-2, r
 
 
 NARROW_CASES = [CASES[1], CASES[6], CASES[10], CASES[12], CASES[13], CASES[4]]
