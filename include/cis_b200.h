@@ -239,6 +239,10 @@ int cis_upsample_nn2x_bwd(const void* ddst, int32_t N, int32_t H, int32_t W, int
  * multi-crop test-time augmentation of test_generator_ensemble (data/davis2016_data_utils.py:130-134, 328-354) on the device */
 int cis_crop_resize_bilinear_f32(const float* src, int32_t Hs, int32_t Ws, int32_t C, int32_t y0, int32_t x0, int32_t ch, int32_t cw, float* dst,
                                  int32_t OH, int32_t OW, cis_stream_t stream);
+/* the same crop and resize of ONE Hs x Ws x 2 flow field, whose vectors follow the resize: channel 0 times s0, channel 1 times s1
+ * (PWC-Net's channel order: s0 = OH / ch for rows, s1 = OW / cw for columns) -- the supplied flow of the multi-crop ensemble */
+int cis_crop_resize_flow_f32(const float* src, int32_t Hs, int32_t Ws, int32_t y0, int32_t x0, int32_t ch, int32_t cw, float* dst, int32_t OH,
+                             int32_t OW, float s0, float s1, cis_stream_t stream);
 /* tf.image.resize_images(NEAREST_NEIGHBOR) for GT masks (adversarial_learner.py:92-94) */
 int cis_resize_nn_f32(const float* src, int32_t N, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW,
                       cis_stream_t stream);

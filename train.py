@@ -1,5 +1,6 @@
 """Training CLI with the reference's flag surface (its train.py:16-43): fixed seed 8964, flag dump, then
-`AdversarialLearner().train(FLAGS)`.  Under torchrun every rank runs this file; only rank 0 prints."""
+`AdversarialLearner().train(FLAGS)`.  Under torchrun every rank runs this file; only rank 0 prints.  --flow_dir (flow_flags.py)
+trains on supplied flow instead of PWC-Net's; --flow_ckpt is then not read."""
 import os
 import pprint
 import random
@@ -9,6 +10,7 @@ import numpy as np
 import torch
 from absl import flags as absl_flags
 
+from unsupervised_detection_b200 import flow_flags
 from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES
 from unsupervised_detection_b200.models.adversarial_learner import AdversarialLearner
 
@@ -23,7 +25,7 @@ def seed_everything(seed=SEED):
 def run(config):
     seed_everything()
     if int(os.environ.get('RANK', '0')) == 0:
-        pprint.pprint({name: getattr(config, name) for name in FLAG_NAMES})
+        pprint.pprint({name: getattr(config, name) for name in FLAG_NAMES + ['flow_dir']})
     if config.checkpoint_dir:
         os.makedirs(config.checkpoint_dir, exist_ok=True)
     AdversarialLearner().train(config)
@@ -32,6 +34,7 @@ def run(config):
 def main(argv):
     try:
         FLAGS(argv)
+        flow_flags.check(FLAGS)
     except absl_flags.Error as err:
         sys.exit('%s\nUsage: %s ARGS\n%s' % (err, argv[0], FLAGS))
     run(FLAGS)

@@ -86,6 +86,7 @@ _PROTOS = {
     'cis_upsample_nn2x': [_p, _i32, _i32, _i32, _i32, _p],
     'cis_upsample_nn2x_bwd': [_p, _i32, _i32, _i32, _i32, _p, _i32],
     'cis_crop_resize_bilinear_f32': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32],
+    'cis_crop_resize_flow_f32': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _f32, _f32],
     'cis_resize_nn_f32': [_p, _i32, _i32, _i32, _i32, _p, _i32, _i32],
     'cis_resize_f32': [_p, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32, _i32],
     'cis_resize_f32_bwd': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32, _i32],

@@ -654,9 +654,12 @@ __global__ void resize_bilinear_f32_kernel(const float* __restrict__ src, int N,
   }
 }
 // central crop + legacy-bilinear resize back to OH x OW of ONE fp32 NHWC image (the multi-crop ensemble inputs,
-// davis2016_data_utils.py:328-354 / 130-134): crop box (y0, x0, ch, cw) of the Hs x Ws source, same interpolation rule as above
+// davis2016_data_utils.py:328-354 / 130-134): crop box (y0, x0, ch, cw) of the Hs x Ws source, same interpolation rule as above.
+// FLOW = true: a 2-channel flow field whose vectors follow the resize, channel 0 times s0 and channel 1 times s1 (cis_crop_resize_flow_f32);
+// FLOW = false reads neither scale and is the plain image crop.
+template <bool FLOW>
 __global__ void crop_resize_f32_kernel(const float* __restrict__ src, int Ws, int C, int y0, int x0, int ch, int cw, float* __restrict__ dst,
-                                       int OH, int OW) {
+                                       int OH, int OW, float s0, float s1) {
   pdl_launch_dependents();
   pdl_wait();
   const int pix = blockIdx.x * blockDim.x + threadIdx.x;
@@ -669,7 +672,8 @@ __global__ void crop_resize_f32_kernel(const float* __restrict__ src, int Ws, in
     const float tl = r0[(x0 + lx.lo) * C + c], tr = r0[(x0 + lx.hi) * C + c];
     const float bl = r1[(x0 + lx.lo) * C + c], br = r1[(x0 + lx.hi) * C + c];
     const float t = tl + (tr - tl) * lx.f, bo = bl + (br - bl) * lx.f;
-    dst[(size_t)pix * C + c] = t + (bo - t) * ly.f;
+    const float v = t + (bo - t) * ly.f;
+    dst[(size_t)pix * C + c] = FLOW ? v * (c == 0 ? s0 : s1) : v;
   }
 }
 // transpose of the fp32 legacy resize (times `scale`, the factor of cis_resize_bilinear_f32), result stored as a bf16 8-channel chunk
@@ -1949,8 +1953,15 @@ int cis_crop_resize_bilinear_f32(const float* src, int32_t Hs, int32_t Ws, int32
                                  int32_t OH, int32_t OW, cis_stream_t stream) {
   if (!src || !dst || y0 < 0 || x0 < 0 || ch < 1 || cw < 1 || y0 + ch > Hs || x0 + cw > Ws || OH < 1 || OW < 1)
     return cis_set_error(CIS_ERR_BAD_ARG, "cis_crop_resize_bilinear_f32: crop box outside the image");
-  CIS_LAUNCH(crop_resize_f32_kernel, nblk((size_t)OH * OW), 256, 0, ST, src, Ws, C, y0, x0, ch, cw, dst, OH, OW);
+  CIS_LAUNCH(crop_resize_f32_kernel<false>, nblk((size_t)OH * OW), 256, 0, ST, src, Ws, C, y0, x0, ch, cw, dst, OH, OW, 1.f, 1.f);
   return cis_check_launch("crop_resize_f32");
+}
+int cis_crop_resize_flow_f32(const float* src, int32_t Hs, int32_t Ws, int32_t y0, int32_t x0, int32_t ch, int32_t cw, float* dst, int32_t OH,
+                             int32_t OW, float s0, float s1, cis_stream_t stream) {
+  if (!src || !dst || y0 < 0 || x0 < 0 || ch < 1 || cw < 1 || y0 + ch > Hs || x0 + cw > Ws || OH < 1 || OW < 1)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_crop_resize_flow_f32: crop box outside the image");
+  CIS_LAUNCH(crop_resize_f32_kernel<true>, nblk((size_t)OH * OW), 256, 0, ST, src, Ws, 2, y0, x0, ch, cw, dst, OH, OW, s0, s1);
+  return cis_check_launch("crop_resize_flow_f32");
 }
 int cis_upsample_nn2x(const void* src, int32_t N, int32_t H, int32_t W, int32_t pitch, void* dst, cis_stream_t stream) {
   if ((size_t)N * 2 * H > 65535) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_upsample_nn2x: too many rows");

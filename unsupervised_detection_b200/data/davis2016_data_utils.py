@@ -5,6 +5,13 @@ Same folder contract (`ImageSets/480p/{train,val,trainval}.txt` listing `/JPEGIm
 /Annotations/480p/<seq>/<frame>.png`), same sampling (frame pairs with a temporal shift in [min,max]_temporal_len forward from
 the head of a sequence / backward from its tail), same preprocessing (x/255-0.5, legacy-bilinear resize to 384x640, random
 flips applied to both frames, random / central crop resized back).  JPEG decoding and augmentation stay on the CPU.
+
+Supplied flow (flow_dir, not in the reference): the flow of a frame pair is one Middlebury .flo file under flow_dir (flow_file gives its
+name), read next to the frames and added to every batch as a fifth element, (img1, img2, seg1, fnames, flow [B,384,640,2]) in PWC-Net's
+channel order and sign.  It goes through the Flying Chairs conversion: resampled to 384x640 with its vectors rescaled
+(flow_to_grid), then flipped and cropped with the frames' own draws (augment_flow) for a training pair, or cut to the same central
+test_crop box for a test pair, and finally pwc_flow_from_uv.  This is a geometric transform of the field: PWC-Net run on the augmented
+frames gives the same flow only for no flip and a crop of 1.0.  Without flow_dir every batch is what it was.
 """
 import collections
 import copy
@@ -21,6 +28,18 @@ import torch
 from .. import _lib
 
 ORIG_H, ORIG_W = 384, 640   # preprocess_image :87-90
+
+
+def flow_file(flow_dir, root_dir, f1, f2):
+    """The .flo file of the frame pair (f1, f2), frame paths under root_dir: <flow_dir>/<directory of f1 relative to root_dir>/<file
+    name of f1 without extension>__<file name of f2 without extension>.flo, e.g. JPEGImages/480p/bear/00003__00001.flo for frame 3 to
+    frame 1.  One file per ordered pair, so every temporal shift and direction has its own.  The two frames must share a directory
+    (the readers never pair frames of two sequences); ValueError otherwise, and for a frame outside root_dir."""
+    d1, d2 = (os.path.dirname(os.path.relpath(f, root_dir)) for f in (f1, f2))
+    if d1 != d2 or d1 == os.pardir or d1.startswith(os.pardir + os.sep):
+        raise ValueError('frame pair %s, %s: both frames must lie in one directory under %s' % (f1, f2, root_dir))
+    stem = lambda f: os.path.splitext(os.path.basename(f))[0]
+    return os.path.join(flow_dir, d1, '%s__%s.flo' % (stem(f1), stem(f2)))
 
 
 class DirectoryIterator(object):
@@ -193,8 +212,10 @@ class _Iter(object):
 
     @staticmethod
     def _collect(futs):
+        """-> [img1, img2, seg1, fnames] (+ [flow] when the samples carry a supplied flow field as a fifth element)."""
         res = [f.result() for f in futs]
-        return [torch.from_numpy(np.stack([r[k] for r in res])) for k in range(3)] + [[r[3] for r in res]]
+        out = [torch.from_numpy(np.stack([r[k] for r in res])) for k in range(3)] + [[r[3] for r in res]]
+        return out + [torch.from_numpy(np.stack([r[4] for r in res]))] if len(res[0]) > 4 else out
 
     def _make(self, n):
         return self._collect(self._submit(n))
@@ -247,17 +268,18 @@ class _Iter(object):
                 raise out
         else:
             out = self._make(n)
-        ts = out[:3]
+        ts = out[:3] + out[4:]
         if pinned and torch.cuda.is_available():
             ts = [t.pin_memory() for t in ts]
-        return ts[0], ts[1], ts[2], out[3]
+        return (ts[0], ts[1], ts[2], out[3]) + tuple(ts[3:])
 
 
 class Davis2016Reader(object):
     """davis2016_data_utils.py:68-354."""
 
-    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=1, num_threads=6, seed=8964):
-        self.root_dir = root_dir
+    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=1, num_threads=6, seed=8964, flow_dir=''):
+        """flow_dir: root of the supplied .flo files (flow_file); '' = frames only."""
+        self.root_dir, self.flow_dir = root_dir, flow_dir
         self.max_temporal_len, self.min_temporal_len = max_temporal_len, min_temporal_len
         assert min_temporal_len < max_temporal_len, "Temporal lenghts are not consistenst"
         assert min_temporal_len > 0, "Min temporal len should be positive"
@@ -297,29 +319,77 @@ class Davis2016Reader(object):
         c = img[y0:y0 + ch, x0:x0 + cw]
         return nn_resize(c, h, w) if nearest else legacy_resize(c, h, w)   # the reference resizes masks bilinearly here too (:133)
 
+    # ---- supplied flow
+    def flow_path(self, f1, f2):
+        """The .flo file of the frame pair (f1, f2) under self.flow_dir (flow_file)."""
+        return flow_file(self.flow_dir, self.root_dir, f1, f2)
+
+    def _with_flow(self, sample, f1, f2, case, box):
+        """sample + (the supplied flow of (f1, f2) after flip `case` and crop `box` = (y0, x0, ch, cw) of the 384x640 grid,) when a
+        flow_dir is set.  IOError naming the file when it is missing or unreadable."""
+        if not self.flow_dir:
+            return sample
+        from .flyingchairs_data_utils import augment_flow, flow_to_grid, pwc_flow_from_uv, read_flo
+        path = self.flow_path(f1, f2)
+        if not os.path.isfile(path):
+            raise IOError('missing flow file %s (frame pair %s -> %s)' % (path, f1, f2))
+        return sample + (pwc_flow_from_uv(augment_flow(flow_to_grid(read_flo(path)), case, *box)).astype(np.float32),)
+
     # ---- samples
+    def _train_frames(self, pair, t_shift):
+        """(frame 1, frame 2) file names of training pair `pair` = (index of frame 1, direction) at temporal shift t_shift."""
+        i1, direction = pair
+        return self.filenames[i1], self.filenames[int(t_shift * direction + i1)]
+
+    def _test_frames(self, pair):
+        """(frame 1, frame 2) file names of test pair `pair`."""
+        i1, direction = pair
+        return self.filenames[i1], self.filenames[int(self.test_t_len * direction + i1)]
+
     def _train_sample(self, pair, seed):
         """dataset_map :150-178 + augment_pair :136-148 + aug_flips.random_flip_images."""
         r = random.Random(seed)
-        i1, direction = pair
-        t_shift = r.randint(self.min_temporal_len, self.max_temporal_len)
-        i2 = int(t_shift * direction + i1)
-        a, b = self.preprocess_image(self.filenames[i1]), self.preprocess_image(self.filenames[i2])
+        f1, f2 = self._train_frames(pair, r.randint(self.min_temporal_len, self.max_temporal_len))
+        a, b = self.preprocess_image(f1), self.preprocess_image(f2)
         h, w = a.shape[:2]
         case, y0, x0, ch, cw = train_augmentation(r, self.train_crop, h, w)
         a = crop_resized(flip(a, case), y0, x0, ch, cw)
         b = crop_resized(flip(b, case), y0, x0, ch, cw)
-        return a.astype(np.float32), b.astype(np.float32), np.ones((h, w, 1), np.float32), self.filenames[i1]
+        sample = a.astype(np.float32), b.astype(np.float32), np.ones((h, w, 1), np.float32), f1
+        return self._with_flow(sample, f1, f2, case, (y0, x0, ch, cw))
 
     def _test_sample(self, pair, seed):
         """test_dataset_map :293-326."""
-        i1, direction = pair
-        i2 = int(self.test_t_len * direction + i1)
-        a, b = self.preprocess_image(self.filenames[i1]), self.preprocess_image(self.filenames[i2])
-        s = self.preprocess_mask(self.annotation_filenames[i1])
+        f1, f2 = self._test_frames(pair)
+        a, b = self.preprocess_image(f1), self.preprocess_image(f2)
+        s = self.preprocess_mask(self.annotation_filenames[pair[0]])
         c = self.test_crop
-        return (self.central_cropping(a, c).astype(np.float32), self.central_cropping(b, c).astype(np.float32),
-                self.central_cropping(s, c).astype(np.float32), self.filenames[i1])
+        sample = (self.central_cropping(a, c).astype(np.float32), self.central_cropping(b, c).astype(np.float32),
+                  self.central_cropping(s, c).astype(np.float32), f1)
+        return self._with_flow(sample, f1, f2, 0, central_crop_box(ORIG_H, ORIG_W, c))
+
+    # ---- the frame pairs a partition can draw (the files export_flow.py writes and a flow_dir must hold).  They are read off the
+    # iterators themselves, built on a copy of the reader so that neither its state nor its random stream moves.
+    def _probe(self):
+        rd = copy.copy(self)
+        rd.rng, rd.prefetch = random.Random(0), 0
+        return rd
+
+    def train_frame_pairs(self, partition='train'):
+        """Every (frame 1, frame 2) file pair image_inputs(partition=partition) can draw: each forward / backward pair at each shift in
+        [min_temporal_len, max_temporal_len]."""
+        it = self._probe().image_inputs(partition=partition)
+        shifts = range(self.min_temporal_len, self.max_temporal_len + 1)
+        return [it.view._train_frames(pr, s) for pr in it.pairs for s in shifts]
+
+    def test_frame_pairs(self, partition='val', t_len=2):
+        """The (frame 1, frame 2) file pairs of test_inputs(partition=partition, t_len=t_len), in its order."""
+        it = self._probe().test_inputs(partition=partition, t_len=t_len)
+        return [it.view._test_frames(pr) for pr in it.pairs]
+
+    def frame_pairs(self, partition, t_len):
+        """Sorted, without repeats: every pair a training iterator and a test iterator at temporal shift t_len of `partition` read."""
+        return sorted(set(self.train_frame_pairs(partition)) | set(self.test_frame_pairs(partition, t_len)))
 
     # ---- iterators
     def image_inputs(self, batch_size=32, partition='train', train_crop=1.0, num_threads=6):

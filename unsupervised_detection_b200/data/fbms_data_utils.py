@@ -17,7 +17,7 @@ import re
 import cv2
 import numpy as np
 
-from .davis2016_data_utils import Davis2016Reader, _Iter, nn_resize, ORIG_H, ORIG_W
+from .davis2016_data_utils import Davis2016Reader, _Iter, central_crop_box, nn_resize, ORIG_H, ORIG_W
 
 
 def _read_bmf(path):
@@ -113,8 +113,8 @@ class FBMS59Reader(Davis2016Reader):
     """fbms_data_utils.py:179-389.  image_inputs / augmentation / central cropping are inherited (identical code in the
     reference); only the directory layout and the test tuples differ."""
 
-    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=2, num_threads=6, seed=8964):
-        Davis2016Reader.__init__(self, root_dir, max_temporal_len, min_temporal_len, num_threads, seed)
+    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=2, num_threads=6, seed=8964, flow_dir=''):
+        Davis2016Reader.__init__(self, root_dir, max_temporal_len, min_temporal_len, num_threads, seed, flow_dir)
 
     def get_filenames_list(self, partition):
         it = DirectoryIterator(self.root_dir, partition)
@@ -128,14 +128,18 @@ class FBMS59Reader(Davis2016Reader):
         self.num_categories = len(it.samples_per_cat)
         return it.test_tuples
 
+    def _test_frames(self, tup):
+        return tup[0], tup[1]
+
     def _test_sample(self, tup, seed):
         """test_dataset_map :337-359."""
         f1, f2, ann, cat, weird, _ = tup
         a, b = self.preprocess_image(f1), self.preprocess_image(f2)
         s = nn_resize(binarise_gt(ann, cat, weird).astype(np.float32)[..., None] / np.float32(255.0), ORIG_H, ORIG_W)
         c = self.test_crop
-        return (self.central_cropping(a, c).astype(np.float32), self.central_cropping(b, c).astype(np.float32),
-                self.central_cropping(s, c).astype(np.float32), f1)
+        sample = (self.central_cropping(a, c).astype(np.float32), self.central_cropping(b, c).astype(np.float32),
+                  self.central_cropping(s, c).astype(np.float32), f1)
+        return self._with_flow(sample, f1, f2, 0, central_crop_box(ORIG_H, ORIG_W, c))
 
     def test_inputs(self, batch_size=32, partition='val', t_len=2, with_fname=False, test_crop=1.0):
         """:311-335 -> ordered iterator over the annotated frames of every category."""

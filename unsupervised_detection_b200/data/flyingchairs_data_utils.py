@@ -36,6 +36,18 @@ def read_flo(path):
     return flow
 
 
+def write_flo(path, uv):
+    """float32 [H,W,2] (u, v) -> Middlebury .flo at `path` (the layout read_flo reads), written to a temporary name and renamed into
+    place, so a reader never sees a partial file.  Parent directories are created."""
+    uv = np.ascontiguousarray(uv, dtype='<f4')
+    h, w = uv.shape[:2]
+    os.makedirs(os.path.dirname(os.path.abspath(path)), exist_ok=True)
+    tmp = '%s.%d.tmp' % (path, os.getpid())
+    with open(tmp, 'wb') as f:
+        f.write(np.float32(FLO_TAG).astype('<f4').tobytes() + np.array([w, h], '<i4').tobytes() + uv.tobytes())
+    os.replace(tmp, path)
+
+
 def pwc_flow_from_uv(uv):
     """Middlebury flow (u, v) [...,2] -> the flow PWC-Net hands to the recover net: channel 0 = -v, channel 1 = -u.
 
@@ -47,6 +59,11 @@ def pwc_flow_from_uv(uv):
     flow1 = -u: the field that makes the network's own warp consistent is (row, column) ordered and points from frame 2 back to frame 1.
     This follows from the warp alone; it has not been compared with the output of a trained PWC-Net checkpoint."""
     return np.stack([-uv[..., 1], -uv[..., 0]], axis=-1)
+
+
+def uv_from_pwc_flow(flow):
+    """The exact inverse of pwc_flow_from_uv: PWC-Net's flow [...,2] -> Middlebury (u, v) = (-flow1, -flow0)."""
+    return np.stack([-flow[..., 1], -flow[..., 0]], axis=-1)
 
 
 def flow_to_grid(uv):

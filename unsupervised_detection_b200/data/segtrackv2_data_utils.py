@@ -53,8 +53,8 @@ class DirectoryIterator(object):
 class SegTrackV2Reader(Davis2016Reader):
     """segtrackv2_data_utils.py:73-308 (no partitions: training and evaluation both walk the whole dataset)."""
 
-    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=2, num_threads=6, seed=8964):
-        Davis2016Reader.__init__(self, root_dir, max_temporal_len, min_temporal_len, num_threads, seed)
+    def __init__(self, root_dir, max_temporal_len=3, min_temporal_len=2, num_threads=6, seed=8964, flow_dir=''):
+        Davis2016Reader.__init__(self, root_dir, max_temporal_len, min_temporal_len, num_threads, seed, flow_dir)
 
     def get_filenames_list(self, partition=None):
         it = DirectoryIterator(self.root_dir)

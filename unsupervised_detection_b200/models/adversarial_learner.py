@@ -3,7 +3,9 @@
 Kept API: AdversarialLearner().train(config) / .setup_inference(config, aug_test=False) / .inference(sess) with the same
 result keys (:617-619), plus .step() = one iteration of the loop body (:380-409) and .pretrain_recover(config) = pretraining of the
 recover net on box-shaped occlusions (the pre-training behind --recover_ckpt that the reference's README describes), on PWC-Net's flow or
-a dataset's ground-truth flow, with .validate_recover() = its held-out inpainting error.  `sess` arguments are accepted and
+a dataset's ground-truth flow, with .validate_recover() = its held-out inpainting error.  With config.flow_dir set (not in the
+reference), every graph takes a supplied flow field in place of PWC-Net's (CISGraph(flow_source='input')): training, validation IoU,
+inference and the multi-crop ensemble, with no PWC-Net built and no --flow_ckpt read.  `sess` arguments are accepted and
 ignored (there is no tf.Session).  Data parallelism (not in the reference): one process per GPU, the frame-pair batch is
 sharded over ranks and the active network's flat gradient buffer is summed with ONE NCCL all-reduce per step
 (SURVEY.md section 8e); clip / noise test / Adam then run identically on every rank.
@@ -21,6 +23,7 @@ from .PWCNet import model_pwcnet
 from ..data.synthetic import SyntheticReader
 from .. import params_init
 from .. import checkpoint as ckpt_io
+from .. import flow_flags                               # defines --flow_dir for every script that drives the learner
 from .utils.general_utils import compute_all_IoU
 
 
@@ -28,6 +31,13 @@ from .utils.general_utils import compute_all_IoU
 PIPELINE = os.environ.get('CIS_PIPELINE', '1') != '0'
 # datasets whose batches carry ground-truth flow (img1, img2, flow, names): recover-net pretraining with pretrain_flow=gt
 FLOW_DATASETS = ('FLYINGCHAIRS',)
+# datasets with masks; with a flow_dir their batches carry the supplied flow as a fifth element (img1, img2, seg1, names, flow)
+MASK_DATASETS = ('DAVIS2016', 'FBMS', 'SEGTRACK')
+
+
+def has_flow(dataset, flow_dir):
+    """True when the batches of `dataset` carry flow: ground-truth flow (FLOW_DATASETS), or a mask dataset read with a flow_dir."""
+    return dataset in FLOW_DATASETS or (dataset in MASK_DATASETS and bool(flow_dir))
 
 
 def _dist():
@@ -50,11 +60,14 @@ class AdversarialLearner(object):
     _pretrain = False                                   # recover-net pretraining: datasets with flow (FLYINGCHAIRS) are accepted
     val_graph = None                                    # forward-only boxes graph of validate_recover, built on first use
     min_val_epe = math.inf
+    _summary_img2 = None                                # frame 2 of the last summary step's batch (an input-flow graph has no img2)
 
     # ------------------------------------------------------------------------------------------------ data
     def load_training_data(self):
         """adversarial_learner.py:22-70.  Dataset readers are host-side code outside the accelerated path (SURVEY 8f-2);
-        'SYNTHETIC' yields seeded frame pairs of the readers' shape.  Unknown datasets raise IOError like the reference."""
+        'SYNTHETIC' yields seeded frame pairs of the readers' shape.  Unknown datasets raise IOError like the reference.  A flow_dir
+        needs a mask dataset (ValueError) and an existing directory (IOError)."""
+        flow_flags.validate(self.config)
         ds = self.config.dataset
         if ds == 'SYNTHETIC':
             self.reader = SyntheticReader(PWC_H, PWC_W, seed=8964 + self.rank)
@@ -69,7 +82,7 @@ class AdversarialLearner(object):
             self.reader = self.dataset_reader.image_inputs(batch_size=cfg.batch_size, train_crop=cfg.train_crop)
             self.num_samples_val = self.dataset_reader.val_samples
             return
-        if ds in ('DAVIS2016', 'FBMS', 'SEGTRACK'):
+        if ds in MASK_DATASETS:
             cfg = self.config
             if ds == 'DAVIS2016':
                 from ..data.davis2016_data_utils import Davis2016Reader as Reader
@@ -80,7 +93,7 @@ class AdversarialLearner(object):
             else:
                 from ..data.segtrackv2_data_utils import SegTrackV2Reader as Reader
             rd = Reader(cfg.root_dir, max_temporal_len=cfg.max_temporal_len, min_temporal_len=cfg.min_temporal_len,
-                        num_threads=cfg.num_threads, seed=8964 + self.rank)
+                        num_threads=cfg.num_threads, seed=8964 + self.rank, flow_dir=self.flow_dir())
             self.dataset_reader = rd
             if self._inference:
                 self.reader = rd.test_inputs(batch_size=cfg.batch_size, t_len=cfg.test_temporal_shift, with_fname=True,
@@ -101,6 +114,13 @@ class AdversarialLearner(object):
         raise IOError("Dataset should be DAVIS2016 / FBMS / SEGTRACK")
 
     # ------------------------------------------------------------------------------------------------ graphs
+    def flow_dir(self):
+        """config.flow_dir: the directory of supplied .flo files, '' (or absent) = PWC-Net's flow."""
+        return getattr(self.config, 'flow_dir', '') or ''
+
+    def _flow_source(self):
+        return 'input' if self.flow_dir() else 'pwc'
+
     def _init_dist(self):
         self.world, self.rank, self.local_rank = 1, 0, 0
         if int(os.environ.get('WORLD_SIZE', '1')) > 1:
@@ -123,7 +143,7 @@ class AdversarialLearner(object):
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
                               flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
-                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
+                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self.val_steps_per_epoch = int(np.ceil(float(self.num_samples_val) / cfg.batch_size))
         self._init_params()
@@ -165,16 +185,8 @@ class AdversarialLearner(object):
         p.update(params_init.init_generator())
         p.update(params_init.init_recover())
         g = self.graph
-        fc = getattr(cfg, 'flow_ckpt', '')
-        if g.flow_source == 'input':
-            pass                                                                # ground-truth flow: the graph has no PWC-Net
-        elif fc.startswith('synthetic'):
-            p.update(params_init.init_pwcnet(g.pwc_store.entries))
-        elif self._is_ckpt(fc):
-            p.update(self._read_ckpt(fc, self._names('pwcnet'))[0])               # flow_saver.restore, adversarial_learner.py:339-341
-            print("Flow net loaded from {}".format(fc))
-        else:
-            raise IOError("Could not find flow ckpt file. Aborting.")          # adversarial_learner.py:343
+        if g.flow_source != 'input':                                            # supplied flow: the graph has no PWC-Net
+            p.update(self.flow_net_params())
         if getattr(cfg, 'resume_train', False):
             ck = cfg.full_model_ckpt if self._is_ckpt(cfg.full_model_ckpt) else self._latest_checkpoint(cfg.checkpoint_dir)
             assert ck, "Found no checkpoint to resume training!"               # :351
@@ -191,6 +203,18 @@ class AdversarialLearner(object):
         else:
             print("No recover checkpoint found! Train Recover from Scratch")   # :360
         g.load_params(p)
+
+    def flow_net_params(self):
+        """PWC-Net's parameters for self.graph from config.flow_ckpt ('synthetic...' = the seeded stand-in) -> dict; IOError without
+        a checkpoint."""
+        fc = getattr(self.config, 'flow_ckpt', '')
+        if fc.startswith('synthetic'):
+            return params_init.init_pwcnet(self.graph.pwc_store.entries)
+        if self._is_ckpt(fc):
+            p = self._read_ckpt(fc, self._names('pwcnet'))[0]                    # flow_saver.restore, adversarial_learner.py:339-341
+            print("Flow net loaded from {}".format(fc))
+            return p
+        raise IOError("Could not find flow ckpt file. Aborting.")              # adversarial_learner.py:343
 
     @staticmethod
     def _latest_checkpoint(d):
@@ -266,7 +290,9 @@ class AdversarialLearner(object):
         if batch is None:
             batch = self.reader.batch(self.local_batch)
         summarize = summarize and step % cfg.summary_freq == 0                 # :391-394 (same decision on every rank)
-        other_grads = self._train_on(mode, batch, next_batch, use_graph, summarize)
+        if summarize:
+            self._summary_img2 = batch[1]
+        other_grads = self._train_on(mode, self._uploads(batch), self._uploads(next_batch), use_graph, summarize)
         res = {"global_step": self.global_step, "train_op": mode}
         fetch = fetch_losses if fetch_losses is not None else (step % cfg.summary_freq == 0)
         if fetch or summarize:
@@ -346,7 +372,7 @@ class AdversarialLearner(object):
         rec = pred[:B] * mask + flow * (1.0 - mask)                            # self.pred_flow, :251
         rec_c = pred[:B] * (1.0 - mask) + flow * mask                          # self.pred_flow_compl, :252 (the PRIMARY prediction, as the reference)
         w.add_image("input_image", g.image[:1].cpu().numpy())                  # :265-268
-        w.add_image("next_image", g.img2[:1].cpu().numpy())
+        w.add_image("next_image", (g.img2 if g.img2 is not None else self._summary_img2)[:1].cpu().numpy())
         flow_img = flow_to_image_pm(flow)
         w.add_image("masked_flow", flow_img * (1.0 - disambiguate_forw_back(mask)))   # :269-272
         w.add_image("PWC_Flow", flow_img)
@@ -398,8 +424,9 @@ class AdversarialLearner(object):
         validation_iou = 0.0
         vr = self.val_reader or self.reader
         for _ in range(self.val_steps_per_epoch):
-            img1, img2, gt, _ = vr.batch(self.local_batch)
-            self.feed(img1, img2)
+            batch = vr.batch(self.local_batch)
+            gt = batch[2]
+            self.feed(*self._uploads(batch))
             self.graph.forward()
             masks = self.graph.mask.cpu().numpy()
             gtr = torch.nn.functional.interpolate(gt.permute(0, 3, 1, 2), size=masks.shape[1:3], mode='nearest').permute(0, 2, 3, 1).numpy()
@@ -427,7 +454,8 @@ class AdversarialLearner(object):
         """The recover step of adversarial_learner.py:72-258 with one random box per sample as the mask: PWC-Net -> resize -> box masks ->
         3x recover -> losses -> train_recover_op.  No generator runs.  config.box_min / box_max = box side range as fractions of the
         image sides (defaults 0.1 / 0.5).  config.pretrain_flow = 'pwc' (default: PWC-Net's flow of the frame pair) or 'gt' (the
-        dataset's ground-truth flow, FLYINGCHAIRS: no PWC-Net is built and --flow_ckpt is not read)."""
+        dataset's ground-truth flow, FLYINGCHAIRS, or the supplied flow of a mask dataset with config.flow_dir: no PWC-Net is built and
+        --flow_ckpt is not read)."""
         cfg = self.config
         self._init_dist()
         if cfg.batch_size % self.world:
@@ -435,8 +463,11 @@ class AdversarialLearner(object):
         self.local_batch = cfg.batch_size // self.world
         box = box_sides(getattr(cfg, 'box_min', 0.1), getattr(cfg, 'box_max', 0.5), cfg.img_height, cfg.img_width)
         gt = getattr(cfg, 'pretrain_flow', 'pwc') == 'gt'
-        if gt and cfg.dataset not in FLOW_DATASETS:
-            raise ValueError('pretrain_flow=gt needs a dataset with ground-truth flow (%s), got %s' % (', '.join(FLOW_DATASETS), cfg.dataset))
+        if gt and not has_flow(cfg.dataset, self.flow_dir()):
+            raise ValueError('pretrain_flow=gt needs a dataset with ground-truth flow (%s) or a mask dataset (%s) with a flow_dir, got %s'
+                             % (', '.join(FLOW_DATASETS), ', '.join(MASK_DATASETS), cfg.dataset))
+        if self.flow_dir() and not gt:
+            raise ValueError('a flow_dir replaces PWC-Net: recover-net pretraining on it needs pretrain_flow=gt')
         self._pretrain = True
         self.load_training_data()
         # sample_offset: sample b of rank r is global sample r * local_batch + b, so a DP job draws the boxes of one GPU running the global batch
@@ -448,11 +479,14 @@ class AdversarialLearner(object):
         self._init_params()
 
     def _uploads(self, batch):
-        """The two tensors of a reader batch (img1, img2, ... ) that the graph uploads: (frame 1, frame 2), or (frame 1, its flow) under
-        ground-truth flow (a flow reader's batch is (img1, img2, flow, names))."""
+        """The two tensors of a reader batch (img1, img2, ... ) that the graph uploads: (frame 1, frame 2), or (frame 1, its flow) for an
+        input-flow graph (a Flying Chairs batch is (img1, img2, flow, names), a mask dataset's with a flow_dir (img1, img2, seg1, names,
+        flow))."""
         if batch is None:
             return None
-        return (batch[0], batch[2]) if self.graph.flow_source == 'input' else (batch[0], batch[1])
+        if getattr(self.graph, 'flow_source', 'pwc') != 'input':         # host-side graph stubs model the default graph
+            return batch[0], batch[1]
+        return batch[0], batch[4 if len(batch) > 4 else 2]
 
     def pretrain_step(self, batch, next_batch=None, fetch_losses=False, use_graph=True):
         """One pretraining iteration: train_recover_op on `batch` under box masks (one NCCL all-reduce of the recover gradient under
@@ -570,7 +604,7 @@ class AdversarialLearner(object):
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
                               cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False,
-                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
+                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 
@@ -584,7 +618,7 @@ class AdversarialLearner(object):
         self._inference = True
         self.load_training_data()
         self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
-                              with_pwc=True, train=False, pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS)
+                              with_pwc=True, train=False, pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 
@@ -598,7 +632,8 @@ class AdversarialLearner(object):
             self.build_test_graph()
 
     def restore(self, ckpt_file):
-        """test_generator.py:45-58: restores ALL trainables (incl. PWC-Net) from one checkpoint (TF V2 bundle or native `.pt`)."""
+        """test_generator.py:45-58: restores ALL trainables (incl. PWC-Net) from one checkpoint (TF V2 bundle or native `.pt`).  An
+        input-flow graph has no PWC-Net, so its variables are neither needed nor read."""
         if ckpt_file.startswith('synthetic'):
             p = {}
             p.update(params_init.init_generator())
@@ -614,7 +649,9 @@ class AdversarialLearner(object):
 
     def _device_crops(self, img1, img2, gt):
         """Multi-crop test-time augmentation on the device: host [1,Hs,Ws,C] tensors -> g.img1 / g.img2 rows (one per crop) and the
-        nearest-resized ground-truth crops [ncrop,H,W,1] (numpy).  Same geometry and interpolation as data/crops.central_crops."""
+        nearest-resized ground-truth crops [ncrop,H,W,1] (numpy).  Same geometry and interpolation as data/crops.central_crops.  For an
+        input-flow graph img2 is frame 1's flow [1,Hs,Ws,2]: its crops go to g.flow_full with the vectors scaled to the resize
+        (cis_crop_resize_flow_f32: rows by Hs/ch, columns by Ws/cw)."""
         from ..data.davis2016_data_utils import central_crop_box
         from .. import _lib
         g = self.graph
@@ -629,8 +666,12 @@ class AdversarialLearner(object):
             self._gt_small = torch.empty(nc, g.H, g.W, 1, dtype=torch.float32, device=dev)
         for i, c in enumerate(self.test_crops):
             y0, x0, ch, cw = central_crop_box(hs, ws, c)
-            for src, dst, C_ in ((d1, g.img1[i], 3), (d2, g.img2[i], 3), (dg, self._gt_crops[i], 1)):
+            frames = [(d1, g.img1[i], 3)] + ([(d2, g.img2[i], 3)] if g.img2 is not None else [])
+            for src, dst, C_ in frames + [(dg, self._gt_crops[i], 1)]:
                 _lib.call('cis_crop_resize_bilinear_f32', src.data_ptr(), hs, ws, C_, y0, x0, ch, cw, dst.data_ptr(), hs, ws, st)
+            if g.img2 is None:
+                _lib.call('cis_crop_resize_flow_f32', d2.data_ptr(), hs, ws, y0, x0, ch, cw, g.flow_full[i].data_ptr(), hs, ws, hs / ch, ws / cw,
+                          st)
         _lib.call('cis_resize_nn_f32', self._gt_crops.data_ptr(), nc, hs, ws, 1, self._gt_small.data_ptr(), g.H, g.W, st)
         self._keep_crop_src = (d1, d2, dg)
         return self._gt_small.cpu().numpy()
@@ -640,7 +681,7 @@ class AdversarialLearner(object):
         g = self.graph
         if batch is None:
             batch = self.reader.batch(1 if self.aug_test else self.local_batch)
-        img1, img2, gt, names = batch
+        (img1, img2), gt, names = self._uploads(batch), batch[2], batch[3]
         H, W = g.H, g.W
         if self.aug_test:
             # crops [0.85,0.9,0.95,1.0] of ONE frame pair, each resized back to 384x640 (davis2016_data_utils.py:328-354): the frame

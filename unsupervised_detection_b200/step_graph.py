@@ -4,6 +4,7 @@ One `CISGraph` owns the parameters (flat fp32 master copies per scope), all acti
 (batch, 384x640 -> HxW) geometry, and the launch lists: forward (PWC-Net -> resize -> generator -> mask (x) flow ->
 3x recover -> Charbonnier losses), backward for the recover step, backward for the generator step, and clip + TF-Adam.
 With masks='boxes' the same graph pretrains the recover net: random boxes (cis_box_masks) replace the generator, which is not built.
+With flow_source='input' a supplied flow field replaces PWC-Net, for either mask source.
 """
 import torch
 
@@ -29,25 +30,32 @@ def box_sides(box_min, box_max, H, W):
 
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
-                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks='generator', box=None,
+                 beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks=None, box=None,
                  sample_offset=0, flow_source='pwc'):
         """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS).
-        masks: 'generator' (the adversarial graph) or 'boxes' (pretraining of the recover net): one random box per sample, drawn on the
-        device by cis_box_masks, replaces the generator's mask; the generator is neither run nor trained and only the recover step
+        masks: 'generator' (the adversarial graph; None means it on PWC-Net's flow) or 'boxes' (pretraining of the recover net): one
+        random box per sample, drawn on the device by cis_box_masks, replaces the generator's mask; the generator is neither run nor trained and only the recover step
         exists.  box = (lo_h, hi_h, lo_w, hi_w) box sides in pixels (None = box_sides(0.1, 0.5, H, W)); sample_offset = global index of
         this rank's first sample (rank * batch under data parallelism), so that every sample of the global batch gets its own box.
         with_pwc=False: no 384x640 inputs at all; image and flow are written at HxW directly (no stage, no pipelined schedule).
-        flow_source: where the flow at 384x640 comes from.  'pwc' (the default): PWC-Net run on the frame pair img1 / img2.  'input'
-        (masks='boxes' only): a known flow field uploaded into flow_full next to img1, in PWC-Net's channel order and sign; no PWC-Net
-        is built.  The flow then reaches the recover net through the same resize and 1/flow_normalizer as PWC-Net's output, and the
-        stage, the pipelined schedule and the batch hand-over work on the pair (img1, flow_full) in place of (img1, img2)."""
+        flow_source: where the flow at 384x640 comes from.  'pwc' (the default): PWC-Net run on the frame pair img1 / img2.  'input':
+        a known flow field uploaded into flow_full next to img1, in PWC-Net's channel order and sign; no PWC-Net is built.  The flow
+        then reaches the generator and the recover net through the same resize and 1/flow_normalizer as PWC-Net's output, every launch
+        after take_stage is the 'pwc' graph's, and the stage, the pipelined schedule and the batch hand-over work on the pair
+        (img1, flow_full) in place of (img1, img2).  Both mask sources and train=True / False accept it, named explicitly: supplied
+        flow serves the recover-net pretraining (masks='boxes') as well as the adversarial graph (masks='generator'), and a graph that
+        silently became the other one would train the wrong network.  with_pwc=False does not accept it."""
+        if masks is None:
+            if flow_source == 'input':
+                raise ValueError("flow_source='input' needs the mask source named: masks='generator' or masks='boxes'")
+            masks = 'generator'
         _lib.load()
         if masks not in ('generator', 'boxes'):
             raise ValueError("masks must be 'generator' or 'boxes', got %r" % (masks,))
         if flow_source not in ('pwc', 'input'):
             raise ValueError("flow_source must be 'pwc' or 'input', got %r" % (flow_source,))
-        if flow_source == 'input' and (masks != 'boxes' or not with_pwc):
-            raise ValueError("flow_source='input' needs masks='boxes' and the 384x640 inputs (with_pwc=True)")
+        if flow_source == 'input' and not with_pwc:
+            raise ValueError("flow_source='input' needs the 384x640 inputs (with_pwc=True)")
         self.masks, self.flow_source = masks, flow_source
         boxes = masks == 'boxes'
         # Two attributes, two meanings: self.staged = the graph takes 384x640 uploads (self.inputs) that fwd.ops[:_pwc_ops] resizes into
@@ -284,6 +292,16 @@ class CISGraph(object):
             self._capture_plans('masks', [self._mask_plan]).replay()
         else:
             self._mask_plan.run()
+
+    def forward_flow(self):
+        """The frozen flow network alone on the frame pair in img1 / img2 -> self.flow_full [B,384,640,2] (PWC-Net's output, before the
+        resize to HxW): what export_flow.py writes.  ValueError for a graph without PWC-Net."""
+        if not self.with_pwc:
+            raise ValueError('forward_flow needs a graph that runs PWC-Net')
+        self._ensure_packed()
+        self.pipeline_drain()
+        self.stage_for = None
+        self._pipe_pwc.run()
 
     def set_sample_offset(self, sample_offset):
         """Global index of the first sample for the box draws of the next eager forward() (a validation pass sets it per batch).  The
