@@ -105,6 +105,12 @@ typedef struct {
   /* halo kernel, BN >= 64: 2 = two MMA warpgroups share every weight stage, each owning MT stacked tiles, so the CTA covers 2*MT tiles
    * (16*2*MT output rows per column of tiles; split-K scratch and the grid count CTAs of that height).  0/1: one warpgroup. */
   int32_t nwg;
+  /* halo kernel, stride 1, undilated, sources totalling 8 or 16 channels: the compact K-dense operand format.  0: 64-channel
+   * SWIZZLE_128B chunks, one K=16 step per tap.  8 / 16: the halo is staged without swizzle at 16 bytes per pixel, one plane per 8
+   * channels, so 8 consecutive halo pixels are one wgmma core matrix; a K=16 step covers two taps (8: taps 2s, 2s+1, LBO = the distance of
+   * their origins, which the host lists in increasing order) or one tap (16: LBO = the plane distance).  wpack / sub[].wpack then hold
+   * cis_pack_weights_tiled(thin) tiles. */
+  int32_t thin;
 } CisConv;
 
 /* Weight gradient of the same convolution: dWp[co][(t,c)] = sum_rows g[row][co] * A[row][(t,c)]  (fp32).  The reduction over rows
@@ -159,9 +165,11 @@ int cis_conv_wgrad(const CisWgrad* d, cis_stream_t stream);
 int cis_pack_weights(const float* w, const int32_t* kmap, int32_t K_pad, int32_t rows, int32_t cout, int32_t sn, const int32_t* nmap,
                      void* wp, cis_stream_t stream);
 /* halo-kernel operand: out[(ny, chunk, tap)][n][64] bf16 blocks of BN x 128 B with the SWIZZLE_128B pattern pre-applied; kmap is the
- * same tap-major map (k = tap*cin8 + channel). */
+ * same tap-major map (k = tap*cin8 + channel).  thin = 8 / 16 (CisConv.thin, cin8 == thin): out[(ny, step)] = BN x 32 B no-swizzle
+ * K=16 tiles instead, core matrix (n / 8, kgroup) at (n / 8) * 256 + kgroup * 128 bytes; kgroup j of step s is tap 2s + j (thin 8, zero
+ * past the last tap) or channels 8j .. 8j + 7 of tap s (thin 16). */
 int cis_pack_weights_tiled(const float* w, const int32_t* kmap, int32_t cin8, int32_t ntaps, int32_t n_tiles, int32_t BN, int32_t cout,
-                           int32_t sn, const int32_t* nmap, void* out, cis_stream_t stream);
+                           int32_t sn, const int32_t* nmap, void* out, int32_t thin, cis_stream_t stream);
 /* dw[kmap[k] + n*sn] = sum_{s < nsplit} dwp[s](n, k) for kmap[k] >= 0, n < cout (fixed summation order);
  * and, when colpart != NULL, the bias gradient db[c] = sum_{b < nblocks} colpart[b][c], c < nch (the partials of cis_colsum).
  * layout bits 0-7 = how cis_conv_wgrad stored a slice: 0 = [cout][K_pad] (CisWgrad.tma == 2), 1 = float4 columns [K_pad/4][cout][4]

@@ -582,8 +582,7 @@ struct HaloMaps {
 template <int NK, int MT, int BN, int MTM>
 __device__ __forceinline__ void halo_issue_stage(float (&acc)[MTM][BN], const uint32_t hlo, uint32_t blo, const uint32_t* s_aoff, const int gt,
                                                  const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep, const uint32_t a_half,
-                                                 const bool first) {
-  const uint32_t bstep = (uint32_t)(BN * 128) >> 4;
+                                                 const uint32_t bstep, const bool first) {
   uint32_t off0 = s_aoff[0], off1 = gt > 1 ? s_aoff[1] : 0u;
   int tt = 0;
 #pragma unroll 1
@@ -607,26 +606,43 @@ __device__ __forceinline__ void halo_issue_stage(float (&acc)[MTM][BN], const ui
 template <int MT, int BN, int MTM>
 __device__ __forceinline__ void halo_issue_nk(const int nk16, float (&acc)[MTM][BN], const uint32_t hlo, const uint32_t blo, const uint32_t* s_aoff,
                                               const int gt, const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep, const uint32_t a_half,
-                                              const bool first) {
-  if (nk16 == 4) halo_issue_stage<4, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
-  else if (nk16 == 1) halo_issue_stage<1, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
-  else if (nk16 == 2) halo_issue_stage<2, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
-  else halo_issue_stage<3, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+                                              const uint32_t bstep, const bool first) {
+  if (nk16 == 4) halo_issue_stage<4, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
+  else if (nk16 == 1) halo_issue_stage<1, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
+  else if (nk16 == 2) halo_issue_stage<2, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
+  else halo_issue_stage<3, MT>(acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
 }
 template <int BN, int MTM>
 __device__ __forceinline__ void halo_issue_any(const int nk16, float (&acc)[MTM][BN], const uint32_t hlo, const uint32_t blo, const uint32_t* s_aoff,
                                                const int gt, const int MT, const uint32_t ahi, const uint32_t bhi, const uint32_t a_mstep,
-                                               const uint32_t a_half, const bool first) {
+                                               const uint32_t a_half, const uint32_t bstep, const bool first) {
   static_assert(MTM >= 1 && MTM <= 4, "1..4 stacked tiles");
-  if (MT == 1) halo_issue_nk<1>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+  if (MT == 1) halo_issue_nk<1>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
   else if constexpr (MTM >= 2) {
-    if (MT == 2) halo_issue_nk<2>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+    if (MT == 2) halo_issue_nk<2>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
     else if constexpr (MTM >= 3) {
-      if (MT == 3) halo_issue_nk<3>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
-      else if constexpr (MTM >= 4) halo_issue_nk<4>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, first);
+      if (MT == 3) halo_issue_nk<3>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
+      else if constexpr (MTM >= 4) halo_issue_nk<4>(nk16, acc, hlo, blo, s_aoff, gt, ahi, bhi, a_mstep, a_half, bstep, first);
     }
   }
   wg_wait<0>();
+}
+
+// Compact thin-input halo (CisConv.thin = 8 / 16): one plane per 8 channels, 16 bytes per pixel, planes 128-byte aligned.
+__host__ __device__ __forceinline__ int thin_plane_bytes(int HP) { return (HP * 16 + 127) & ~127; }
+// K=16 steps of a tap list: one per tap, or one per tap pair in the compact 8-channel format
+__host__ __device__ __forceinline__ int halo_nsteps(int thin, int ntaps) { return thin == 8 ? (ntaps + 1) / 2 : ntaps; }
+// s_aoff entry of K=16 step s over the taps dh/dw[t0 .. t0 + nt): start of the step's A operand inside the halo in descriptor start-field
+// units (16 B).  Compact format: OR-ed with its LBO (bits 16+), the distance to the second core matrix along K -- the next tap's origin
+// (thin 8; the host lists the taps in increasing order of origin; an odd last tap pairs with itself against zero weights) or plane 1
+// (thin 16).
+__device__ __forceinline__ uint32_t halo_step_off(const CisConv& p, const int t0, const int nt, const int s, const int Wh, const uint32_t plane16) {
+  if (!p.thin) return (uint32_t)((p.dh[t0 + s] * Wh + p.dw[t0 + s]) * 8);   // * 128 B / 16
+  const int ta = p.thin == 8 ? 2 * s : s;
+  const uint32_t o0 = (uint32_t)(p.dh[t0 + ta] * Wh + p.dw[t0 + ta]);
+  if (p.thin == 16) return o0 | (plane16 << 16);
+  const uint32_t o1 = ta + 1 < nt ? (uint32_t)(p.dh[t0 + ta + 1] * Wh + p.dw[t0 + ta + 1]) : o0;
+  return o0 | ((o1 - o0) << 16);
 }
 
 template <int BN, int NWG>
@@ -648,7 +664,9 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
   const int MT = p.MT, MTC = NWG * MT, d = p.dil;   // MT tiles per MMA warpgroup, MTC per CTA
   const int nph = p.nph > 1 ? p.nph : 1;       // stride-2 forward conv: 4 space-to-depth phases, each with its own halo and tap range
   const int Wh = 8 + p.ex, Hh = 16 * MTC + p.ey, HP = Wh * Hh;
-  const uint32_t stage_bytes = (uint32_t)G * kBStage;
+  const int thin = p.thin;
+  const uint32_t wstep = thin ? BN * 32 : kBStage;                  // weight bytes of one K=16 step (compact) or one tap (64-channel chunk)
+  const uint32_t stage_bytes = (uint32_t)G * wstep;
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t h_base = tile_base;                                // NHS halo stages
   const uint32_t b_base = tile_base + NHS * halo_stage_bytes;       // BS weight stages of G tap tiles each
@@ -660,6 +678,7 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
   // ---- grouped launch: blockIdx.z selects one of nsub sub-problems (own taps, halo origin, weights, output extent / offset)
   const bool grouped = p.nsub > 1;
   const int tap0 = grouped ? p.sub[blockIdx.z].tap0 : 0, ntaps = grouped ? p.sub[blockIdx.z].ntaps : p.ntaps;
+  const int nst = halo_nsteps(thin, ntaps);    // K=16 steps (compact) or taps (64-channel chunks) per chunk
   const int hoy = grouped ? p.sub[blockIdx.z].hoy : p.hoy, hox = grouped ? p.sub[blockIdx.z].hox : p.hox;
   const int OHs = grouped ? p.sub[blockIdx.z].OH : p.OH, OWs = grouped ? p.sub[blockIdx.z].OW : p.OW;
   const int oa = grouped ? p.sub[blockIdx.z].oa : p.oa, ob = grouped ? p.sub[blockIdx.z].ob : p.ob;
@@ -685,7 +704,7 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
   __shared__ __align__(16) float s_bias[BN];
   pdl_launch_dependents();
 
-  if (tid < ntaps) s_aoff[tid] = (uint32_t)((p.dh[tap0 + tid] * Wh + p.dw[tap0 + tid]) * 8);   // * 128 B / 16
+  if (tid < nst) s_aoff[tid] = halo_step_off(p, tap0, ntaps, tid, Wh, (uint32_t)thin_plane_bytes(HP) >> 4);
   if (tid < p.nsrc) {
     s_src[tid].ptr = reinterpret_cast<const __nv_bfloat16*>(p.src[tid].ptr);
     s_src[tid].pitch = p.src[tid].pitch;
@@ -738,6 +757,22 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
             ++si;
           }
           const int nmod = s_src[si].n_mod;
+          if (thin) {
+            // compact halo (single chunk, undilated, one phase): one no-swizzle plane of 8 channels per 8-channel slice of the sources
+            const int npl = thin / 8, pb16 = thin_plane_bytes(HP);
+            mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(npl * HP * 16));
+            for (int q = 0; q < npl; ++q) {
+              int cq = q, sq = 0;
+              while (sq < p.nsrc - 1 && cq >= s_src[sq].chunks) {
+                cq -= s_src[sq].chunks;
+                ++sq;
+              }
+              const int nm = s_src[sq].n_mod;
+              tma_load_4d(h_base + hs * halo_stage_bytes + q * pb16, &maps.m[sq], bar_hfull + 8 * hs, cq * 8, tx * 8 + hox, ty * 16 * MTC + hoy,
+                          nm ? (n % nm) : n);
+            }
+            continue;
+          }
           mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
           // dilated layer: the map strides by d pixels from any start, the start carries this CTA's phase (pa, pb)
           tma_load_4d(h_base + hs * halo_stage_bytes, &maps.m[si * nph + ph], bar_hfull + 8 * hs, c * 8, pb + d * (tx * 8 + hox),
@@ -797,17 +832,17 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
     if (tid == 64) {
       // weights: pre-swizzled [n-tile][chunk][tap] tiles of BN x 128 B (cis_pack_weights_tiled); the tiles of the G taps of a stage
       // are adjacent in that layout -> ONE bulk copy per pipeline stage
-      const uint8_t* wt = reinterpret_cast<const uint8_t*>(wpack) + ((size_t)ny * nchunks_all + cc_lo) * ntaps * kBStage;
+      const uint8_t* wt = reinterpret_cast<const uint8_t*>(wpack) + ((size_t)ny * nchunks_all + cc_lo) * nst * wstep;
       int bs = 0;
       uint32_t bph = 1;           // parity to wait for on the empty barrier: the first pass over the ring finds every stage free
       for (int vc = 0; vc < nchunks * nph; ++vc) {
         const int cc = vc / nph, ph = vc - cc * nph;
-        const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : ntaps;
+        const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : nst;
         for (int t0 = tlo; t0 < thi; t0 += G) {
-          const uint32_t bytes = (uint32_t)min(G, thi - t0) * kBStage;
+          const uint32_t bytes = (uint32_t)min(G, thi - t0) * wstep;
           mbar_wait(bar_bempty + 8 * bs, bph);
           mbar_expect_tx(bar_bfull + 8 * bs, bytes);
-          bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * ntaps + t0) * kBStage, bytes, bar_bfull + 8 * bs);
+          bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
           if (++bs == BS) {
             bs = 0;
             bph ^= 1u;
@@ -824,28 +859,31 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
     const int wtid = tid - (kHMmaWarp_ + 4 * wg) * 32;
     constexpr int MTM = Cfg::kMaxMT;
     float acc[MTM][BN];
-    const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
-    const uint32_t a_mstep = (uint32_t)(16 * Wh * 128) >> 4;   // descriptor start-field step between stacked M tiles
-    const uint32_t a_half = (uint32_t)(8 * Wh * 128) >> 4;     // rows 64..127 of a tile: 8 halo rows further
+    // pixel pitch of the halo: 128 B (64-channel SWIZZLE_128B chunk) or 16 B (compact no-swizzle plane); B: 8-row groups 1024 / 256 B apart
+    const uint32_t pix = thin ? 16u : 128u;
+    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix), bhi = thin ? desc_hi_ns(256) : desc_hi(1024);
+    const uint32_t a_mstep = (16u * Wh * pix) >> 4;   // descriptor start-field step between stacked M tiles
+    const uint32_t a_half = (8u * Wh * pix) >> 4;     // rows 64..127 of a tile: 8 halo rows further
     const uint32_t a_wg = (uint32_t)(wg * MT) * a_mstep;        // this warpgroup's first tile inside the halo
     int bs = 0, hs = 0, it = 0;
     uint32_t bph = 0, hph = 0;
     bool any = false;
     for (int vc = 0; vc < nchunks * nph; ++vc) {
       const int cc = vc / nph, ph = vc - cc * nph;
-      const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : ntaps;
+      const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : nst;
       if (thi == tlo) continue;
       const int rem = m_chunks - (cc_lo + cc) * 8;
       const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
       mbar_wait(bar_hfull + 8 * hs, hph);
       if (vc == 0 && wtid == 0 && wg == 0) CIS_TRACE_AT(1);
-      const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16) + a_wg;
+      // compact format: the LBO of every step comes with its s_aoff entry
+      const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, thin ? 0 : 16) + a_wg;
       for (int t0 = tlo; t0 < thi; t0 += G, ++it) {
         const int gt = min(G, thi - t0);
         mbar_wait(bar_bfull + 8 * bs, bph);
         if (wtid == 0 && wg == 0) CIS_TRACE_AT(8 + 2 * it);
-        const uint32_t blo = desc_lo(b_base + bs * stage_bytes, 16);
-        halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, !any);
+        const uint32_t blo = desc_lo(b_base + bs * stage_bytes, thin ? 128 : 16);
+        halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, wstep >> 4, !any);
         if (wtid == 0) {   // one release per warpgroup
           mbar_arrive(bar_bempty + 8 * bs);
           if (t0 + G >= thi) mbar_arrive(bar_hempty + 8 * hs);
@@ -999,7 +1037,11 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int MT = p.MT;
   const int Wh = 8 + p.ex, Hh = 16 * MT + p.ey, HP = Wh * Hh;
-  const uint32_t stage_bytes = (uint32_t)G * kBStage;
+  const int thin = p.thin;
+  const bool grouped = p.nsub > 1;             // grouped launch: the sub-problems' tiles one after the other in the work list
+  const int nsb = grouped ? p.nsub : 1;
+  const uint32_t wstep = thin ? BN * 32 : kBStage;                  // weight bytes of one K=16 step (compact) or one tap (64-channel chunk)
+  const uint32_t stage_bytes = (uint32_t)G * wstep;
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   const uint32_t acc_bytes = (uint32_t)(MT * BN) * kAccColBytes;     // one accumulator stage (a multiple of 8 KB)
   const uint32_t acc_base = tile_base, h_base = tile_base + AS * acc_bytes, b_base = h_base + NHS * halo_stage_bytes;
@@ -1007,14 +1049,30 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
   const uint32_t bar_bfull = smem_u32(&bars[2 * kMaxHS]), bar_bempty = smem_u32(&bars[2 * kMaxHS + kHaloMaxBStages]);
   const uint32_t bar_tfull = smem_u32(&bars[2 * kMaxHS + 2 * kHaloMaxBStages]), bar_tempty = smem_u32(&bars[2 * kMaxHS + 2 * kHaloMaxBStages + 2]);
 
-  const int tiles_x = (p.OW + 7) / 8, tiles_y = (p.OH + 16 * MT - 1) / (16 * MT);
-  const int total = tiles_x * tiles_y * p.N;
+  __shared__ int s_tcum[5], s_sbase[5];      // per sub-problem: first work item, first K=16 step (tap) in s_aoff and the resident weights
   int m_chunks = 0;
   for (int i = 0; i < p.nsrc; ++i) m_chunks += p.src[i].chunks;
   const int nchunks = (m_chunks + 7) / 8;
 
   pdl_launch_dependents();
-  if (tid < p.ntaps) s_aoff[tid] = (uint32_t)((p.dh[tid] * Wh + p.dw[tid]) * 8);
+  {
+    int tc = 0, sb = 0;
+    for (int z = 0; z < nsb; ++z) {
+      const int nt = grouped ? p.sub[z].ntaps : p.ntaps, t0 = grouped ? p.sub[z].tap0 : 0, ns = halo_nsteps(thin, nt);
+      const int oh = grouped ? p.sub[z].OH : p.OH, ow = grouped ? p.sub[z].OW : p.OW;
+      if (tid >= sb && tid < sb + ns) s_aoff[tid] = halo_step_off(p, t0, nt, tid - sb, Wh, (uint32_t)thin_plane_bytes(HP) >> 4);
+      if (tid == 0) {
+        s_tcum[z] = tc;
+        s_sbase[z] = sb;
+      }
+      tc += ((ow + 7) / 8) * ((oh + 16 * MT - 1) / (16 * MT)) * p.N;
+      sb += ns;
+    }
+    if (tid == 0) {
+      s_tcum[nsb] = tc;
+      s_sbase[nsb] = sb;
+    }
+  }
   if (tid == 0) {
     for (int s = 0; s < NHS; ++s) {
       mbar_init(bar_hfull + 8 * s, 1);
@@ -1034,6 +1092,17 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
   pdl_wait();
   if (tid < BN) s_bias[tid] = p.bias ? p.bias[tid] : 0.f;
   __syncthreads();
+  const int total = s_tcum[nsb];
+  // work item w -> (sub-problem z, tile column tx, tile row ty, image n)
+  auto decode = [&](const int w, int& z, int& tx, int& ty, int& n) {
+    z = 0;
+    while (z + 1 < nsb && w >= s_tcum[z + 1]) ++z;
+    const int tiles_x = ((grouped ? p.sub[z].OW : p.OW) + 7) / 8, tiles_y = ((grouped ? p.sub[z].OH : p.OH) + 16 * MT - 1) / (16 * MT);
+    const int l = w - s_tcum[z];
+    tx = l % tiles_x;
+    ty = (l / tiles_x) % tiles_y;
+    n = l / (tiles_x * tiles_y);
+  };
   if (tid == 0) {
     CIS_TRACE_AT(0);
     CIS_TRACE_AT(4);      // slot 4 marks a persistent-kernel trace (tools/trace_persist.py)
@@ -1045,7 +1114,9 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
       int hs = 0;
       uint32_t hph = 1;
       for (int w = blockIdx.x; w < total; w += gridDim.x) {
-        const int tx = w % tiles_x, r1 = w / tiles_x, ty = r1 % tiles_y, n = r1 / tiles_y;
+        int z, tx, ty, n;
+        decode(w, z, tx, ty, n);
+        const int hox = grouped ? p.sub[z].hox : p.hox, hoy = grouped ? p.sub[z].hoy : p.hoy;
         for (int cc = 0; cc < nchunks; ++cc) {
           mbar_wait(bar_hempty + 8 * hs, hph);
           int c = cc * 8, si = 0;
@@ -1057,9 +1128,25 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
           if (si == 1) nmod = p.src[1].n_mod;
           if (si == 2) nmod = p.src[2].n_mod;
           if (si == 3) nmod = p.src[3].n_mod;
-          mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
-          tma_load_4d(h_base + hs * halo_stage_bytes, &maps.m[si], bar_hfull + 8 * hs, c * 8, tx * 8 + p.hox, ty * 16 * MT + p.hoy,
-                      nmod ? (n % nmod) : n);
+          if (thin) {
+            // compact halo: one no-swizzle plane of 8 channels per 8-channel slice of the sources (see conv_halo_kernel)
+            const int npl = thin / 8, pb16 = thin_plane_bytes(HP);
+            mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(npl * HP * 16));
+            for (int q = 0; q < npl; ++q) {
+              int cq = q, sq = 0;
+              while (sq < p.nsrc - 1 && cq >= p.src[sq].chunks) {
+                cq -= p.src[sq].chunks;
+                ++sq;
+              }
+              const int nm = p.src[sq].n_mod;
+              tma_load_4d(h_base + hs * halo_stage_bytes + q * pb16, &maps.m[sq], bar_hfull + 8 * hs, cq * 8, tx * 8 + hox, ty * 16 * MT + hoy,
+                          nm ? (n % nm) : n);
+            }
+          } else {
+            mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
+            tma_load_4d(h_base + hs * halo_stage_bytes, &maps.m[si], bar_hfull + 8 * hs, c * 8, tx * 8 + hox, ty * 16 * MT + hoy,
+                        nmod ? (n % nmod) : n);
+          }
           if (++hs == NHS) {
             hs = 0;
             hph ^= 1u;
@@ -1071,13 +1158,18 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
     // ------------------------------------------------------------------ weight producer
     if (lane == 0) {
       const uint8_t* wt = reinterpret_cast<const uint8_t*>(p.wpack);
-      const int per_tile = nchunks * p.ntaps;
+      const int nst = s_sbase[1];          // ungrouped: weight tiles per chunk
       if (ws) {
+        // the resident set: every sub-problem's tiles at its first step (grouped launches have one chunk; the host checks)
         if ((int)blockIdx.x < total) {
-          mbar_expect_tx(bar_bfull, (uint32_t)(per_tile * kBStage));
-          for (int it = 0; it < per_tile; it += 8) {      // bulk copies of up to 8 tiles (<= 128 KB each)
-            const int nt = min(8, per_tile - it);
-            bulk_g2s(b_base + it * kBStage, wt + (size_t)it * kBStage, (uint32_t)(nt * kBStage), bar_bfull);
+          mbar_expect_tx(bar_bfull, (uint32_t)(nchunks * s_sbase[nsb] * wstep));
+          for (int z = 0; z < nsb; ++z) {
+            const uint8_t* wz = grouped ? reinterpret_cast<const uint8_t*>(p.sub[z].wpack) : wt;
+            const int per = nchunks * (s_sbase[z + 1] - s_sbase[z]);
+            for (int it = 0; it < per; it += 8) {      // bulk copies of up to 8 tiles (<= 128 KB each)
+              const int nt = min(8, per - it);
+              bulk_g2s(b_base + (s_sbase[z] + it) * wstep, wz + (size_t)it * wstep, (uint32_t)(nt * wstep), bar_bfull);
+            }
           }
         }
       } else {
@@ -1085,11 +1177,11 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
         uint32_t bph = 1;
         for (int w = blockIdx.x; w < total; w += gridDim.x) {
           for (int cc = 0; cc < nchunks; ++cc) {
-            for (int t0 = 0; t0 < p.ntaps; t0 += G) {
-              const uint32_t bytes = (uint32_t)min(G, p.ntaps - t0) * kBStage;
+            for (int t0 = 0; t0 < nst; t0 += G) {
+              const uint32_t bytes = (uint32_t)min(G, nst - t0) * wstep;
               mbar_wait(bar_bempty + 8 * bs, bph);
               mbar_expect_tx(bar_bfull + 8 * bs, bytes);
-              bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * p.ntaps + t0) * kBStage, bytes, bar_bfull + 8 * bs);
+              bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
               if (++bs == BS) {
                 bs = 0;
                 bph ^= 1u;
@@ -1104,30 +1196,35 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
     const int wtid = tid;
     constexpr int MTM = (kPMaxAccCols / BN) < 4 ? kPMaxAccCols / BN : 4;
     float acc[MTM][BN];
-    const uint32_t ahi = desc_hi((uint32_t)(Wh * 128)), bhi = desc_hi(1024);
-    const uint32_t a_mstep = (uint32_t)(16 * Wh * 128) >> 4;
-    const uint32_t a_half = (uint32_t)(8 * Wh * 128) >> 4;
+    const uint32_t pix = thin ? 16u : 128u;       // halo pixel pitch (see conv_halo_kernel)
+    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix), bhi = thin ? desc_hi_ns(256) : desc_hi(1024);
+    const uint32_t a_mstep = (16u * Wh * pix) >> 4;
+    const uint32_t a_half = (8u * Wh * pix) >> 4;
     int hs = 0, bs = 0, as = 0;
     uint32_t hph = 0, bph = 0, tph = 1;
     if (ws && (int)blockIdx.x < total) mbar_wait(bar_bfull, 0u);      // the resident weight set; never released
     int wi = 0;
     for (int w = blockIdx.x; w < total; w += gridDim.x, ++wi) {
       if (wtid == 0) CIS_TRACE_AT(8 + 5 * wi);
+      int z, tx, ty, n;
+      decode(w, z, tx, ty, n);
+      const int nst = s_sbase[z + 1] - s_sbase[z];
+      const uint32_t* so = s_aoff + s_sbase[z];
       for (int cc = 0; cc < nchunks; ++cc) {
         const int rem = m_chunks - cc * 8;
         const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
         mbar_wait(bar_hfull + 8 * hs, hph);
         if (cc == 0 && wtid == 0) CIS_TRACE_AT(10 + 5 * wi);
-        const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, 16);
-        const int gstep = ws ? p.ntaps : G;
-        for (int t0 = 0; t0 < p.ntaps; t0 += gstep) {
-          const int gt = min(gstep, p.ntaps - t0);
+        const uint32_t hlo = desc_lo(h_base + hs * halo_stage_bytes, thin ? 0 : 16);
+        const int gstep = ws ? nst : G;
+        for (int t0 = 0; t0 < nst; t0 += gstep) {
+          const int gt = min(gstep, nst - t0);
           if (!ws) mbar_wait(bar_bfull + 8 * bs, bph);
-          const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(cc * p.ntaps) * kBStage : b_base + bs * stage_bytes, 16);
-          halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, (cc | t0) == 0);
+          const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(s_sbase[z] + cc * nst) * wstep : b_base + bs * stage_bytes, thin ? 128 : 16);
+          halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, so + t0, gt, MT, ahi, bhi, a_mstep, a_half, wstep >> 4, (cc | t0) == 0);
           if (wtid == 0) {
             if (!ws) mbar_arrive(bar_bempty + 8 * bs);
-            if (t0 + gstep >= p.ntaps) mbar_arrive(bar_hempty + 8 * hs);
+            if (t0 + gstep >= nst) mbar_arrive(bar_hempty + 8 * hs);
           }
           if (!ws && ++bs == BS) {
             bs = 0;
@@ -1161,13 +1258,16 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
       int wi = 0;
       for (int w = blockIdx.x; w < total; w += gridDim.x, ++wi) {
         if (wi % AS != grp) continue;
-        const int tx = w % tiles_x, r1 = w / tiles_x, ty = r1 % tiles_y, n = r1 / tiles_y;
+        int z, tx, ty, n;
+        decode(w, z, tx, ty, n);
+        const int OHs = grouped ? p.sub[z].OH : p.OH, OWs = grouped ? p.sub[z].OW : p.OW;
+        const int oa = grouped ? p.sub[z].oa : p.oa, ob = grouped ? p.sub[z].ob : p.ob;
         mbar_wait(bar_tfull + 8 * grp, tph);
         tph ^= 1u;
         for (int m = 0; m < MT; ++m) {
           const int oy = ty * 16 * MT + 16 * m + (r >> 3), ox = tx * 8 + (r & 7);
-          const bool valid = oy < p.OH && ox < p.OW;
-          const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + p.oa) * p.DW + ox * p.osw + p.ob) : 0;
+          const bool valid = oy < OHs && ox < OWs;
+          const size_t dpix = valid ? ((size_t)(n * p.DH + oy * p.osh + oa) * p.DW + ox * p.osw + ob) : 0;
           epi_row<BN>(p, acc_base + grp * acc_bytes + (uint32_t)r * 16 + (uint32_t)(m * BN) * kAccColBytes, 0, dpix, valid, s_bias);
         }
         __syncwarp();
@@ -1728,9 +1828,12 @@ template <int BN, int NWG>
 static int launch_halo(const CisConv* d, cudaStream_t st) {
   const int MTC = d->MT * NWG;                                 // stacked 16x8 tiles per CTA
   const int Wh = 8 + d->ex, Hh = 16 * MTC + d->ey, HP = Wh * Hh;
-  const int halo_stage = (HP * 128 + 1023) & ~1023;
+  const int thin = d->thin;
+  const int halo_stage = ((thin ? thin / 8 * thin_plane_bytes(HP) : HP * 128) + 1023) & ~1023;
   int chunks = 0;
   for (int i = 0; i < d->nsrc; ++i) chunks += d->src[i].chunks;
+  if (thin && ((thin != 8 && thin != 16) || chunks * 8 != thin || d->dil != 1 || d->nph > 1))
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): the compact format needs 8 or 16 undilated input channels");
   const int nchunks = (chunks + 7) / 8;
   const int nsub = d->nsub > 1 ? d->nsub : 1;                  // grouped launch: grid.z = sub-problem, no split-K
   const int nsp = (nsub == 1 && d->splits > 1) ? d->splits : 1;
@@ -1754,14 +1857,24 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
     const int Hp0 = (d->OH + dd - 1) / dd, Wp0 = (d->OW + dd - 1) / dd;
     tiles = ((Wp0 + 7) / 8) * ((Hp0 + 16 * MTC - 1) / (16 * MTC));
   }
+  if (thin == 8) {
+    // a K=16 step reads its second tap at a positive LBO from the first: every sub-problem lists its taps in increasing halo offset
+    for (int i = 0; i < nsub; ++i) {
+      const int t0 = nsub > 1 ? d->sub[i].tap0 : 0, nt = nsub > 1 ? d->sub[i].ntaps : d->ntaps;
+      for (int t = t0 + 1; t < t0 + nt; ++t)
+        if (d->dh[t] * (8 + d->ex) + d->dw[t] < d->dh[t - 1] * (8 + d->ex) + d->dw[t - 1])
+          return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): compact 8-channel taps must be listed in increasing halo offset");
+    }
+  }
+  const int nst_max = halo_nsteps(thin, ntaps_max);            // weight tiles (K=16 steps or taps) per chunk
   const long ncta_all = (long)tiles * dd * dd * d->N * d->n_tiles * nsp * nsub;
   // ---- weight pipeline: G taps per stage (one bulk copy, one wait / commit of the MMA thread), BS stages
   static const int g_env = getenv("CIS_HALO_G") ? atoi(getenv("CIS_HALO_G")) : 0;            // experiments: force the group size
   static const int stage_kb = getenv("CIS_HALO_STAGE_KB") ? atoi(getenv("CIS_HALO_STAGE_KB")) : 48;
-  const int kB = BN * 128;
+  const int kB = thin ? BN * 32 : BN * 128;
   int G = g_env > 0 ? g_env : (stage_kb * 1024) / kB;
   if (G < 1) G = 1;
-  if (G > ntaps_max) G = ntaps_max;
+  if (G > nst_max) G = nst_max;
   const int fixed = nhs * halo_stage + HP * 4 + 1024;
   // two co-resident CTAs per SM overlap one CTA's epilogue with the other's main loop -- when the grid has that many CTAs
   static const int lim_small_kb = getenv("CIS_HALO_SMALL_KB") ? atoi(getenv("CIS_HALO_SMALL_KB")) : 226;   // grids of <= one CTA per SM
@@ -1772,7 +1885,7 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   int limit = (ncta_all > nsm && fixed + 2 * kB <= lim_kb * 1024) ? lim_kb * 1024 : 226 * 1024;
   if (ncta_all <= nsm && fixed + 2 * kB <= lim_small_kb * 1024) limit = lim_small_kb * 1024;
   while (G > 1 && fixed + 2 * G * kB > limit) --G;
-  const int groups = cper * ((nsub > 1 ? 1 : (ntaps_max + G - 1) / G));   // pipeline stages one CTA walks (grouped: at least one per chunk)
+  const int groups = cper * ((nsub > 1 ? 1 : (nst_max + G - 1) / G));   // pipeline stages one CTA walks (grouped: at least one per chunk)
   int BS = (limit - fixed) / (G * kB);
   if (BS > (ncta_all > nsm ? 4 : kHaloMaxBStages)) BS = ncta_all > nsm ? 4 : kHaloMaxBStages;
   if (BS > groups) BS = groups;
@@ -1799,14 +1912,17 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   const int nph = d->nph > 1 ? d->nph : 1;
   static const int dil_tma = getenv("CIS_DIL_TMA") ? atoi(getenv("CIS_DIL_TMA")) : 1;
   int use_tma = ((d->dil == 1 || dil_tma) && Wh * d->dil <= 256 && Hh * d->dil <= 256) ? 1 : 0;
-  for (int i = 0; use_tma && i < d->nsrc - 1; ++i)
+  for (int i = 0; use_tma && !thin && i < d->nsrc - 1; ++i)
     if (d->src[i].chunks % 8) use_tma = 0;
   for (int i = 0; use_tma && i < d->nsrc; ++i) {
     if (((uintptr_t)d->src[i].ptr + (size_t)d->src[i].c_off * 2) % 16) use_tma = 0;
     for (int ph = 0; use_tma && ph < nph; ++ph)
-      if (!encode_src_map(&maps.m[i * nph + ph], d->src[i], d->N, d->H, d->W, Wh, Hh, nph > 1 ? 2 : 1, ph >> 1, ph & 1, d->dil)) use_tma = 0;
+      if (!(thin ? encode_src_map(&maps.m[i], d->src[i], d->N, d->H, d->W, Wh, Hh, 1, 0, 0, 1, 8, CU_TENSOR_MAP_SWIZZLE_NONE)
+                 : encode_src_map(&maps.m[i * nph + ph], d->src[i], d->N, d->H, d->W, Wh, Hh, nph > 1 ? 2 : 1, ph >> 1, ph & 1, d->dil)))
+        use_tma = 0;
   }
   if (!use_tma) memset(&maps, 0, sizeof(maps));
+  if (thin && !use_tma) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): the compact format needs the TMA halo path");
   if (nph > 1 && !use_tma) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): stride-2 phases need the TMA halo path");
   // persistent variant (conv_halo_persist_kernel): layers with many tiles per SM.  CIS_PERSIST_MODE / cis_set_persist_mode:
   //   0 off | 1 (default) layers whose whole weight set stays resident in shared memory and that have >= 2 tiles per SM |
@@ -1815,9 +1931,17 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   static const int p_min_tiles = getenv("CIS_PERSIST_MIN_TILES") ? atoi(getenv("CIS_PERSIST_MIN_TILES")) : 296;
   static const int p_ws_kb = getenv("CIS_PERSIST_WS_KB") ? atoi(getenv("CIS_PERSIST_WS_KB")) : 112;
   if constexpr (BN <= kPMaxAccCols && NWG == 1) {
-   if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && nsub == 1 && dd == 1 && d->MT * BN <= kPMaxAccCols) {
-    const int total = tiles * d->N;
-    const int per_tile = nchunks * d->ntaps;
+   // grouped launches (one chunk, whole weight set resident): the sub-problems' tiles form one work list
+   if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && (nsub == 1 || nchunks == 1) && dd == 1 &&
+       d->MT * BN <= kPMaxAccCols) {
+    int total = tiles * d->N, per_tile = nchunks * nst_max;
+    if (nsub > 1) {
+      total = per_tile = 0;
+      for (int i = 0; i < nsub; ++i) {
+        total += ((d->sub[i].OW + 7) / 8) * ((d->sub[i].OH + 16 * d->MT - 1) / (16 * d->MT)) * d->N;
+        per_tile += halo_nsteps(thin, d->sub[i].ntaps);
+      }
+    }
     const int acc_stage = d->MT * BN * (int)kAccColBytes;           // one shared-memory accumulator stage
     const int AS = 2;
     const int fixed_p = AS * acc_stage + 1024;
@@ -1835,7 +1959,7 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
       if (p_bs > 4) p_bs = 4;
       p_smem = p_nhs * halo_stage + fixed_p + p_bs * G * kB;
     }
-    if (take && p_bs >= (ws_fits ? 1 : 2)) {
+    if (take && (ws_fits || nsub == 1) && p_bs >= (ws_fits ? 1 : 2)) {
       static int attr_p = 0;   // largest dynamic-smem limit set so far on conv_halo_persist_kernel<BN>
       if (p_smem > attr_p) {
         cudaError_t e = cudaFuncSetAttribute(conv_halo_persist_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, p_smem);

@@ -97,6 +97,31 @@ __device__ __forceinline__ void pack_weights_tiled_tile(int blk, const float* __
     o[idx] = __float2bfloat16(tile[kk * ld + n]);
   }
 }
+// Compact (thin = 8 / 16 input channels) tiles of the halo kernel: block (ny, step s) = BN x 32 B, the no-swizzle K-major operand of
+// one K=16 step.  Element (n, kgroup j, e) at ((n / 8) * 2 + j) * 64 + (n % 8) * 8 + e; kgroup j is tap 2s + j, channel e (thin 8) or
+// tap s, channel 8j + e (thin 16).  i >= the tile set's size returns (the job's block count is that of the 64-channel layout).
+__device__ __forceinline__ void pack_weights_thin_body(size_t i, const float* __restrict__ w, const int* __restrict__ kmap, int cin8, int ntaps,
+                                                       int n_tiles, int BN, int cout, int sn, const int* __restrict__ nmap, int thin,
+                                                       bf16* __restrict__ out) {
+  const int nst = thin == 8 ? (ntaps + 1) / 2 : ntaps;
+  if (i >= (size_t)n_tiles * nst * BN * 16) return;
+  const int e = (int)(i % 8);
+  const int n8 = (int)((i / 8) % 8);
+  const int j = (int)((i / 64) % 2);
+  size_t r = i / 128;
+  const int ng8 = (int)(r % (BN / 8));
+  r /= BN / 8;
+  const int s = (int)(r % nst), ny = (int)(r / nst);
+  const int t = thin == 8 ? 2 * s + j : s, c = thin == 8 ? e : 8 * j + e;
+  float v = 0.f;
+  if (t < ntaps && c < cin8) {
+    const int km = kmap[t * cin8 + c];
+    const int ng = ny * BN + ng8 * 8 + n8;
+    const int ne = nmap ? nmap[ng] : (ng < cout ? ng : -1);
+    if (km >= 0 && ne >= 0) v = w[(size_t)km + (size_t)ne * sn];
+  }
+  out[i] = __float2bfloat16(v);
+}
 __device__ __forceinline__ void unpack_wgrad_body(size_t i, const float* __restrict__ dwp, const int* __restrict__ kmap, int K_pad, int cout,
                                                   int nsplit, float* __restrict__ dw, const float* __restrict__ colpart, int nblocks, int nch,
                                                   float* __restrict__ db, int layout) {
@@ -181,11 +206,12 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, const int* __re
   pack_weights_body((size_t)blockIdx.x * blockDim.x + threadIdx.x, w, kmap, K_pad, rows, cout, sn, nmap, wp);
 }
 __global__ void pack_weights_tiled_kernel(const float* __restrict__ w, const int* __restrict__ kmap, int cin8, int ntaps, int n_tiles, int BN,
-                                          int cout, int sn, const int* __restrict__ nmap, bf16* __restrict__ out) {
+                                          int cout, int sn, const int* __restrict__ nmap, bf16* __restrict__ out, int thin) {
   pdl_launch_dependents();
   pdl_wait();
   __shared__ float tile[64 * 129];
-  if (sn == 1) pack_weights_tiled_tile(blockIdx.x, w, kmap, cin8, ntaps, n_tiles, BN, cout, nmap, out, tile);
+  if (thin) pack_weights_thin_body((size_t)blockIdx.x * blockDim.x + threadIdx.x, w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, thin, out);
+  else if (sn == 1) pack_weights_tiled_tile(blockIdx.x, w, kmap, cin8, ntaps, n_tiles, BN, cout, nmap, out, tile);
   else pack_weights_tiled_body((size_t)blockIdx.x * blockDim.x + threadIdx.x, w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, out);
 }
 __global__ void unpack_wgrad_kernel(const float* __restrict__ dwp, const int* __restrict__ kmap, int K_pad, int cout, int nsplit,
@@ -229,7 +255,12 @@ __global__ void param_multi_kernel(const CisParamJob* __restrict__ jobs, int njo
       pack_weights_body(i, (const float*)j.p[0], (const int*)j.p[1], j.i[0], j.i[1], j.i[2], j.i[3], (const int*)j.p[2], (bf16*)j.p[3]);
       break;
     case CIS_JOB_PACK_TILED:
-      if (j.i[5] == 1)       // forward orientation: one block per tile, transposed through shared memory
+      if (j.i[6]) {          // compact thin-input tiles (a fraction of the 64-channel layout the job's blocks are counted for)
+        const size_t per = j.i[5] == 1 ? (size_t)j.i[3] * 64 : blockDim.x;
+        for (size_t q = threadIdx.x; q < per; q += blockDim.x)
+          pack_weights_thin_body((size_t)blk * per + q, (const float*)j.p[0], (const int*)j.p[1], j.i[0], j.i[1], j.i[2], j.i[3], j.i[4], j.i[5],
+                                 (const int*)j.p[2], j.i[6], (bf16*)j.p[3]);
+      } else if (j.i[5] == 1)       // forward orientation: one block per tile, transposed through shared memory
         pack_weights_tiled_tile(blk, (const float*)j.p[0], (const int*)j.p[1], j.i[0], j.i[1], j.i[2], j.i[3], j.i[4], (const int*)j.p[2],
                                 (bf16*)j.p[3], tile);
       else
@@ -1823,11 +1854,13 @@ int cis_pack_weights(const float* w, const int32_t* kmap, int32_t K_pad, int32_t
   return cis_check_launch("pack_weights");
 }
 int cis_pack_weights_tiled(const float* w, const int32_t* kmap, int32_t cin8, int32_t ntaps, int32_t n_tiles, int32_t BN, int32_t cout, int32_t sn,
-                           const int32_t* nmap, void* out, cis_stream_t stream) {
-  const size_t total = (size_t)n_tiles * ((cin8 + 63) / 64) * ntaps * BN * 64;
-  const unsigned blocks = sn == 1 ? (unsigned)(n_tiles * ((cin8 + 63) / 64) * ntaps) : nblk(total);
+                           const int32_t* nmap, void* out, int32_t thin, cis_stream_t stream) {
+  const size_t total = thin ? (size_t)n_tiles * (thin == 8 ? (ntaps + 1) / 2 : ntaps) * BN * 16
+                            : (size_t)n_tiles * ((cin8 + 63) / 64) * ntaps * BN * 64;
+  const unsigned blocks = (sn == 1 && !thin) ? (unsigned)(n_tiles * ((cin8 + 63) / 64) * ntaps) : nblk(total);
   if (BN > 128) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_pack_weights_tiled: BN > 128");
-  CIS_LAUNCH(pack_weights_tiled_kernel, blocks, 256, 0, ST, w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, (mbf)out);
+  if (thin && (cin8 != thin || (thin != 8 && thin != 16))) return cis_set_error(CIS_ERR_BAD_ARG, "cis_pack_weights_tiled: thin must be 8 or 16 = cin8");
+  CIS_LAUNCH(pack_weights_tiled_kernel, blocks, 256, 0, ST, w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, (mbf)out, thin);
   return cis_check_launch("pack_weights_tiled");
 }
 int cis_unpack_wgrad(const float* dwp, const int32_t* kmap, int32_t K_pad, int32_t cout, int32_t nsplit, float* dw, const float* colpart,

@@ -162,6 +162,8 @@ template <int TA, int TB> struct Wgmma<128, TA, TB> {
 // halo taps) offset from a 1024-aligned, swizzle-written tile keep base_offset = 0.
 // Split form for hot issue loops: hi word is loop-invariant, lo word = start>>4 | LBO>>4<<16 advances by (bytes>>4) per K step.
 __device__ __forceinline__ uint32_t desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 30); }
+// no-swizzle K-major layout (layout = 0): core matrices of 8 rows x 16 contiguous bytes; LBO = next core matrix along K, SBO = next 8 rows
+__device__ __forceinline__ uint32_t desc_hi_ns(uint32_t sbo_bytes) { return (sbo_bytes >> 4) & 0x3FFF; }
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
   return ((saddr & 0x3FFFF) >> 4) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
 }

@@ -128,11 +128,12 @@ class Plan(object):
                 j.kind, blocks = JOB_PACK, -(-(rows * K_pad) // 256)
                 ptrs, ints = [w, kmap, nmap, wp], [K_pad, rows, cout, sn]
             elif name == 'cis_pack_weights_tiled':
-                w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, out = a
+                w, kmap, cin8, ntaps, n_tiles, BN, cout, sn, nmap, out, thin = a
                 j.kind, blocks = JOB_PACK_TILED, -(-(n_tiles * (-(-cin8 // 64)) * ntaps * BN * 64) // 256)
                 if sn == 1:               # forward orientation: one block per BN x 64 tile (transposed through shared memory)
                     blocks = n_tiles * (-(-cin8 // 64)) * ntaps
-                ptrs, ints = [w, kmap, nmap, out], [cin8, ntaps, n_tiles, BN, cout, sn]
+                # the compact thin-input tiles are smaller: the kernel walks them over the same blocks
+                ptrs, ints = [w, kmap, nmap, out], [cin8, ntaps, n_tiles, BN, cout, sn, thin]
             elif name == 'cis_unpack_wgrad':
                 dwp, kmap, K_pad, cout, nsplit, dw, colpart, nblocks, nch, db, layout = a
                 j.kind, blocks = JOB_UNPACK, -(-(cout * K_pad + nch) // 256)
@@ -516,8 +517,21 @@ def setup_halo(d, taps, dil, n_tiles):
         return False
     d.halo, d.dil, d.MT, d.hoy, d.hox, d.ey, d.ex = 1, dil, best[1], hoy, hox, ey, ex
     d.nwg = halo_nwg(d, best[1], Hp0, Wp0, dil, n_tiles, ntaps, nchunks, ey, ex)
-    _fill_taps(d, rel)
+    d.thin = thin_format(m_chunks, dil)
+    _fill_taps(d, [rel[i] for i in thin_tap_order(d.thin, rel)])
     return True
+
+
+def thin_format(m_chunks, dil):
+    """CisConv.thin of an undilated halo launch whose sources total m_chunks 8-channel chunks: 8 or 16 channels take the compact K-dense
+    format (a 16-byte-per-pixel halo; one K=16 step per tap pair or per tap instead of one per tap of a mostly-zero 64-channel chunk)."""
+    return m_chunks * 8 if dil == 1 and m_chunks in (1, 2) else 0
+
+
+def thin_tap_order(thin, taps):
+    """Order of the taps in a halo launch and in its pre-tiled weights: the compact 8-channel format pairs consecutive taps in one K=16
+    step whose second tap must lie at a positive offset from the first, so it lists them in increasing (dy, dx); else as given."""
+    return sorted(range(len(taps)), key=lambda i: tuple(taps[i])) if thin == 8 else list(range(len(taps)))
 
 
 # stride-2 forward convolutions on the halo kernel (4 space-to-depth phase tensor maps, CisConv.nph = 4).  Off by default: every tap
@@ -587,7 +601,7 @@ def merge_parity_launches(descs):
         return None
     d0 = descs[0]
     same = ('N', 'H', 'W', 'BN', 'n_tiles', 'nsrc', 'act', 'DH', 'DW', 'osh', 'osw', 'out', 'out_pitch', 'out_coff', 'out_ch', 'outf', 'outf_pitch',
-            'outf_coff', 'outf_ch', 'add_pre', 'add_pre_pitch', 'add_pre_coff', 'add_post', 'addf_pre', 'mode', 'bias')
+            'outf_coff', 'outf_ch', 'add_pre', 'add_pre_pitch', 'add_pre_coff', 'add_post', 'addf_pre', 'mode', 'bias', 'thin')
     for d in descs:
         if not d.halo or d.dil != 1 or d.splits > 1 or d.nph > 1 or any(getattr(d, f) != getattr(d0, f) for f in same):
             return None
@@ -676,7 +690,7 @@ class Pack:
     """One packed bf16 weight operand of a conv layer.  a, b: output parity of a parity launch; taps: its (dy, dx) offsets (forward
     operand: the tap indices, in its tiled copy's order); kmap: packed K position -> flat weight offset; w: row pack [rows][K_pad] of
     the gather kernel; nmap: row -> output channel (None = identity); wt: tiled copy of the halo kernel, allocated when the first launch
-    goes there, wt_kmap its kmap if the tap order differs; rows_used: None until a launch is placed (rows packed), False while only halo
+    goes there, wt_kmap its kmap if the tap order differs, thin its CisConv.thin format; rows_used: None until a launch is placed (rows packed), False while only halo
     launches read the operand; wg_splits / dwp: per-mode split count and fp32 slices of the parity's weight gradient (transposed conv)."""
     a: int = 0
     b: int = 0
@@ -690,6 +704,7 @@ class Pack:
     w: torch.Tensor = None
     wt: torch.Tensor = None
     wt_kmap: torch.Tensor = None
+    thin: int = 0
     rows_used: bool = None
     wg_splits: dict = dataclasses.field(default_factory=dict)
     dwp: torch.Tensor = None
@@ -795,10 +810,17 @@ class ConvLayer(object):
             return
         if pk.wt is None:
             pk.wt = self._alloc_tiles(len(taps), kch, pk.BN, pk.n_tiles)
+            pk.thin = d.thin
             if order is not None:
                 pk.taps = list(order)
                 pk.wt_kmap, _ = self._kmap(pk.taps, self.in_chanmap, self.cin * self.cout, self.cout)
+            perm = thin_tap_order(d.thin, taps)
+            if perm != sorted(perm):         # the compact 8-channel tiles follow the launch's tap order
+                n = len(taps)
+                pk.wt_kmap = pk.kmap.clone()
+                pk.wt_kmap[:n * kch] = pk.kmap[:n * kch].view(n, kch)[perm].reshape(-1)
         assert order is None or pk.taps == list(order), self.name
+        assert pk.thin == d.thin, self.name
         d.wpack = pk.wt.data_ptr()
         if pk.rows_used is None:
             pk.rows_used = False
@@ -826,7 +848,7 @@ class ConvLayer(object):
         for pk, kch, nch, sn in packs:
             if pk.wt is not None:
                 plan.add('cis_pack_weights_tiled', self.w_src_ptr(), (pk.kmap if pk.wt_kmap is None else pk.wt_kmap).data_ptr(), kch,
-                         len(pk.taps), pk.n_tiles, pk.BN, nch, sn, _ptr(pk.nmap), pk.wt.data_ptr())
+                         len(pk.taps), pk.n_tiles, pk.BN, nch, sn, _ptr(pk.nmap), pk.wt.data_ptr(), pk.thin)
             if pk.rows_used is not False:
                 plan.add('cis_pack_weights', self.w_src_ptr(), pk.kmap.data_ptr(), pk.K_pad, pk.rows, nch, sn, _ptr(pk.nmap), pk.w.data_ptr())
 
