@@ -84,7 +84,9 @@ typedef struct {
   int32_t* sk_counters;  /* must be NULL (the single-launch ticket mode of round 1 was removed; the field keeps the struct layout) */
   /* Stride-2 forward convolution on the halo kernel (halo = 1, sh = sw = 1 in this descriptor, H x W = the INPUT size): the input is
    * read as nph = 4 space-to-depth phases in(2y + py, 2x + px), phase index py*2 + px; taps are listed phase by phase in PHASE
-   * coordinates (dh/dw relative to the halo origin of the phase images) and taps [ph_tap[i], ph_tap[i+1]) belong to phase i.
+   * coordinates (dh/dw relative to the halo origin of the phase images) and taps [ph_tap[i], ph_tap[i+1]) belong to phase i.  With
+   * `thin` set, ph_tap still counts taps, not K=16 steps: one halo stage holds the planes of the four phases, phase-major, so an
+   * 8-channel step pairs taps 2s and 2s+1 even where they belong to two phases (the second one's origin lies in a later plane).
    * nph = 0/1: ordinary stride-1 gather. */
   int32_t nph;
   int32_t ph_tap[5];
@@ -105,7 +107,7 @@ typedef struct {
   /* halo kernel, BN >= 64: 2 = two MMA warpgroups share every weight stage, each owning MT stacked tiles, so the CTA covers 2*MT tiles
    * (16*2*MT output rows per column of tiles; split-K scratch and the grid count CTAs of that height).  0/1: one warpgroup. */
   int32_t nwg;
-  /* halo kernel, stride 1, undilated, sources totalling 8 or 16 channels: the compact K-dense operand format.  0: 64-channel
+  /* halo kernel, undilated (stride 1 or nph = 4), sources totalling 8 or 16 channels: the compact K-dense operand format.  0: 64-channel
    * SWIZZLE_128B chunks, one K=16 step per tap.  8 / 16: the halo is staged without swizzle at 16 bytes per pixel, one plane per 8
    * channels, so 8 consecutive halo pixels are one wgmma core matrix; a K=16 step covers two taps (8: taps 2s, 2s+1, LBO = the distance of
    * their origins, which the host lists in increasing order) or one tap (16: LBO = the plane distance).  wpack / sub[].wpack then hold
@@ -153,7 +155,12 @@ uint32_t cis_crc32c(uint32_t crc, const void* data, size_t n);
 int cis_host_resize_bilinear_legacy(const float* src, int32_t H, int32_t W, int32_t C, float* dst, int32_t OH, int32_t OW);
 int cis_host_bgr8_to_rgb_resized(const unsigned char* bgr, int32_t H, int32_t W, float* dst, int32_t OH, int32_t OW);
 
+/* A gather launch (halo = 0) with stride 2 whose sources total 8 or 16 channels and whose grid has at least 296 16x8 tiles runs on the
+ * halo kernels as a compact phase-halo launch (nph = 4, thin set) that reads its weights in place from the row pack wpack.  cis_conv_s2_phase_plan (host only, no stream) returns 1
+ * and that launch's descriptor in *h, with the row-pack K column of kgroup j of K=16 step s in wk[2 s + j] (2 * CIS_MAX_TAPS entries),
+ * or 0 when cis_conv_igemm runs d on the gather kernel. */
 int cis_conv_igemm(const CisConv* d, cis_stream_t stream);
+int cis_conv_s2_phase_plan(const CisConv* d, CisConv* h, int16_t* wk);
 /* which launches use the persistent warp-specialised halo kernel: 0 none, 1 thin single-chunk layers (default), 2 all eligible,
  * 3 = 1 + the weight-stationary variant for thin layers whose whole weight set fits in shared memory (experimental),
  * -1 back to the default / CIS_PERSIST_MODE environment variable.  Host-side switch, not a stream operation. */

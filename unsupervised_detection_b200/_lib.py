@@ -126,7 +126,7 @@ _PROTOS = {
                                _p, _i32, _i32, _i32, _p, _p, _p, _i32],
 }
 EXPORTS = sorted(list(_PROTOS) + ['cis_last_error', 'cis_version', 'cis_set_persist_mode', 'cis_crc32c', 'cis_host_resize_bilinear_legacy',
-                                  'cis_host_bgr8_to_rgb_resized'])
+                                  'cis_host_bgr8_to_rgb_resized', 'cis_conv_s2_phase_plan'])
 
 _lib = None
 
@@ -149,6 +149,8 @@ def load():
         lib.cis_host_resize_bilinear_legacy.restype = C.c_int
         lib.cis_host_bgr8_to_rgb_resized.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_int32]
         lib.cis_host_bgr8_to_rgb_resized.restype = C.c_int
+        lib.cis_conv_s2_phase_plan.argtypes = [C.POINTER(CisConv), C.POINTER(CisConv), C.POINTER(C.c_int16)]
+        lib.cis_conv_s2_phase_plan.restype = C.c_int
         for name, args in _PROTOS.items():
             fn = getattr(lib, name)
             fn.argtypes = list(args) + [C.c_void_p]

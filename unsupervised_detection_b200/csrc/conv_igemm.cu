@@ -572,8 +572,21 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
 static constexpr int kHaloMaxBStages = 8;
 struct HaloMaps {
   // one 4-D (C, W, H, N) SWIZZLE_128B map per (concat source, stride-2 phase): index si * nph + phase; box = (64, Wh, Hh, 1)
+  // (compact format: SWIZZLE_NONE, box (8, Wh, Hh, 1))
   CUtensorMap m[CIS_MAX_SRC * 4];
+  // wrow = 1 (compact format only): the weights are read in place from a gather launch's row pack [n_tiles * BN][K_pad] through the 2-D
+  // no-swizzle map w, box (8, BN): kgroup j of K=16 step s is the 8 K columns from wk[2 s + j], landed as BN rows of 16 B at
+  // s * BN * 32 + j * BN * 16 (B descriptor: SBO 128, LBO BN * 16).  wrow = 0: pre-tiled weights at wpack.
+  CUtensorMap w;
+  int wrow;
+  int16_t wk[2 * CIS_MAX_TAPS];
 };
+// weights of the K=16 steps [s0, s0 + ns) of output channels [n0, n0 + BN) from the row pack (HaloMaps::wrow) to dst
+__device__ __forceinline__ void wrow_load(const HaloMaps& maps, const uint32_t dst, const uint32_t bar, const int s0, const int ns, const int n0,
+                                          const int BN) {
+  for (int s = 0; s < ns; ++s)
+    for (int j = 0; j < 2; ++j) tma_load_2d(dst + (uint32_t)(s * BN * 32 + j * BN * 16), &maps.w, bar, maps.wk[2 * (s0 + s) + j], n0);
+}
 
 // wgmma of one weight stage (gt taps of one 64-channel chunk, MT stacked tiles, NK K=16 steps each), issued by the MMA warpgroup into
 // the register accumulators acc[m] of the MT tiles.  The tap offsets come from a shared-memory table (a broadcast read); the offset
@@ -635,14 +648,43 @@ __host__ __device__ __forceinline__ int halo_nsteps(int thin, int ntaps) { retur
 // s_aoff entry of K=16 step s over the taps dh/dw[t0 .. t0 + nt): start of the step's A operand inside the halo in descriptor start-field
 // units (16 B).  Compact format: OR-ed with its LBO (bits 16+), the distance to the second core matrix along K -- the next tap's origin
 // (thin 8; the host lists the taps in increasing order of origin; an odd last tap pairs with itself against zero weights) or plane 1
-// (thin 16).
+// (thin 16).  Stride-2 phases (nph = 4): the planes of phase q follow those of phases 0 .. q-1, so the taps, listed phase by phase,
+// still lie at increasing offsets and a pair may span two phases.
+__device__ __forceinline__ uint32_t halo_tap_off(const CisConv& p, const int t, const int Wh, const uint32_t plane16) {
+  int ph = 0;
+  if (p.nph > 1)
+    while (ph < p.nph - 1 && t >= p.ph_tap[ph + 1]) ++ph;
+  return (uint32_t)(ph * (p.thin / 8)) * plane16 + (uint32_t)(p.dh[t] * Wh + p.dw[t]);
+}
 __device__ __forceinline__ uint32_t halo_step_off(const CisConv& p, const int t0, const int nt, const int s, const int Wh, const uint32_t plane16) {
   if (!p.thin) return (uint32_t)((p.dh[t0 + s] * Wh + p.dw[t0 + s]) * 8);   // * 128 B / 16
   const int ta = p.thin == 8 ? 2 * s : s;
-  const uint32_t o0 = (uint32_t)(p.dh[t0 + ta] * Wh + p.dw[t0 + ta]);
+  const uint32_t o0 = halo_tap_off(p, t0 + ta, Wh, plane16);
   if (p.thin == 16) return o0 | (plane16 << 16);
-  const uint32_t o1 = ta + 1 < nt ? (uint32_t)(p.dh[t0 + ta + 1] * Wh + p.dw[t0 + ta + 1]) : o0;
+  const uint32_t o1 = ta + 1 < nt ? halo_tap_off(p, t0 + ta + 1, Wh, plane16) : o0;
   return o0 | ((o1 - o0) << 16);
+}
+// compact halo of a TMA producer: per stride-2 phase with steps (one phase when nph <= 1), one no-swizzle plane of 8 channels per 8-channel
+// slice of the sources, phase-major.  expect_tx covers every plane.  src: CisSrc array (kernel parameters or their shared-memory copy).
+template <typename Src>
+__device__ __forceinline__ void thin_halo_load(const CisConv& p, const Src* src, const HaloMaps& maps, const uint32_t dst, const uint32_t bar,
+                                               const int HP, const int x0, const int y0, const int n) {
+  const int nph = p.nph > 1 ? p.nph : 1, npl = p.thin / 8, pb16 = thin_plane_bytes(HP);
+  int nld = 0;
+  for (int ph = 0; ph < nph; ++ph) nld += nph == 1 || p.ph_tap[ph + 1] > p.ph_tap[ph];
+  mbar_expect_tx(bar, (uint32_t)(nld * npl * HP * 16));
+  for (int ph = 0; ph < nph; ++ph) {
+    if (nph > 1 && p.ph_tap[ph + 1] == p.ph_tap[ph]) continue;      // phase without taps (kernel size 1)
+    for (int q = 0; q < npl; ++q) {
+      int cq = q, sq = 0;
+      while (sq < p.nsrc - 1 && cq >= src[sq].chunks) {
+        cq -= src[sq].chunks;
+        ++sq;
+      }
+      const int nm = src[sq].n_mod;
+      tma_load_4d(dst + (ph * npl + q) * pb16, &maps.m[sq * nph + ph], bar, cq * 8, x0, y0, nm ? (n % nm) : n);
+    }
+  }
 }
 
 template <int BN, int NWG>
@@ -662,9 +704,10 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int MT = p.MT, MTC = NWG * MT, d = p.dil;   // MT tiles per MMA warpgroup, MTC per CTA
-  const int nph = p.nph > 1 ? p.nph : 1;       // stride-2 forward conv: 4 space-to-depth phases, each with its own halo and tap range
+  const int nph = p.nph > 1 ? p.nph : 1;       // stride-2 forward conv: 4 space-to-depth phases, each with its own halo planes and tap range
   const int Wh = 8 + p.ex, Hh = 16 * MTC + p.ey, HP = Wh * Hh;
   const int thin = p.thin;
+  const int nhph = thin ? 1 : nph;             // halo stages per chunk: the compact format stages every phase's planes in one
   const uint32_t wstep = thin ? BN * 32 : kBStage;                  // weight bytes of one K=16 step (compact) or one tap (64-channel chunk)
   const uint32_t stage_bytes = (uint32_t)G * wstep;
   const uint32_t tile_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -745,9 +788,9 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
       if (tid == 0) {
         // halo through the TMA engine: one 4-D tiled load per 64-channel chunk (x phase), out-of-image pixels / channels are zero-filled
         int hcount = 0;
-        for (int vc = 0; vc < nchunks * nph; ++vc) {
-          const int cc = vc / nph, ph = vc - cc * nph;
-          if (nph > 1 && p.ph_tap[ph + 1] == p.ph_tap[ph]) continue;      // phase without taps (kernel size 1)
+        for (int vc = 0; vc < nchunks * nhph; ++vc) {
+          const int cc = vc / nhph, ph = vc - cc * nhph;
+          if (nhph > 1 && p.ph_tap[ph + 1] == p.ph_tap[ph]) continue;      // phase without taps (kernel size 1)
           const int hs = hcount % NHS;
           mbar_wait(bar_hempty + 8 * hs, (uint32_t)(((hcount / NHS) & 1) ^ 1));
           ++hcount;
@@ -758,19 +801,8 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
           }
           const int nmod = s_src[si].n_mod;
           if (thin) {
-            // compact halo (single chunk, undilated, one phase): one no-swizzle plane of 8 channels per 8-channel slice of the sources
-            const int npl = thin / 8, pb16 = thin_plane_bytes(HP);
-            mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(npl * HP * 16));
-            for (int q = 0; q < npl; ++q) {
-              int cq = q, sq = 0;
-              while (sq < p.nsrc - 1 && cq >= s_src[sq].chunks) {
-                cq -= s_src[sq].chunks;
-                ++sq;
-              }
-              const int nm = s_src[sq].n_mod;
-              tma_load_4d(h_base + hs * halo_stage_bytes + q * pb16, &maps.m[sq], bar_hfull + 8 * hs, cq * 8, tx * 8 + hox, ty * 16 * MTC + hoy,
-                          nm ? (n % nm) : n);
-            }
+            // compact halo (single chunk, undilated): the planes of every phase in one stage
+            thin_halo_load(p, s_src, maps, h_base + hs * halo_stage_bytes, bar_hfull + 8 * hs, HP, tx * 8 + hox, ty * 16 * MTC + hoy, n);
             continue;
           }
           mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
@@ -835,14 +867,15 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
       const uint8_t* wt = reinterpret_cast<const uint8_t*>(wpack) + ((size_t)ny * nchunks_all + cc_lo) * nst * wstep;
       int bs = 0;
       uint32_t bph = 1;           // parity to wait for on the empty barrier: the first pass over the ring finds every stage free
-      for (int vc = 0; vc < nchunks * nph; ++vc) {
-        const int cc = vc / nph, ph = vc - cc * nph;
-        const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : nst;
+      for (int vc = 0; vc < nchunks * nhph; ++vc) {
+        const int cc = vc / nhph, ph = vc - cc * nhph;
+        const int tlo = nhph > 1 ? p.ph_tap[ph] : 0, thi = nhph > 1 ? p.ph_tap[ph + 1] : nst;
         for (int t0 = tlo; t0 < thi; t0 += G) {
           const uint32_t bytes = (uint32_t)min(G, thi - t0) * wstep;
           mbar_wait(bar_bempty + 8 * bs, bph);
           mbar_expect_tx(bar_bfull + 8 * bs, bytes);
-          bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
+          if (maps.wrow) wrow_load(maps, b_base + bs * stage_bytes, bar_bfull + 8 * bs, t0, min(G, thi - t0), ny * BN, BN);
+          else bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
           if (++bs == BS) {
             bs = 0;
             bph ^= 1u;
@@ -860,17 +893,19 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
     constexpr int MTM = Cfg::kMaxMT;
     float acc[MTM][BN];
     // pixel pitch of the halo: 128 B (64-channel SWIZZLE_128B chunk) or 16 B (compact no-swizzle plane); B: 8-row groups 1024 / 256 B apart
+    // (row-pack weights: 128 B, the two kgroups BN * 16 B apart)
     const uint32_t pix = thin ? 16u : 128u;
-    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix), bhi = thin ? desc_hi_ns(256) : desc_hi(1024);
+    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix);
+    const uint32_t bhi = thin ? desc_hi_ns(maps.wrow ? 128u : 256u) : desc_hi(1024), b_lbo = maps.wrow ? BN * 16u : thin ? 128u : 16u;
     const uint32_t a_mstep = (16u * Wh * pix) >> 4;   // descriptor start-field step between stacked M tiles
     const uint32_t a_half = (8u * Wh * pix) >> 4;     // rows 64..127 of a tile: 8 halo rows further
     const uint32_t a_wg = (uint32_t)(wg * MT) * a_mstep;        // this warpgroup's first tile inside the halo
     int bs = 0, hs = 0, it = 0;
     uint32_t bph = 0, hph = 0;
     bool any = false;
-    for (int vc = 0; vc < nchunks * nph; ++vc) {
-      const int cc = vc / nph, ph = vc - cc * nph;
-      const int tlo = nph > 1 ? p.ph_tap[ph] : 0, thi = nph > 1 ? p.ph_tap[ph + 1] : nst;
+    for (int vc = 0; vc < nchunks * nhph; ++vc) {
+      const int cc = vc / nhph, ph = vc - cc * nhph;
+      const int tlo = nhph > 1 ? p.ph_tap[ph] : 0, thi = nhph > 1 ? p.ph_tap[ph + 1] : nst;
       if (thi == tlo) continue;
       const int rem = m_chunks - (cc_lo + cc) * 8;
       const int nk16 = rem >= 8 ? 4 : (rem + 1) / 2;
@@ -882,7 +917,7 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
         const int gt = min(G, thi - t0);
         mbar_wait(bar_bfull + 8 * bs, bph);
         if (wtid == 0 && wg == 0) CIS_TRACE_AT(8 + 2 * it);
-        const uint32_t blo = desc_lo(b_base + bs * stage_bytes, thin ? 128 : 16);
+        const uint32_t blo = desc_lo(b_base + bs * stage_bytes, b_lbo);
         halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, s_aoff + t0, gt, MT, ahi, bhi, a_mstep, a_half, wstep >> 4, !any);
         if (wtid == 0) {   // one release per warpgroup
           mbar_arrive(bar_bempty + 8 * bs);
@@ -1129,19 +1164,8 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
           if (si == 2) nmod = p.src[2].n_mod;
           if (si == 3) nmod = p.src[3].n_mod;
           if (thin) {
-            // compact halo: one no-swizzle plane of 8 channels per 8-channel slice of the sources (see conv_halo_kernel)
-            const int npl = thin / 8, pb16 = thin_plane_bytes(HP);
-            mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(npl * HP * 16));
-            for (int q = 0; q < npl; ++q) {
-              int cq = q, sq = 0;
-              while (sq < p.nsrc - 1 && cq >= p.src[sq].chunks) {
-                cq -= p.src[sq].chunks;
-                ++sq;
-              }
-              const int nm = p.src[sq].n_mod;
-              tma_load_4d(h_base + hs * halo_stage_bytes + q * pb16, &maps.m[sq], bar_hfull + 8 * hs, cq * 8, tx * 8 + hox, ty * 16 * MT + hoy,
-                          nm ? (n % nm) : n);
-            }
+            // compact halo, every stride-2 phase's planes in one stage (see conv_halo_kernel)
+            thin_halo_load(p, p.src, maps, h_base + hs * halo_stage_bytes, bar_hfull + 8 * hs, HP, tx * 8 + hox, ty * 16 * MT + hoy, n);
           } else {
             mbar_expect_tx(bar_hfull + 8 * hs, (uint32_t)(HP * 128));
             tma_load_4d(h_base + hs * halo_stage_bytes, &maps.m[si], bar_hfull + 8 * hs, c * 8, tx * 8 + hox, ty * 16 * MT + hoy,
@@ -1163,7 +1187,8 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
         // the resident set: every sub-problem's tiles at its first step (grouped launches have one chunk; the host checks)
         if ((int)blockIdx.x < total) {
           mbar_expect_tx(bar_bfull, (uint32_t)(nchunks * s_sbase[nsb] * wstep));
-          for (int z = 0; z < nsb; ++z) {
+          if (maps.wrow) wrow_load(maps, b_base, bar_bfull, 0, nst, 0, BN);      // one chunk, one n-tile, not grouped (the host checks)
+          for (int z = 0; z < nsb && !maps.wrow; ++z) {
             const uint8_t* wz = grouped ? reinterpret_cast<const uint8_t*>(p.sub[z].wpack) : wt;
             const int per = nchunks * (s_sbase[z + 1] - s_sbase[z]);
             for (int it = 0; it < per; it += 8) {      // bulk copies of up to 8 tiles (<= 128 KB each)
@@ -1181,7 +1206,8 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
               const uint32_t bytes = (uint32_t)min(G, nst - t0) * wstep;
               mbar_wait(bar_bempty + 8 * bs, bph);
               mbar_expect_tx(bar_bfull + 8 * bs, bytes);
-              bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
+              if (maps.wrow) wrow_load(maps, b_base + bs * stage_bytes, bar_bfull + 8 * bs, t0, min(G, nst - t0), 0, BN);
+              else bulk_g2s(b_base + bs * stage_bytes, wt + (size_t)(cc * nst + t0) * wstep, bytes, bar_bfull + 8 * bs);
               if (++bs == BS) {
                 bs = 0;
                 bph ^= 1u;
@@ -1197,7 +1223,8 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
     constexpr int MTM = (kPMaxAccCols / BN) < 4 ? kPMaxAccCols / BN : 4;
     float acc[MTM][BN];
     const uint32_t pix = thin ? 16u : 128u;       // halo pixel pitch (see conv_halo_kernel)
-    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix), bhi = thin ? desc_hi_ns(256) : desc_hi(1024);
+    const uint32_t ahi = thin ? desc_hi_ns((uint32_t)Wh * pix) : desc_hi((uint32_t)Wh * pix);
+    const uint32_t bhi = thin ? desc_hi_ns(maps.wrow ? 128u : 256u) : desc_hi(1024), b_lbo = maps.wrow ? BN * 16u : thin ? 128u : 16u;
     const uint32_t a_mstep = (16u * Wh * pix) >> 4;
     const uint32_t a_half = (8u * Wh * pix) >> 4;
     int hs = 0, bs = 0, as = 0;
@@ -1220,7 +1247,7 @@ __global__ void __launch_bounds__(kPThreads, 1) conv_halo_persist_kernel(const _
         for (int t0 = 0; t0 < nst; t0 += gstep) {
           const int gt = min(gstep, nst - t0);
           if (!ws) mbar_wait(bar_bfull + 8 * bs, bph);
-          const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(s_sbase[z] + cc * nst) * wstep : b_base + bs * stage_bytes, thin ? 128 : 16);
+          const uint32_t blo = desc_lo(ws ? b_base + (uint32_t)(s_sbase[z] + cc * nst) * wstep : b_base + bs * stage_bytes, b_lbo);
           halo_issue_any<BN, MTM>(nk16, acc, hlo, blo, so + t0, gt, MT, ahi, bhi, a_mstep, a_half, wstep >> 4, (cc | t0) == 0);
           if (wtid == 0) {
             if (!ws) mbar_arrive(bar_bempty + 8 * bs);
@@ -1824,15 +1851,19 @@ extern "C" int cis_set_persist_mode(int mode) {
   return CIS_OK;
 }
 
+// wk: NULL = the weights are cis_pack_weights_tiled tiles at d->wpack; else (compact format) d->wpack is a gather launch's row pack
+// [n_tiles * BN][K_pad] and wk[2 s + j] the K column of kgroup j of step s (HaloMaps::wrow)
 template <int BN, int NWG>
-static int launch_halo(const CisConv* d, cudaStream_t st) {
+static int launch_halo(const CisConv* d, cudaStream_t st, const int16_t* wk = nullptr) {
   const int MTC = d->MT * NWG;                                 // stacked 16x8 tiles per CTA
   const int Wh = 8 + d->ex, Hh = 16 * MTC + d->ey, HP = Wh * Hh;
   const int thin = d->thin;
-  const int halo_stage = ((thin ? thin / 8 * thin_plane_bytes(HP) : HP * 128) + 1023) & ~1023;
+  const int nph = d->nph > 1 ? d->nph : 1;
+  // compact format: the planes of every stride-2 phase share one stage
+  const int halo_stage = ((thin ? nph * (thin / 8) * thin_plane_bytes(HP) : HP * 128) + 1023) & ~1023;
   int chunks = 0;
   for (int i = 0; i < d->nsrc; ++i) chunks += d->src[i].chunks;
-  if (thin && ((thin != 8 && thin != 16) || chunks * 8 != thin || d->dil != 1 || d->nph > 1))
+  if (thin && ((thin != 8 && thin != 16) || chunks * 8 != thin || d->dil != 1))
     return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): the compact format needs 8 or 16 undilated input channels");
   const int nchunks = (chunks + 7) / 8;
   const int nsub = d->nsub > 1 ? d->nsub : 1;                  // grouped launch: grid.z = sub-problem, no split-K
@@ -1858,11 +1889,13 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
     tiles = ((Wp0 + 7) / 8) * ((Hp0 + 16 * MTC - 1) / (16 * MTC));
   }
   if (thin == 8) {
-    // a K=16 step reads its second tap at a positive LBO from the first: every sub-problem lists its taps in increasing halo offset
+    // a K=16 step reads its second tap at a positive LBO from the first: every sub-problem (stride-2 phases: every phase, whose planes
+    // follow the previous phase's) lists its taps in increasing halo offset
     for (int i = 0; i < nsub; ++i) {
       const int t0 = nsub > 1 ? d->sub[i].tap0 : 0, nt = nsub > 1 ? d->sub[i].ntaps : d->ntaps;
       for (int t = t0 + 1; t < t0 + nt; ++t)
-        if (d->dh[t] * (8 + d->ex) + d->dw[t] < d->dh[t - 1] * (8 + d->ex) + d->dw[t - 1])
+        if (!(nph > 1 && (t == d->ph_tap[1] || t == d->ph_tap[2] || t == d->ph_tap[3])) &&
+            d->dh[t] * (8 + d->ex) + d->dw[t] < d->dh[t - 1] * (8 + d->ex) + d->dw[t - 1])
           return cis_set_error(CIS_ERR_BAD_ARG, "cis_conv_igemm(halo): compact 8-channel taps must be listed in increasing halo offset");
     }
   }
@@ -1909,7 +1942,6 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   dim3 grid(tiles * dd * dd * d->N, d->n_tiles, nsub > 1 ? nsub : splits);
   // TMA halo path: undilated, every concat source except the last a multiple of 64 channels (a chunk never straddles sources)
   HaloMaps maps;
-  const int nph = d->nph > 1 ? d->nph : 1;
   static const int dil_tma = getenv("CIS_DIL_TMA") ? atoi(getenv("CIS_DIL_TMA")) : 1;
   int use_tma = ((d->dil == 1 || dil_tma) && Wh * d->dil <= 256 && Hh * d->dil <= 256) ? 1 : 0;
   for (int i = 0; use_tma && !thin && i < d->nsrc - 1; ++i)
@@ -1917,13 +1949,26 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   for (int i = 0; use_tma && i < d->nsrc; ++i) {
     if (((uintptr_t)d->src[i].ptr + (size_t)d->src[i].c_off * 2) % 16) use_tma = 0;
     for (int ph = 0; use_tma && ph < nph; ++ph)
-      if (!(thin ? encode_src_map(&maps.m[i], d->src[i], d->N, d->H, d->W, Wh, Hh, 1, 0, 0, 1, 8, CU_TENSOR_MAP_SWIZZLE_NONE)
+      if (!(thin ? encode_src_map(&maps.m[i * nph + ph], d->src[i], d->N, d->H, d->W, Wh, Hh, nph > 1 ? 2 : 1, ph >> 1, ph & 1, 1, 8,
+                                  CU_TENSOR_MAP_SWIZZLE_NONE)
                  : encode_src_map(&maps.m[i * nph + ph], d->src[i], d->N, d->H, d->W, Wh, Hh, nph > 1 ? 2 : 1, ph >> 1, ph & 1, d->dil)))
         use_tma = 0;
   }
   if (!use_tma) memset(&maps, 0, sizeof(maps));
   if (thin && !use_tma) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): the compact format needs the TMA halo path");
   if (nph > 1 && !use_tma) return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): stride-2 phases need the TMA halo path");
+  maps.wrow = 0;
+  if (wk) {
+    EncodeTiledFn enc = get_encode_tiled();
+    const cuuint64_t dims[2] = {(cuuint64_t)d->K_pad, (cuuint64_t)d->n_tiles * BN}, strides[1] = {(cuuint64_t)d->K_pad * 2};
+    const cuuint32_t box[2] = {8, (cuuint32_t)BN}, es[2] = {1, 1};
+    if (!thin || nsub > 1 || !enc ||
+        enc(&maps.w, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(d->wpack), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+      return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm(halo): row-pack weight map");
+    maps.wrow = 1;
+    memcpy(maps.wk, wk, sizeof(maps.wk));
+  }
   // persistent variant (conv_halo_persist_kernel): layers with many tiles per SM.  CIS_PERSIST_MODE / cis_set_persist_mode:
   //   0 off | 1 (default) layers whose whole weight set stays resident in shared memory and that have >= 2 tiles per SM |
   //   2 every eligible layer (tests) | 3 every layer whose weight set fits, whatever the tile count (tests)
@@ -1931,8 +1976,9 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   static const int p_min_tiles = getenv("CIS_PERSIST_MIN_TILES") ? atoi(getenv("CIS_PERSIST_MIN_TILES")) : 296;
   static const int p_ws_kb = getenv("CIS_PERSIST_WS_KB") ? atoi(getenv("CIS_PERSIST_WS_KB")) : 112;
   if constexpr (BN <= kPMaxAccCols && NWG == 1) {
-   // grouped launches (one chunk, whole weight set resident): the sub-problems' tiles form one work list
-   if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && nph == 1 && (nsub == 1 || nchunks == 1) && dd == 1 &&
+   // grouped launches (one chunk, whole weight set resident): the sub-problems' tiles form one work list.  Stride-2 phases: compact
+   // format only (one halo stage holds every phase)
+   if (persist_mode > 0 && use_tma && d->n_tiles == 1 && splits == 1 && (nph == 1 || thin) && (nsub == 1 || nchunks == 1) && dd == 1 &&
        d->MT * BN <= kPMaxAccCols) {
     int total = tiles * d->N, per_tile = nchunks * nst_max;
     if (nsub > 1) {
@@ -1990,6 +2036,90 @@ static int launch_halo(const CisConv* d, cudaStream_t st) {
   return cis_check_launch("conv_halo");
 }
 
+// A stride-2 gather launch whose sources total 8 or 16 channels, as a compact phase-halo launch (CisConv.nph = 4): input pixel
+// (2 oh + u, 2 ow + v) of tap (u, v) is pixel (oh + u / 2, ow + v / 2) of the space-to-depth phase (u & 1, v & 1) (floor division).
+// The taps are listed phase by phase, each phase in the gather order (increasing (dy, dx), as the compact 8-channel pairs need), and
+// wk gives the row-pack K column of every step's two kgroups: the row pack's K index is tap * cin8 + channel; the second kgroup of an odd
+// last 8-channel step starts at K_pad, outside the map, which the TMA engine fills with zeros.  The tile stack MT follows the planner's wave model (engine.setup_halo_s2).  Returns false
+// (the gather kernel runs the launch) where the halo path does not apply.
+static bool s2_phase_plan(const CisConv* g, CisConv* h, int16_t* wk) {
+  int chunks = 0;
+  for (int i = 0; i < g->nsrc; ++i) {
+    chunks += g->src[i].chunks;
+    if (((uintptr_t)g->src[i].ptr + (size_t)g->src[i].c_off * 2) % 16) return false;
+  }
+  const int thin = chunks * 8, BN = g->BN;
+  if (g->sh != 2 || g->sw != 2 || (thin != 8 && thin != 16) || g->splits > 1 || g->nsub > 1 || g->nph > 1 || g->dil > 1 || g->H < 2 ||
+      g->W < 2 || BN > 128 || g->K_pad > 32767)
+    return false;
+  const int nt = g->ntaps;
+  int order[CIS_MAX_TAPS], bounds[5] = {0, 0, 0, 0, 0}, k = 0;
+  for (int q = 0; q < 4; ++q) {
+    for (int t = 0; t < nt; ++t)
+      if (((g->dh[t] & 1) << 1 | (g->dw[t] & 1)) == q) order[k++] = t;
+    bounds[q + 1] = k;
+  }
+  int hoy = 1 << 20, hox = 1 << 20, ey = 0, ex = 0;
+  for (int t = 0; t < nt; ++t) {
+    hoy = min(hoy, g->dh[t] >> 1);
+    hox = min(hox, g->dw[t] >> 1);
+  }
+  *h = *g;
+  for (int i = 0; i < nt; ++i) {
+    h->dh[i] = (int16_t)((g->dh[order[i]] >> 1) - hoy);
+    h->dw[i] = (int16_t)((g->dw[order[i]] >> 1) - hox);
+    ey = max(ey, (int)h->dh[i]);
+    ex = max(ex, (int)h->dw[i]);
+  }
+  // MT: the planner's wave model for the compact format (weights through the TMA engine and halo bytes ~40 B/clk/SM, K=16 steps)
+  const int nst = halo_nsteps(thin, nt), kb = BN * 32, tiles_x = (g->OW + 7) / 8, nsm = cis_num_sms();
+  int best_mt = 0;
+  double best = 0.0;
+  for (int MT = 1; MT <= 4; ++MT) {
+    if (MT * BN > kMaxAccCols || 8 + ex > 256 || 16 * MT + ey > 256) continue;
+    const int HP = (8 + ex) * (16 * MT + ey);
+    const int halo = (4 * (thin / 8) * thin_plane_bytes(HP) + 1023) & ~1023, smem = halo + HP * 4 + 2048 + 2 * kb;
+    if (smem > 227 * 1024) continue;
+    const int tiles_y = (g->OH + 16 * MT - 1) / (16 * MT);
+    if ((double)g->OH * g->OW < 0.2 * tiles_y * 16 * MT * tiles_x * 8) continue;
+    const long ncta = (long)g->N * tiles_x * tiles_y * g->n_tiles;
+    const int cps = max(1, min(225 * 1024 / smem, 4));
+    const double t_mma = MT * 2.0 * BN * nst * 0.25, t_mem = (double)kb * nst / 40.0 + halo / 40.0;
+    const double t_cta = fmax(t_mma, t_mem) + (4000.0 + 1500.0 * MT) / cps;
+    const double cost = (double)((ncta + (long)nsm * cps - 1) / ((long)nsm * cps)) * cps * t_cta / fmin((double)cps, fmax(1.0, (double)ncta / nsm));
+    if (!best_mt || cost < best - 1e-9) {
+      best = cost;
+      best_mt = MT;
+    }
+  }
+  // grids under the persistent kernel's 296 tiles run one short CTA per tile that fetches its own weights: there the gather kernel is
+  // faster (64x112x4, 5x5 on 16 channels, H100 SXM at 700 W: 10.2 us against 17.9 us)
+  if (!best_mt || (long)g->N * tiles_x * ((g->OH + 16 * best_mt - 1) / (16 * best_mt)) * g->n_tiles < 296) return false;
+  h->halo = 1;
+  h->sh = h->sw = 1;                   // the phases absorb the stride; H x W stay the input size (tensor maps)
+  h->dil = 1;
+  h->MT = best_mt;
+  h->nwg = 1;
+  h->hoy = hoy;
+  h->hox = hox;
+  h->ey = ey;
+  h->ex = ex;
+  h->nph = 4;
+  for (int q = 0; q < 5; ++q) h->ph_tap[q] = bounds[q];
+  h->thin = thin;
+  h->splits = 0;
+  h->sk_cluster = 0;
+  for (int s = 0; s < nst; ++s)
+    for (int j = 0; j < 2; ++j) {
+      const int i = thin == 8 ? 2 * s + j : s;
+      wk[2 * s + j] = (int16_t)(thin == 8 ? (i < nt ? order[i] * 8 : g->K_pad) : order[i] * 16 + 8 * j);
+    }
+  return true;
+}
+extern "C" int cis_conv_s2_phase_plan(const CisConv* d, CisConv* h, int16_t* wk) {
+  return d && h && wk && !d->halo && s2_phase_plan(d, h, wk) ? 1 : 0;
+}
+
 extern "C" int cis_conv_igemm(const CisConv* d, cis_stream_t stream) {
   if (!d || d->ntaps < 1 || d->ntaps > CIS_MAX_TAPS || d->nsrc < 1 || d->nsrc > CIS_MAX_SRC || d->K_pad % 64 != 0 || d->K_pad <= 0 ||
       d->n_tiles < 1 || !d->wpack)
@@ -2015,6 +2145,16 @@ extern "C" int cis_conv_igemm(const CisConv* d, cis_stream_t stream) {
       case 64: return d->nwg == 2 ? launch_halo<64, 2>(d, st) : launch_halo<64, 1>(d, st);
       case 128: return d->nwg == 2 ? launch_halo<128, 2>(d, st) : launch_halo<128, 1>(d, st);
       default: return cis_set_error(CIS_ERR_UNSUPPORTED, "cis_conv_igemm: BN must be 16/32/64/128");
+    }
+  }
+  CisConv h;
+  int16_t wk[2 * CIS_MAX_TAPS];
+  if (s2_phase_plan(d, &h, wk)) {     // thin stride-2 launch: halo bytes ~1x the input tile instead of the gather's ~k*k/4x
+    switch (h.BN) {
+      case 16: return launch_halo<16, 1>(&h, st, wk);
+      case 32: return launch_halo<32, 1>(&h, st, wk);
+      case 64: return launch_halo<64, 1>(&h, st, wk);
+      case 128: return launch_halo<128, 1>(&h, st, wk);
     }
   }
   switch (d->BN) {
