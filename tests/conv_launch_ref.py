@@ -306,8 +306,9 @@ class Walker(object):
     """Replays plans with every recorded conv launch checked.  results[label] = list of worst bound ratios; failures = messages;
     controls[name] = negative-control ratio (> 1: the bound rejected the corrupted comparison)."""
 
-    def __init__(self, rec, controls=False):
+    def __init__(self, rec, controls=False, glue=None):
         self.rec = rec
+        self.glue = glue            # a second checker for the ops it owns (glue_launch_ref.Glue), keyed on the entry point
         self.results = collections.defaultdict(list)
         self.persist = collections.Counter()
         self.failures = []
@@ -322,16 +323,22 @@ class Walker(object):
     def run(self, plan):
         st = torch.cuda.current_stream().cuda_stream
         modes = set()
-        for op in plan.ops:
+        if self.glue is not None:
+            self.glue.start_plan(plan.name)
+        for i, op in enumerate(plan.ops):
             fn, args, name = op[0], op[1], op[2]
             ck = self.rec.by_op.get(id(op))
             if ck is not None and ck.ops[0] is op:
                 self._before(ck)
+            gctx = self.glue.before(op, i) if (self.glue is not None and ck is None and self.glue.owns(name)) else None
             if fn is None:
                 if args is not None:
                     args()
             else:
                 _lib.check(fn(*args, st), name)
+            if gctx is not None:
+                torch.cuda.synchronize()
+                self.glue.after(op, gctx)
             if ck is not None and ck.ops[-1] is op:
                 torch.cuda.synchronize()
                 self._after(ck)
