@@ -45,6 +45,15 @@ Per-element bound, no normalisation by the tensor maximum:
 Stray writes: after each checked launch, every element of the destination buffer outside the launch's rows x [out_coff, out_coff+out_ch)
 must be bit-identical to its snapshot, and the padding channels inside the window must be exactly 0 (a NaN there would poison the next
 layer: its zero weights do not mask it).
+
+Negative controls (Walker(controls=True); a ratio > 1 means the bound rejected the corruption), made on the reference or on a copy of the
+result, each for the first launch that qualifies:
+  fwd.halo, fwd.gather, dgrad.parity_group, wgrad.<kind>: the reference without the centre tap of the weights;
+  tile: one 16 x 8 tile of one channel of a bf16 output scaled by 1 + 2^-5, at the largest output;
+  tile.partial: the same on the last 16 x 8 tile of a launch whose OW is not a multiple of 8 (a partial tile: columns past OW do not
+    exist), at the sample and channel where that tile is largest;
+  thin<t>.cin<c>: a compact thin-input launch (CisConv.thin = t) of a layer with c < t real input channels, against the reference without
+    input channel c - 1 (the last real one; channels c .. t - 1 are the zero padding the format reads).
 """
 import collections
 import contextlib
@@ -537,25 +546,42 @@ class Walker(object):
 
     # ---- negative controls: act on the reference and the copied result only
     def _controls_output(self, ck, got, rr):
-        L, r = ck.layer, self.snap['ref']
+        L, r, d = ck.layer, self.snap['ref'], ck.descs()[0]
         if L.transposed or ck.info['mask_mode'] or rr > 1.0:
             return
-        kind = 'fwd.%s' % ('halo' if ck.descs()[0].halo else 'gather')
+
+        def bound_ratio(g, y):    # g against reference y, within the bound of the intact reference
+            return ratio(g, y, r['S'], E_BF16, r['gamma'] * (1 + 2 ** -7), DELTA_ELU if L.act == ACT_ELU else 0.0)
+
+        def with_weights(w):
+            y = _act(L, _conv(L, r['x'], w) + _bias(L) + (ck.info['addf'][:r['N']].double() if ck.info['addf'] is not None else 0))
+            return y + _real(ck.info['post_add'], r['N']) if ck.info['post_add'] is not None else y
+        kind = 'fwd.%s' % ('halo' if d.halo else 'gather')
         if kind not in self.controls:
             w = r['w'].clone()
             w[L.k // 2, L.k // 2] = 0          # centre tap dropped; the bound of the intact reference is kept
-            y = _act(L, _conv(L, r['x'], w) + _bias(L) + (ck.info['addf'][:r['N']].double() if ck.info['addf'] is not None else 0))
-            if ck.info['post_add'] is not None:
-                y = y + _real(ck.info['post_add'], r['N'])
-            self._control(kind, ratio(got, y, r['S'], E_BF16, r['gamma'] * (1 + 2 ** -7), DELTA_ELU if L.act == ACT_ELU else 0.0))
+            self._control(kind, bound_ratio(got, with_weights(w)))
+        y = r['y']
         if 'tile' not in self.controls:
             # one 16 x 8 tile of one channel scaled by 1 + 2^-5, at the largest output
-            y = r['y']
             n, h, x, c = [int(v) for v in torch.unravel_index(y.abs().argmax(), y.shape)]
             h0, x0 = h // 16 * 16, x // 8 * 8
             bad = got.clone()
             bad[n, h0:h0 + 16, x0:x0 + 8, c] *= 1 + 2 ** -5
-            self._control('tile', ratio(bad, y, r['S'], E_BF16, r['gamma'] * (1 + 2 ** -7), DELTA_ELU if L.act == ACT_ELU else 0.0))
+            self._control('tile', bound_ratio(bad, y))
+        if d.OW % 8 and 'tile.partial' not in self.controls:
+            # the last 16 x 8 tile (partial in x) of one channel scaled by 1 + 2^-5, at the sample and channel where it is largest
+            h0, x0 = (d.OH - 1) // 16 * 16, (d.OW - 1) // 8 * 8
+            n, c = [int(v) for v in torch.unravel_index(y[:, h0:, x0:].abs().amax((1, 2)).argmax(), (y.shape[0], y.shape[3]))]
+            bad = got.clone()
+            bad[n, h0:, x0:, c] *= 1 + 2 ** -5
+            self._control('tile.partial', bound_ratio(bad, y))
+        name = 'thin%d.cin%d' % (d.thin, L.cin)
+        if d.thin and L.cin < d.thin and name not in self.controls:
+            # the last real input channel dropped (the compact format reads cin real channels and thin - cin zero padding channels)
+            w = r['w'].clone()
+            w[:, :, L.cin - 1] = 0
+            self._control(name, bound_ratio(got, with_weights(w)))
 
     def _controls_dgrad(self, ck, got, rr):
         L, r, d = ck.layer, self.snap['ref'], ck.descs()[0]

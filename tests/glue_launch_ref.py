@@ -38,7 +38,12 @@ Per-element bound, no normalisation by the tensor maximum (the form of conv_laun
     eps_q = 2^-23 (|q| + |fs flow|) per axis.  Bilinear is continuous in q, so the warped value moves by <= eps_q 2 M, M = max |c2| over
     the 4 x 4 neighbourhood of the cell; with the lerps' 2^-21 sum |corners| this is Werr.  The correlation sums Cp products in fp32:
     bound_pre = (Cp + 6) 2^-23 S_pre + corr(|c1|, Werr) / C (the 1 / C multiply inside the +6).  Where |pre_ref| <= bound_pre either
-    slope of the leaky is accepted.  Outside the (2R+1)^2 channels at `oo` the destination is bit-identical.
+    slope of the leaky is accepted.  The bound is per (pixel, displacement), so it does not depend on the search range R.  The window is
+    the (2R+1)^2 channels at `oo`, dy outer, padded to a multiple of 8; the padding channels must be +0 bit for bit (at R = 1 a compact
+    16-channel conv reads all 16), and outside the window the destination is bit-identical.  At R = 4 too: channels 81-87 lie inside the
+    88-channel window, where they are held to +0 instead of to their bits before the launch.
+  cis_warp_costvol_r, cis_warp_costvol_bwd_r: the same references with R = the trailing argument r (1 .. 4): (2r+1)^2 = 9 / 25 / 49
+    channels in windows of 16 / 32 / 56 for r = 1 / 2 / 3.
   cis_warp_costvol_bwd: the same composite transposed in fp64 (dc1 = sum_d g' warp[p+d], dwarp = sum_d g'[q-d] c1[q-d], dc2 = the
     bilinear scatter of dwarp, d(flow) = -fs sum_c dwarp (d warp / dq), zero where q - floor leaves [0, 1]), acc bits honoured.  The gate
     is recomputed in fp32, so the (pixel, displacement) pairs with |pre_ref| <= bound_pre may be gated either way: their contribution at
@@ -52,7 +57,8 @@ buffer) must be exactly 0.
 
 Negative controls (a ratio > 1 means the bound rejected the corruption); they act on the reference or on a copy of the result only:
   resize.row_off_by_one, rc_bwd.fold_dropped, rc_bwd.overwrite, dact.d_at_y, colsum.block_dropped, add_slice.acc_dropped,
-  warp_costvol.fs_x1.25, costvol_bwd.gate_one, and tile.<entry point>: one 16 x 8 tile of one channel of a bf16 result scaled by 1 + 2^-5.
+  warp_costvol.fs_x1.25, warp_costvol_r1.dx_outer (the r = 1 cost volume with its displacements listed dx outer), costvol_bwd.gate_one,
+  and tile.<entry point>: one 16 x 8 tile of one channel of a bf16 result scaled by 1 + 2^-5.
 """
 import bisect
 import collections
@@ -92,6 +98,9 @@ ARGS = {
     'cis_pack_generator_input': 'image flow stats B hw dst',
     'cis_warp_costvol': 'c1 c1p c1o c2 c2p c2o flow fs B h w C out op oo',
     'cis_warp_costvol_bwd': 'c1 c1p c1o c2 c2p c2o flow fs B h w C dcorr dcp dco dc1 dc1p dc1o dc2 dc2p dc2o dflow dfp dfo acc gs ws ds',
+    'cis_warp_costvol_r': 'c1 c1p c1o c2 c2p c2o flow fs B h w C out op oo r',
+    'cis_warp_costvol_bwd_r': 'c1 c1p c1o c2 c2p c2o flow fs B h w C dcorr dcp dco dc1 dc1p dc1o dc2 dc2p dc2o dflow dfp dfo acc gs ws ds '
+                              'r',
 }
 
 # entry points of the step pinned per launch by other tests (the ownership test of tests/test_glue_launches_cpu.py)
@@ -806,16 +815,25 @@ class Glue(object):
         bound = (Cp + 6) * U23 * S + _corr(x1.abs(), wp.Werr, R) / C
         return pre, bound
 
-    def _pre_warp_costvol(self, a):
+    def _pre_warp_costvol(self, a, R=4):
         C = a['C']
         c1, c2, flow, Cp = self._cv_operands(a)
         wp = _Warp(c2.double(), flow, a['fs'])
-        pre, bound = self._cv_pre(c1, wp, C, Cp)
-        ctx = dict(pre=pre, bound=bound, reads=[c1, c2] + ([flow] if flow is not None else []),
-                   dests=[(a['out'], torch.bfloat16, a['B'] * a['h'] * a['w'], a['op'], a['oo'], a['oo'] + 81)])
+        pre, bound = self._cv_pre(c1, wp, C, Cp, R)
+        nd = (2 * R + 1) ** 2
+        # the window is the (2R+1)^2 channels padded to a multiple of 8: the padding channels must stay exactly 0
+        ctx = dict(pre=pre, bound=bound, nd=nd, label='cis_warp_costvol_r' if 'r' in a else 'cis_warp_costvol',
+                   reads=[c1, c2] + ([flow] if flow is not None else []),
+                   dests=[(a['out'], torch.bfloat16, a['B'] * a['h'] * a['w'], a['op'], a['oo'], a['oo'] + 8 * (-(-nd // 8)))])
         if self.controls is not None and flow is not None and 'warp_costvol.fs_x1.25' not in self.controls:
-            ctx['bad'] = self._cv_pre(c1, _Warp(c2.double(), flow, a['fs'], fs_scale=1.25), C, Cp)[0]
+            ctx['bad'] = self._cv_pre(c1, _Warp(c2.double(), flow, a['fs'], fs_scale=1.25), C, Cp, R)[0]
+        if self.controls is not None and R == 1 and 'warp_costvol_r1.dx_outer' not in self.controls:
+            # the displacements listed dx outer instead of dy outer
+            ctx['dx_outer'] = pre.view(pre.shape[:-1] + (3, 3)).transpose(-1, -2).reshape(pre.shape)
         return ctx
+
+    def _pre_warp_costvol_r(self, a):
+        return self._pre_warp_costvol(a, a['r'])
 
     def _cv_ratio(self, got, pre, bound):
         ref = F.leaky_relu(pre, 0.1)
@@ -829,12 +847,21 @@ class Glue(object):
         return float((err / b).max())
 
     def _post_warp_costvol(self, a, ctx):
-        got = self.mem.view(a['out'], torch.bfloat16, (a['B'], a['h'], a['w'], a['op']))[..., a['oo']:a['oo'] + 81]
-        self._rec('cis_warp_costvol', 'cost volume', self._cv_ratio(got, ctx['pre'], ctx['bound']))
+        label, nd = ctx['label'], ctx['nd']
+        out = self.mem.view(a['out'], torch.bfloat16, (a['B'], a['h'], a['w'], a['op']))
+        got = out[..., a['oo']:a['oo'] + nd]
+        if not bool((out[..., a['oo'] + nd:a['oo'] + 8 * (-(-nd // 8))].view(torch.int16) == 0).all()):
+            self.failures.append('%s launch %d %s: padding channels not +0' % (self.where + (label,)))
+        self._rec(label, 'cost volume', self._cv_ratio(got, ctx['pre'], ctx['bound']))
         if 'bad' in ctx:
             self._control('warp_costvol.fs_x1.25', self._cv_ratio(got, ctx['bad'], ctx['bound']))
-        if self.controls is not None and 'tile.cis_warp_costvol' not in self.controls:
-            self._control('tile.cis_warp_costvol', self._cv_ratio(_tile(got), ctx['pre'], ctx['bound']))
+        if 'dx_outer' in ctx:
+            self._control('warp_costvol_r1.dx_outer', self._cv_ratio(got, ctx['dx_outer'], ctx['bound']))
+        if self.controls is not None and 'tile.' + label not in self.controls:
+            self._control('tile.' + label, self._cv_ratio(_tile(got), ctx['pre'], ctx['bound']))
+
+    def _post_warp_costvol_r(self, a, ctx):
+        self._post_warp_costvol(a, ctx)
 
     def _pre_warp_costvol_bwd(self, a, R=4):
         B, h, w, C = a['B'], a['h'], a['w'], a['C']
@@ -862,7 +889,8 @@ class Glue(object):
         EW = sum(_shift(amb[..., k:k + 1] * x1.abs(), -dy, -dx) for k, (dy, dx) in enumerate(_disps(R)))
         errW = gam * SW + EW                               # what the fp32 dwarp may be off by
         npix = B * h * w
-        out = dict(reads=[c1, c2, dcorr] + ([flow] if flow is not None else []), dests=[], checks=[])
+        out = dict(reads=[c1, c2, dcorr] + ([flow] if flow is not None else []), dests=[], checks=[],
+                   label='cis_warp_costvol_bwd_r' if 'r' in a else 'cis_warp_costvol_bwd')
 
         def add(p, pitch, off, nch, ref, err, bit, what):
             old = self.mem.view(p, torch.bfloat16, (B, h, w, pitch))[..., off:off + nch].double()
@@ -898,11 +926,17 @@ class Glue(object):
         for p, pitch, off, nch, ref, err, what in ctx['checks']:
             got = self.mem.view(p, torch.bfloat16, (B, h, w, pitch))[..., off:off + nch]
             b = E_BF16 * ref.abs() + err * (1 + 2 ** -7)
-            self._rec('cis_warp_costvol_bwd', what, ratio(got, ref, b))
+            self._rec(ctx['label'], what, ratio(got, ref, b))
             if what == 'dc1' and 'bad_dc1' in ctx:
                 # the largest over the levels: where the correlations are almost all positive the gate hardly matters
                 r = ratio(got, ref + ctx['bad_dc1'], b)
                 self.controls['costvol_bwd.gate_one'] = max(r, self.controls.get('costvol_bwd.gate_one', 0.0))
+
+    def _pre_warp_costvol_bwd_r(self, a):
+        return self._pre_warp_costvol_bwd(a, a['r'])
+
+    def _post_warp_costvol_bwd_r(self, a, ctx):
+        self._post_warp_costvol_bwd(a, ctx)
 
     # ---- summary
     def summary(self):

@@ -7,14 +7,16 @@ poisoned-buffer replay showing that each plan reads only what it wrote.
   defaults     192x384, batch 16, flow given directly
   odd          100x172, batch 3, flow given: the generic (non-x2) resize-concat and its transpose
   direct       the branches no graph reaches: the nx > 8 fallback of the resize-concat transpose, 1-pixel sources, 3 replicas with
-               accumulate, the bf16 resize pair at a non-binary ratio
+               accumulate, the bf16 resize pair at a non-binary ratio; the warp + cost-volume transpose on independent random features
+               (about half the correlations negative, so the leaky gate shows) at R = 4 and, through cis_warp_costvol_bwd_r, at r = 1, 2, 3
 
 The conv launches run unchecked here (tests/test_conv_launches_gpu.py checks them per launch).  One summary line per label (count, worst
 bound ratio) is printed with pytest -s.  Measured worst ratios on an H100 80GB HBM3, over all graphs and direct calls: 0 for every
 bit-exact kind; 0.996 for the bf16 resize-concat (x2, generic), its transposes (same, x2, generic), the nearest x2 transpose, the bf16
-resize pair and the generator input; 0.994 cis_resize_f32_bwd_to_bf16_scaled; 0.993 cis_warp_costvol_bwd; 0.992 cis_warp_costvol;
-0.154 cis_resize_bilinear_f32; 0.009 the dact_colsum partials; 0.001 cis_colsum; 0.0004 cis_flow_stats.  The bf16 kinds sit at the
-rounding term 2^-8 |ref|.  The whole file runs in about 16 s."""
+resize pair and the generator input; 0.994 cis_resize_f32_bwd_to_bf16_scaled; 0.993 cis_warp_costvol_bwd; 0.984 the direct
+cis_warp_costvol_bwd_r at r = 1, 2, 3 (gate_one controls 4.5e4 - 1.0e5); 0.992 cis_warp_costvol; 0.154 cis_resize_bilinear_f32;
+0.009 the dact_colsum partials; 0.001 cis_colsum; 0.0004 cis_flow_stats.  The bf16 kinds sit at the rounding term 2^-8 |ref|.  The whole
+file runs in about 16 s."""
 import pytest
 import torch
 
@@ -118,6 +120,30 @@ def test_direct_warp_costvol_bwd_gate():
                                               88, 0, dc1.data_ptr(), C, 0, dc2.data_ptr(), C, 0, dfl.data_ptr(), 8, 0, 0, gs.data_ptr(),
                                               ws.data_ptr(), ds.data_ptr()))])
     _report('direct_costvol_bwd', glue)
+    assert not glue.failures, '\n'.join(glue.failures[:20])
+    assert glue.controls['costvol_bwd.gate_one'] > 1.0, glue.controls
+
+
+@pytest.mark.parametrize('r', [1, 2, 3])
+def test_direct_warp_costvol_bwd_r_gate(r):
+    """The same for the search-range entry point cis_warp_costvol_bwd_r: the PWC-Net graphs at ranges 1-3 hardly show the gate, so here
+    the gate_one control shows that the bound rejects a wrong transpose at each range."""
+    gen = torch.Generator().manual_seed(23 + r)
+    B, h, w, C = 1, 12, 20, 16
+    nd = (2 * r + 1) ** 2
+    pad = 8 * (-(-nd // 8))
+    c1, c2 = _bf(gen, B, h, w, C), _bf(gen, B, h, w, C)
+    flow = R.smooth(B, h, w, 2, 1.5, gen, div=4).cuda()
+    dcorr = _bf(gen, B, h, w, pad)
+    dc1, dc2, dfl = (torch.zeros(B, h, w, n, dtype=torch.bfloat16, device='cuda') for n in (C, C, 8))
+    npix = B * h * w
+    gs, ws = torch.zeros(npix * nd, device='cuda'), torch.zeros(npix * C, device='cuda')
+    ds = torch.zeros(npix * C, dtype=torch.float64, device='cuda')
+    args = (c1.data_ptr(), C, 0, c2.data_ptr(), C, 0, flow.data_ptr(), 2.5, B, h, w, C, dcorr.data_ptr(), pad, 0, dc1.data_ptr(), C, 0,
+            dc2.data_ptr(), C, 0, dfl.data_ptr(), 8, 0, 0, gs.data_ptr(), ws.data_ptr(), ds.data_ptr(), r)
+    glue = _direct([('cis_warp_costvol_bwd_r', args)])
+    _report('direct_costvol_bwd_r%d' % r, glue)
+    assert glue.counts['cis_warp_costvol_bwd_r'] == 1
     assert not glue.failures, '\n'.join(glue.failures[:20])
     assert glue.controls['costvol_bwd.gate_one'] > 1.0, glue.controls
 
@@ -260,11 +286,14 @@ def _targets(g, plans):
     for L in list(g.gen.all_layers()) + list(g.rec.all_layers()) + (list(g.pwc.all_layers()) if g.with_pwc else []):
         walk(L)
     # scalars[5:8] are slots no kernel writes (cis_cis_loss_reduce defines [0, 5))
-    named = [g.image, g.flow, g.mask, g.flow1, g.pred, g.dpred, g.dmask, g.sums, g.scalars[:5], g.coef]
-    named += [t for t in (getattr(g, 'stats', None), getattr(g, 'image_st', None), getattr(g, 'flow_st', None)) if t is not None]
+    named = [g.image, g.flow, g.mask, g.flow1, g.pred, g.dmask, g.sums, g.scalars[:5], g.coef]
+    named += [t for t in (getattr(g, 'dpred', None), getattr(g, 'stats', None), getattr(g, 'image_st', None), getattr(g, 'flow_st', None))
+              if t is not None]
     if g.with_pwc:
         named.append(g.flow_full)
-    inputs = {t.data_ptr() for t in (g.img1, g.img2) if t is not None}
+    # what a batch upload writes (the two buffers of a staged graph, image and flow otherwise) is input, not poisoned
+    inputs = {t.data_ptr() for t in (g.inputs if g.staged else (g.image, g.flow))}
+    named = [t for t in named if t.data_ptr() not in inputs]
     full = {t.data_ptr() for t in named}
     f32 = named + [t for t in f32 if t.data_ptr() not in inputs and t.data_ptr() not in full]
     return acts, f32, b16
