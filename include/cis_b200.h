@@ -413,6 +413,38 @@ int cis_warp_costvol_bwd_r(const void* c1, int32_t c1_pitch, int32_t c1_coff, co
 int cis_parity_split_bf16(const void* src, int32_t s_pitch, int32_t s_coff, int32_t N, int32_t H, int32_t W, int32_t C, void* dst,
                           int32_t d_pitch, cis_stream_t stream);
 
+/* ---- PWC-Net training (tfoptflow's multi-scale objective, as defined in DESIGN.md: not checked against TensorFlow) ----
+ * Level i = 0..4 is pyramid level l = 6 - i: flow[i] = the refined fp32 flow [B, H >> l, W >> l, 2] of the network at input size H x W;
+ * grad[i] = the bf16 gradient of that level's flow Act (element (pixel, c) at grad[i][pixel * pitch[i] + c_off[i] + c], c = 0, 1),
+ * overwritten or, with accumulate[i], added to; weight[i] = the backward's factor alpha_l / global batch. */
+typedef struct {
+  const float* flow[5];
+  void* grad[5];
+  int32_t pitch[5];
+  int32_t c_off[5];
+  int32_t accumulate[5];
+  float weight[5];
+} CisFlowPyr;
+/* gt = fp32 [B, GH, GW, 2], the ground-truth flow in PWC-Net's channel order.  Target of level l: g_l = R_l(gt) * (s_c / 2^l) for channel
+ * c, R_l = the legacy bilinear resize to the level's size (cis_resize_bilinear_f32's rule), sampled on the fly; s0, s1 = the vectors' scale
+ * from the gt grid to the input grid (1 when GH x GW = H x W).  rho(d), d = flow_l - g_l: robust = 0: ||d||_2; robust = 1:
+ * (|d0| + |d1| + eps)^q.  out = double [B, 5]: out[b * 5 + i] = sum over level i's pixels of sample b of rho.  The sums are double,
+ * reduced in a fixed order through scratch (double [5 * B * 64], need not be initialised), no atomics: bit-identical run to run.
+ * gt and flow[0..4] are read as pairs of floats and must be 8-byte aligned (a tensor's base address is).
+ * CIS_ERR_BAD_ARG unless H and W are multiples of 64, 1 <= B <= 65535, GH, GW >= 1, and the alignment holds. */
+int cis_flow_multiscale_loss(const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW, float s0,
+                             float s1, int32_t robust, float eps, float q, double* scratch, double* out, cis_stream_t stream);
+/* its backward, all five levels in one launch: grad[i] (=|+=) weight[i] * d rho / d flow_l per pixel.  The gradient of ||d||_2 is
+ * d / ||d||_2, and 0 at d = 0; that of |d_c| is sign(d_c), 0 at d_c = 0. */
+int cis_flow_multiscale_loss_bwd(const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW, float s0,
+                                 float s1, int32_t robust, float eps, float q, cis_stream_t stream);
+/* TF-Adam with L2 weight decay, no clip: g' = grad + decay * param inside the segments seg = int64 [nseg][2] {start, end} (device,
+ * sorted and disjoint: the kernel variables), g' = grad elsewhere; then cis_clip_adam's update (lr_t = lr * sqrt(1 - b2^t) / (1 - b1^t),
+ * t = step_state[0] + 1) over [0, n).  lr = device float [1], read when the kernel runs (a rate schedule needs no re-capture).
+ * step_state is advanced by this call. */
+int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, const int64_t* seg, int32_t nseg, float decay, const float* lr,
+                float beta1, float beta2, float eps, int64_t* step_state, cis_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

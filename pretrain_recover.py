@@ -13,7 +13,7 @@ from absl import flags as absl_flags
 
 from train import seed_everything
 from unsupervised_detection_b200 import flow_flags
-from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES
+from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES, define_validate
 from unsupervised_detection_b200.step_graph import box_sides
 
 PRETRAIN_FLAGS = ['box_min', 'box_max', 'pretrain_flow', 'validate', 'flow_dir']
@@ -23,8 +23,7 @@ if 'box_min' not in FLAGS:
     absl_flags.DEFINE_enum('pretrain_flow', 'pwc', ['pwc', 'gt'], "flow the recover net learns to inpaint: 'pwc' = PWC-Net's flow of "
                            "the frame pair (needs --flow_ckpt), 'gt' = the dataset's ground-truth flow (FLYINGCHAIRS, or DAVIS2016 / FBMS / "
                            "SEGTRACK with --flow_dir)")
-    absl_flags.DEFINE_bool('validate', False, 'score the held-out EPE inside the boxes on the val split every epoch and save '
-                           'recover-best when it improves (FLYINGCHAIRS with its split file)')
+define_validate()
 
 
 def check_flags(config):

@@ -61,6 +61,11 @@ class CisWgrad(C.Structure):
                 ('nh', C.c_int32), ('nwg', C.c_int32)]
 
 
+class CisFlowPyr(C.Structure):
+    _fields_ = [('flow', C.c_void_p * 5), ('grad', C.c_void_p * 5), ('pitch', C.c_int32 * 5), ('c_off', C.c_int32 * 5),
+                ('accumulate', C.c_int32 * 5), ('weight', C.c_float * 5)]
+
+
 _i32, _i64, _f32, _p, _u64 = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_uint64
 
 # name -> argtypes (the trailing stream argument is appended automatically)
@@ -119,6 +124,10 @@ _PROTOS = {
     'cis_warp_costvol_bwd': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32,
                              _p, _i32, _i32, _i32, _p, _p, _p],
     'cis_parity_split_bf16': [_p, _i32, _i32, _i32, _i32, _i32, _i32, _p, _i32],
+    # PWC-Net training: multi-scale flow loss forward / backward, TF-Adam with L2 weight decay on the kernel segments
+    'cis_flow_multiscale_loss': [C.POINTER(CisFlowPyr), _p, _i32, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _f32, _f32, _p, _p],
+    'cis_flow_multiscale_loss_bwd': [C.POINTER(CisFlowPyr), _p, _i32, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _f32, _f32],
+    'cis_adam_l2': [_p, _p, _p, _p, _i64, _p, _i32, _f32, _p, _f32, _f32, _f32, _p],
     # search-range variants: the arguments of the three entry points above plus search_range (1..4)
     'cis_warp_costvol_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32],
     'cis_cost_volume_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _i32],

@@ -58,6 +58,15 @@ def _define():
 _define()
 
 
+def define_validate():
+    """--validate, shared by pretrain_recover.py and train_flow.py (not one of the reference's flags, so not in FLAG_NAMES): defined once,
+    with one help text, by whichever of the two scripts is imported first."""
+    if 'validate' not in FLAGS:
+        gflags.DEFINE_bool('validate', False, 'score the held-out end-point error on the val split at every epoch end and save the '
+                                              'best checkpoint (recover-best / pwcnet-best) when it improves; needs --dataset=FLYINGCHAIRS '
+                                              'with its split file')
+
+
 class Config(object):
     """Plain-attribute stand-in for the parsed FLAGS object (handy for tests / bench): same names and defaults."""
 

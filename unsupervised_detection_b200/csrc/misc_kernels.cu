@@ -1846,6 +1846,130 @@ static int warp_costvol_bwd(const void* c1, int32_t c1p, int32_t c1o, const void
     default: return cis_set_error(CIS_ERR_BAD_ARG, what ": search_range must be 1, 2, 3 or 4");                       \
   }
 
+// ------------------------------------------------------------------------------------------------ PWC-Net training
+// Multi-scale flow loss (cis_flow_multiscale_loss).  Level i = 0..4 is pyramid level l = 6 - i at (H >> l) x (W >> l).  The target is
+// sampled from the ground truth on the fly with the legacy bilinear rule of resize_bilinear_f32_kernel<false>, vectors times f = s_c / 2^l.
+struct FlowLossArgs {
+  CisFlowPyr pyr;
+  const float* gt;
+  int B, H, W, GH, GW;
+  float s0, s1;
+  int robust;
+  float eps, q;
+};
+__device__ __forceinline__ float2 flow_level_diff(const FlowLossArgs& a, int i, int b, int y, int x) {
+  const int l = 6 - i, h = a.H >> l, w = a.W >> l;
+  const Lerp ly = legacy_lerp(y, a.GH, (float)a.GH / (float)h), lx = legacy_lerp(x, a.GW, (float)a.GW / (float)w);
+  const float* g = a.gt + (size_t)b * a.GH * a.GW * 2;
+  const float2 tl = *reinterpret_cast<const float2*>(g + ((size_t)ly.lo * a.GW + lx.lo) * 2);
+  const float2 tr = *reinterpret_cast<const float2*>(g + ((size_t)ly.lo * a.GW + lx.hi) * 2);
+  const float2 bl = *reinterpret_cast<const float2*>(g + ((size_t)ly.hi * a.GW + lx.lo) * 2);
+  const float2 br = *reinterpret_cast<const float2*>(g + ((size_t)ly.hi * a.GW + lx.hi) * 2);
+  const float t0 = tl.x + (tr.x - tl.x) * lx.f, b0 = bl.x + (br.x - bl.x) * lx.f;
+  const float t1 = tl.y + (tr.y - tl.y) * lx.f, b1 = bl.y + (br.y - bl.y) * lx.f;
+  const float inv = 1.f / (float)(1 << l);   // exact
+  const float2 f = *reinterpret_cast<const float2*>(a.pyr.flow[i] + (((size_t)b * h + y) * w + x) * 2);
+  return make_float2(f.x - (t0 + (b0 - t0) * ly.f) * (a.s0 * inv), f.y - (t1 + (b1 - t1) * ly.f) * (a.s1 * inv));
+}
+// pass 1: block x of (sample b, level i) sums rho over a fixed pixel subset (grid-stride) in double, reduced warp butterfly -> the 8 warps
+// in index order into part[(i * B + b) * kFlowStdBlocks + x]
+__global__ void flow_loss_sums_kernel(FlowLossArgs a, double* __restrict__ part) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ double sm[8];
+  const int b = blockIdx.y, i = blockIdx.z, l = 6 - i, w = a.W >> l;
+  const size_t hw = (size_t)(a.H >> l) * w;
+  double s = 0;
+  for (size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x; p < hw; p += (size_t)gridDim.x * blockDim.x) {
+    const float2 d = flow_level_diff(a, i, b, (int)(p / w), (int)(p % w));
+    if (a.robust) s += pow(fabs((double)d.x) + fabs((double)d.y) + (double)a.eps, (double)a.q);
+    else s += sqrt((double)d.x * d.x + (double)d.y * d.y);
+  }
+  s = warp_sum_d(s);
+  if ((threadIdx.x & 31) == 0) sm[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) t += sm[k];
+    part[((size_t)i * a.B + b) * gridDim.x + blockIdx.x] = t;
+  }
+}
+// pass 2: one block per sample, thread i adds level i's kFlowStdBlocks partials in block order
+__global__ void flow_loss_reduce_kernel(const double* __restrict__ part, int B, double* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x, i = threadIdx.x;
+  double t = 0;
+  for (int q = 0; q < kFlowStdBlocks; ++q) t += part[((size_t)i * B + b) * kFlowStdBlocks + q];
+  out[b * 5 + i] = t;
+}
+// backward: one thread per pixel of the five levels, levels laid end to end (i = 0 first)
+__global__ void flow_loss_bwd_kernel(FlowLossArgs a, size_t total) {
+  pdl_launch_dependents();
+  pdl_wait();
+  size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= total) return;
+  int i = 0;
+  for (; i < 4; ++i) {
+    const size_t n = (size_t)a.B * (a.H >> (6 - i)) * (a.W >> (6 - i));
+    if (p < n) break;
+    p -= n;
+  }
+  const int l = 6 - i, h = a.H >> l, w = a.W >> l;
+  const int x = (int)(p % w), y = (int)((p / w) % h), b = (int)(p / ((size_t)w * h));
+  const float2 d = flow_level_diff(a, i, b, y, x);
+  float g0, g1;
+  if (a.robust) {
+    const float k = a.q * powf(fabsf(d.x) + fabsf(d.y) + a.eps, a.q - 1.f);
+    g0 = d.x > 0.f ? k : (d.x < 0.f ? -k : 0.f);
+    g1 = d.y > 0.f ? k : (d.y < 0.f ? -k : 0.f);
+  } else {
+    const float n = sqrtf(d.x * d.x + d.y * d.y);
+    g0 = n > 0.f ? d.x / n : 0.f;
+    g1 = n > 0.f ? d.y / n : 0.f;
+  }
+  const float wt = a.pyr.weight[i];
+  const Bf16Out o{(bf16*)a.pyr.grad[i], a.pyr.pitch[i], a.pyr.c_off[i], a.pyr.accumulate[i]};
+  o.put(p, 0, wt * g0);
+  o.put(p, 1, wt * g1);
+}
+// TF-Adam on grad + decay * param inside the kernel segments (binary search over the sorted segment starts), no clip
+__global__ void adam_l2_kernel(float* __restrict__ param, float* __restrict__ m, float* __restrict__ v, const float* __restrict__ grad, size_t n,
+                               const long long* __restrict__ seg, int nseg, float decay, const float* __restrict__ lr, float b1, float b2, float eps,
+                               const long long* __restrict__ step) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int lo = 0, hi = nseg;                      // first segment whose start is > i
+  while (lo < hi) {
+    const int mid = (lo + hi) >> 1;
+    if (seg[2 * mid] <= (long long)i) lo = mid + 1;
+    else hi = mid;
+  }
+  const float w = param[i];
+  float g = grad[i];
+  if (lo > 0 && (long long)i < seg[2 * (lo - 1) + 1]) g += decay * w;
+  const long long t = step[0] + 1;
+  const float lr_t = lr[0] * sqrtf(1.f - powf(b2, (float)t)) / (1.f - powf(b1, (float)t));
+  const float mi = b1 * m[i] + (1.f - b1) * g;
+  const float vi = b2 * v[i] + (1.f - b2) * g * g;
+  m[i] = mi;
+  v[i] = vi;
+  param[i] = w - lr_t * mi / (sqrtf(vi) + eps);
+}
+static int flow_loss_args(const char* what, const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW,
+                          float s0, float s1, int32_t robust, float eps, float q, FlowLossArgs& a) {
+  if (!pyr || !gt || B < 1 || B > 65535 || H < 64 || W < 64 || H % 64 || W % 64 || GH < 1 || GW < 1 || (robust != 0 && robust != 1))
+    return cis_set_error(CIS_ERR_BAD_ARG, what);
+  // gt and the level flows are read as float2: 8-byte aligned pairs
+  if ((uintptr_t)gt & 7) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  for (int i = 0; i < 5; ++i)
+    if (!pyr->flow[i] || ((uintptr_t)pyr->flow[i] & 7)) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  a = FlowLossArgs{*pyr, gt, B, H, W, GH, GW, s0, s1, robust, eps, q};
+  return CIS_OK;
+}
+
 extern "C" {
 
 int cis_pack_weights(const float* w, const int32_t* kmap, int32_t K_pad, int32_t rows, int32_t cout, int32_t sn, const int32_t* nmap, void* wp,
@@ -2232,6 +2356,39 @@ int cis_parity_split_bf16(const void* src, int32_t sp, int32_t sc, int32_t N, in
   if (C < 1 || C > 8 || dp < 8 || (dp & 7)) return cis_set_error(CIS_ERR_BAD_ARG, "cis_parity_split_bf16: 1..8 channels into 8-aligned planes");
   CIS_LAUNCH(parity_split_bf16_kernel, nblk((size_t)4 * N * H * W), 256, 0, ST, (cbf)src, sp, sc, N, H, W, C, (mbf)dst, dp);
   return cis_check_launch("parity_split_bf16");
+}
+int cis_flow_multiscale_loss(const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW, float s0,
+                             float s1, int32_t robust, float eps, float q, double* scratch, double* out, cis_stream_t stream) {
+  FlowLossArgs a;
+  const int rc = flow_loss_args("cis_flow_multiscale_loss: bad pyramid, size, rho or alignment", pyr, gt, B, H, W, GH, GW, s0, s1, robust, eps, q, a);
+  if (rc) return rc;
+  if (!scratch || !out) return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_multiscale_loss: no scratch or output");
+  CIS_LAUNCH(flow_loss_sums_kernel, dim3(kFlowStdBlocks, B, 5), 256, 0, ST, a, scratch);
+  CIS_LAUNCH(flow_loss_reduce_kernel, B, 5, 0, ST, (const double*)scratch, B, out);
+  return cis_check_launch("flow_multiscale_loss");
+}
+int cis_flow_multiscale_loss_bwd(const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW, float s0,
+                                 float s1, int32_t robust, float eps, float q, cis_stream_t stream) {
+  FlowLossArgs a;
+  const int rc = flow_loss_args("cis_flow_multiscale_loss_bwd: bad pyramid, size, rho or alignment", pyr, gt, B, H, W, GH, GW, s0, s1, robust, eps, q, a);
+  if (rc) return rc;
+  size_t total = 0;
+  for (int i = 0; i < 5; ++i) {
+    if (!pyr->grad[i] || pyr->pitch[i] < 2 || pyr->c_off[i] < 0 || pyr->c_off[i] + 2 > pyr->pitch[i])
+      return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_multiscale_loss_bwd: bad gradient slice");
+    total += (size_t)B * (H >> (6 - i)) * (W >> (6 - i));
+  }
+  CIS_LAUNCH(flow_loss_bwd_kernel, nblk(total), 256, 0, ST, a, total);
+  return cis_check_launch("flow_multiscale_loss_bwd");
+}
+int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, const int64_t* seg, int32_t nseg, float decay, const float* lr,
+                float beta1, float beta2, float eps, int64_t* step_state, cis_stream_t stream) {
+  if (!param || !m || !v || !grad || n < 1 || nseg < 0 || (nseg > 0 && !seg) || !lr || !step_state)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_adam_l2: bad buffer, size or segment list");
+  CIS_LAUNCH(adam_l2_kernel, nblk((size_t)n), 256, 0, ST, param, m, v, grad, (size_t)n, (const long long*)seg, nseg, decay, lr, beta1, beta2, eps,
+             (const long long*)step_state);
+  CIS_LAUNCH(step_inc_kernel, 1, 1, 0, ST, (long long*)step_state);
+  return cis_check_launch("adam_l2");
 }
 
 }  // extern "C"

@@ -259,7 +259,7 @@ class AdversarialLearner(object):
         for old in ckpt_io.update_checkpoint_state(checkpoint_dir, base, keep=40):
             for suf in ('.index', '.data-00000-of-00001', '.pt'):
                 fp = os.path.join(checkpoint_dir, old + suf)
-                if os.path.isfile(fp) and old not in ('model.best', 'recover-best'):
+                if os.path.isfile(fp) and old not in ('model.best', 'recover-best', 'pwcnet-best'):
                     os.remove(fp)
 
     # ------------------------------------------------------------------------------------------------ stepping

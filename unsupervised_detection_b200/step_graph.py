@@ -28,6 +28,81 @@ def box_sides(box_min, box_max, H, W):
     return tuple(out)
 
 
+def capture_plans(graphs, key, plans, lane_key=0, warm=True):
+    """The CUDA graph of `plans` cached in the dict `graphs` under `key`, captured on first use.  warm: run the plans once outside
+    capture first (sets function attributes, lazy allocations) -- never for plans that change state (the optimiser step)."""
+    g = graphs.get(key)
+    if g is None:
+        torch.cuda.synchronize()
+        if warm:
+            s = torch.cuda.Stream()
+            s.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(s):
+                for pl in plans:
+                    pl.run(lane_key=lane_key)
+            torch.cuda.current_stream().wait_stream(s)
+            torch.cuda.synchronize()
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g):
+            for pl in plans:
+                pl.run(lane_key=lane_key)
+        graphs[key] = g
+    return g
+
+
+class UploadSlots(object):
+    """Host -> device batch uploads on a copy stream for a graph whose batch fills the device buffers `like`: prefetch() copies an
+    upcoming batch into one of two device staging slots, so that it overlaps the kernels queued now, and take() hands it over into the
+    graph's inputs on the current stream.  Write-after-read: a slot is overwritten only once the main stream's last read of it has
+    executed (the host can run steps ahead of the GPU).  copy_stream: callable -> the copy stream (made on first use)."""
+
+    def __init__(self, like, copy_stream):
+        self._like, self._copy_stream = tuple(like), copy_stream
+        self._slots = None                  # two device staging slots, made on first prefetch
+        self._slot = 0                      # the slot the last prefetch wrote
+        self._read = [None, None]           # per slot: event after the main stream's last read of it (take)
+        self._staged = None                 # (first host tensor, slot, copy-done event) of the last prefetched batch
+
+    def upload(self, after, dst, srcs):
+        """Host -> device copy of srcs into the device tensors dst on the copy stream, once event `after` (if any) has completed -> the
+        event after the copy."""
+        copy = self._copy_stream()
+        if after is not None:
+            copy.wait_event(after)
+        with torch.cuda.stream(copy):
+            for d, s in zip(dst, srcs):
+                d.copy_(s, non_blocking=True)
+            ready = torch.cuda.Event()
+            ready.record(copy)
+        return ready
+
+    def prefetch(self, srcs):
+        if self._slots is None:
+            self._slots = [tuple(torch.empty_like(t) for t in self._like) for _ in range(2)]
+        self._slot ^= 1
+        self._staged = (srcs[0], self._slot, self.upload(self._read[self._slot], self._slots[self._slot], srcs))
+
+    def take(self, key, dst):
+        """When the last prefetch staged the batch whose first host tensor is `key`: copy it from its slot into dst on the current stream
+        -> True; else False (nothing done)."""
+        st = self._staged
+        if st is None or st[0] is not key:
+            return False
+        _, slot, ready = st
+        cur = torch.cuda.current_stream()
+        cur.wait_event(ready)
+        for d, s in zip(dst, self._slots[slot]):
+            d.copy_(s, non_blocking=True)
+        self._read[slot] = torch.cuda.Event()
+        self._read[slot].record(cur)
+        self._staged = None
+        return True
+
+    def drop(self):
+        """Forget the staged batch: take() then hands nothing over until the next prefetch."""
+        self._staged = None
+
+
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
                  beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks=None, box=None,
@@ -226,10 +301,7 @@ class CISGraph(object):
         # ---- device-only state, made on first use (a CISGraph is also built with device='cpu' to inspect its plans)
         self.graphs = {}                    # CUDA graphs by key (_capture_plans)
         self._side = self._copy = None      # streams of the pipelined flow-network branch and of batch uploads (_streams)
-        self._slots = None                  # two device staging slots (img1, img2) of prefetch
-        self._slot = 0                      # the slot the last prefetch wrote
-        self._slot_read = [None, None]      # per slot: event after the main stream's last read of it (feed)
-        self._staged = None                 # (host img1, slot, copy-done event) of the last prefetched batch
+        self._uploads = UploadSlots(self.inputs or (), lambda: self._streams()[1])     # copy-stream uploads of (img1, img2)
         self._pipe_done = None              # event: the last pipelined step's flow-network branch has filled the stage
         self._pipe_free = None              # event: prime_pipeline has finished reading img1 / img2
         # Which frame pair is where.  A frame pair is named by its host img1 tensor when feed_next uploaded it, and by the device
@@ -367,25 +439,7 @@ class CISGraph(object):
         return sp
 
     def _capture_plans(self, key, plans, lane_key=0, warm=True):
-        """One CUDA graph of `plans`.  warm: run them once outside capture first (sets function attributes, lazy allocations) -- never
-        for plans that change state (the optimiser step)."""
-        g = self.graphs.get(key)
-        if g is None:
-            torch.cuda.synchronize()
-            if warm:
-                s = torch.cuda.Stream()
-                s.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(s):
-                    for pl in plans:
-                        pl.run(lane_key=lane_key)
-                torch.cuda.current_stream().wait_stream(s)
-                torch.cuda.synchronize()
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g):
-                for pl in plans:
-                    pl.run(lane_key=lane_key)
-            self.graphs[key] = g
-        return g
+        return capture_plans(self.graphs, key, plans, lane_key, warm)
 
     def _streams(self):
         """(side, copy): the stream of the pipelined flow-network branch and the stream of the host-to-device batch uploads."""
@@ -399,48 +453,22 @@ class CISGraph(object):
         flow_source='input' the second tensor is frame 1's flow [B,384,640,2] and goes to flow_full."""
         self.pipeline_drain()          # a pipelined flow-network branch may still be reading img1 / img2
         self.inputs_for = self.img1
-        st = self._staged
-        if st is not None and st[0] is img1:
-            _, slot, ready = st
-            cur = torch.cuda.current_stream()
-            cur.wait_event(ready)
-            for dst, src in zip(self.inputs, self._slots[slot]):
-                dst.copy_(src, non_blocking=True)
-            # the staging slot may be overwritten by a later prefetch only after these two reads have executed
-            self._slot_read[slot] = torch.cuda.Event()
-            self._slot_read[slot].record(cur)
-            self._staged = None
+        if self._uploads.take(img1, self.inputs):
             return
         self.inputs[0].copy_(img1, non_blocking=True)
         self.inputs[1].copy_(img2, non_blocking=True)
 
-    def _upload(self, after, dst, img1, img2):
-        """Host -> device copy of a frame pair into the device tensors dst = (d1, d2) on the copy stream, once event `after` (if any)
-        has completed -> the event after the copy."""
-        copy = self._streams()[1]
-        if after is not None:
-            copy.wait_event(after)
-        with torch.cuda.stream(copy):
-            dst[0].copy_(img1, non_blocking=True)
-            dst[1].copy_(img2, non_blocking=True)
-            ready = torch.cuda.Event()
-            ready.record(copy)
-        return ready
-
     def prefetch(self, img1, img2):
         """Starts the host -> device copy of an upcoming batch into a staging slot on the copy stream, so that it overlaps the kernels
         queued now; feed(img1, img2) then hands it over on the device."""
-        if self._slots is None:
-            self._slots = [tuple(torch.empty_like(t) for t in self.inputs) for _ in range(2)]
-        self._slot ^= 1
-        # write-after-read: the slot's last hand-over must have executed (the host can run steps ahead of the GPU)
-        self._staged = (img1, self._slot, self._upload(self._slot_read[self._slot], self._slots[self._slot], img1, img2))
+        self._uploads.prefetch((img1, img2))
 
     def feed_next(self, img1, img2):
         """Host -> device copy of the frame pair that the next pipelined train_step runs the flow network on, on the copy stream
         once the flow network has finished reading img1 / img2 -> the event to pass as train_step(inputs_ready=)."""
-        ready = self._upload(self.pipeline_inputs_free(), self.inputs, img1, img2)
-        self.inputs_for, self._staged = img1, None
+        ready = self._uploads.upload(self.pipeline_inputs_free(), self.inputs, (img1, img2))
+        self.inputs_for = img1
+        self._uploads.drop()
         return ready
 
     def prime_pipeline(self):
