@@ -445,6 +445,32 @@ int cis_flow_multiscale_loss_bwd(const CisFlowPyr* pyr, const float* gt, int32_t
 int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, const int64_t* seg, int32_t nseg, float decay, const float* lr,
                 float beta1, float beta2, float eps, int64_t* step_state, cis_stream_t stream);
 
+/* ---- Unsupervised fine-tuning of PWC-Net (occlusion-masked census + second-order smoothness, restated from UnFlow's published
+ * recipe as defined in DESIGN.md: not checked against any other implementation) ----
+ * img1, img2 = fp32 RGB [B, H, W, 3] in [-0.5, 0.5]; flow = fp32 [2B, H, W, 2] in PWC-Net's order and sign, pixels of H x W: direction
+ * n < B is the pair (img1[n], img2[n]), n >= B the swapped pair (img2[n-B], img1[n-B]); S / T = its first / second frame, n' = n -+ B its
+ * partner direction.  Per pixel p = (y, x) of direction n, with F = flow[n]:
+ *   g(I) = 255 (0.2989 R + 0.5870 G + 0.1140 B) of I + 0.5;  q = (y - F0, x - F1);  T~(p) = g(T) sampled at q by dense_image_warp's rule
+ *   (floor clamped to [0, size-2], alpha = clip(q - floor, 0, 1));  V = [0 <= q_y <= H-1 and 0 <= q_x <= W-1];  F^ = flow[n'] sampled at q
+ *   by the same rule;  O = [|F + F^|^2 > 0.01 (|F|^2 + |F^|^2) + 0.5];  M = V (1 - O), which carries no gradient.
+ *   Census over the offsets d != 0 of the 7x7 window with p + d inside the frame: t_X = v / sqrt(0.81 + v^2), v = X(p+d) - X(p), for X =
+ *   g(S) and X = T~;  c = sum_d e^2 / (0.1 + e^2), e = t_S - t_T~;  psi = (c + 0.01)^0.4.
+ *   Smoothness, for each axis a with p +- e_a inside the frame: s_a = sum_c |l_c|, l_c = F_c(p+e_a) - 2 F_c(p) + F_c(p-e_a) (gradient of
+ *   |.|: sign, 0 at 0), where l_c counts as 0 when |l_c| <= 2^-18 (|F_c(p+e_a)| + 2 |F_c(p)| + |F_c(p-e_a)|), the rounding level of fp32
+ *   flows; w_a = exp(-10 * mean over RGB of |S(p+e_a) - S(p-e_a)| / 2).
+ * out = double [2B, 2]: out[n] = {sum_p M psi, sum_p sum_a w_a s_a}; the sums are double, reduced in a fixed order through scratch
+ * (double [2 * 2B * 64], need not be initialised), no atomics: bit-identical run to run.  Per-pixel buffers for the backward, fp32
+ * [2B, H, W]: warped = T~, mask = M, coef = M psi'(c).  Three launches: warp + mask, census + smoothness with block partials, reduction.
+ * flow is read as pairs of floats and must be 8-byte aligned.  CIS_ERR_BAD_ARG unless 1 <= B <= 65535, H, W >= 3 and the alignment holds. */
+int cis_unsup_flow_loss(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, float* warped, float* mask,
+                        float* coef, double* scratch, double* out, cis_stream_t stream);
+/* its backward, one launch: dflow = fp32 [2B, H, W, 2] (overwritten, 8-byte aligned) = w_photo * d(sum_p M psi) / dF + w_smooth *
+ * d(sum_p sum_a w_a s_a) / dF, each direction's own flow only (M and F^ carry no gradient).  The census term is a gather: T~(r) collects
+ * coef * dc / dT~(r) from the <= 49 windows holding r, then dense_image_warp's dflow rule (alpha passes it where 0 <= q - floor <= 1);
+ * the smoothness term is a 5-point gather.  No atomics.  warped / coef: the forward's buffers.  Same argument checks as the forward. */
+int cis_unsup_flow_loss_bwd(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, const float* warped,
+                            const float* coef, float w_photo, float w_smooth, float* dflow, cis_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -128,6 +128,9 @@ _PROTOS = {
     'cis_flow_multiscale_loss': [C.POINTER(CisFlowPyr), _p, _i32, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _f32, _f32, _p, _p],
     'cis_flow_multiscale_loss_bwd': [C.POINTER(CisFlowPyr), _p, _i32, _i32, _i32, _i32, _i32, _f32, _f32, _i32, _f32, _f32],
     'cis_adam_l2': [_p, _p, _p, _p, _i64, _p, _i32, _f32, _p, _f32, _f32, _f32, _p],
+    # PWC-Net fine-tuning without ground truth: census + smoothness loss forward / backward
+    'cis_unsup_flow_loss': [_p, _p, _p, _i32, _i32, _i32, _p, _p, _p, _p, _p],
+    'cis_unsup_flow_loss_bwd': [_p, _p, _p, _i32, _i32, _i32, _p, _p, _f32, _f32, _p],
     # search-range variants: the arguments of the three entry points above plus search_range (1..4)
     'cis_warp_costvol_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32],
     'cis_cost_volume_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _i32],

@@ -64,7 +64,8 @@ def define_validate():
     if 'validate' not in FLAGS:
         gflags.DEFINE_bool('validate', False, 'score the held-out end-point error on the val split at every epoch end and save the '
                                               'best checkpoint (recover-best / pwcnet-best) when it improves; needs --dataset=FLYINGCHAIRS '
-                                              'with its split file')
+                                              'with its split file, or for train_flow.py --flow_loss=unsupervised a mask dataset '
+                                              'with val pairs (scored by the unsupervised objective)')
 
 
 class Config(object):

@@ -1970,6 +1970,245 @@ static int flow_loss_args(const char* what, const CisFlowPyr* pyr, const float* 
   return CIS_OK;
 }
 
+// ------------------------------------------------------------------------------------------------ unsupervised flow loss
+// Occlusion-masked census + edge-aware second-order smoothness (cis_unsup_flow_loss, formulas in cis_b200.h).  Direction n < B runs
+// pair (img1, img2) of sample n, direction n >= B the swapped pair of sample n - B; S / T = first / second frame of the direction.
+// Launches: (1) unsup_warp_mask_kernel, one thread per pixel: T~ and M;  (2) unsup_census_kernel, 64 blocks per direction walking
+// 16x32 tiles whose 22x38 halo (3-pixel apron) of g(S) and T~ sits in shared memory: c, psi, k = M psi'(c), and the smoothness term
+// read from global memory, summed in double, block partials in a fixed order;  (3) unsup_reduce_kernel: the 64 partials per direction
+// in block order.  The backward is one launch of unsup_bwd_kernel over the same tiles (g(S), T~ and k halos).
+constexpr int kUnsupTY = 16, kUnsupTX = 32, kUnsupR = 3, kUnsupHY = kUnsupTY + 2 * kUnsupR, kUnsupHX = kUnsupTX + 2 * kUnsupR;
+constexpr int kUnsupBlocks = 64;
+struct UnsupArgs {
+  const float* flow;
+  const float* img1;
+  const float* img2;
+  int B, H, W;
+};
+__device__ __forceinline__ const float* unsup_frame(const UnsupArgs& a, int n, bool second) {
+  const bool fwd = n < a.B;
+  const float* f = (fwd != second) ? a.img1 : a.img2;
+  return f + (size_t)(fwd ? n : n - a.B) * a.H * a.W * 3;
+}
+// g(I) = 255 (0.2989 R + 0.5870 G + 0.1140 B) of I + 0.5, I = one frame's fp32 RGB.  In double, rounded once: the census divides
+// gray-level differences by sqrt(0.81 + v^2), so their fp32 rounding (not the frames') sets the precision of the loss.
+__device__ __forceinline__ float unsup_gray(const float* f, size_t pix) {
+  const float* p = f + pix * 3;
+  return (float)(255.0 * (0.2989 * ((double)p[0] + 0.5) + 0.5870 * ((double)p[1] + 0.5) + 0.1140 * ((double)p[2] + 0.5)));
+}
+// dense_image_warp's sample of g(T) at q: the four corners, the clamped floor, alpha and r = q - floor (the gradient passes where
+// 0 <= r <= 1).  q = p - F in double: in fp32 its rounding (2^-17 at x = 640) moves the sample by more than the census resolves.
+struct UnsupSample {
+  int y0, x0;
+  float ay, ax, tl, tr, bl, br;
+  bool pass_y, pass_x;
+};
+__device__ __forceinline__ void unsup_coords(double q, int size, int& lo, float& a, bool& pass) {
+  const double fl = fmin(fmax(floor(q), 0.0), (double)(size - 2)), r = q - fl;
+  lo = (int)fl;
+  a = (float)fmin(fmax(r, 0.0), 1.0);
+  pass = r >= 0.0 && r <= 1.0;
+}
+__device__ __forceinline__ UnsupSample unsup_sample(const float* T, int H, int W, double qy, double qx) {
+  UnsupSample s;
+  unsup_coords(qy, H, s.y0, s.ay, s.pass_y);
+  unsup_coords(qx, W, s.x0, s.ax, s.pass_x);
+  const size_t q00 = (size_t)s.y0 * W + s.x0;
+  s.tl = unsup_gray(T, q00);
+  s.tr = unsup_gray(T, q00 + 1);
+  s.bl = unsup_gray(T, q00 + W);
+  s.br = unsup_gray(T, q00 + W + 1);
+  return s;
+}
+// the census transform's soft sign of a difference, t = v / sqrt(0.81 + v^2)
+__device__ __forceinline__ float unsup_t(float v) { return v * rsqrtf(0.81f + v * v); }
+// second-order smoothness of axis (dy, dx) at (y, x), the centre inside [1, size-2] along the axis: weight w and the second differences
+// l_c = F_c(p+e) - 2F_c(p) + F_c(p-e), in double and set to 0 when |l_c| <= 2^-18 (|F_c(p+e)| + 2|F_c(p)| + |F_c(p-e)|): fp32 flows
+// cannot hold an exactly linear run (the final x4 bilinear upsampling makes three pixels in four one), so its second difference is
+// rounding noise, whose sign -- the gradient of |.| -- would be noise too
+__device__ __forceinline__ void unsup_smooth_terms(const UnsupArgs& a, int n, int y, int x, int dy, int dx, float& w, double l[2]) {
+  const float* S = unsup_frame(a, n, false);
+  const size_t pp = (size_t)(y + dy) * a.W + (x + dx), pm = (size_t)(y - dy) * a.W + (x - dx), p0 = (size_t)y * a.W + x;
+  const float e = fabsf(S[pp * 3] - S[pm * 3]) + fabsf(S[pp * 3 + 1] - S[pm * 3 + 1]) + fabsf(S[pp * 3 + 2] - S[pm * 3 + 2]);
+  w = expf(-10.f * (e * (1.f / 3.f)) * 0.5f);
+  const float2* F = reinterpret_cast<const float2*>(a.flow) + (size_t)n * a.H * a.W;
+  const float2 fp = F[pp], f0 = F[p0], fm = F[pm];
+  l[0] = (double)fp.x - 2.0 * (double)f0.x + (double)fm.x;
+  l[1] = (double)fp.y - 2.0 * (double)f0.y + (double)fm.y;
+  if (fabs(l[0]) <= 0x1p-18 * (fabs((double)fp.x) + 2.0 * fabs((double)f0.x) + fabs((double)fm.x))) l[0] = 0.0;
+  if (fabs(l[1]) <= 0x1p-18 * (fabs((double)fp.y) + 2.0 * fabs((double)f0.y) + fabs((double)fm.y))) l[1] = 0.0;
+}
+// (1) per pixel of direction n: T~(p) = g(T) at q = p - F(p), and M(p) = V(p) (1 - O(p)) with the partner direction's flow sampled at q
+__global__ void unsup_warp_mask_kernel(UnsupArgs a, float* __restrict__ warped, float* __restrict__ mask) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t hw = (size_t)a.H * a.W, i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= 2 * (size_t)a.B * hw) return;
+  const int n = (int)(i / hw), p = (int)(i % hw), y = p / a.W, x = p % a.W;
+  const float2 f = reinterpret_cast<const float2*>(a.flow)[i];
+  const double qy = (double)y - f.x, qx = (double)x - f.y;
+  const UnsupSample s = unsup_sample(unsup_frame(a, n, true), a.H, a.W, qy, qx);
+  const float top = s.ax * (s.tr - s.tl) + s.tl, bot = s.ax * (s.br - s.bl) + s.bl;
+  warped[i] = s.ay * (bot - top) + top;
+  const int m = n < a.B ? n + a.B : n - a.B;
+  const float2* G = reinterpret_cast<const float2*>(a.flow) + (size_t)m * hw + (size_t)s.y0 * a.W + s.x0;
+  const float2 g00 = G[0], g01 = G[1], g10 = G[a.W], g11 = G[a.W + 1];
+  const float t0 = s.ax * (g01.x - g00.x) + g00.x, b0 = s.ax * (g11.x - g10.x) + g10.x;
+  const float t1 = s.ax * (g01.y - g00.y) + g00.y, b1 = s.ax * (g11.y - g10.y) + g10.y;
+  const float h0 = s.ay * (b0 - t0) + t0, h1 = s.ay * (b1 - t1) + t1;
+  const float s0 = f.x + h0, s1 = f.y + h1;
+  const bool vis = qy >= 0.0 && qy <= (double)(a.H - 1) && qx >= 0.0 && qx <= (double)(a.W - 1);
+  const bool occ = s0 * s0 + s1 * s1 > 0.01f * (f.x * f.x + f.y * f.y + h0 * h0 + h1 * h1) + 0.5f;
+  mask[i] = (vis && !occ) ? 1.f : 0.f;
+}
+// the halo of tile (ty0, tx0) of direction n: g(S), T~ and, for the backward, k; zero outside the frame (never read there)
+__device__ __forceinline__ void unsup_load_halo(const UnsupArgs& a, int n, int ty0, int tx0, const float* __restrict__ warped,
+                                                const float* __restrict__ coef, float (*gs)[kUnsupHX], float (*tw)[kUnsupHX],
+                                                float (*kk)[kUnsupHX]) {
+  const float* S = unsup_frame(a, n, false);
+  const size_t base = (size_t)n * a.H * a.W;
+  for (int e = threadIdx.x; e < kUnsupHY * kUnsupHX; e += blockDim.x) {
+    const int hy = e / kUnsupHX, hx = e % kUnsupHX, y = ty0 + hy - kUnsupR, x = tx0 + hx - kUnsupR;
+    const bool in = y >= 0 && y < a.H && x >= 0 && x < a.W;
+    const size_t p = in ? (size_t)y * a.W + x : 0;
+    gs[hy][hx] = in ? unsup_gray(S, p) : 0.f;
+    tw[hy][hx] = in ? warped[base + p] : 0.f;
+    if (kk) kk[hy][hx] = in ? coef[base + p] : 0.f;
+  }
+}
+// (2) census + smoothness.  Block x of direction n walks tiles x, x + 64, ...; each thread owns two pixels of a tile.  Partials:
+// part[(n * 64 + x) * 2 + {0, 1}] = {sum M psi, sum w s} of the block's pixels (warp butterfly, then the 8 warps in index order).
+__global__ void __launch_bounds__(256) unsup_census_kernel(UnsupArgs a, const float* __restrict__ warped, const float* __restrict__ mask,
+                                                           float* __restrict__ coef, double* __restrict__ part) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float gs[kUnsupHY][kUnsupHX], tw[kUnsupHY][kUnsupHX];
+  __shared__ double red[8][2];
+  const int n = blockIdx.x / kUnsupBlocks, blk = blockIdx.x % kUnsupBlocks;
+  const int tiles_x = (a.W + kUnsupTX - 1) / kUnsupTX, tiles = tiles_x * ((a.H + kUnsupTY - 1) / kUnsupTY);
+  const size_t base = (size_t)n * a.H * a.W;
+  double photo = 0, smooth = 0;
+  for (int t = blk; t < tiles; t += kUnsupBlocks) {
+    const int ty0 = (t / tiles_x) * kUnsupTY, tx0 = (t % tiles_x) * kUnsupTX;
+    __syncthreads();                                  // the previous tile's reads are done
+    unsup_load_halo(a, n, ty0, tx0, warped, nullptr, gs, tw, nullptr);
+    __syncthreads();
+    for (int e = threadIdx.x; e < kUnsupTY * kUnsupTX; e += blockDim.x) {
+      const int ly = e / kUnsupTX, lx = e % kUnsupTX, y = ty0 + ly, x = tx0 + lx;
+      if (y >= a.H || x >= a.W) continue;
+      const int cy = ly + kUnsupR, cx = lx + kUnsupR;
+      const float s0 = gs[cy][cx], w0 = tw[cy][cx];
+      float c = 0.f;
+      for (int dy = -kUnsupR; dy <= kUnsupR; ++dy) {
+        if (y + dy < 0 || y + dy >= a.H) continue;
+#pragma unroll
+        for (int dx = -kUnsupR; dx <= kUnsupR; ++dx) {
+          if ((dy == 0 && dx == 0) || x + dx < 0 || x + dx >= a.W) continue;
+          const float d = unsup_t(gs[cy + dy][cx + dx] - s0) - unsup_t(tw[cy + dy][cx + dx] - w0);
+          c += d * d / (0.1f + d * d);
+        }
+      }
+      const size_t p = base + (size_t)y * a.W + x;
+      const float m = mask[p];
+      photo += (double)(m * powf(c + 0.01f, 0.4f));
+      coef[p] = m * 0.4f * powf(c + 0.01f, -0.6f);
+      for (int ax = 0; ax < 2; ++ax) {
+        const int dy = ax == 0, dx = ax == 1;
+        if ((ax == 0 && (y < 1 || y > a.H - 2)) || (ax == 1 && (x < 1 || x > a.W - 2))) continue;
+        float w;
+        double l[2];
+        unsup_smooth_terms(a, n, y, x, dy, dx, w, l);
+        smooth += (double)w * (fabs(l[0]) + fabs(l[1]));
+      }
+    }
+  }
+  photo = warp_sum_d(photo);
+  smooth = warp_sum_d(smooth);
+  if ((threadIdx.x & 31) == 0) {
+    red[threadIdx.x >> 5][0] = photo;
+    red[threadIdx.x >> 5][1] = smooth;
+  }
+  __syncthreads();
+  if (threadIdx.x < 2) {
+    double s = 0;
+    for (int k = 0; k < (int)(blockDim.x >> 5); ++k) s += red[k][threadIdx.x];
+    part[((size_t)n * kUnsupBlocks + blk) * 2 + threadIdx.x] = s;
+  }
+}
+// (3) one block per direction, thread i adds component i of the 64 partials in block order
+__global__ void unsup_reduce_kernel(const double* __restrict__ part, double* __restrict__ out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int n = blockIdx.x, i = threadIdx.x;
+  double s = 0;
+  for (int k = 0; k < kUnsupBlocks; ++k) s += part[((size_t)n * kUnsupBlocks + k) * 2 + i];
+  out[n * 2 + i] = s;
+}
+// backward, one thread per pixel r of a 16x32 tile (grid: tiles x 2B).  Census: dT~(r) = -sum_delta (k(r+delta) + k(r)) h(r, r+delta),
+// h = d/du of (dt^2 / (0.1 + dt^2)), dt = t_S - t(u), u = T~(r+delta) - T~(r) (each window's term is odd in the pair's order, so the
+// gather over the windows holding r folds into one sweep of r's own window), chained through dense_image_warp's dflow rule.
+// Smoothness: the 5-point gather of w_a sign(second difference) from the centres r - e_a, r, r + e_a.
+__global__ void __launch_bounds__(256) unsup_bwd_kernel(UnsupArgs a, const float* __restrict__ warped, const float* __restrict__ coef,
+                                                        float w_photo, float w_smooth, float* __restrict__ dflow) {
+  pdl_launch_dependents();
+  pdl_wait();
+  __shared__ float gs[kUnsupHY][kUnsupHX], tw[kUnsupHY][kUnsupHX], kk[kUnsupHY][kUnsupHX];
+  const int tiles_x = (a.W + kUnsupTX - 1) / kUnsupTX, tiles = tiles_x * ((a.H + kUnsupTY - 1) / kUnsupTY);
+  const int n = blockIdx.x / tiles, t = blockIdx.x % tiles;
+  const int ty0 = (t / tiles_x) * kUnsupTY, tx0 = (t % tiles_x) * kUnsupTX;
+  unsup_load_halo(a, n, ty0, tx0, warped, coef, gs, tw, kk);
+  __syncthreads();
+  const size_t base = (size_t)n * a.H * a.W;
+  for (int e = threadIdx.x; e < kUnsupTY * kUnsupTX; e += blockDim.x) {
+    const int ly = e / kUnsupTX, lx = e % kUnsupTX, y = ty0 + ly, x = tx0 + lx;
+    if (y >= a.H || x >= a.W) continue;
+    const int cy = ly + kUnsupR, cx = lx + kUnsupR;
+    const float s0 = gs[cy][cx], w0 = tw[cy][cx], k0 = kk[cy][cx];
+    float g = 0.f;
+    for (int dy = -kUnsupR; dy <= kUnsupR; ++dy) {
+      if (y + dy < 0 || y + dy >= a.H) continue;
+#pragma unroll
+      for (int dx = -kUnsupR; dx <= kUnsupR; ++dx) {
+        if ((dy == 0 && dx == 0) || x + dx < 0 || x + dx >= a.W) continue;
+        const float u = tw[cy + dy][cx + dx] - w0, iu = rsqrtf(0.81f + u * u);
+        const float d = unsup_t(gs[cy + dy][cx + dx] - s0) - u * iu, den = 0.1f + d * d;
+        g += (kk[cy + dy][cx + dx] + k0) * (-0.2f * d / (den * den)) * (0.81f * iu * iu * iu);
+      }
+    }
+    const float dtw = -g * w_photo;
+    const size_t pix = base + (size_t)y * a.W + x;
+    const float2 f = reinterpret_cast<const float2*>(a.flow)[pix];
+    const UnsupSample s = unsup_sample(unsup_frame(a, n, true), a.H, a.W, (double)y - f.x, (double)x - f.y);
+    const float top = s.ax * (s.tr - s.tl) + s.tl, bot = s.ax * (s.br - s.bl) + s.bl;
+    float d0 = s.pass_y ? -dtw * (bot - top) : 0.f;
+    float d1 = s.pass_x ? -dtw * (s.ay * (s.br - s.bl) + (1.f - s.ay) * (s.tr - s.tl)) : 0.f;
+    float sm0 = 0.f, sm1 = 0.f;
+    for (int ax = 0; ax < 2; ++ax) {
+      const int dy = ax == 0, dx = ax == 1, pos = ax == 0 ? y : x, size = ax == 0 ? a.H : a.W;
+      for (int o = -1; o <= 1; ++o) {                // centre r + o e_a: coefficient -2 at o = 0, 1 at o = +-1
+        const int c = pos + o;
+        if (c < 1 || c > size - 2) continue;
+        float w;
+        double l[2];
+        unsup_smooth_terms(a, n, y + o * dy, x + o * dx, dy, dx, w, l);
+        const float cw = (o == 0 ? -2.f : 1.f) * w;
+        sm0 += cw * (float)((l[0] > 0) - (l[0] < 0));
+        sm1 += cw * (float)((l[1] > 0) - (l[1] < 0));
+      }
+    }
+    d0 += w_smooth * sm0;
+    d1 += w_smooth * sm1;
+    reinterpret_cast<float2*>(dflow)[pix] = make_float2(d0, d1);
+  }
+}
+static int unsup_args(const char* what, const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W,
+                      UnsupArgs& a) {
+  // the flow is read as float2: 8-byte aligned pairs
+  if (!flow || !img1 || !img2 || B < 1 || B > 65535 || H < 3 || W < 3 || ((uintptr_t)flow & 7)) return cis_set_error(CIS_ERR_BAD_ARG, what);
+  a = UnsupArgs{flow, img1, img2, B, H, W};
+  return CIS_OK;
+}
+
 extern "C" {
 
 int cis_pack_weights(const float* w, const int32_t* kmap, int32_t K_pad, int32_t rows, int32_t cout, int32_t sn, const int32_t* nmap, void* wp,
@@ -2389,6 +2628,28 @@ int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, 
              (const long long*)step_state);
   CIS_LAUNCH(step_inc_kernel, 1, 1, 0, ST, (long long*)step_state);
   return cis_check_launch("adam_l2");
+}
+int cis_unsup_flow_loss(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, float* warped, float* mask,
+                        float* coef, double* scratch, double* out, cis_stream_t stream) {
+  UnsupArgs a;
+  const int rc = unsup_args("cis_unsup_flow_loss: bad frames, flow alignment or size (B 1..65535, H, W >= 3)", flow, img1, img2, B, H, W, a);
+  if (rc) return rc;
+  if (!warped || !mask || !coef || !scratch || !out) return cis_set_error(CIS_ERR_BAD_ARG, "cis_unsup_flow_loss: no buffer, scratch or output");
+  CIS_LAUNCH(unsup_warp_mask_kernel, nblk((size_t)2 * B * H * W), 256, 0, ST, a, warped, mask);
+  CIS_LAUNCH(unsup_census_kernel, 2 * B * kUnsupBlocks, 256, 0, ST, a, (const float*)warped, (const float*)mask, coef, scratch);
+  CIS_LAUNCH(unsup_reduce_kernel, 2 * B, 2, 0, ST, (const double*)scratch, out);
+  return cis_check_launch("unsup_flow_loss");
+}
+int cis_unsup_flow_loss_bwd(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, const float* warped,
+                            const float* coef, float w_photo, float w_smooth, float* dflow, cis_stream_t stream) {
+  UnsupArgs a;
+  const int rc = unsup_args("cis_unsup_flow_loss_bwd: bad frames, flow alignment or size (B 1..65535, H, W >= 3)", flow, img1, img2, B, H, W, a);
+  if (rc) return rc;
+  const size_t blocks = (size_t)((H + kUnsupTY - 1) / kUnsupTY) * ((W + kUnsupTX - 1) / kUnsupTX) * 2 * B;
+  if (!warped || !coef || !dflow || ((uintptr_t)dflow & 7) || blocks > 0x7fffffff)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_unsup_flow_loss_bwd: bad buffer, dflow alignment or grid size");
+  CIS_LAUNCH(unsup_bwd_kernel, (unsigned)blocks, 256, 0, ST, a, warped, coef, w_photo, w_smooth, dflow);
+  return cis_check_launch("unsup_flow_loss_bwd");
 }
 
 }  // extern "C"
