@@ -471,6 +471,51 @@ int cis_unsup_flow_loss(const float* flow, const float* img1, const float* img2,
 int cis_unsup_flow_loss_bwd(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, const float* warped,
                             const float* coef, float w_photo, float w_smooth, float* dflow, cis_stream_t stream);
 
+/* ---- Geometric + photometric augmentation of supervised PWC-Net training pairs (restated from the FlowNet / PWC-Net papers'
+ * description, as defined in DESIGN.md; the ranges are chosen here and not checked against any other implementation) ----
+ * Pixel centres are at integer (x, y) of the H x W grid, c = ((W-1)/2, (H-1)/2), R(th) = [[cos th, -sin th], [sin th, cos th]] on (x, y).
+ * Frame 1 and the ground truth sample their source at T1(p) = c + t + R(th)(p - c)/s; frame 2 at T2 = T1 o Tr, Tr(p) = c + t_r +
+ * R(th_r)(p - c)/s_r.  Every range below is [lo, hi], drawn uniformly; angles in degrees; translations as fractions of (W, H). */
+typedef struct {
+  float scale[2];          /* s                      default [0.9, 2.0] */
+  float rotate[2];         /* th                     default [-17, 17] */
+  float translate[2];      /* t = (u W, u' H)        default [-0.2, 0.2] */
+  float rel_scale[2];      /* s_r                    default [0.95, 1.05] */
+  float rel_rotate[2];     /* th_r                   default [-3, 3] */
+  float rel_translate[2];  /* t_r = (u W, u' H)      default [-0.03, 0.03] */
+  float color[2];          /* m_c, log-uniform       default [0.5, 2] */
+  float contrast[2];       /* kappa                  default [-0.8, 0.4] */
+  float brightness;        /* std of beta ~ N(0, .)  default 0.2 */
+  float gamma[2];          /* gamma                  default [0.7, 1.5] */
+  float noise[2];          /* sigma                  default [0, 0.04] */
+} CisFlowAug;
+#define CIS_FLOW_AUG_ROW 32
+/* Per-sample parameters: params = fp32 [B, CIS_FLOW_AUG_ROW], row b for the global sample g = sample_offset + b at step t = step[0]
+ * (device int64, read when the kernel runs: the Adam step counter, so CUDA-graph replays draw new parameters; data-parallel ranks with
+ * sample_offset = rank * local batch draw what one GPU running the global batch draws).  Draw k is r_k = hash32(seed ^ D ^ t<<40 ^ g<<10 ^
+ * k), D = 0x466c6f774175676d, hash32 = the 64-bit MurmurHash3 finaliser truncated to 32 bits (cis_box_masks'), U_k = (r_k + 0.5) / 2^32.
+ * Geometry attempt a = 0..63 draws k = 8a + j: j = 0 s, 1 th, 2 t_x, 3 t_y, 4 s_r, 5 th_r, 6 t_r.x, 7 t_r.y (lo + (hi - lo) U_k, in
+ * double).  It is accepted when the four corners (0,0), (W-1,0), (0,H-1), (W-1,H-1) map under T1 and under T2 into [0, W-1] x [0, H-1]
+ * (tested in double); the first accepted attempt is used, and after 64 rejections the identity.  Photometric draws k = 512 + j: j = 0..2
+ * m_c = exp(ln lo + (ln hi - ln lo) U_k), 3 kappa, 4 and 5 beta = brightness sqrt(-2 ln U_516) cos(2 pi U_517), 6 gamma, 7 sigma, 8 the
+ * noise key r_520.  Row layout (each affine map as (r0, r1, r2, r3, r4, r5): q = (r0 x + r1 y + r2, r3 x + r4 y + r5), formed in double
+ * and rounded): [0, 6) T1, [6, 12) T2, [12, 18) T2^-1, [18, 21) m_c, 21 1 + kappa, 22 beta, 23 gamma, 24 sigma, 25 the noise key (uint32
+ * bits), 26 the accepted attempt (64 = identity), [27, 32) 0.  One thread per sample, no atomics.  CIS_ERR_BAD_ARG unless 1 <= B <= 65535,
+ * H, W >= 2, sample_offset >= 0, the buffers are non-null and every range has lo <= hi with scale, rel_scale and color lo > 0. */
+int cis_flow_aug_params(const CisFlowAug* ranges, int32_t B, int32_t H, int32_t W, int64_t sample_offset, const long long* step,
+                        uint64_t seed, float* params, cis_stream_t stream);
+/* The augmented pair and flow, one pass, one thread per output pixel p of each sample: img1, img2 = fp32 RGB [B, H, W, 3] in [-0.5, 0.5],
+ * gt = fp32 [B, H, W, 2] in PWC-Net's order (ch0 = -v, ch1 = -u).  Samples use dense_image_warp's bilinear rule (floor clamped to
+ * [0, size-2], fraction clamped to [0, 1]).  img1_out(p) = phot(img1 at T1(p)), img2_out(p) = phot(img2 at T2(p)); flow: q = T1(p), (u, v)
+ * = gt at q (converted from PWC-Net's order), p2 = T2^-1(q + (u, v)), gt_out(p) = p2 - p in PWC-Net's order.  phot, on v = sample + 0.5
+ * per channel c: v *= m_c; v = 0.5 + (1 + kappa)(v - 0.5); v += beta; v = clamp(v, 0, 1)^gamma; v = clamp(v + sigma n, 0, 1); out = v -
+ * 0.5, n = sqrt(-2 ln U1) cos(2 pi U2), U1 = (hash32(N ^ key<<32 ^ 2i) + 0.5) / 2^32, U2 the same with 2i + 1, N = 0x4175674e6f697365,
+ * i = ((f H + y) W + x) 3 + c, f = 0 for frame 1 and 1 for frame 2 (sigma = 0 skips n).  gt and gt_out are read / written as float pairs and must be 8-byte
+ * aligned; the outputs must not alias the inputs.  CIS_ERR_BAD_ARG unless 1 <= B <= 65535, H, W >= 2, 6 H W < 2^31, the buffers are
+ * non-null and the alignment holds. */
+int cis_flow_augment(const float* img1, const float* img2, const float* gt, const float* params, int32_t B, int32_t H, int32_t W,
+                     float* img1_out, float* img2_out, float* gt_out, cis_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -9,7 +9,10 @@ frame-pairs/s, and the peak device memory of each network's step.
 --flow_loss unsupervised times the 'lg' network's unsupervised step (census + smoothness, the network on both directions of each pair)
 against its multi-scale step instead, alternated the same way, and then, in a separate torch.profiler run, the kernels of
 cis_unsup_flow_loss and cis_unsup_flow_loss_bwd against their HBM byte roofline (bytes per pixel from the shapes, unsup_bytes below).
-Usage: python tools/time_flow_train.py [--flow_loss multiscale|unsupervised] [--rounds 5] [--steps 20] [--warmup 5]"""
+
+--flow_aug times the 'lg' network's multi-scale step with and without the augmentation of its batch (FlowTrainGraph(augment=True)),
+alternated the same way, and then, in a separate torch.profiler run, cis_flow_augment's kernel against its HBM byte roofline (AUG_BYTES).
+Usage: python tools/time_flow_train.py [--flow_loss multiscale|unsupervised] [--flow_aug] [--rounds 5] [--steps 20] [--warmup 5]"""
 import argparse
 import json
 import os
@@ -25,6 +28,9 @@ from unsupervised_detection_b200.flow_train_graph import FlowTrainGraph  # noqa:
 B, H, W = 8, 384, 640
 NETS = {'lg': None, 'sm': {'use_dense_cx': False}}
 HBM_TBS = 3.35                                       # H100 SXM data-sheet HBM3 bandwidth
+# HBM bytes per output pixel of one sample that cis_flow_augment must move, each element read or written once (the bilinear corners come
+# from cache): fp32 img1, img2 [3] and gt [2] read, the same written
+AUG_BYTES = 4 * (3 + 3 + 2) * 2
 
 
 def unsup_bytes():
@@ -36,11 +42,11 @@ def unsup_bytes():
 
 
 class Case(object):
-    def __init__(self, name, options, seed=0, loss='multiscale'):
+    def __init__(self, name, options, seed=0, loss='multiscale', augment=False):
         self.name = name
         base = torch.cuda.memory_allocated()               # the networks built before this one
         torch.cuda.reset_peak_memory_stats()
-        self.graph = g = FlowTrainGraph(H, W, B, options=options, loss=loss)
+        self.graph = g = FlowTrainGraph(H, W, B, options=options, loss=loss, augment=augment)
         g.load_params(params_init.init_pwcnet(g.store.entries))
         gen = torch.Generator().manual_seed(seed)
         a = torch.rand(B, H, W, 3, generator=gen) - 0.5
@@ -58,8 +64,9 @@ class Case(object):
         return dict(step_ms=ms, pairs_per_s=B / (ms / 1e3))
 
 
-def profile_unsup(case, steps=5):
-    """Mean device time of each unsupervised-loss kernel over `steps` eager steps under torch.profiler, against its byte roofline."""
+def profile_kernels(case, per, npix, steps=5):
+    """{kernel name: [device times, us]} of the kernels named in `per` over `steps` eager steps under torch.profiler; printed against
+    their byte roofline (per[k] bytes per pixel, npix pixels)."""
     from torch.profiler import ProfilerActivity, profile
     g = case.graph
     for _ in range(2):
@@ -69,14 +76,11 @@ def profile_unsup(case, steps=5):
         for _ in range(steps):
             g.train_step()
         torch.cuda.synchronize()
-    per = unsup_bytes()
     times = {}
     for e in prof.events():
         for k in per:
             if k in e.name:
                 times.setdefault(k, []).append(e.device_time_total if hasattr(e, 'device_time_total') else e.cuda_time_total)
-    npix = 2 * B * H * W
-    print('unsupervised loss kernels (%d directions x %dx%d, mean of %d launches each, torch.profiler):' % (2 * B, H, W, steps))
     for k, b in per.items():
         t = times.get(k)
         if not t:
@@ -89,9 +93,20 @@ def profile_unsup(case, steps=5):
                               share_of_bw_roofline=round(floor / us, 3))))
 
 
+def profile_unsup(case, steps=5):
+    print('unsupervised loss kernels (%d directions x %dx%d, mean of %d launches each, torch.profiler):' % (2 * B, H, W, steps))
+    profile_kernels(case, unsup_bytes(), 2 * B * H * W, steps)
+
+
+def profile_aug(case, steps=5):
+    print('augmentation kernel (%d samples x %dx%d, mean of %d launches, torch.profiler):' % (B, H, W, steps))
+    profile_kernels(case, {'flow_augment_kernel': AUG_BYTES}, B * H * W, steps)
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
     ap.add_argument('--flow_loss', default='multiscale', choices=['multiscale', 'unsupervised'])
+    ap.add_argument('--flow_aug', action='store_true', help='time the multi-scale step with and without augmentation')
     ap.add_argument('--rounds', type=int, default=5)
     ap.add_argument('--steps', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=5)
@@ -99,7 +114,9 @@ def main():
     torch.cuda.set_device(0)
     print('card: %s' % card())
     print('PWC-Net training step %dx%d batch %d, CUDA graphs; %d rounds x %d steps (warm-up %d)' % (H, W, B, args.rounds, args.steps, args.warmup))
-    if args.flow_loss == 'unsupervised':
+    if args.flow_aug:
+        cases = [Case('lg-multiscale', None), Case('lg-multiscale-aug', None, augment=True)]
+    elif args.flow_loss == 'unsupervised':
         cases = [Case('lg-multiscale', None), Case('lg-unsup', None, loss='unsupervised')]
     else:
         cases = [Case(n, o) for n, o in NETS.items()]
@@ -118,7 +135,9 @@ def main():
     for n in rows:
         s = {k: med([m[k] for m in rows[n]]) for k in rows[n][0]}
         print('  %-3s %7.2f ms/step  %6.1f frame-pairs/s' % (n, s['step_ms'], s['pairs_per_s']))
-    if args.flow_loss == 'unsupervised':
+    if args.flow_aug:
+        profile_aug(cases[1])
+    elif args.flow_loss == 'unsupervised':
         profile_unsup(cases[1])
 
 

@@ -3,7 +3,8 @@ frame pairs of a video dataset with the unsupervised census + smoothness loss, b
 unsupervised_detection_b200/flow_train_graph.py.  Same flags, seed and flag dump as pretrain_recover.py, plus --flow_loss
 (multiscale | robust | unsupervised), --smooth_weight (lambda_s of the unsupervised loss), --learning_rate, --lr_boundaries (steps after
 which the rate halves), --weight_decay (L2 on the conv kernels) and --validate (every epoch: the end-point error on Flying Chairs' val split,
-or the mean unsupervised objective over a video dataset's val pairs; pwcnet-best on improvement).  --flow_ckpt, when given, is the starting
+or the mean unsupervised objective over a video dataset's val pairs; pwcnet-best on improvement) and --flow_aug (random affine and
+photometric augmentation of every supervised training batch on the device, the ground-truth flow transformed to match).  --flow_ckpt, when given, is the starting
 point (fine-tuning); otherwise training starts from params_init.init_pwcnet.  The network input is img_height x img_width (multiples of
 64, at least 128).
 
@@ -23,7 +24,7 @@ from train import seed_everything
 from unsupervised_detection_b200 import flow_flags
 from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES, define_validate
 
-TRAIN_FLOW_FLAGS = ['flow_loss', 'smooth_weight', 'learning_rate', 'lr_boundaries', 'weight_decay', 'validate']
+TRAIN_FLOW_FLAGS = ['flow_loss', 'smooth_weight', 'learning_rate', 'lr_boundaries', 'weight_decay', 'validate', 'flow_aug']
 UNSUP_DATASETS = ('FLYINGCHAIRS', 'DAVIS2016', 'FBMS', 'SEGTRACK')
 if 'flow_loss' not in FLAGS:
     absl_flags.DEFINE_enum('flow_loss', 'multiscale', ['multiscale', 'robust', 'unsupervised'], "flow loss: 'multiscale' = ||d||_2 to "
@@ -33,6 +34,9 @@ if 'flow_loss' not in FLAGS:
     absl_flags.DEFINE_float('learning_rate', 1e-4, 'Adam learning rate of the first step')
     absl_flags.DEFINE_list('lr_boundaries', [], 'steps after which the learning rate halves (comma-separated, increasing)')
     absl_flags.DEFINE_float('weight_decay', 4e-4, 'L2 weight decay gamma of the conv kernels (loss term gamma/2 ||w||^2; biases are not decayed)')
+    absl_flags.DEFINE_bool('flow_aug', False, 'augment every training pair on the GPU: random translation, rotation and zoom of the pair, a '
+                           'small extra transform of the second frame, colour / contrast / brightness / gamma / noise, with the ground-truth '
+                           'flow transformed to match (multiscale / robust losses; validation is not augmented)')
 define_validate()
 
 
@@ -56,6 +60,8 @@ def check_flags(config):
                                                % (' / '.join(UNSUP_DATASETS), config.dataset))
     if not unsup and config.dataset != 'FLYINGCHAIRS':
         raise absl_flags.IllegalFlagValueError('train_flow.py trains on Flying Chairs: --dataset=FLYINGCHAIRS, not %s' % config.dataset)
+    if unsup and config.flow_aug:
+        raise absl_flags.IllegalFlagValueError('--flow_aug is for the supervised losses: --flow_loss=unsupervised scores the frames themselves')
     if unsup and config.flow_dir:
         raise absl_flags.IllegalFlagValueError('--flow_dir replaces PWC-Net, which --flow_loss=unsupervised trains: drop one of them')
     if not config.smooth_weight >= 0:

@@ -66,6 +66,15 @@ class CisFlowPyr(C.Structure):
                 ('accumulate', C.c_int32 * 5), ('weight', C.c_float * 5)]
 
 
+class CisFlowAug(C.Structure):
+    _fields_ = [('scale', C.c_float * 2), ('rotate', C.c_float * 2), ('translate', C.c_float * 2), ('rel_scale', C.c_float * 2),
+                ('rel_rotate', C.c_float * 2), ('rel_translate', C.c_float * 2), ('color', C.c_float * 2), ('contrast', C.c_float * 2),
+                ('brightness', C.c_float), ('gamma', C.c_float * 2), ('noise', C.c_float * 2)]
+
+
+FLOW_AUG_ROW = 32                                   # CIS_FLOW_AUG_ROW: floats per sample of cis_flow_aug_params' table
+
+
 _i32, _i64, _f32, _p, _u64 = C.c_int32, C.c_int64, C.c_float, C.c_void_p, C.c_uint64
 
 # name -> argtypes (the trailing stream argument is appended automatically)
@@ -131,6 +140,9 @@ _PROTOS = {
     # PWC-Net fine-tuning without ground truth: census + smoothness loss forward / backward
     'cis_unsup_flow_loss': [_p, _p, _p, _i32, _i32, _i32, _p, _p, _p, _p, _p],
     'cis_unsup_flow_loss_bwd': [_p, _p, _p, _i32, _i32, _i32, _p, _p, _f32, _f32, _p],
+    # augmentation of the supervised training pairs: per-sample parameter draws, the augmented frames and flow
+    'cis_flow_aug_params': [C.POINTER(CisFlowAug), _i32, _i32, _i32, _i64, _p, _u64, _p],
+    'cis_flow_augment': [_p, _p, _p, _p, _i32, _i32, _i32, _p, _p, _p],
     # search-range variants: the arguments of the three entry points above plus search_range (1..4)
     'cis_warp_costvol_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _i32],
     'cis_cost_volume_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _i32, _i32, _p, _p, _p, _i32],

@@ -1399,6 +1399,146 @@ __global__ void box_masks_kernel(float* __restrict__ mask, int H, int W, int lo_
   const uint32_t y = (uint32_t)(i / W), x = (uint32_t)(i - (size_t)y * W);
   mask[blockIdx.y * hw + i] = (y - y0 < bh && x - x0 < bw) ? 1.f : 0.f;   // unsigned: y < y0 wraps around and fails the test
 }
+// Augmentation of the supervised PWC-Net training pairs (cis_flow_aug_params / cis_flow_augment in include/cis_b200.h state the draws,
+// the row layout and the rules).  The draws and the affine maps are formed in double so that the host restatement reproduces the
+// accept / reject choices exactly; the per-pixel pass is fp32.
+constexpr uint64_t kAugDomain = 0x466c6f774175676dULL;     // "FlowAugm"
+constexpr uint64_t kAugNoiseDomain = 0x4175674e6f697365ULL; // "AugNoise"
+__device__ __forceinline__ double aug_u(unsigned long long seed, long long t, long long g, int k) {
+  return ((double)hash32((uint64_t)seed ^ kAugDomain ^ ((uint64_t)t << 40) ^ ((uint64_t)g << 10) ^ (uint64_t)k) + 0.5) * 0x1p-32;
+}
+__device__ __forceinline__ double aug_range(const float* r, double u) { return (double)r[0] + ((double)r[1] - (double)r[0]) * u; }
+// the affine map c + t + R(th)(p - c)/s as (r0..r5)
+__device__ __forceinline__ void aug_affine(double s, double deg, double tx, double ty, double cx, double cy, double* m) {
+  double sn, cs;
+  sincos(deg * (3.14159265358979323846 / 180.0), &sn, &cs);
+  m[0] = cs / s; m[1] = -sn / s; m[3] = sn / s; m[4] = cs / s;
+  m[2] = cx + tx - (m[0] * cx + m[1] * cy);
+  m[5] = cy + ty - (m[3] * cx + m[4] * cy);
+}
+__device__ __forceinline__ bool aug_corners_inside(const double* m, double w1, double h1) {
+  bool ok = true;
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const double x = (k & 1) ? w1 : 0.0, y = (k & 2) ? h1 : 0.0;
+    const double qx = m[0] * x + m[1] * y + m[2], qy = m[3] * x + m[4] * y + m[5];
+    ok = ok && qx >= 0.0 && qx <= w1 && qy >= 0.0 && qy <= h1;
+  }
+  return ok;
+}
+__global__ void flow_aug_params_kernel(const CisFlowAug a, int B, int H, int W, long long sample_offset, const long long* __restrict__ step,
+                                       unsigned long long seed, float* __restrict__ params) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  const long long t = step[0], g = sample_offset + b;
+  const double w1 = W - 1, h1 = H - 1, cx = 0.5 * w1, cy = 0.5 * h1;
+  double t1[6] = {1, 0, 0, 0, 1, 0}, t2[6] = {1, 0, 0, 0, 1, 0};
+  int att = 64;
+  for (int k = 0; k < 64; ++k) {
+    double m1[6], mr[6], m2[6];
+    aug_affine(aug_range(a.scale, aug_u(seed, t, g, 8 * k)), aug_range(a.rotate, aug_u(seed, t, g, 8 * k + 1)),
+               aug_range(a.translate, aug_u(seed, t, g, 8 * k + 2)) * W, aug_range(a.translate, aug_u(seed, t, g, 8 * k + 3)) * H, cx, cy, m1);
+    aug_affine(aug_range(a.rel_scale, aug_u(seed, t, g, 8 * k + 4)), aug_range(a.rel_rotate, aug_u(seed, t, g, 8 * k + 5)),
+               aug_range(a.rel_translate, aug_u(seed, t, g, 8 * k + 6)) * W, aug_range(a.rel_translate, aug_u(seed, t, g, 8 * k + 7)) * H,
+               cx, cy, mr);
+    m2[0] = m1[0] * mr[0] + m1[1] * mr[3]; m2[1] = m1[0] * mr[1] + m1[1] * mr[4]; m2[2] = m1[0] * mr[2] + m1[1] * mr[5] + m1[2];
+    m2[3] = m1[3] * mr[0] + m1[4] * mr[3]; m2[4] = m1[3] * mr[1] + m1[4] * mr[4]; m2[5] = m1[3] * mr[2] + m1[4] * mr[5] + m1[5];
+    if (aug_corners_inside(m1, w1, h1) && aug_corners_inside(m2, w1, h1)) {
+#pragma unroll
+      for (int j = 0; j < 6; ++j) { t1[j] = m1[j]; t2[j] = m2[j]; }
+      att = k;
+      break;
+    }
+  }
+  const double det = t2[0] * t2[4] - t2[1] * t2[3];
+  const double i0 = t2[4] / det, i1 = -t2[1] / det, i3 = -t2[3] / det, i4 = t2[0] / det;
+  float* row = params + (size_t)b * CIS_FLOW_AUG_ROW;
+#pragma unroll
+  for (int j = 0; j < 6; ++j) { row[j] = (float)t1[j]; row[6 + j] = (float)t2[j]; }
+  row[12] = (float)i0; row[13] = (float)i1; row[14] = (float)(-(i0 * t2[2] + i1 * t2[5]));
+  row[15] = (float)i3; row[16] = (float)i4; row[17] = (float)(-(i3 * t2[2] + i4 * t2[5]));
+  const double lc0 = log((double)a.color[0]), lc1 = log((double)a.color[1]);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) row[18 + c] = (float)exp(lc0 + (lc1 - lc0) * aug_u(seed, t, g, 512 + c));
+  row[21] = (float)(1.0 + aug_range(a.contrast, aug_u(seed, t, g, 515)));
+  row[22] = (float)((double)a.brightness * sqrt(-2.0 * log(aug_u(seed, t, g, 516))) * cospi(2.0 * aug_u(seed, t, g, 517)));
+  row[23] = (float)aug_range(a.gamma, aug_u(seed, t, g, 518));
+  row[24] = (float)aug_range(a.noise, aug_u(seed, t, g, 519));
+  row[25] = __uint_as_float(hash32((uint64_t)seed ^ kAugDomain ^ ((uint64_t)t << 40) ^ ((uint64_t)g << 10) ^ 520ull));
+  row[26] = (float)att;
+#pragma unroll
+  for (int j = 27; j < CIS_FLOW_AUG_ROW; ++j) row[j] = 0.f;
+}
+// dense_image_warp's bilinear rule on one fp32 pixel-interleaved plane: floor clamped to [0, size-2], fraction clamped to [0, 1]
+__device__ __forceinline__ void aug_tap(float qx, float qy, int H, int W, int& i00, float& ax, float& ay) {
+  int x0, y0;
+  warp_coords(qx, W, x0, ax);
+  warp_coords(qy, H, y0, ay);
+  i00 = y0 * W + x0;
+}
+__device__ __forceinline__ float aug_lerp(float tl, float tr, float bl, float br, float ax, float ay) {
+  const float t = ax * (tr - tl) + tl, b = ax * (br - bl) + bl;
+  return ay * (b - t) + t;
+}
+__device__ __forceinline__ float aug_noise(uint32_t key, uint32_t i) {
+  const uint64_t base = kAugNoiseDomain ^ ((uint64_t)key << 32) ^ ((uint64_t)i << 1);
+  const float u1 = ((float)hash32(base) + 0.5f) * 0x1p-32f, u2 = ((float)hash32(base ^ 1ull) + 0.5f) * 0x1p-32f;
+  return sqrtf(-2.f * logf(u1)) * cospif(2.f * u2);
+}
+// one frame's sample at q through the photometric chain -> out[0..2]
+__device__ __forceinline__ void aug_frame(const float* __restrict__ img, float qx, float qy, int H, int W, const float* __restrict__ row,
+                                          uint32_t nbase, float* __restrict__ out) {
+  int i00;
+  float ax, ay;
+  aug_tap(qx, qy, H, W, i00, ax, ay);
+  const float* p = img + (size_t)i00 * 3;
+  const float ck = __ldg(row + 21), beta = __ldg(row + 22), gam = __ldg(row + 23), sig = __ldg(row + 24);
+  const uint32_t key = __float_as_uint(__ldg(row + 25));
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    float v = aug_lerp(__ldg(p + c), __ldg(p + 3 + c), __ldg(p + (size_t)W * 3 + c), __ldg(p + (size_t)W * 3 + 3 + c), ax, ay) + 0.5f;
+    v *= __ldg(row + 18 + c);
+    v = 0.5f + ck * (v - 0.5f);
+    v += beta;
+    v = powf(fminf(fmaxf(v, 0.f), 1.f), gam);
+    if (sig != 0.f) v += sig * aug_noise(key, nbase + (uint32_t)c);
+    out[c] = fminf(fmaxf(v, 0.f), 1.f) - 0.5f;
+  }
+}
+__global__ void flow_augment_kernel(const float* __restrict__ img1, const float* __restrict__ img2, const float* __restrict__ gt,
+                                    const float* __restrict__ params, int H, int W, float* __restrict__ img1_out, float* __restrict__ img2_out,
+                                    float* __restrict__ gt_out) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const int hw = H * W;
+  const int pix = blockIdx.x * blockDim.x + threadIdx.x;
+  if (pix >= hw) return;
+  const int b = blockIdx.y;
+  const int y = pix / W, x = pix - y * W;
+  const float fx = (float)x, fy = (float)y;
+  const float* row = params + (size_t)b * CIS_FLOW_AUG_ROW;
+  const float q1x = __ldg(row + 0) * fx + __ldg(row + 1) * fy + __ldg(row + 2), q1y = __ldg(row + 3) * fx + __ldg(row + 4) * fy + __ldg(row + 5);
+  const float q2x = __ldg(row + 6) * fx + __ldg(row + 7) * fy + __ldg(row + 8), q2y = __ldg(row + 9) * fx + __ldg(row + 10) * fy + __ldg(row + 11);
+  const size_t o = (size_t)b * hw;
+  float c1[3], c2[3];
+  aug_frame(img1 + o * 3, q1x, q1y, H, W, row, (uint32_t)pix * 3u, c1);
+  aug_frame(img2 + o * 3, q2x, q2y, H, W, row, (uint32_t)(hw + pix) * 3u, c2);
+  // the flow: gt at q1 in PWC-Net's order (-v, -u), moved by T2^-1, minus p
+  int i00;
+  float ax, ay;
+  aug_tap(q1x, q1y, H, W, i00, ax, ay);
+  const float2* g = reinterpret_cast<const float2*>(gt) + o + i00;
+  const float2 tl = __ldg(g), tr = __ldg(g + 1), bl = __ldg(g + W), br = __ldg(g + W + 1);
+  const float sx = q1x - aug_lerp(tl.y, tr.y, bl.y, br.y, ax, ay), sy = q1y - aug_lerp(tl.x, tr.x, bl.x, br.x, ax, ay);   // q + (u, v)
+  const float p2x = __ldg(row + 12) * sx + __ldg(row + 13) * sy + __ldg(row + 14), p2y = __ldg(row + 15) * sx + __ldg(row + 16) * sy + __ldg(row + 17);
+  float* d1 = img1_out + (o + pix) * 3;
+  float* d2 = img2_out + (o + pix) * 3;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) { d1[c] = c1[c]; d2[c] = c2[c]; }
+  reinterpret_cast<float2*>(gt_out)[o + pix] = make_float2(fy - p2y, fx - p2x);    // (-v', -u') = -(p2 - p)
+}
 __global__ void abs_sum_kernel(const float* __restrict__ g, size_t n, float* __restrict__ out) {
   pdl_launch_dependents();
   pdl_wait();
@@ -2653,3 +2793,24 @@ int cis_unsup_flow_loss_bwd(const float* flow, const float* img1, const float* i
 }
 
 }  // extern "C"
+static bool aug_range_ok(const float* r, bool positive) { return r[0] <= r[1] && (!positive || r[0] > 0.f); }
+int cis_flow_aug_params(const CisFlowAug* ranges, int32_t B, int32_t H, int32_t W, int64_t sample_offset, const long long* step, uint64_t seed,
+                        float* params, cis_stream_t stream) {
+  if (!ranges || !step || !params || B < 1 || B > 65535 || H < 2 || W < 2 || sample_offset < 0)
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_aug_params: bad buffer, batch, size (H, W >= 2) or sample offset");
+  const CisFlowAug& a = *ranges;
+  if (!aug_range_ok(a.scale, true) || !aug_range_ok(a.rotate, false) || !aug_range_ok(a.translate, false) || !aug_range_ok(a.rel_scale, true) ||
+      !aug_range_ok(a.rel_rotate, false) || !aug_range_ok(a.rel_translate, false) || !aug_range_ok(a.color, true) ||
+      !aug_range_ok(a.contrast, false) || !aug_range_ok(a.gamma, false) || !aug_range_ok(a.noise, false))
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_aug_params: every range needs lo <= hi, and scale, rel_scale and color lo > 0");
+  CIS_LAUNCH(flow_aug_params_kernel, nblk((size_t)B, 64), 64, 0, ST, a, B, H, W, (long long)sample_offset, step, (unsigned long long)seed, params);
+  return cis_check_launch("flow_aug_params");
+}
+int cis_flow_augment(const float* img1, const float* img2, const float* gt, const float* params, int32_t B, int32_t H, int32_t W, float* img1_out,
+                     float* img2_out, float* gt_out, cis_stream_t stream) {
+  if (!img1 || !img2 || !gt || !params || !img1_out || !img2_out || !gt_out || B < 1 || B > 65535 || H < 2 || W < 2 ||
+      6 * (int64_t)H * W >= ((int64_t)1 << 31) || ((uintptr_t)gt & 7) || ((uintptr_t)gt_out & 7))
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_flow_augment: bad buffer, gt alignment, batch or size (H, W >= 2, 6 H W < 2^31)");
+  CIS_LAUNCH(flow_augment_kernel, dim3(nblk((size_t)H * W), B), 256, 0, ST, img1, img2, gt, params, H, W, img1_out, img2_out, gt_out);
+  return cis_check_launch("flow_augment");
+}

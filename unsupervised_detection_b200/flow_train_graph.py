@@ -20,6 +20,13 @@ gradients, loss backward into the five level-flow gradients) -> the builder's re
 [one all-reduce] -> cis_adam_l2 -> re-pack of the bf16 operands.  The images carry no gradient dependency, so no conv1a data gradient is
 emitted.  The unsupervised step seeds only the final flow: the loss backward writes d L / d flow at H x W, and the transpose of the
 final x4 resize carries it into the level-2 flow gradient; levels 3-6 get theirs from the reverse tape alone.
+
+augment=True (supervised losses only) puts a random affine and photometric augmentation in front of that step, restated from the
+FlowNet / PWC-Net papers' description (cis_flow_aug_params and cis_flow_augment in include/cis_b200.h define it; the ranges, AUG_RANGES
+below, are chosen here).  Its parameters are drawn on the device from a counter hash of (seed, the Adam step, the global sample index):
+CUDA-graph replays draw new ones with no host involvement, and a data-parallel job with sample_offset = rank * batch draws what one GPU
+running the global batch draws.  The step's resize, pack and loss then read the augmented copies of the uploaded batch; forward() copies
+the batch unchanged into those buffers, so validation and epe() see the frames as uploaded.
 """
 import ctypes as C
 
@@ -35,6 +42,23 @@ WEIGHT_DECAY = 4e-4                               # gamma
 ROBUST_EPS, ROBUST_Q = 0.01, 0.4
 SMOOTH_WEIGHT = 3.0                               # lambda_s of the unsupervised loss: UnFlow's second-order weight, not tuned here
 FLOW_LOSSES = ('multiscale', 'robust', 'unsupervised')
+# augment=True: the default ranges of CisFlowAug (include/cis_b200.h states what each one draws)
+AUG_RANGES = dict(scale=(0.9, 2.0), rotate=(-17.0, 17.0), translate=(-0.2, 0.2), rel_scale=(0.95, 1.05), rel_rotate=(-3.0, 3.0),
+                  rel_translate=(-0.03, 0.03), color=(0.5, 2.0), contrast=(-0.8, 0.4), brightness=0.2, gamma=(0.7, 1.5), noise=(0.0, 0.04))
+AUG_SEED = 8964
+
+
+def flow_aug_ranges(**changes):
+    """A CisFlowAug holding AUG_RANGES with `changes` (field name -> value) applied."""
+    r = _lib.CisFlowAug()
+    for k, v in dict(AUG_RANGES, **changes).items():
+        if k not in AUG_RANGES:
+            raise ValueError('unknown augmentation range %r' % k)
+        if isinstance(v, tuple):
+            getattr(r, k)[:] = [float(x) for x in v]
+        else:
+            setattr(r, k, float(v))
+    return r
 
 
 def check_size(H, W):
@@ -57,11 +81,13 @@ class FlowTrainGraph(object):
     are resized to H x W on the device and the loss samples its targets from the uploaded flow, its vectors scaled to the H x W grid.
     loss: 'multiscale', 'robust' or 'unsupervised'; alphas, weight_decay, eps, q: the objective's constants; smooth_weight: lambda_s of
     the unsupervised loss; lr, beta1, beta2, adam_eps: TF-Adam.  With loss='unsupervised' the network batch is 2 * batch (forward pairs,
-    then backward pairs) and self.flow holds both halves; the ground truth is only read by epe()."""
+    then backward pairs) and self.flow holds both halves; the ground truth is only read by epe().
+    augment: train_step augments each uploaded batch at in_hw before the step (supervised losses only); aug_ranges: a CisFlowAug
+    (flow_aug_ranges(); None = AUG_RANGES); sample_offset: the global index of this rank's first sample (rank * batch under data parallelism)."""
 
     def __init__(self, H, W, batch, options=None, global_batch=None, device='cuda', in_hw=None, loss='multiscale', alphas=ALPHAS,
                  weight_decay=WEIGHT_DECAY, eps=ROBUST_EPS, q=ROBUST_Q, lr=1e-4, beta1=0.9, beta2=0.999, adam_eps=1e-8, name='pwcnet',
-                 smooth_weight=SMOOTH_WEIGHT):
+                 smooth_weight=SMOOTH_WEIGHT, augment=False, aug_ranges=None, sample_offset=0):
         from .models.PWCNet.model_pwcnet import PWCNetBuilder
         check_size(H, W)
         if loss not in FLOW_LOSSES:
@@ -70,6 +96,10 @@ class FlowTrainGraph(object):
             raise ValueError('alphas: one weight per level 6..2, got %r' % (alphas,))
         if not smooth_weight >= 0:
             raise ValueError('smooth_weight must be >= 0, got %r' % (smooth_weight,))
+        if augment and loss == 'unsupervised':
+            raise ValueError('augment=True is for the supervised losses: the unsupervised loss scores the frames themselves')
+        if sample_offset < 0:
+            raise ValueError('sample_offset must be >= 0, got %r' % (sample_offset,))
         _lib.load()
         self.H, self.W, self.B = H, W, batch
         self.GB = global_batch or batch
@@ -92,13 +122,31 @@ class FlowTrainGraph(object):
         f32 = bld.f32
         self.img1, self.img2, self.gt = f32(B, ih, iw, 3), f32(B, ih, iw, 3), f32(B, ih, iw, 2)
         self.inputs = (self.img1, self.img2, self.gt)       # the three device buffers one batch upload writes
+        self.augment, self.sample_offset = bool(augment), int(sample_offset)
+        self.aug, self.copy_in = Plan('aug_P'), Plan('copy_P')
+        if self.augment:
+            # the step reads augmented copies of the upload: aug draws each sample's parameters and writes them; copy_in (forward())
+            # writes the upload unchanged
+            self.aug_ranges = aug_ranges if aug_ranges is not None else flow_aug_ranges()
+            self.aug_seed = AUG_SEED
+            self.aug_params = torch.zeros(B, _lib.FLOW_AUG_ROW, dtype=torch.float32, device=device)
+            self.batch = (f32(B, ih, iw, 3), f32(B, ih, iw, 3), f32(B, ih, iw, 2))
+            self.aug.keep += [self.aug_ranges, self.aug_params]
+            self.aug.add('cis_flow_aug_params', C.byref(self.aug_ranges), B, ih, iw, self.sample_offset, self.step_state.data_ptr(),
+                         self.aug_seed, self.aug_params.data_ptr())
+            self.aug.add('cis_flow_augment', *(t.data_ptr() for t in self.inputs), self.aug_params.data_ptr(), B, ih, iw,
+                         *(t.data_ptr() for t in self.batch))
+            for dst, src in zip(self.batch, self.inputs):
+                self.copy_in.add_py(lambda d=dst, s=src: d.copy_(s), 'copy')
+        else:
+            self.batch = self.inputs
         # the images carry no gradient dependency: the backward emits conv1a's weight gradient but no data gradient
         i1, i2 = Act(N, H, W, 3, device, name='img1_8'), Act(N, H, W, 3, device, name='img2_8')
         self.img_acts = bld.hold((i1, i2))
-        src = (self.img1, self.img2)
+        src = self.batch[:2]
         if (ih, iw) != (H, W):
             src = (f32(B, H, W, 3), f32(B, H, W, 3))
-            for a, b in zip((self.img1, self.img2), src):
+            for a, b in zip(self.batch[:2], src):
                 P.add('cis_resize_bilinear_f32', a.data_ptr(), B, ih, iw, 3, b.data_ptr(), H, W, 1.0)
         if unsup:
             # network pairs n < B: (img1, img2); n >= B: (img2, img1) -- each frame packed into one half of each image Act
@@ -156,7 +204,7 @@ class FlowTrainGraph(object):
         self.pyr = pyr
         self.sums = torch.zeros(B, 5, dtype=torch.float64, device=device)
         self._scratch = torch.zeros(5 * B * 64, dtype=torch.float64, device=device)
-        self._loss_args = (self.gt.data_ptr(), B, H, W, ih, iw, H / ih, W / iw, 1 if self.loss == 'robust' else 0, float(eps), float(q))
+        self._loss_args = (self.batch[2].data_ptr(), B, H, W, ih, iw, H / ih, W / iw, 1 if self.loss == 'robust' else 0, float(eps), float(q))
         P.keep.append(pyr)
         P.add('cis_flow_multiscale_loss', C.byref(pyr), *self._loss_args, self._scratch.data_ptr(), self.sums.data_ptr())
         # ---- backward: zero the DenseNet level gradients, seed the five level-flow gradients, reverse tape, weight-gradient reduction
@@ -240,22 +288,24 @@ class FlowTrainGraph(object):
             self._dirty = False
 
     def forward(self):
-        """PWC-Net forward and the loss forward on the batch in img1 / img2 / gt (-> self.flow, self.sums)."""
+        """PWC-Net forward and the loss forward on the batch in img1 / img2 / gt (-> self.flow, self.sums), not augmented."""
         self._ensure_packed()
+        self.copy_in.run()
         self.fwd.run()
 
     def train_step(self, allreduce=None, use_graph=False):
-        """One step on the batch in img1 / img2 / gt: forward, loss, backward, [allreduce(flat gradient)], Adam + L2, re-pack.
-        use_graph replays two CUDA graphs (forward + backward, optimiser + pack) around the all-reduce."""
+        """One step on the batch in img1 / img2 / gt: [augmentation], forward, loss, backward, [allreduce(flat gradient)], Adam + L2,
+        re-pack.  use_graph replays two CUDA graphs (augmentation + forward + backward, optimiser + pack) around the all-reduce."""
         self._ensure_packed()
         if use_graph:
-            fwd_bwd = self._capture('fwd_bwd', [self.fwd, self.bwd])
+            fwd_bwd = self._capture('fwd_bwd', [self.aug, self.fwd, self.bwd])
             opt = self._capture('adam', [self.adam, self.pack], warm=False)
             fwd_bwd.replay()
             if allreduce is not None:
                 allreduce(self.store.grad)
             opt.replay()
             return
+        self.aug.run()
         self.fwd.run()
         self.bwd.run()
         if allreduce is not None:
@@ -267,7 +317,7 @@ class FlowTrainGraph(object):
         return capture_plans(self.graphs, key, plans, warm=warm)
 
     def launches_per_step(self):
-        return self.fwd.count() + self.bwd.count() + self.adam.count() + self.pack.count()
+        return self.aug.count() + self.fwd.count() + self.bwd.count() + self.adam.count() + self.pack.count()
 
     # ------------------------------------------------------------------------------------------------ results
     def losses(self, reduce=None):
@@ -296,7 +346,7 @@ class FlowTrainGraph(object):
 
     def epe(self):
         """End-point error of the last forward's final flow (self.flow, the level-2 flow x4; its forward half for the unsupervised loss)
-        against the ground truth, on the ground truth's grid -> self.epe_sums, fp64 [B,4] on the device: per sample {sum e, 0, pixels, 0},
+        against the ground truth it was trained or scored on (the augmented flow after an augmented train_step), on the ground truth's grid -> self.epe_sums, fp64 [B,4] on the device: per sample {sum e, 0, pixels, 0},
         e = ||pred - gt||_2 (cis_masked_epe with an all-ones mask; fixed-order sums).  When in_hw differs from H x W the prediction is first resized to in_hw with its vectors
         scaled to that grid (cis_crop_resize_flow_f32 over the whole frame)."""
         st = torch.cuda.current_stream().cuda_stream
@@ -305,6 +355,6 @@ class FlowTrainGraph(object):
             for b in range(self.B):
                 _lib.call('cis_crop_resize_flow_f32', self.flow[b].data_ptr(), H, W, 0, 0, H, W, self._pred_gt_grid[b].data_ptr(), ih, iw,
                           ih / H, iw / W, st)
-        _lib.call('cis_masked_epe', self._pred_gt_grid.data_ptr(), self.gt.data_ptr(), self._ones.data_ptr(), self.B, ih * iw,
+        _lib.call('cis_masked_epe', self._pred_gt_grid.data_ptr(), self.batch[2].data_ptr(), self._ones.data_ptr(), self.B, ih * iw,
                   self._epe_scratch.data_ptr(), self.epe_sums.data_ptr(), st)
         return self.epe_sums

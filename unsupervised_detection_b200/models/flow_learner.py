@@ -38,7 +38,9 @@ class FlowLearner(AdversarialLearner):
     def build_flow_graph(self):
         """FlowTrainGraph at img_height x img_width on the 384x640 batches (the frames are resized on the device; the supervised losses
         sample their targets from the 384x640 flow); parameters from --flow_ckpt when given, else params_init.init_pwcnet.  The
-        unsupervised loss also reads the training pairs of a mask dataset (--train_partition, --train_crop, the temporal shifts)."""
+        unsupervised loss also reads the training pairs of a mask dataset (--train_partition, --train_crop, the temporal shifts).  With
+        --flow_aug every training batch is augmented on the device; sample b of rank r is global sample r * local_batch + b, so a
+        data-parallel job draws the augmentation of one GPU running the global batch."""
         cfg = self.config
         loss = getattr(cfg, 'flow_loss', 'multiscale')
         ok = FLOW_DATASETS + (MASK_DATASETS if loss == 'unsupervised' else ())
@@ -53,7 +55,8 @@ class FlowLearner(AdversarialLearner):
         self.graph = FlowTrainGraph(cfg.img_height, cfg.img_width, self.local_batch, options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS,
                                     global_batch=cfg.batch_size, device=self.device, in_hw=(PWC_H, PWC_W),
                                     loss=loss, weight_decay=getattr(cfg, 'weight_decay', 4e-4),
-                                    lr=self._rate(1), beta1=cfg.beta1, smooth_weight=getattr(cfg, 'smooth_weight', 3.0))
+                                    lr=self._rate(1), beta1=cfg.beta1, smooth_weight=getattr(cfg, 'smooth_weight', 3.0),
+                                    augment=getattr(cfg, 'flow_aug', False), sample_offset=self.rank * self.local_batch)
         self._lr = self._rate(1)
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         names = [e[0] for e in self.graph.store.entries]
