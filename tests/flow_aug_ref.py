@@ -1,7 +1,8 @@
 """fp64 restatement of the augmentation of supervised PWC-Net training pairs (cis_flow_aug_params / cis_flow_augment, include/cis_b200.h).
 
 The counter hash is restated in uint64, so every draw is the kernel's bit for bit; the parameters and the per-pixel pass are then
-evaluated in double.  Parameter rows use the kernel's layout (ROW floats per sample)."""
+evaluated in double.  Parameter rows use the kernel's layout (ROW floats per sample).  tolerances() bounds how far the kernel's fp32
+per-pixel pass may lie from augment()."""
 import math
 
 import numpy as np
@@ -10,6 +11,7 @@ ROW = 32
 AUG_DOMAIN = 0x466c6f774175676d
 NOISE_DOMAIN = 0x4175674e6f697365
 _M = (1 << 64) - 1
+EPS = 2.0 ** -24          # fp32 unit roundoff, for the tolerances of the kernel's fp32 positions
 # the defaults of flow_train_graph.AUG_RANGES, restated
 DEFAULTS = dict(scale=(0.9, 2.0), rotate=(-17.0, 17.0), translate=(-0.2, 0.2), rel_scale=(0.95, 1.05), rel_rotate=(-3.0, 3.0),
                 rel_translate=(-0.03, 0.03), color=(0.5, 2.0), contrast=(-0.8, 0.4), brightness=0.2, gamma=(0.7, 1.5), noise=(0.0, 0.04))
@@ -190,3 +192,37 @@ def table_rows(table):
     P = t.astype(np.float64)
     P[:, 25] = t[:, 25].view(np.uint32).astype(np.float64)
     return P
+
+
+def lipschitz(a):
+    """max |difference| between neighbouring pixels of a [H, W, C] field: its Lipschitz bound per pixel of the bilinear sample."""
+    return max(float(np.abs(np.diff(a, axis=0)).max()), float(np.abs(np.diff(a, axis=1)).max()))
+
+
+def position_error(m, H, W):
+    """bound on the fp32 error of r0 x + r1 y + r2 (and the second row) over the grid"""
+    return 4 * EPS * max(abs(m[0]) * W + abs(m[1]) * H + abs(m[2]), abs(m[3]) * W + abs(m[4]) * H + abs(m[5]))
+
+
+def tolerances(img1, img2, gt, r):
+    """Per-element tolerances of cis_flow_augment's result for one sample (fp64 img1, img2 [H,W,3], gt [H,W,2], parameter row r) against
+    augment(): (frame 1 [H,W,3], frame 2 [H,W,3], flow scalar).  They come from the fp32 rounding of the sample positions."""
+    H, W = gt.shape[:2]
+    y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing='ij')
+    out = []
+    for src, m in ((img1, r[0:6]), (img2, r[6:12])):
+        # the sample moves by at most 2 * position error * Lipschitz bound; the affine part of the chain scales it by m_c (1 + kappa),
+        # gamma maps the interval around the pre-gamma value; fp32 arithmetic adds a few ulps of 1
+        qx, qy = apply(m, x, y)
+        s = bilinear(src, qx, qy)
+        pre = 0.5 + r[21] * ((s + 0.5) * r[18:21] - 0.5) + r[22]
+        e = np.abs(r[21] * r[18:21]) * 2 * position_error(m, H, W) * lipschitz(src) + 1e-6
+        g_ = lambda v: np.clip(v, 0, 1) ** r[23]  # noqa: E731
+        out.append(g_(pre + e) - g_(pre - e) + 8e-6)
+    # flow: q moves by dq; gt at q by 2 dq Lip(gt); T2^-1 scales the sum by its row norm and adds its own rounding; then - p
+    dq = position_error(r[0:6], H, W)
+    s_max = float(max(W, H) + np.abs(gt).max())
+    inv = r[12:18]
+    row = max(abs(inv[0]) + abs(inv[1]), abs(inv[3]) + abs(inv[4]))
+    out.append(row * (dq + 2 * dq * lipschitz(gt) + 4 * EPS * s_max) + 4 * EPS * (row * s_max + max(abs(inv[2]), abs(inv[5]))) + 2 * EPS * max(W, H))
+    return out

@@ -51,6 +51,52 @@ Per-element bound, no normalisation by the tensor maximum (the form of conv_laun
     flow gradient jumps where q crosses an integer (a clamp edge is one): positions within eps_q of one take 4 M |dwarp| fs per channel
     into delta, and their scatter is spread over the 4 x 4 neighbourhood.
 
+The PWC-Net training step (FlowTrainGraph; the kernels in csrc/misc_kernels.cu, built without --use_fast_math: sqrtf and division are
+correctly rounded, powf within CUDA's documented 4 ulp, rsqrtf and expf within 2 ulp).  U = 2^-24 is fp32's unit roundoff.
+  cis_flow_multiscale_loss: the [B, 5] sums against fp64 sums of rho(flow_l - g_l), g_l the legacy-bilinear sample of gt (fp32 source
+    positions, as lerp_axis forms them) times fp32(s_c) 2^-l.  The kernel's fp32 difference is within e_c = 2^-21 S_c |s_c 2^-l| + 2^-23
+    (|flow_c| + |g_c|) per channel (the lerps and the scale product as for cis_resize_bilinear_f32, then the subtraction).  ||.|| is
+    1-Lipschitz: rho moves by <= e_0 + e_1; robust rho by <= q max(x - E, eps)^(q-1) E, x = |d_0| + |d_1| + eps, E = e_0 + e_1 (the
+    local derivative at the interval's low end).  The sums are fp64: + (hw + 128) 2^-53 sum rho.  scratch and out are destinations.
+  cis_flow_multiscale_loss_bwd: the five bf16 level gradients weight[i] d rho / d flow (+ the snapshot where accumulate[i]).  ||.||:
+    d / ||d|| moves by <= 2 ||e|| / ||d||, + 2^-21 for the fp32 squares, sum, sqrtf, division and weight product; where ||d|| <= 4 E any
+    vector of norm <= weight is accepted.  Robust: k = q powf(x, q - 1) with x within E + 2^-23 x, so k within q (1 - q) x_lo^(q-2) (that)
+    + k (4 2^-23 + 2^-24 + |ln x| 2^-24) (powf, the product, the fp32 exponent q - 1); a component with |d_c| <= e_c may take either sign
+    or 0.  Destinations are exactly [c_off, c_off + 2) of each level; the padding channels of the level-gradient buffers must be +0 after
+    the launch (up_flow's data gradient and the predict-flow convs read them).
+  cis_adam_l2: fp64 TF-Adam from snapshots of param, m, v, grad, lr and step, decay inside the decoded segments only.  Per element, from
+    the fp32 operation count: e_g = U (2 |decay w| + |g|), e_m = 2U (b1 |m| + (1 - b1) |g|) + (1 - b1) e_g, e_v = 3U (b2 v + (1 - b2) g^2)
+    + 2 (1 - b2) |g| e_g; lr_t relative 2^-23 / (1 - b2^t) + 2^-22 / (1 - b1^t) + 4U (powf's 4 ulp on b^t in [0.5, 1), 1 - b^t exact by
+    Sterbenz, sqrtf, two products); sqrt(v') + eps within min(e_v / (2 sqrt v'), sqrt e_v) + 2U (sqrt v' + eps); the update
+    lr_t m' / (sqrt v' + eps) relative (that + 3U) plus lr_t e_m / (sqrt v' + eps); the parameter + U |w'|.  step_state must advance by
+    exactly 1 and grad stay bit-identical.
+  cis_flow_aug_params: flow_aug_ref's draw from the decoded ranges, seed and sample_offset at the step read from step_state before the
+    launch.  The accepted attempt (26), the noise key (25, as uint32) and the zero tail are bit-identical; columns 0-24 within one fp32 ulp
+    of fp32(the fp64 value) (the ratio is in ulps).
+  cis_flow_augment: flow_aug_ref.augment's fp64 per-pixel pass for both frames and the flow, within flow_aug_ref.tolerances (the bounds
+    tests/test_flow_aug_gpu.py uses too: fp32 sample positions through the Lipschitz bound of the sampled field and the photometric chain;
+    the flow through T2^-1's row norm).
+  cis_unsup_flow_loss: the occlusion test runs in fp32 on the partner flow h sampled at q (lerps and fp32 alphas: 2^-20 sum |corners|
+    = eh per channel), so lhs = |f + h|^2 and rhs = 0.01f (|f|^2 + |h|^2) + 0.5f are within e_lhs = sum_c 2 |s_c| (eh_c + 2^-23 |s_c|)
+    + eh_c^2 + 3 2^-23 lhs and e_rhs = 0.01 sum_c (2 |h_c| eh_c + eh_c^2) + |0.01f - 0.01| (|f|^2 + |h|^2) + 6 2^-23 rhs; the mask must be
+    the fp64 one except where |lhs - rhs| <= 2 (e_lhs + e_rhs).  The frame-border test is exact: q = p - F is formed in double from the
+    fp32 flow by the kernel and the reference alike.  Where the mask is ambiguous the references use the launch's own bit.  warped: the
+    fp64 sample of the gray levels, within 2^-20 sum |corners| (fp32 gray levels and alphas, the lerps).  The census is recomputed from
+    the launch's own warped (checked above) and the fp64 gray levels of S; c within e_c (_census_bound: the fp32 rounding of the gray
+    levels and differences through t's slope, t within 8U |t|, e = t_S - t_T through phi's largest slope on the interval, phi within 8U
+    phi, the 48-term fp32 sum).  psi = powf(c + 0.01f, 0.4f) within 0.4 c_lo^-0.6 Dc + psi (|ln(c + 0.01)| |0.4f - 0.4| + 4 2^-23), Dc =
+    e_c + 2^-23 (c + 0.01) + |0.01f - 0.01|, c_lo = max(c - Dc, 0) + 0.01; coef = M 0.4f powf(c + 0.01f, -0.6f) likewise (slope 0.24
+    c_lo^-1.6).  Smoothness: w within rel_w = 5 (e/3) 8U + 3 2^-23 (fp32 differences, the 1/3f and -10 products, expf), l in double as
+    the kernel forms it; where |l_c| is within 2^-50 (|a| + 2|b| + |c|) of the ROUNDING threshold w |l_c| joins delta.  Sums fp64:
+    + (hw + 128) 2^-53 sum M psi and (2 hw + 128) 2^-53 sum w s.
+  cis_unsup_flow_loss_bwd: checked on its own from the forward's warped and coef buffers.  Reference: unsup_bwd_gather, the explicit
+    fp64 gather (test_flow_train_launches_cpu.py proves it equals autograd of unsup_flow_loss_ref).  Per window term (k(r+d) + k(r)) h,
+    h = -0.2 e / (0.1 + e^2)^2 0.81 iu^3: the fp32 e within e_e (as in the forward) through |dh/de| <= 0.2 (0.1 + 3x) / (0.1 + x)^3
+    0.81 iu^3 at x = max(|e| - e_e, 0)^2 (it falls with x), and 33 U |h| for the term's own fp32 operations; the 48-term sum 48 2^-23
+    sum |terms| (S: the same gather over |terms|); the chain factor (bot - top etc.) within 2^-20 sum |corners|.  The sample point q is
+    exact in double on both sides, so floor, clamps and pass flags agree and no jump enters delta.  Smoothness: w rel_w per stencil term,
+    6 2^-23 sum |c w| for the fp32 sum, |c w| where the centre's sign is ambiguous.  Then 2^-23 |dflow| for the final additions.
+
 Stray writes: every destination storage is snapshotted whole; after the launch every byte outside the windows the launch owns (rows x
 channel window of each destination) must be unchanged, and the padding channels inside the windows (padding in every Act that views the
 buffer) must be exactly 0.
@@ -59,6 +105,10 @@ Negative controls (a ratio > 1 means the bound rejected the corruption); they ac
   resize.row_off_by_one, rc_bwd.fold_dropped, rc_bwd.overwrite, dact.d_at_y, colsum.block_dropped, add_slice.acc_dropped,
   warp_costvol.fs_x1.25, warp_costvol_r1.dx_outer (the r = 1 cost volume with its displacements listed dx outer), costvol_bwd.gate_one,
   and tile.<entry point>: one 16 x 8 tile of one channel of a bf16 result scaled by 1 + 2^-5.
+  The training step's: ms_loss.axes_swapped (s0 and s1 exchanged; only made where they differ), ms_loss.level_scale (targets at
+  2^-(l-1)), ms_loss_bwd.weights_reversed, unsup.mask_ones, unsup_bwd.smooth_dropped, aug_params.step_frozen (rows drawn at step 0, made
+  from step 1 on), augment.flow_unmapped (the flow resampled at T1 but not passed through T2^-1), adam.decay_everywhere and
+  adam.t_off_by_one (made from t = 2 on).  pack.unswapped lives in tests/test_flow_train_launches_gpu.py.
 """
 import bisect
 import collections
@@ -69,6 +119,7 @@ import torch.nn.functional as F
 
 from oracle import losses as OL
 from unsupervised_detection_b200 import engine as E
+from unsupervised_detection_b200 import _lib
 from unsupervised_detection_b200._lib import ACT_ELU
 
 U23 = 2.0 ** -23
@@ -101,6 +152,14 @@ ARGS = {
     'cis_warp_costvol_r': 'c1 c1p c1o c2 c2p c2o flow fs B h w C out op oo r',
     'cis_warp_costvol_bwd_r': 'c1 c1p c1o c2 c2p c2o flow fs B h w C dcorr dcp dco dc1 dc1p dc1o dc2 dc2p dc2o dflow dfp dfo acc gs ws ds '
                               'r',
+    # the PWC-Net training step (FlowTrainGraph)
+    'cis_flow_multiscale_loss': 'pyr gt B H W GH GW s0 s1 robust eps q scratch out',
+    'cis_flow_multiscale_loss_bwd': 'pyr gt B H W GH GW s0 s1 robust eps q',
+    'cis_unsup_flow_loss': 'flow img1 img2 B H W warped mask coef scratch out',
+    'cis_unsup_flow_loss_bwd': 'flow img1 img2 B H W warped coef w_photo w_smooth dflow',
+    'cis_flow_aug_params': 'ranges B H W sample_offset step seed params',
+    'cis_flow_augment': 'img1 img2 gt params B H W img1_out img2_out gt_out',
+    'cis_adam_l2': 'param m v grad n seg nseg decay lr beta1 beta2 eps step_state',
 }
 
 # entry points of the step pinned per launch by other tests (the ownership test of tests/test_glue_launches_cpu.py)
@@ -350,6 +409,172 @@ class _Warp(object):
                 idx = ((self.bidx * h + (self.ly + dy).clamp(0, h - 1)) * w + (self.lx + dx).clamp(0, w - 1)).reshape(-1)
                 out.index_add_(0, idx, v.reshape(-1, C))
         return out.view(B, h, w, C)
+
+
+# ------------------------------------------------------------------------------------------------------------ unsupervised loss
+U24 = 2.0 ** -24
+
+
+def _unsup_sample(img, flow):
+    """dense_image_warp's sample of img [N,H,W,C] at q = p - flow (fp64, exact alphas): val, abs = sum of the four |corners|, the
+    derivative factors cy = bot - top and cx = ay (br - bl) + (1 - ay)(tr - tl), and the pass flags of the alphas."""
+    import unsup_flow_loss_ref as UR
+    N, H, W, C = img.shape
+    qy, qx = UR.sample_points(flow)
+
+    def prep(q, size):
+        fl = torch.clamp(torch.floor(q), 0.0, float(size - 2))
+        r = q - fl
+        return fl.long(), torch.clamp(r, 0.0, 1.0).unsqueeze(-1), (r >= 0) & (r <= 1)
+    fy, ay, py = prep(qy, H)
+    fx, ax, px = prep(qx, W)
+    flat = img.reshape(N, H * W, C)
+
+    def at(yy, xx):
+        return torch.gather(flat, 1, (yy * W + xx).reshape(N, H * W, 1).expand(-1, -1, C)).reshape(N, H, W, C)
+    tl, tr, bl, br = at(fy, fx), at(fy, fx + 1), at(fy + 1, fx), at(fy + 1, fx + 1)
+    top, bot = tl + ax * (tr - tl), bl + ax * (br - bl)
+    return dict(val=top + ay * (bot - top), abs=tl.abs() + tr.abs() + bl.abs() + br.abs(), cy=bot - top,
+                cx=ay * (br - bl) + (1 - ay) * (tr - tl), pass_y=py, pass_x=px)
+
+
+def _tsoft(v):
+    return v / torch.sqrt(0.81 + v * v)
+
+
+def _tsoft_slope(v):
+    """max of |t'| over |v'| >= |v| (t' = 0.81 / (0.81 + v^2)^1.5 falls with |v|)."""
+    return 0.81 / (0.81 + v * v) ** 1.5
+
+
+def _census_bound(gS, tw):
+    """c of unsup_flow_loss_ref.census and the bound e on the kernel's fp32 c: gray levels of S rounded to fp32 (2^-24 each), T~ read
+    as is, differences rounded, t(v) = v rsqrtf(0.81 + v^2) within 8 2^-24 |t| (rsqrtf 2 ulp, three roundings, the constant 0.81f),
+    the difference e = t_S - t_T carried through phi(e) = e^2 / (0.1 + e^2) by its largest slope on [|e| - e_e, |e| + e_e], phi's own
+    roundings 8 2^-24 phi, and the 48-term fp32 sum (48 2^-23 c)."""
+    import unsup_flow_loss_ref as UR
+    c, e = torch.zeros_like(tw), torch.zeros_like(tw)
+    xs = (0.1 / 3) ** 0.5                                 # phi' = 0.2 x / (0.1 + x^2)^2 peaks there
+    for dy in range(-3, 4):
+        for dx in range(-3, 4):
+            if dy == 0 and dx == 0:
+                continue
+            s2, ins = UR._shift(gS, dy, dx)
+            t2, _ = UR._shift(tw, dy, dx)
+            vS, vT = s2 - gS, t2 - tw
+            e_vS, e_vT = U24 * (s2.abs() + gS.abs() + vS.abs()), U24 * vT.abs()
+            tS, tT = _tsoft(vS), _tsoft(vT)
+            e_d = (_tsoft_slope(torch.clamp(vS.abs() - e_vS, min=0)) * e_vS + 8 * U24 * tS.abs() +
+                   _tsoft_slope(torch.clamp(vT.abs() - e_vT, min=0)) * e_vT + 8 * U24 * tT.abs())
+            d = tS - tT
+            e_d = e_d + U24 * d.abs()
+            x = torch.clamp(torch.full_like(d, xs), min=torch.clamp(d.abs() - e_d, min=0), max=d.abs() + e_d)
+            phi = d * d / (0.1 + d * d)
+            c = c + ins * phi
+            e = e + ins * (0.2 * x / (0.1 + x * x) ** 2 * e_d + 8 * U24 * phi)
+    return dict(c=c, e=e + 48 * U23 * c)
+
+
+def _unsup_smooth_terms(fd, S):
+    """Per pixel of the 2B directions: val = sum_a w_a s_a (the kernel's per-pixel smoothness term) and err, its bound: w_a within
+    rel_w (fp32 differences and sums of the frame, the 1/3f and -10 products, expf 2 ulp), and where |l_c| is within 2^-50 (|a| + 2|b|
+    + |c|) of the ROUNDING threshold (the double second difference may land on either side) w |l_c| more.  Per axis, for the backward's
+    gather: X = w sign(l) per centre, A = w, Rw = w rel_w, Z = w at centres whose sign is ambiguous ([N,H,W,2]; 0 where no centre)."""
+    import unsup_flow_loss_ref as UR
+    N, H, W, _ = fd.shape
+    val, err = torch.zeros(N, H, W, dtype=fd.dtype, device=fd.device), torch.zeros(N, H, W, dtype=fd.dtype, device=fd.device)
+    axes = []
+    for dim in (1, 2):
+        n = fd.shape[dim]
+        a, b, c = fd.narrow(dim, 2, n - 2), fd.narrow(dim, 1, n - 2), fd.narrow(dim, 0, n - 2)
+        l = a - 2 * b + c
+        mag = a.abs() + 2 * b.abs() + c.abs()
+        amb = (l.abs() - UR.ROUNDING * mag).abs() <= 2.0 ** -50 * mag
+        lz = UR.second_difference(a, b, c)
+        e3 = (S.narrow(dim, 2, n - 2) - S.narrow(dim, 0, n - 2)).abs().sum(-1)
+        w = torch.exp(-10.0 * (e3 / 3) / 2)
+        rel_w = 5 * (e3 / 3) * 8 * U24 + 3 * U23
+        s = lz.abs().sum(-1)
+        v_in = w * s
+        e_in = rel_w * v_in + w * (amb * l.abs()).sum(-1) + 2.0 ** -50 * v_in
+        pad = [0, 0] * (2 - dim) + [1, 1]
+        val = val + F.pad(v_in, pad)
+        err = err + F.pad(e_in, pad)
+        pad4 = [0, 0] + pad
+        X = F.pad(w.unsqueeze(-1) * torch.sign(lz), pad4)
+        A = F.pad(w.unsqueeze(-1) * torch.ones_like(lz), pad4)
+        Rw = F.pad((w * rel_w).unsqueeze(-1) * torch.ones_like(lz), pad4)
+        Z = F.pad(w.unsqueeze(-1) * amb, pad4)
+        axes.append((dim, X, A, Rw, Z))
+    return dict(val=val, err=err, axes=axes)
+
+
+def _stencil(X, dim, centre):
+    """out[r] = X[r + e] + X[r - e] + centre X[r] along dim (0 outside)."""
+    n = X.shape[dim]
+    out = centre * X
+    z = torch.zeros_like(X.narrow(dim, 0, 1))
+    out = out + torch.cat([X.narrow(dim, 1, n - 1), z], dim) + torch.cat([z, X.narrow(dim, 0, n - 1)], dim)
+    return out
+
+
+def unsup_bwd_gather(flow, img1, img2, warped, coef, w_photo, w_smooth, bounds=False):
+    """cis_unsup_flow_loss_bwd restated as an explicit fp64 gather on any device: the census term folded into one sweep of each pixel's
+    own 7x7 window, dT~(r) = -w_photo sum_d (k(r+d) + k(r)) h(r, r+d), h = d/du of phi(t_S - t(u)) at u = T~(r+d) - T~(r), chained
+    through dense_image_warp's dflow rule at r's own sample point; plus w_smooth times the 5-point gather of w sign(l) from the centres
+    r - e_a (x1), r (x-2), r + e_a (x1).  flow [2B,H,W,2], frames [B,H,W,3], warped / coef [2B,H,W] (the forward's T~ and M psi'(c)).
+    -> dict(ref, photo (the census part alone), smooth) and with bounds=True err, the bound on the kernel's fp32 result."""
+    import unsup_flow_loss_ref as UR
+    S, T = UR.directions(img1, img2)
+    gS = UR.gray(S)
+    G, eG, SG = torch.zeros_like(warped), torch.zeros_like(warped), torch.zeros_like(warped)
+    for dy in range(-3, 4):
+        for dx in range(-3, 4):
+            if dy == 0 and dx == 0:
+                continue
+            s2, ins = UR._shift(gS, dy, dx)
+            t2, _ = UR._shift(warped, dy, dx)
+            k2, _ = UR._shift(coef, dy, dx)
+            vS, u = s2 - gS, t2 - warped
+            iu = 1 / torch.sqrt(0.81 + u * u)
+            d = _tsoft(vS) - u * iu
+            hh = -0.2 * d / (0.1 + d * d) ** 2 * 0.81 * iu ** 3
+            term = ins * (k2 + coef) * hh
+            G = G + term
+            if bounds:
+                # |d(-0.2 d / (0.1 + d^2)^2) / dd| <= 0.2 (0.1 + 3x) / (0.1 + x)^3, x = d^2, which falls with x; ~33 fp32 roundings
+                # (rsqrtf 2 ulp, iu^3, den^2, the products, the constants 0.2f and 0.81f, k2 + k) on the term itself
+                e_vS, e_u = U24 * (s2.abs() + gS.abs() + vS.abs()), U24 * u.abs()
+                e_d = (_tsoft_slope(torch.clamp(vS.abs() - e_vS, min=0)) * e_vS + 8 * U24 * _tsoft(vS).abs() +
+                       _tsoft_slope(torch.clamp(u.abs() - e_u, min=0)) * e_u + 8 * U24 * (u * iu).abs())
+                e_d = e_d + U24 * d.abs()
+                x = torch.clamp(d.abs() - e_d, min=0) ** 2
+                slope = 0.2 * (0.1 + 3 * x) / (0.1 + x) ** 3 * 0.81 * iu ** 3
+                eG = eG + ins * (k2 + coef).abs() * (slope * e_d + 33 * U24 * hh.abs())
+                SG = SG + term.abs()
+    dtw = -G * w_photo
+    st = _unsup_sample(UR.gray(T).unsqueeze(-1), flow)
+    cy, cx = st['cy'][..., 0], st['cx'][..., 0]
+    photo = torch.stack([torch.where(st['pass_y'], -dtw * cy, torch.zeros_like(cy)), torch.where(st['pass_x'], -dtw * cx, torch.zeros_like(cx))], -1)
+    sm = _unsup_smooth_terms(flow, S)
+    smooth = torch.zeros_like(flow)
+    absw, relw, ambw = torch.zeros_like(flow), torch.zeros_like(flow), torch.zeros_like(flow)
+    for dim, X, A, Rw, Z in sm['axes']:
+        smooth = smooth + _stencil(X, dim, -2.0)
+        absw = absw + _stencil(A, dim, 2.0)
+        relw = relw + _stencil(Rw, dim, 2.0)
+        ambw = ambw + _stencil(Z, dim, 2.0)
+    ref = photo + w_smooth * smooth
+    out = dict(ref=ref, photo=photo, smooth=smooth)
+    if bounds:
+        e_dtw = w_photo * (eG + 48 * U23 * SG) + U24 * dtw.abs()
+        e_chain = 2.0 ** -20 * st['abs'][..., 0]              # fp32 gray corners and alphas, the lerps
+        pas = torch.stack([st['pass_y'], st['pass_x']], -1)
+        e_photo = pas * ((dtw.abs() * e_chain).unsqueeze(-1) + torch.stack([cy, cx], -1).abs() * e_dtw.unsqueeze(-1) + U24 * photo.abs())
+        # the weights' own error, the 6-term fp32 sum, the ambiguous signs
+        e_sm = w_smooth * (relw + 6 * U23 * absw + ambw) + U24 * (w_smooth * smooth).abs()
+        out['err'] = e_photo + e_sm + U23 * ref.abs()
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------ the checker
@@ -937,6 +1162,361 @@ class Glue(object):
 
     def _post_warp_costvol_bwd_r(self, a, ctx):
         self._post_warp_costvol_bwd(a, ctx)
+
+    # ---- multi-scale flow loss and its backward
+    def _ms_levels(self, a, scale=(1.0, 1.0), level_shift=0):
+        """Per level i: the fp32 flow read, d = flow - target in fp64 and e = the per-channel bound on the kernel's fp32 d.
+        scale / level_shift: corrupted targets (negative controls)."""
+        pyr, B, H, W, GH, GW = a['pyr']._obj, a['B'], a['H'], a['W'], a['GH'], a['GW']
+        gt = self.mem.view(a['gt'], torch.float32, (B, GH, GW, 2)).clone()
+        x = gt.double()
+        s = (float(_f32(a['s0'])) * scale[0], float(_f32(a['s1'])) * scale[1])
+        out = []
+        for i in range(5):
+            l = 6 - i
+            h, w = H >> l, W >> l
+            f = self.mem.view(pyr.flow[i], torch.float32, (B, h, w, 2)).clone()
+            (My, Iy), (Mx, Ix) = lerp_axis(GH, h), lerp_axis(GW, w)
+            sc = torch.tensor([s[0], s[1]], dtype=torch.float64, device='cuda') * 2.0 ** -(l - level_shift)
+            t = apply2(My, Mx, x) * sc
+            d = f.double() - t
+            e = G_LERP * apply2(Iy, Ix, x.abs()) * sc.abs() + U23 * (f.double().abs() + t.abs())
+            out.append(dict(f=f, d=d, e=e, h=h, w=w))
+        return gt, out
+
+    @staticmethod
+    def _rho(d, e, robust, eps, q):
+        """(rho(d), bound on |rho(d') - rho(d)| for |d'_c - d_c| <= e_c) per pixel, fp64."""
+        E = e.sum(-1)
+        if robust:
+            x = d.abs().sum(-1) + eps
+            r = x ** q
+            return r, q * torch.clamp(x - E, min=eps) ** (q - 1) * E + 2.0 ** -50 * r
+        r = torch.sqrt((d * d).sum(-1))
+        return r, E + 2.0 ** -50 * r                 # ||.|| is 1-Lipschitz
+
+    def _pre_flow_multiscale_loss(self, a):
+        B = a['B']
+        robust, eps, q = a['robust'], float(_f32(a['eps'])), float(_f32(a['q']))
+        gt, lv = self._ms_levels(a)
+
+        def sums(levels):
+            ref, err = [], []
+            for L in levels:
+                r, er = self._rho(L['d'], L['e'], robust, eps, q)
+                hw = L['h'] * L['w']
+                ref.append(r.sum((1, 2)))
+                err.append(er.sum((1, 2)) + (hw + 128) * 2.0 ** -53 * r.sum((1, 2)))
+            return torch.stack(ref, 1), torch.stack(err, 1)
+        ref, err = sums(lv)
+        ctx = dict(ref=ref, err=err, reads=[gt] + [L['f'] for L in lv],
+                   dests=[(a['scratch'], torch.float64, 5 * B, 64, 0, 64), (a['out'], torch.float64, B, 5, 0, 5)])
+        if self.controls is not None:
+            if float(_f32(a['s0'])) != float(_f32(a['s1'])):
+                ctx['bad_axes'] = sums(self._ms_levels(a, scale=(float(_f32(a['s1'])) / float(_f32(a['s0'])),
+                                                                float(_f32(a['s0'])) / float(_f32(a['s1']))))[1])[0]
+            ctx['bad_level'] = sums(self._ms_levels(a, level_shift=1)[1])[0]
+        return ctx
+
+    def _post_flow_multiscale_loss(self, a, ctx):
+        got = self.mem.view(a['out'], torch.float64, (a['B'], 5))
+        self._rec('cis_flow_multiscale_loss', 'level sums', ratio(got, ctx['ref'], ctx['err']))
+        if 'bad_axes' in ctx:
+            self._control('ms_loss.axes_swapped', ratio(got, ctx['bad_axes'], ctx['err']))
+        if 'bad_level' in ctx:
+            self._control('ms_loss.level_scale', ratio(got, ctx['bad_level'], ctx['err']))
+
+    def _ms_grad(self, L, robust, eps, q):
+        """(d rho / d flow, its bound, where the kernel's value may be any vector of norm <= 1) per pixel, before the weight."""
+        d, e = L['d'], L['e']
+        if robust:
+            E = e.sum(-1, keepdim=True)
+            x = d.abs().sum(-1, keepdim=True) + eps
+            Dx = E + U23 * x                                  # the kernel's fp32 |d0| + |d1| + eps
+            xl = torch.clamp(x - Dx, min=eps * (1 - U23))
+            k = q * x ** (q - 1)
+            ek = q * (1 - q) * xl ** (q - 2) * Dx + k * (4 * U23 + 2.0 ** -24 + x.log().abs() * 2.0 ** -24)
+            amb = d.abs() <= e                                # sign(d_c) may go either way
+            g = torch.where(amb, torch.zeros_like(d), torch.sign(d) * k)
+            err = torch.where(amb, q * xl ** (q - 1) * (1 + 2 * U23), ek.expand_as(d))
+            return g, err, None
+        n = torch.sqrt((d * d).sum(-1, keepdim=True))
+        E = e.sum(-1, keepdim=True)
+        amb = n <= 4 * E
+        g = torch.where(amb, torch.zeros_like(d), d / torch.where(amb, torch.ones_like(n), n))
+        err = torch.where(amb, torch.ones_like(d) * (1 + 2.0 ** -20), 2 * E / torch.clamp(n - E, min=FLOOR) + 2.0 ** -21)
+        return g, err, amb[..., 0]
+
+    def _pre_flow_multiscale_loss_bwd(self, a, weights=None):
+        pyr, B = a['pyr']._obj, a['B']
+        robust, eps, q = a['robust'], float(_f32(a['eps'])), float(_f32(a['q']))
+        gt, lv = self._ms_levels(a)
+        wts = [float(pyr.weight[i]) for i in range(5)]
+        checks, dests, reads = [], [], [gt]
+        bad = []
+        for i, L in enumerate(lv):
+            g, err, amb = self._ms_grad(L, robust, eps, q)
+            n = B * L['h'] * L['w']
+            p, pitch, c0 = pyr.grad[i], pyr.pitch[i], pyr.c_off[i]
+            old = self._bf(p, n, pitch)[:, c0:c0 + 2].double().view(B, L['h'], L['w'], 2)
+            acc = bool(pyr.accumulate[i])
+            ref = wts[i] * g + (old if acc else 0.0)
+            e = wts[i] * err * (1 + 2 * U23) + (U23 * (old.abs() + wts[i] * g.abs()) if acc else 0.0)
+            checks.append(dict(p=p, pitch=pitch, c0=c0, n=n, shape=(B, L['h'], L['w'], 2), ref=ref, e=e, amb=amb, wt=wts[i], old=old,
+                               acc=acc, pads=self.mem.pads(p, pitch, 0, pitch)))
+            bad.append(wts[4 - i] * g + (old if acc else 0.0))
+            dests.append((p, torch.bfloat16, n, pitch, c0, c0 + 2))
+            reads.append(L['f'])
+        return dict(checks=checks, dests=dests, reads=reads, bad=bad if wts != wts[::-1] else None)
+
+    def _post_flow_multiscale_loss_bwd(self, a, ctx):
+        worst_bad = 0.0
+        for i, c in enumerate(ctx['checks']):
+            got = self._bf(c['p'], c['n'], c['pitch'])[:, c['c0']:c['c0'] + 2].view(c['shape'])
+            b = E_BF16 * c['ref'].abs() + c['e'] * (1 + 2 ** -7)
+            self._rec('cis_flow_multiscale_loss_bwd', 'level %d gradient' % (6 - i), ratio(got, c['ref'], b))
+            if c['amb'] is not None and bool(c['amb'].any()):
+                # where ||d|| is within a few e_d of 0: any vector of norm <= weight
+                v = got.double() - (c['old'] if c['acc'] else 0.0)
+                nrm = torch.sqrt((v * v).sum(-1))[c['amb']]
+                self._rec('cis_flow_multiscale_loss_bwd', 'near-zero norm', float(nrm.max()) / (c['wt'] * (1 + 2 ** -6)))
+            if c['pads']:
+                pv = self._bf(c['p'], c['n'], c['pitch'])[:, c['pads']]
+                if not bool((pv.view(torch.int16) == 0).all()):
+                    self.failures.append('%s launch %d cis_flow_multiscale_loss_bwd: level %d gradient padding channels %s not +0'
+                                         % (self.where + (6 - i, c['pads'])))
+            if ctx['bad'] is not None:
+                worst_bad = max(worst_bad, ratio(got, ctx['bad'][i], b))
+            self._control('tile.cis_flow_multiscale_loss_bwd', ratio(_tile(got), c['ref'], b))
+        if ctx['bad'] is not None:
+            self._control('ms_loss_bwd.weights_reversed', worst_bad)
+
+    # ---- TF-Adam with L2 on the kernel segments
+    @staticmethod
+    def _adam_ref(w, m, v, g0, inseg, decay, lr, b1, b2, eps, t):
+        g = g0 + torch.where(inseg, decay * w, torch.zeros_like(w))
+        lr_t = lr * (1 - b2 ** t) ** 0.5 / (1 - b1 ** t)
+        m1 = b1 * m + (1 - b1) * g
+        v1 = b2 * v + (1 - b2) * g * g
+        return g, m1, v1, lr_t, w - lr_t * m1 / (v1.sqrt() + eps)
+
+    def _pre_adam_l2(self, a):
+        n = a['n']
+        snap = [self.mem.view(a[k], torch.float32, (n,)).clone() for k in ('param', 'm', 'v', 'grad')]
+        seg = self.mem.view(a['seg'], torch.int64, (a['nseg'], 2)).clone() if a['nseg'] else torch.zeros(0, 2, dtype=torch.int64)
+        lr = float(self.mem.view(a['lr'], torch.float32, (1,)))
+        step = int(self.mem.view(a['step_state'], torch.int64, (1,)))
+        w, m, v, g0 = (x.double() for x in snap)
+        inseg = torch.zeros(n, dtype=torch.bool, device='cuda')
+        for s0, s1 in seg.tolist():
+            inseg[s0:s1] = True
+        decay, b1, b2, eps = (float(_f32(a[k])) for k in ('decay', 'beta1', 'beta2', 'eps'))
+        t = step + 1
+        g, m1, v1, lr_t, w1 = self._adam_ref(w, m, v, g0, inseg, decay, lr, b1, b2, eps, t)
+        u = 2.0 ** -24
+        e_g = u * (2 * (decay * w).abs() * inseg + g.abs())
+        e_m = 2 * u * (b1 * m.abs() + (1 - b1) * g.abs()) + (1 - b1) * e_g
+        e_v = 3 * u * (b2 * v + (1 - b2) * g * g) + (1 - b2) * 2 * g.abs() * e_g
+        # lr_t: powf within 4 ulp (2^-22 on b^t in [0.5, 1)), 1 - b^t exact (Sterbenz), sqrtf, two products
+        rel_lr = 0.5 * 2.0 ** -22 / (1 - b2 ** t) + 2.0 ** -22 / (1 - b1 ** t) + 4 * u
+        den = v1.sqrt() + eps
+        e_den = torch.minimum(e_v / (2 * v1.sqrt()).clamp(min=FLOOR), e_v.sqrt()) + 2 * u * den
+        U = lr_t * m1 / den
+        e_U = U.abs() * (rel_lr + 3 * u + e_den / den) + lr_t * e_m / den
+        ctx = dict(ref=(w1, m1, v1), err=(u * w1.abs() + e_U, e_m, e_v), grad=snap[3], step=step,
+                   reads=snap, dests=[(a[k], torch.float32, 1, n, 0, n) for k in ('param', 'm', 'v')] +
+                   [(a['step_state'], torch.int64, 1, 1, 0, 1)])
+        if self.controls is not None:
+            ctx['bad_decay'] = self._adam_ref(w, m, v, g0, torch.ones_like(inseg), decay, lr, b1, b2, eps, t)[1:]
+            if t >= 2:
+                ctx['bad_t'] = self._adam_ref(w, m, v, g0, inseg, decay, lr, b1, b2, eps, t - 1)[1:]
+        return ctx
+
+    def _post_adam_l2(self, a, ctx):
+        n = a['n']
+        got = [self.mem.view(a[k], torch.float32, (n,)) for k in ('param', 'm', 'v')]
+        for what, x, r, e in zip(('param', 'm', 'v'), got, ctx['ref'], ctx['err']):
+            self._rec('cis_adam_l2', what, ratio(x, r, e))
+        step = int(self.mem.view(a['step_state'], torch.int64, (1,)))
+        self._rec('cis_adam_l2', 'step advanced by one', 0.0 if step == ctx['step'] + 1 else float('inf'))
+        self._rec('cis_adam_l2', 'grad unchanged', exact(self.mem.view(a['grad'], torch.float32, (n,)), ctx['grad']))
+        for name, key in (('adam.decay_everywhere', 'bad_decay'), ('adam.t_off_by_one', 'bad_t')):
+            if key in ctx:
+                bad = ctx[key]
+                self._control(name, max(ratio(got[0], bad[3], ctx['err'][0]), ratio(got[1], bad[0], ctx['err'][1]),
+                                        ratio(got[2], bad[1], ctx['err'][2])))
+
+    # ---- augmentation: parameter rows and the per-pixel pass
+    @staticmethod
+    def _aug_ranges(r):
+        out = {}
+        for name, _ in r._fields_:
+            v = getattr(r, name)
+            out[name] = float(v) if isinstance(v, float) else tuple(float(x) for x in v)
+        return out
+
+    def _aug_rows_ratio(self, got, ref):
+        """0 / inf for the accepted attempt, the noise key and the zero tail, else max |got - fp32(ref)| / (one fp32 ulp) over
+        columns 0..24."""
+        import numpy as np
+        g = got.cpu().numpy()
+        if not (np.array_equal(g[:, 26], ref[:, 26]) and np.array_equal(g[:, 25].view(np.uint32).astype(np.float64), ref[:, 25])
+                and not g[:, 27:].any()):
+            return float('inf')
+        r32 = ref[:, :25].astype(np.float32)
+        ulp = np.spacing(np.abs(r32)).astype(np.float64)
+        return float((np.abs(g[:, :25].astype(np.float64) - r32.astype(np.float64)) / ulp).max())
+
+    def _pre_flow_aug_params(self, a):
+        import flow_aug_ref as AR
+        B = a['B']
+        t = int(self.mem.view(a['step'], torch.int64, (1,)))
+        rg = self._aug_ranges(a['ranges']._obj)
+        ref = AR.params(rg, B, a['H'], a['W'], a['sample_offset'], t, a['seed'])
+        ctx = dict(ref=ref, t=t, dests=[(a['params'], torch.float32, B, _lib.FLOW_AUG_ROW, 0, _lib.FLOW_AUG_ROW)])
+        if self.controls is not None and t >= 1:
+            ctx['bad'] = AR.params(rg, B, a['H'], a['W'], a['sample_offset'], 0, a['seed'])
+        return ctx
+
+    def _post_flow_aug_params(self, a, ctx):
+        got = self.mem.view(a['params'], torch.float32, (a['B'], _lib.FLOW_AUG_ROW))
+        self._rec('cis_flow_aug_params', 'parameter rows (fp32 ulps)', self._aug_rows_ratio(got, ctx['ref']))
+        if 'bad' in ctx:
+            self._control('aug_params.step_frozen', self._aug_rows_ratio(got, ctx['bad']))
+
+    def _pre_flow_augment(self, a):
+        import flow_aug_ref as AR
+        B, H, W = a['B'], a['H'], a['W']
+        src = [self.mem.view(a[k], torch.float32, (B, H, W, c)).clone() for k, c in (('img1', 3), ('img2', 3), ('gt', 2))]
+        table = self.mem.view(a['params'], torch.float32, (B, _lib.FLOW_AUG_ROW)).clone()
+        P = AR.table_rows(table.cpu().numpy())
+        host = [s.cpu().numpy().astype('float64') for s in src]
+        ref = AR.augment(*host, P)
+        tol = [AR.tolerances(host[0][b], host[1][b], host[2][b], P[b]) for b in range(B)]
+        ctx = dict(ref=ref, tol=tol, reads=src + [table], dests=[(a[k], torch.float32, B * H * W, c, 0, c)
+                                                                 for k, c in (('img1_out', 3), ('img2_out', 3), ('gt_out', 2))])
+        if self.controls is not None:
+            # the flow resampled at T1 but not passed through T2^-1: p2 = q + (u, v)
+            import numpy as np
+            y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing='ij')
+            bad = np.empty_like(host[2])
+            for b in range(B):
+                q1x, q1y = AR.apply(P[b][0:6], x, y)
+                gq = AR.bilinear(host[2][b], q1x, q1y)
+                bad[b] = np.stack([y - (q1y - gq[..., 0]), x - (q1x - gq[..., 1])], -1)
+            ctx['bad'] = bad
+        return ctx
+
+    def _post_flow_augment(self, a, ctx):
+        import numpy as np
+        B, H, W = a['B'], a['H'], a['W']
+        got = [self.mem.view(a[k], torch.float32, (B, H, W, c)).cpu().numpy().astype(np.float64)
+               for k, c in (('img1_out', 3), ('img2_out', 3), ('gt_out', 2))]
+        for f, what in enumerate(('frame 1', 'frame 2', 'flow')):
+            r = 0.0
+            for b in range(B):
+                if not np.isfinite(got[f][b]).all():
+                    r = float('inf')
+                    break
+                r = max(r, float((np.abs(got[f][b] - ctx['ref'][f][b]) / ctx['tol'][b][f]).max()))
+            self._rec('cis_flow_augment', what, r)
+        if 'bad' in ctx:
+            self._control('augment.flow_unmapped', max(float((np.abs(got[2][b] - ctx['bad'][b]) / ctx['tol'][b][2]).max())
+                                                       for b in range(B)))
+
+    # ---- unsupervised census + smoothness loss and its backward
+    def _unsup_read(self, a):
+        B, H, W = a['B'], a['H'], a['W']
+        flow = self.mem.view(a['flow'], torch.float32, (2 * B, H, W, 2)).clone()
+        i1 = self.mem.view(a['img1'], torch.float32, (B, H, W, 3)).clone()
+        i2 = self.mem.view(a['img2'], torch.float32, (B, H, W, 3)).clone()
+        return flow, i1, i2
+
+    def _pre_unsup_flow_loss(self, a):
+        import unsup_flow_loss_ref as UR
+        B, H, W = a['B'], a['H'], a['W']
+        N = 2 * B
+        flow, i1, i2 = self._unsup_read(a)
+        fd = flow.double()
+        S, T = UR.directions(i1.double(), i2.double())
+        gT = UR.gray(T)
+        M, V, lhs, rhs = UR.mask(fd)
+        # the occlusion test in fp32: the partner flow h sampled at q (lerps 2^-21 sum |corners|, alpha rounded to fp32), s = f + h
+        sp = _unsup_sample(UR.partner(fd), fd)
+        h = sp['val']
+        eh = 2.0 ** -20 * sp['abs']
+        s = fd + h
+        e_lhs = (2 * s.abs() * (eh + U23 * s.abs()) + eh * eh).sum(-1) + 3 * U23 * lhs
+        e_rhs = (0.01 * (2 * h.abs() * eh + eh * eh)).sum(-1) + abs(float(_f32(0.01)) - 0.01) * ((fd * fd).sum(-1) + (h * h).sum(-1)) \
+            + 6 * U23 * rhs
+        amb = (lhs - rhs).abs() <= 2 * (e_lhs + e_rhs)
+        # T~: lerps of fp32 gray levels (each rounded from double) with fp32 alphas
+        st = _unsup_sample(gT.unsqueeze(-1), fd)
+        ctx = dict(M=M, V=V, amb=amb, warped=st['val'][..., 0], e_warped=2.0 ** -20 * st['abs'][..., 0], S=S, fd=fd,
+                   reads=[flow, i1, i2], dests=[(a[k], torch.float32, N, H * W, 0, H * W) for k in ('warped', 'mask', 'coef')] +
+                   [(a['scratch'], torch.float64, N, 128, 0, 128), (a['out'], torch.float64, N, 2, 0, 2)])
+        ctx['smooth'] = _unsup_smooth_terms(fd, S)
+        return ctx
+
+    def _post_unsup_flow_loss(self, a, ctx):
+        import unsup_flow_loss_ref as UR
+        B, H, W = a['B'], a['H'], a['W']
+        N = 2 * B
+        got_w = self.mem.view(a['warped'], torch.float32, (N, H, W))
+        got_m = self.mem.view(a['mask'], torch.float32, (N, H, W)).double()
+        got_k = self.mem.view(a['coef'], torch.float32, (N, H, W))
+        got_s = self.mem.view(a['out'], torch.float64, (N, 2))
+        self._rec('cis_unsup_flow_loss', 'warped frame', ratio(got_w, ctx['warped'], ctx['e_warped']))
+        # the mask: the fp64 one except where the occlusion test is within its epsilon (the border test is exact: q is formed in
+        # double from the fp32 flow on both sides)
+        wrong = (got_m != ctx['M']) & ~ctx['amb']
+        self._rec('cis_unsup_flow_loss', 'mask', 0.0 if not bool(wrong.any()) and bool(((got_m == 0) | (got_m == 1)).all()) else float('inf'))
+        self.unsup_mask = dict(differ=int((got_m != ctx['M']).sum()), near=int(ctx['amb'].sum()), pixels=got_m.numel(),
+                               out=int((ctx['V'] == 0).sum()), occluded=int(((ctx['V'] == 1) & (ctx['M'] == 0)).sum()))
+        m = torch.where(ctx['amb'], got_m, ctx['M'])
+        cen = _census_bound(UR.gray(ctx['S']), got_w.double())
+        c, e_c = cen['c'], cen['e']
+
+        def photo(mm):
+            # psi = powf(c + 0.01f, 0.4f) and k = 0.4f powf(c + 0.01f, -0.6f): the perturbation Dc of c + 0.01 (the census bound, the
+            # fp32 add and the constant 0.01f), the exponents' fp32 constants, powf's 4 ulp and the product's rounding
+            Dc = e_c + U23 * (c + 0.01) + abs(float(_f32(0.01)) - 0.01)
+            cl = torch.clamp(c - Dc, min=0) + 0.01
+            lg = (c + 0.01).log().abs()
+            psi = (c + 0.01) ** 0.4
+            e_psi = 0.4 * cl ** -0.6 * Dc + psi * (lg * abs(float(_f32(0.4)) - 0.4) + 4 * U23)
+            k = 0.4 * (c + 0.01) ** -0.6
+            e_k = 0.24 * cl ** -1.6 * Dc + k * (lg * abs(float(_f32(-0.6)) + 0.6) + 4 * U23 + abs(float(_f32(0.4)) - 0.4) / 0.4 + U23)
+            return mm * psi, mm * e_psi, mm * k, mm * e_k
+        P, eP, K, eK = photo(m)
+        self._rec('cis_unsup_flow_loss', 'coef', ratio(got_k, K, eK))
+        sm = ctx['smooth']
+        hw = H * W
+        ref = torch.stack([P.sum((1, 2)), sm['val'].sum((1, 2))], 1)
+        err = torch.stack([eP.sum((1, 2)) + (hw + 128) * 2.0 ** -53 * P.sum((1, 2)),
+                           sm['err'].sum((1, 2)) + (2 * hw + 128) * 2.0 ** -53 * sm['val'].sum((1, 2))], 1)
+        self._rec('cis_unsup_flow_loss', 'direction sums', ratio(got_s, ref, err))
+        if self.controls is not None:
+            P1, _, K1, _ = photo(torch.ones_like(m))
+            bad = torch.stack([P1.sum((1, 2)), sm['val'].sum((1, 2))], 1)
+            self._control('unsup.mask_ones', max(ratio(got_s, bad, err), ratio(got_k, K1, eK)))
+
+    def _pre_unsup_flow_loss_bwd(self, a):
+        B, H, W = a['B'], a['H'], a['W']
+        N = 2 * B
+        flow, i1, i2 = self._unsup_read(a)
+        warped = self.mem.view(a['warped'], torch.float32, (N, H, W)).clone()
+        coef = self.mem.view(a['coef'], torch.float32, (N, H, W)).clone()
+        wp, ws = float(_f32(a['w_photo'])), float(_f32(a['w_smooth']))
+        r = unsup_bwd_gather(flow.double(), i1.double(), i2.double(), warped.double(), coef.double(), wp, ws, bounds=True)
+        return dict(r=r, reads=[flow, i1, i2, warped, coef], dests=[(a['dflow'], torch.float32, N * H * W, 2, 0, 2)])
+
+    def _post_unsup_flow_loss_bwd(self, a, ctx):
+        got = self.mem.view(a['dflow'], torch.float32, (2 * a['B'], a['H'], a['W'], 2))
+        r = ctx['r']
+        self._rec('cis_unsup_flow_loss_bwd', 'dflow', ratio(got, r['ref'], r['err']))
+        if self.controls is not None:
+            self._control('unsup_bwd.smooth_dropped', ratio(got, r['photo'], r['err']))
 
     # ---- summary
     def summary(self):

@@ -20,7 +20,6 @@ from unsupervised_detection_b200.flow_train_graph import AUG_SEED, FlowTrainGrap
 from unsupervised_detection_b200.params_init import init_pwcnet  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
-EPS = 2.0 ** -24
 
 
 def _st():
@@ -77,16 +76,6 @@ def _frames(B, H, W, seed):
             _smooth(B, H, W, 2, 6.0, seed + 2))
 
 
-def _lip(a):
-    """max |difference| between neighbouring pixels of a [H, W, C] field: its Lipschitz bound per pixel of the bilinear sample."""
-    return max(float(np.abs(np.diff(a, axis=0)).max()), float(np.abs(np.diff(a, axis=1)).max()))
-
-
-def _pos_err(m, H, W):
-    """bound on the fp32 error of r0 x + r1 y + r2 (and the second row) over the grid"""
-    return 4 * EPS * max(abs(m[0]) * W + abs(m[1]) * H + abs(m[2]), abs(m[3]) * W + abs(m[4]) * H + abs(m[5]))
-
-
 def _check_pass(img1, img2, gt, table):
     B, H, W = gt.shape[:3]
     got = _augment(img1.cuda(), img2.cuda(), gt.cuda(), table)
@@ -95,29 +84,11 @@ def _check_pass(img1, img2, gt, table):
     ref = AR.augment(a1, a2, g, P)
     worst = [0.0, 0.0, 0.0]
     for b in range(B):
-        r = P[b]
-        y, x = np.meshgrid(np.arange(H, dtype=np.float64), np.arange(W, dtype=np.float64), indexing='ij')
-        for f, (src, m) in enumerate(((a1[b], r[0:6]), (a2[b], r[6:12]))):
-            # the sample moves by at most 2 * position error * Lipschitz bound; the affine part of the chain scales it by m_c (1 + kappa),
-            # gamma maps the interval around the pre-gamma value; fp32 arithmetic adds a few ulps of 1
-            qx, qy = AR.apply(m, x, y)
-            s = AR.bilinear(src, qx, qy)
-            pre = 0.5 + r[21] * ((s + 0.5) * r[18:21] - 0.5) + r[22]
-            e = np.abs(r[21] * r[18:21]) * 2 * _pos_err(m, H, W) * _lip(src) + 1e-6
-            g_ = lambda v: np.clip(v, 0, 1) ** r[23]  # noqa: E731
-            tol = g_(pre + e) - g_(pre - e) + 8e-6
+        tols = AR.tolerances(a1[b], a2[b], g[b], P[b])
+        for f in range(3):
             d = np.abs(got[f][b] - ref[f][b])
-            assert (d <= tol).all(), (b, f, float(d.max()))
-            worst[f] = max(worst[f], float((d / tol).max()))
-        # flow: q moves by dq; gt at q by 2 dq Lip(gt); T2^-1 scales the sum by its row norm and adds its own rounding; then - p
-        dq = _pos_err(r[0:6], H, W)
-        s_max = float(max(W, H) + np.abs(g[b]).max())
-        inv = r[12:18]
-        row = max(abs(inv[0]) + abs(inv[1]), abs(inv[3]) + abs(inv[4]))
-        tol = row * (dq + 2 * dq * _lip(g[b]) + 4 * EPS * s_max) + 4 * EPS * (row * s_max + max(abs(inv[2]), abs(inv[5]))) + 2 * EPS * max(W, H)
-        d = np.abs(got[2][b] - ref[2][b])
-        assert (d <= tol).all(), (b, float(d.max()), tol)
-        worst[2] = max(worst[2], float(d.max() / tol))
+            assert (d <= tols[f]).all(), (b, f, float(d.max()))
+            worst[f] = max(worst[f], float((d / tols[f]).max()))
     return worst
 
 
