@@ -133,17 +133,26 @@ class AdversarialLearner(object):
         self.device = 'cuda:%d' % self.local_rank
         torch.cuda.set_device(self.local_rank)
 
+    def _init_training_ranks(self):
+        """_init_dist, then local_batch = this rank's share of the global batch_size; ValueError when the ranks cannot share it evenly."""
+        self._init_dist()
+        if self.config.batch_size % self.world:
+            raise ValueError('batch_size must be divisible by the number of ranks')
+        self.local_batch = self.config.batch_size // self.world
+
+    def _cis_graph(self, **kw):
+        """CISGraph at img_height x img_width on local_batch frame pairs, with PWC-Net's default options; kw = the graph's own arguments."""
+        cfg = self.config
+        return CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
+                        with_pwc=True, pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, **kw)
+
     def build_train_graph(self):
         """adversarial_learner.py:72-258: PWC-Net -> resize -> generator -> 3x recover -> losses -> two train ops."""
         cfg = self.config
-        self._init_dist()
-        if cfg.batch_size % self.world:
-            raise ValueError('batch_size must be divisible by the number of ranks')
-        self.local_batch = cfg.batch_size // self.world
+        self._init_training_ranks()
         self.load_training_data()
-        self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
-                              flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
-                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
+        self.graph = self._cis_graph(global_batch=cfg.batch_size, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, train=True,
+                                     masks='generator', flow_source=self._flow_source())
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self.val_steps_per_epoch = int(np.ceil(float(self.num_samples_val) / cfg.batch_size))
         self._init_params()
@@ -232,27 +241,24 @@ class AdversarialLearner(object):
         tf.train.Saver V2 bundle (`model-<step>.index` + `.data-00000-of-00001` + the `checkpoint` state file, trainables +
         global_step, no Adam slots, max_to_keep=40 :327) that the reference itself can restore, plus the same tensors as a
         native torch file."""
-        if self.rank != 0:
-            return
-        base = 'model.best' if step == 'best' else 'model-%s' % step
-        print(" [*] Saving checkpoint to {}/model-{}".format(checkpoint_dir, step))
-        params = {k: v.cpu() for k, v in self.graph.export_params().items()}
-        self._write_checkpoint(checkpoint_dir, base, params, self.global_step)
+        self._write_checkpoint(checkpoint_dir, 'model.best' if step == 'best' else 'model-%s' % step, self.graph.export_params,
+                               self.global_step, "checkpoint to {}/model-{}".format(checkpoint_dir, step))
 
     def save_recover(self, checkpoint_dir, epoch):
         """The recover net alone, as the reference's recover_saver covers it (adversarial_learner.py:329): `recover-<epoch>` as a TF V2
         bundle of the FlownetS variables (no global_step, no Adam slots) plus the same tensors as a native `.pt`, and the `checkpoint`
         state file.  train.py --recover_ckpt=<dir>/recover-<epoch> and a TF recover_saver.restore both read it.  epoch='best' writes
         recover-best (the lowest validation EPE so far), which later saves never delete."""
+        base = 'recover-%s' % epoch
+        self._write_checkpoint(checkpoint_dir, base, self.graph.rec_store.export, None, "recover net to {}/{}".format(checkpoint_dir, base))
+
+    def _write_checkpoint(self, checkpoint_dir, base, export, bundle_step, what):
+        """On rank 0 only: prints ' [*] Saving <what>' and writes host copies of the tensors export() returns as <base>.pt + the <base>
+        bundle (global_step in the bundle when bundle_step is not None); old entries beyond max_to_keep=40 go."""
         if self.rank != 0:
             return
-        base = 'recover-%s' % epoch
-        print(" [*] Saving recover net to {}/{}".format(checkpoint_dir, base))
-        params = {k: v.cpu() for k, v in self.graph.rec_store.export().items()}
-        self._write_checkpoint(checkpoint_dir, base, params, None)
-
-    def _write_checkpoint(self, checkpoint_dir, base, params, bundle_step):
-        """<base>.pt + the <base> bundle (global_step in the bundle when bundle_step is not None); old entries beyond max_to_keep=40 go."""
+        print(" [*] Saving " + what)
+        params = {k: v.cpu() for k, v in export().items()}
         os.makedirs(checkpoint_dir, exist_ok=True)
         torch.save({'params': params, 'global_step': self.global_step}, os.path.join(checkpoint_dir, base + '.pt'))
         ckpt_io.write_bundle(os.path.join(checkpoint_dir, base), ckpt_io.export_params(params, bundle_step))
@@ -384,40 +390,80 @@ class AdversarialLearner(object):
                 w.add_histogram(ckpt_io.to_tf_name(name) + "/gradients", gv)
         w.flush_step(gs)
 
-    def train(self, config):
-        """adversarial_learner.py:312-420."""
-        self.config = config
-        self.build_train_graph()
-        self.min_val_iou = -1.0e12
+    def _epoch_loop(self, header, step, progress, epoch_end, banner):
+        """The training loop of train, pretrain_recover and train_flow.  Rank 0 prints the two `header` lines between rules and the event
+        file opens (collect_summaries).  Then train_steps_per_epoch (num_samples_train / batch_size) steps per epoch for max_epochs
+        epochs: every step consumes one reader batch, in order, and hands the next one over for the overlapped host -> device copy,
+        step(batch, next_batch, fetch) -> result.  fetch is True every summary_freq steps (the same decision on every rank); then rank 0
+        prints 'Epoch: [e] [s/steps] time: t/it ' + text and writes the scalars, if any, at the result's global_step, where
+        progress(result) -> (text, {tag: scalar}).  Each epoch ends with epoch_end(epoch); after the last one rank 0 prints `banner`
+        between rules and the loop returns."""
+        cfg, steps_per_epoch = self.config, self.train_steps_per_epoch
         if self.rank == 0:
-            print("Number of params: {}".format(self.graph.param_count()))
-            print("-------------------------------------")
-            print("Training {} Recover and {} Generator".format(config.iters_rec, config.iters_gen))
-            print("-------------------------------------")
-        self.collect_summaries()
+            for line in header:
+                print(line)
+                print("-------------------------------------")
+        w = self.collect_summaries()
         batch = self.reader.batch(self.local_batch)
-        for step in count(start=1):
+        for k in count(start=1):
             start_time = time.time()
             # the next batch (already decoded by the reader's background prefetch) is copied to the device on the side stream while this
             # step computes -- the same step(batch, next_batch=...) pattern bench.py's end-to-end arm measures
             nxt = self.reader.batch(self.local_batch)
-            results = self.step(batch, summarize=True, next_batch=nxt)
+            fetch = k % cfg.summary_freq == 0
+            res = step(batch, nxt, fetch)
             batch = nxt
-            if step % config.summary_freq == 0 and self.rank == 0:
-                train_epoch = math.ceil(step / self.train_steps_per_epoch)
-                train_step = step - (train_epoch - 1) * self.train_steps_per_epoch
-                print("Epoch: [%2d] [%5d/%5d] time: %4.4f/it loss_generator: %4.4f loss_recover %4.4f"
-                      % (train_epoch, train_step, self.train_steps_per_epoch, time.time() - start_time,
-                         results["loss_generator"], results["loss_recover"]))
-            if step % self.train_steps_per_epoch == 0:
-                train_epoch = int(step / self.train_steps_per_epoch)
-                self.epoch_end_callback(None, None, train_epoch)
-                if train_epoch == self.config.max_epochs:
+            if fetch and self.rank == 0:
+                epoch = math.ceil(k / steps_per_epoch)
+                text, scalars = progress(res)
+                print("Epoch: [%2d] [%5d/%5d] time: %4.4f/it %s"
+                      % (epoch, k - (epoch - 1) * steps_per_epoch, steps_per_epoch, time.time() - start_time, text))
+                if w is not None and scalars:
+                    for tag, v in scalars.items():
+                        w.add_scalar(tag, v)
+                    w.flush_step(res["global_step"])
+            if k % steps_per_epoch == 0:
+                epoch = k // steps_per_epoch
+                epoch_end(epoch)
+                if epoch == cfg.max_epochs:
                     if self.rank == 0:
                         print("-------------------------------")
-                        print("Training completed successfully")
+                        print(banner)
                         print("-------------------------------")
-                    break
+                    return
+
+    def _save_and_validate(self, epoch, save, validate):
+        """The epoch end of pretrain_recover and train_flow: save(checkpoint_dir, epoch) every save_freq epochs and after the last one.
+        Then, with config.validate, validate() -> (value, text, tag), lower is better: rank 0 prints 'Epoch [e] ' + text and writes
+        value under tag at step epoch, and save(checkpoint_dir, 'best') runs whenever value is strictly below min_val_epe."""
+        cfg = self.config
+        if epoch % cfg.save_freq == 0 or epoch == cfg.max_epochs:
+            save(cfg.checkpoint_dir, epoch)
+        if not getattr(cfg, 'validate', False):
+            return
+        value, text, tag = validate()
+        if self.rank == 0:
+            print("Epoch [{}] {}".format(epoch, text))
+            if self.summary_writer is not None:
+                self.summary_writer.add_scalar(tag, value)
+                self.summary_writer.flush_step(epoch)
+        if value < self.min_val_epe:                # the same all-reduced value on every rank
+            self.min_val_epe = value
+            save(cfg.checkpoint_dir, 'best')
+
+    def train(self, config):
+        """adversarial_learner.py:312-420 in _epoch_loop.  step() decides for itself when to fetch the losses and writes its summaries;
+        every epoch ends with epoch_end_callback, which saves model-<epoch> every save_freq epochs (not after the last one)."""
+        self.config = config
+        self.build_train_graph()
+        self.min_val_iou = -1.0e12
+        self._epoch_loop(
+            header=("Number of params: {}".format(self.graph.param_count()),
+                    "Training {} Recover and {} Generator".format(config.iters_rec, config.iters_gen)),
+            step=lambda batch, nxt, fetch: self.step(batch, summarize=True, next_batch=nxt),
+            progress=lambda r: ("loss_generator: %4.4f loss_recover %4.4f" % (r["loss_generator"], r["loss_recover"]), {}),
+            epoch_end=lambda epoch: self.epoch_end_callback(None, None, epoch),
+            banner="Training completed successfully")
 
     def epoch_end_callback(self, sess, sv, epoch_num):
         """adversarial_learner.py:422-448: validation IoU, save best / every save_freq epochs."""
@@ -431,10 +477,10 @@ class AdversarialLearner(object):
             masks = self.graph.mask.cpu().numpy()
             gtr = torch.nn.functional.interpolate(gt.permute(0, 3, 1, 2), size=masks.shape[1:3], mode='nearest').permute(0, 2, 3, 1).numpy()
             validation_iou += float(np.sum(compute_all_IoU(masks, gtr)))
-        d = _dist()
-        if d is not None and self.world > 1:
+        ar = self._allreduce()
+        if ar is not None:
             t = torch.tensor([validation_iou], device=self.device)
-            d.all_reduce(t)
+            ar(t)
             validation_iou = float(t)
         validation_iou /= self.val_steps_per_epoch * self.config.batch_size
         if self.rank == 0:
@@ -457,10 +503,7 @@ class AdversarialLearner(object):
         dataset's ground-truth flow, FLYINGCHAIRS, or the supplied flow of a mask dataset with config.flow_dir: no PWC-Net is built and
         --flow_ckpt is not read)."""
         cfg = self.config
-        self._init_dist()
-        if cfg.batch_size % self.world:
-            raise ValueError('batch_size must be divisible by the number of ranks')
-        self.local_batch = cfg.batch_size // self.world
+        self._init_training_ranks()
         box = box_sides(getattr(cfg, 'box_min', 0.1), getattr(cfg, 'box_max', 0.5), cfg.img_height, cfg.img_width)
         gt = getattr(cfg, 'pretrain_flow', 'pwc') == 'gt'
         if gt and not has_flow(cfg.dataset, self.flow_dir()):
@@ -471,10 +514,9 @@ class AdversarialLearner(object):
         self._pretrain = True
         self.load_training_data()
         # sample_offset: sample b of rank r is global sample r * local_batch + b, so a DP job draws the boxes of one GPU running the global batch
-        self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
-                              flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, with_pwc=True, train=True,
-                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='boxes', box=box,
-                              sample_offset=self.rank * self.local_batch, flow_source='input' if gt else 'pwc')
+        self.graph = self._cis_graph(global_batch=cfg.batch_size, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, train=True,
+                                     masks='boxes', box=box, sample_offset=self.rank * self.local_batch,
+                                     flow_source='input' if gt else 'pwc')
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self._init_params()
 
@@ -503,61 +545,50 @@ class AdversarialLearner(object):
 
     def pretrain_recover(self, config):
         """Pretrains the recover net (scope FlownetS) to inpaint optical flow under box-shaped occlusions, the pre-training the reference's
-        README describes for --recover_ckpt.  num_samples_train / batch_size steps per epoch for max_epochs epochs; every summary_freq
-        steps rank 0 prints the loss and writes the scalars recover / reconstruction_loss / reconstruction_compl_loss; every save_freq
-        epochs and after the last one it saves recover-<epoch> (save_recover).  --flow_ckpt is mandatory unless pretrain_flow=gt,
-        --recover_ckpt gives the starting weights (else the reference's initialisation).  config.validate: at every epoch end,
-        validate_recover() on the val split; rank 0 prints and logs the EPE inside the boxes, and recover-best is saved whenever it
-        improves."""
+        README describes for --recover_ckpt, in _epoch_loop: the scalars are recover / reconstruction_loss / reconstruction_compl_loss,
+        the checkpoints recover-<epoch> (save_recover), and with config.validate every epoch ends with validate_recover() on the val
+        split, logged as the EPE inside the boxes and kept at its lowest in recover-best.  --flow_ckpt is mandatory unless
+        pretrain_flow=gt, --recover_ckpt gives the starting weights (else the reference's initialisation)."""
         self.config = config
         self.build_pretrain_graph()
-        if self.rank == 0:
-            print("Number of recover params: {}".format(self.graph.rec_store.real_count()))
-            print("-------------------------------------")
-            print("Pretraining Recover on box masks, sides {} px (h lo, h hi, w lo, w hi)".format(self.graph.box))
-            print("-------------------------------------")
-        w = self.collect_summaries()
-        steps_per_epoch = self.train_steps_per_epoch
-        batch = self.reader.batch(self.local_batch)
-        for step in count(start=1):
-            start_time = time.time()
-            nxt = self.reader.batch(self.local_batch)
-            fetch = step % config.summary_freq == 0
-            results = self.pretrain_step(batch, next_batch=nxt, fetch_losses=fetch)
-            batch = nxt
-            if fetch and self.rank == 0:
-                epoch = math.ceil(step / steps_per_epoch)
-                print("Epoch: [%2d] [%5d/%5d] time: %4.4f/it loss_recover %4.4f"
-                      % (epoch, step - (epoch - 1) * steps_per_epoch, steps_per_epoch, time.time() - start_time, results["loss_recover"]))
-                if w is not None:
-                    w.add_scalar("recover", results["loss_recover"])
-                    w.add_scalar("reconstruction_loss", results["reconstruction_loss"])
-                    w.add_scalar("reconstruction_compl_loss", results["reconstruction_compl_loss"])
-                    w.flush_step(results["global_step"])
-            if step % steps_per_epoch == 0:
-                epoch = step // steps_per_epoch
-                last = epoch == config.max_epochs
-                if epoch % config.save_freq == 0 or last:
-                    self.save_recover(config.checkpoint_dir, epoch)
-                if getattr(config, 'validate', False):
-                    self._validation_epoch_end(epoch)
-                if last:
-                    if self.rank == 0:
-                        print("-------------------------------")
-                        print("Pretraining completed successfully")
-                        print("-------------------------------")
-                    break
 
-    def _validation_epoch_end(self, epoch):
-        epe, epe_out = self.validate_recover()
-        if self.rank == 0:
-            print("Epoch [{}] Validation EPE (boxes): {:.4f} (outside the boxes: {:.4f})".format(epoch, epe, epe_out))
-            if self.summary_writer is not None:
-                self.summary_writer.add_scalar("Validation EPE", epe)
-                self.summary_writer.flush_step(epoch)
-        if epe < self.min_val_epe:                  # the same all-reduced value on every rank
-            self.min_val_epe = epe
-            self.save_recover(self.config.checkpoint_dir, 'best')
+        def validate():
+            epe, epe_out = self.validate_recover()
+            return epe, "Validation EPE (boxes): {:.4f} (outside the boxes: {:.4f})".format(epe, epe_out), "Validation EPE"
+        self._epoch_loop(
+            header=("Number of recover params: {}".format(self.graph.rec_store.real_count()),
+                    "Pretraining Recover on box masks, sides {} px (h lo, h hi, w lo, w hi)".format(self.graph.box)),
+            step=lambda batch, nxt, fetch: self.pretrain_step(batch, next_batch=nxt, fetch_losses=fetch),
+            progress=lambda r: ("loss_recover %4.4f" % r["loss_recover"],
+                                {"recover": r["loss_recover"], "reconstruction_loss": r["reconstruction_loss"],
+                                 "reconstruction_compl_loss": r["reconstruction_compl_loss"]}),
+            epoch_end=lambda epoch: self._save_and_validate(epoch, self.save_recover, validate),
+            banner="Pretraining completed successfully")
+
+    def _val_sums(self, it, width, run, sums):
+        """One ordered pass over the num_samples_val pairs of a val split, sharded over ranks like the evaluation -> the `width` fp64
+        sums, added over the batches on the device and merged by one all-reduce, as a list.  it = the split's test_inputs at
+        batch_size; this rank reads local_batch pairs of each global batch, the first with global val index first = k * batch_size +
+        rank * local_batch, and closes the iterator at the end.  run(batch, first) feeds and forwards every batch, padding included;
+        sums(valid) -> the sums of the batch's first `valid` pairs is added only when valid > 0, so the pairs that only pad the last
+        global batch add nothing."""
+        n, GB, lb = self.num_samples_val, self.config.batch_size, self.local_batch
+        tot = torch.zeros(width, dtype=torch.float64, device=self.device)
+        it = it.shard(self.rank, self.world, GB)
+        try:
+            for k in range(-(-n // GB)):
+                batch = it.batch(lb)
+                first = k * GB + self.rank * lb
+                run(batch, first)
+                valid = min(lb, n - first)
+                if valid > 0:
+                    tot += sums(valid)
+        finally:
+            it.close()
+        ar = self._allreduce()
+        if ar is not None:
+            ar(tot)
+        return tot.tolist()
 
     def validate_recover(self):
         """Held-out inpainting error of the recover net -> (EPE inside the boxes, EPE outside them), means over the pixels of the val
@@ -567,31 +598,17 @@ class AdversarialLearner(object):
         pad the last global batch are left out) and merged by one all-reduce."""
         cfg, g = self.config, self.graph
         if self.val_graph is None:
-            self.val_graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, global_batch=cfg.batch_size,
-                                      flow_normalizer=cfg.flow_normalizer, cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False,
-                                      pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='boxes', box=g.box,
-                                      flow_source=g.flow_source)
+            self.val_graph = self._cis_graph(global_batch=cfg.batch_size, cbn=cfg.cbn, epsilon=cfg.epsilon, train=False, masks='boxes',
+                                             box=g.box, flow_source=g.flow_source)
         vg = self.val_graph
         vg.load_params(g.export_params())
-        n, GB, lb = self.num_samples_val, cfg.batch_size, self.local_batch
-        tot = torch.zeros(4, dtype=torch.float64, device=self.device)
-        it = self.dataset_reader.test_inputs(batch_size=GB).shard(self.rank, self.world, GB)     # a fresh ordered pass every call
-        try:
-            for k in range(-(-n // GB)):
-                batch = it.batch(lb)
-                first = k * GB + self.rank * lb
-                vg.set_sample_offset(first)
-                vg.feed(*self._uploads(batch))
-                vg.forward()
-                valid = min(lb, n - first)
-                if valid > 0:
-                    tot += vg.masked_epe()[:valid].sum(0)
-        finally:
-            it.close()
-        d = _dist()
-        if d is not None and self.world > 1:
-            d.all_reduce(tot)
-        s = tot.tolist()
+
+        def run(batch, first):
+            vg.set_sample_offset(first)
+            vg.feed(*self._uploads(batch))
+            vg.forward()
+        s = self._val_sums(self.dataset_reader.test_inputs(batch_size=cfg.batch_size), 4, run,     # a fresh ordered pass every call
+                           lambda valid: vg.masked_epe()[:valid].sum(0))
         return tuple(e / m * cfg.flow_normalizer if m else math.nan for e, m in ((s[0], s[2]), (s[1], s[3])))
 
     # ------------------------------------------------------------------------------------------------ inference
@@ -602,9 +619,7 @@ class AdversarialLearner(object):
         self.local_batch = cfg.batch_size
         self._inference = True
         self.load_training_data()
-        self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
-                              cbn=cfg.cbn, epsilon=cfg.epsilon, with_pwc=True, train=False,
-                              pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
+        self.graph = self._cis_graph(cbn=cfg.cbn, epsilon=cfg.epsilon, train=False, masks='generator', flow_source=self._flow_source())
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 
@@ -612,13 +627,11 @@ class AdversarialLearner(object):
         """adversarial_learner.py:525-592: multi-crop ensemble, batch 1 per crop (the four crops are batched here)."""
         self.test_crops = [0.85, 0.9, 0.95, 1.0]
         print("Evaluating the following crops {}".format(self.test_crops))
-        cfg = self.config
         self._init_dist()
         self.local_batch = len(self.test_crops)
         self._inference = True
         self.load_training_data()
-        self.graph = CISGraph(cfg.img_height, cfg.img_width, self.local_batch, device=self.device, flow_normalizer=cfg.flow_normalizer,
-                              with_pwc=True, train=False, pwc_options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, masks='generator', flow_source=self._flow_source())
+        self.graph = self._cis_graph(train=False, masks='generator', flow_source=self._flow_source())
         self.test_samples = self.reader.val_samples
         self.test_iterator = self.reader
 

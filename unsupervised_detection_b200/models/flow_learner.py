@@ -3,16 +3,13 @@ DAVIS2016 / FBMS / SEGTRACK (or Flying Chairs) with the unsupervised loss (flow_
 that --flow_ckpt of train.py, test_generator*.py, pretrain_recover.py and export_flow.py read.
 
 It is AdversarialLearner's counterpart for the flow network: the same process setup (one process per GPU under torchrun, the global
-batch sharded over ranks, one NCCL all-reduce of the flat gradient per step), reader, summaries and checkpoint writer.  The PWC-Net option
+batch sharded over ranks, one NCCL all-reduce of the flat gradient per step), reader, training loop, sharded validation pass, summaries
+and checkpoint writer.  The PWC-Net option
 set is model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS, as for every other graph.
 """
 import math
-import time
-from itertools import count
 
-import torch
-
-from .adversarial_learner import AdversarialLearner, FLOW_DATASETS, MASK_DATASETS, _dist
+from .adversarial_learner import AdversarialLearner, FLOW_DATASETS, MASK_DATASETS
 from .PWCNet import model_pwcnet
 from .. import params_init
 from ..flow_train_graph import FlowTrainGraph
@@ -33,7 +30,6 @@ def learning_rate_at(step, base, boundaries):
 
 class FlowLearner(AdversarialLearner):
     _lr = None                                          # the rate last written to the graph
-    min_val_epe = math.inf
 
     def build_flow_graph(self):
         """FlowTrainGraph at img_height x img_width on the 384x640 batches (the frames are resized on the device; the supervised losses
@@ -46,10 +42,7 @@ class FlowLearner(AdversarialLearner):
         ok = FLOW_DATASETS + (MASK_DATASETS if loss == 'unsupervised' else ())
         if cfg.dataset not in ok:
             raise IOError('PWC-Net training with the %s loss needs a dataset in %s, got %s' % (loss, ', '.join(ok), cfg.dataset))
-        self._init_dist()
-        if cfg.batch_size % self.world:
-            raise ValueError('batch_size must be divisible by the number of ranks')
-        self.local_batch = cfg.batch_size // self.world
+        self._init_training_ranks()
         self._pretrain = True                           # load_training_data: Flying Chairs' train pairs
         self.load_training_data()
         self.graph = FlowTrainGraph(cfg.img_height, cfg.img_width, self.local_batch, options=model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS,
@@ -103,122 +96,58 @@ class FlowLearner(AdversarialLearner):
     def save_flow(self, checkpoint_dir, epoch):
         """`pwcnet-<epoch>`: a TF V2 bundle of the pwcnet/* variables only (no global_step, no Adam slots) plus the same tensors as a
         native `.pt`, and the `checkpoint` state file.  epoch='best' writes pwcnet-best (the lowest validation EPE so far)."""
-        if self.rank != 0:
-            return
         base = 'pwcnet-%s' % epoch
-        print(" [*] Saving PWC-Net to {}/{}".format(checkpoint_dir, base))
-        self._write_checkpoint(checkpoint_dir, base, {k: v.cpu() for k, v in self.graph.export_params().items()}, None)
+        self._write_checkpoint(checkpoint_dir, base, self.graph.export_params, None, "PWC-Net to {}/{}".format(checkpoint_dir, base))
 
     def train_flow(self, config):
-        """num_samples_train / batch_size steps per epoch for max_epochs epochs.  Every summary_freq steps rank 0 prints and writes
-        the FlowTrainGraph.losses() terms (flow_loss and its parts); every save_freq epochs and after the last one it saves pwcnet-<epoch>.
-        With config.validate every epoch ends with a validation: on Flying Chairs validate_flow(), rank 0 prints and writes
-        `Validation EPE (flow)`; on a mask dataset validate_unsup(), `Validation unsupervised flow loss`.  pwcnet-best is saved whenever
-        the value improves."""
+        """PWC-Net training in _epoch_loop: the scalars are the FlowTrainGraph.losses() terms (flow_loss and its parts), the checkpoints
+        pwcnet-<epoch> (save_flow).  With config.validate every epoch ends with a validation kept at its lowest in pwcnet-best: on Flying
+        Chairs validate_flow(), logged as `Validation EPE (flow)`; on a mask dataset validate_unsup(), `Validation unsupervised flow
+        loss`."""
         self.config = config
         self.build_flow_graph()
         g = self.graph
-        if self.rank == 0:
-            print("Number of PWC-Net params: {}".format(g.store.real_count()))
-            print("-------------------------------------")
-            print("Training PWC-Net ({} loss) on {}x{}, options {}".format(g.loss, g.H, g.W, dict(g.options._asdict())))
-            print("-------------------------------------")
-        w = self.collect_summaries()
-        steps_per_epoch = self.train_steps_per_epoch
-        batch = self.reader.batch(self.local_batch)
-        for step in count(start=1):
-            start_time = time.time()
-            nxt = self.reader.batch(self.local_batch)
-            fetch = step % config.summary_freq == 0
-            res = self.flow_step(batch, next_batch=nxt, fetch_losses=fetch)
-            batch = nxt
-            if fetch and self.rank == 0:
-                epoch = math.ceil(step / steps_per_epoch)
-                print("Epoch: [%2d] [%5d/%5d] time: %4.4f/it flow_loss %4.4f"
-                      % (epoch, step - (epoch - 1) * steps_per_epoch, steps_per_epoch, time.time() - start_time, res['flow_loss']))
-                if w is not None:
-                    for k in SUMMARY_KEYS[g.loss]:
-                        w.add_scalar(k, res[k])
-                    w.flush_step(res['global_step'])
-            if step % steps_per_epoch == 0:
-                epoch = step // steps_per_epoch
-                last = epoch == config.max_epochs
-                if epoch % config.save_freq == 0 or last:
-                    self.save_flow(config.checkpoint_dir, epoch)
-                if getattr(config, 'validate', False):
-                    self._flow_validation_epoch_end(epoch)
-                if last:
-                    if self.rank == 0:
-                        print("-------------------------------")
-                        print("Training completed successfully")
-                        print("-------------------------------")
-                    break
 
-    def _flow_validation_epoch_end(self, epoch):
-        if self.config.dataset in FLOW_DATASETS:
-            tag, val = "Validation EPE (flow)", self.validate_flow()
-        else:
-            tag, val = "Validation unsupervised flow loss", self.validate_unsup()
-        if self.rank == 0:
-            print("Epoch [{}] {}: {:.4f}".format(epoch, tag, val))
-            if self.summary_writer is not None:
-                self.summary_writer.add_scalar(tag, val)
-                self.summary_writer.flush_step(epoch)
-        if val < self.min_val_epe:                  # the same all-reduced value on every rank
-            self.min_val_epe = val
-            self.save_flow(self.config.checkpoint_dir, 'best')
+        def validate():
+            if config.dataset in FLOW_DATASETS:
+                tag, val = "Validation EPE (flow)", self.validate_flow()
+            else:
+                tag, val = "Validation unsupervised flow loss", self.validate_unsup()
+            return val, "{}: {:.4f}".format(tag, val), tag
+        self._epoch_loop(
+            header=("Number of PWC-Net params: {}".format(g.store.real_count()),
+                    "Training PWC-Net ({} loss) on {}x{}, options {}".format(g.loss, g.H, g.W, dict(g.options._asdict()))),
+            step=lambda batch, nxt, fetch: self.flow_step(batch, next_batch=nxt, fetch_losses=fetch),
+            progress=lambda r: ("flow_loss %4.4f" % r['flow_loss'], {k: r[k] for k in SUMMARY_KEYS[g.loss]}),
+            epoch_end=lambda epoch: self._save_and_validate(epoch, self.save_flow, validate),
+            banner="Training completed successfully")
 
     def validate_unsup(self):
         """The unsupervised objective on the val partition of a mask dataset -> the mean over its frame pairs of the pair's two
-        directions' P + lambda_s * Sm (FlowTrainGraph.direction_objective).  The training graph's forward runs the val pairs in order
-        (test_inputs at --test_temporal_shift and --test_crop), sharded over ranks like the evaluation; the sums are added on the device
-        (pairs that only pad the last global batch are left out) and merged by one all-reduce."""
-        g, cfg = self.graph, self.config
-        n, GB, lb = self.num_samples_val, cfg.batch_size, self.local_batch
-        tot = torch.zeros(2, dtype=torch.float64, device=self.device)
-        it = self.dataset_reader.test_inputs(batch_size=GB, t_len=cfg.test_temporal_shift, test_crop=cfg.test_crop,
-                                             partition='val').shard(self.rank, self.world, GB)
-        try:
-            for k in range(-(-n // GB)):
-                batch = it.batch(lb)
-                first = k * GB + self.rank * lb
-                g.feed(batch[0], batch[1])
-                g.forward()
-                valid = min(lb, n - first)
-                if valid > 0:
-                    o = g.direction_objective()
-                    tot[0] += o[:valid].sum() + o[lb:lb + valid].sum()
-                    tot[1] += valid
-        finally:
-            it.close()
-        d = _dist()
-        if d is not None and self.world > 1:
-            d.all_reduce(tot)
-        s = tot.tolist()
-        return s[0] / s[1] if s[1] else math.nan
+        directions' P + lambda_s * Sm (FlowTrainGraph.direction_objective).  The training graph's forward runs the val pairs of
+        test_inputs at --test_temporal_shift and --test_crop in _val_sums."""
+        g, cfg, lb = self.graph, self.config, self.local_batch
+
+        def run(batch, first):
+            g.feed(batch[0], batch[1])
+            g.forward()
+
+        def sums(valid):
+            o = g.direction_objective()
+            return o[:valid].sum() + o[lb:lb + valid].sum()
+        it = self.dataset_reader.test_inputs(batch_size=cfg.batch_size, t_len=cfg.test_temporal_shift, test_crop=cfg.test_crop,
+                                             partition='val')
+        s = self._val_sums(it, 1, run, sums)
+        n = self.num_samples_val                        # _val_sums scores each val pair on exactly one rank
+        return s[0] / n if n else math.nan
 
     def validate_flow(self):
-        """End-point error of the final flow on the val split -> mean over its pixels, in pixels of the 384x640 grid.  The training
-        graph's forward runs the val pairs in order, sharded over ranks like the evaluation; the per-sample sums of FlowTrainGraph.epe
-        are added over the batches on the device (pairs that only pad the last global batch are left out) and merged by one
-        all-reduce."""
+        """End-point error of the final flow on the val split -> mean over its pixels, in pixels of the 384x640 grid: the per-sample sums
+        of FlowTrainGraph.epe after the training graph's forward, in _val_sums."""
         g = self.graph
-        n, GB, lb = self.num_samples_val, self.config.batch_size, self.local_batch
-        tot = torch.zeros(4, dtype=torch.float64, device=self.device)
-        it = self.dataset_reader.test_inputs(batch_size=GB).shard(self.rank, self.world, GB)
-        try:
-            for k in range(-(-n // GB)):
-                batch = it.batch(lb)
-                first = k * GB + self.rank * lb
-                g.feed(batch[0], batch[1], batch[2])
-                g.forward()
-                valid = min(lb, n - first)
-                if valid > 0:
-                    tot += g.epe()[:valid].sum(0)
-        finally:
-            it.close()
-        d = _dist()
-        if d is not None and self.world > 1:
-            d.all_reduce(tot)
-        s = tot.tolist()
+
+        def run(batch, first):
+            g.feed(batch[0], batch[1], batch[2])
+            g.forward()
+        s = self._val_sums(self.dataset_reader.test_inputs(batch_size=self.config.batch_size), 4, run, lambda valid: g.epe()[:valid].sum(0))
         return s[0] / s[2] if s[2] else math.nan
