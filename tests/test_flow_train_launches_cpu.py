@@ -10,9 +10,8 @@ BUILT on CPU tensors (nothing is launched) and checked for what the GPU walk rel
 Every op of the aug, fwd, bwd, adam and pack plans has exactly one owner, the glue and conv launch counts are pinned, and so are the
 arguments that motivate each graph, so that a builder change which silently stops exercising one of them fails here.  The ratchet: every
 entry point of the C ABI binding is owned by a per-launch check or listed in FUNCTION_LEVEL with the test file that checks it, and no
-plan of any graph of the three CPU launch-census files (this one, tests/test_glue_launches_cpu.py, tests/test_graph_variants_launches_cpu.py)
-launches a listed one.  The next kernel added to a step without a per-launch reference fails here."""
-import collections
+plan of any graph of the launch suites (tests/launch_suites.py GRAPHS) launches a listed one.  The next kernel added to a step without a
+per-launch reference fails here."""
 import os
 
 import pytest
@@ -21,38 +20,12 @@ import torch
 import conv_launch_ref as R
 import glue_launch_ref as G
 import unsup_flow_loss_ref as UR
+from launch_suites import CONV, FLOW_TRAIN, GLUE, GRAPHS, attributed, build
 from unsupervised_detection_b200 import _lib
-from unsupervised_detection_b200.flow_train_graph import ALPHAS, LEVELS, FlowTrainGraph
+from unsupervised_detection_b200.flow_train_graph import ALPHAS, LEVELS
 from unsupervised_detection_b200.models.PWCNet.model_pwcnet import FLOW_PRED_LVL
-from test_conv_launches_cpu import _attributed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-PLANS = ('aug', 'fwd', 'bwd', 'adam', 'pack')
-GRAPHS = {
-    'default': ((192, 384, 16), dict(in_hw=(384, 640))),
-    'unsup': ((192, 384, 16), dict(in_hw=(384, 640), loss='unsupervised')),
-    'timed': ((384, 640, 8), {}),
-    'shard': ((192, 384, 4), dict(global_batch=16, in_hw=(384, 640), loss='robust', options={'use_dense_cx': False}, augment=True,
-                                  sample_offset=8)),
-}
-KEYS = list(GRAPHS)
-
-# glue launches per plan
-_BWD = {'cis_zero': 5, 'cis_flow_multiscale_loss_bwd': 1, 'cis_colsum': 18, 'cis_dact_colsum': 91, 'cis_warp_costvol_bwd': 5,
-        'cis_parity_split_bf16': 8}
-_FWD = {'cis_resize_bilinear_f32': 3, 'cis_pack_f32_to_bf16': 2, 'cis_warp_costvol': 5, 'cis_flow_multiscale_loss': 1}
-_ADAM = {'cis_adam_l2': 1}
-DEFAULT = {'aug': {}, 'fwd': _FWD, 'bwd': _BWD, 'adam': _ADAM, 'pack': {}}
-GLUE = {
-    'default': DEFAULT,
-    'unsup': dict(DEFAULT, fwd={'cis_resize_bilinear_f32': 3, 'cis_pack_f32_to_bf16': 4, 'cis_warp_costvol': 5, 'cis_unsup_flow_loss': 1},
-                  bwd=dict({k: v for k, v in _BWD.items() if k != 'cis_flow_multiscale_loss_bwd'}, cis_unsup_flow_loss_bwd=1,
-                           cis_resize_f32_bwd_to_bf16_scaled=1)),
-    'timed': dict(DEFAULT, fwd=dict(_FWD, cis_resize_bilinear_f32=1)),     # no input resize: only the final x4
-    'shard': dict(DEFAULT, aug={'cis_flow_aug_params': 1, 'cis_flow_augment': 1}),
-}
-# conv launches (cis_conv_igemm + cis_conv_wgrad) of fwd + bwd
-CONV = {'default': 367, 'unsup': 367, 'timed': 355, 'shard': 367}
 
 # Entry points no launch plan of the checked graphs uses: each is checked against fp64 at the function level, by the file named.  The
 # groups say how that file reaches them; a file that stops reaching its entry points this way must be replaced here.
@@ -79,25 +52,16 @@ FUNCTION_LEVEL = {
 }
 
 
-def build(key, device):
-    """(FlowTrainGraph, conv Recorder, [(plan name, Plan)]) of one of KEYS."""
-    a, kw = GRAPHS[key]
-    mp = pytest.MonkeyPatch()
-    with R.recorded(mp) as rec:
-        g = FlowTrainGraph(*a, device=device, **kw)
-    return g, rec, [(p, getattr(g, p)) for p in PLANS]
-
-
 @pytest.fixture(scope='module')
 def graphs():
-    return {k: build(k, 'cpu') for k in KEYS}
+    return {k: build(k, 'cpu') for k in FLOW_TRAIN}
 
 
 def _ops(graphs, key, plan):
     return [op for name, p in graphs[key][2] if name == plan for op in p.ops]
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_every_launch_has_one_owner(graphs, key):
     owners = [set(G.ARGS), G.CONV_WALKER, set(G.PINNED_ELSEWHERE), G.STRUCTURAL]
     for name, plan in graphs[key][2]:
@@ -105,7 +69,7 @@ def test_every_launch_has_one_owner(graphs, key):
             assert sum(op[2] in s for s in owners) == 1, (key, name, op[2])
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_glue_launch_counts(graphs, key):
     plans = dict(graphs[key][2])
     assert set(plans) == set(GLUE[key])
@@ -116,10 +80,10 @@ def test_glue_launch_counts(graphs, key):
                 G.decode(op)
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_every_conv_op_is_attributed_once(graphs, key):
     plans = [p for _, p in graphs[key][2]]
-    checks = _attributed(graphs[key][1], plans)
+    checks = attributed(graphs[key][1], plans)
     assert sum(len(R.conv_ops(p)) for p in plans) == sum(len(ck.ops) for ck in checks) == CONV[key]
 
 
@@ -198,22 +162,11 @@ def test_every_entry_point_is_owned_or_listed():
         assert os.path.isfile(os.path.join(ROOT, path)), (name, path)
 
 
-def test_no_checked_graph_launches_a_function_level_entry_point(graphs):
-    import test_glue_launches_cpu as GC
-    import test_graph_variants_launches_cpu as GV
-    from unsupervised_detection_b200.models import functional as FN
-    plans = [(k, n, p) for k, (_, _, ps) in graphs.items() for n, p in ps]
-    for key, args, kw in (('config2', (256, 448, 4), {}), ('defaults', (192, 384, 16), dict(with_pwc=False)),
-                          ('odd', (100, 172, 3), dict(with_pwc=False)), ('boxes', (256, 448, 4), dict(masks='boxes'))):
-        plans += [(key, n, p) for n, p in GC._graph(*args, **kw)[1].items()]
-    r = FN._PWCRunner(2, 384, 640, 'cpu', 'pwcnet', trainable=True)
-    r.ensure_backward()
-    plans += [('pwc_runner', 'fwd', r.bld.fwd), ('pwc_runner', 'bwd', r.bwd)]
-    for key in GV.KEYS:
-        plans += [(key, n, p) for n, p in GV.build(key, 'cpu')[2]]
-    for key, name, plan in plans:
-        for op in plan.ops:
-            assert op[2] not in FUNCTION_LEVEL, (key, name, op[2])
+def test_no_checked_graph_launches_a_function_level_entry_point():
+    for key in GRAPHS:
+        for name, plan in build(key, 'cpu')[2]:
+            for op in plan.ops:
+                assert op[2] not in FUNCTION_LEVEL, (key, name, op[2])
 
 
 # ------------------------------------------------------------------------------------------------ the backward gather restated

@@ -21,7 +21,7 @@ the loss sums must be bit-identical to the walked step's.  Also: epe() at `defau
 the prediction to 384x640 with vectors scaled by (2, 5/3), and the cis_masked_epe sums), and cis_abs_sum against an fp64 sum.
 
 One summary line per graph and label and the controls are printed with pytest -s.  Controls: every control made must be rejected
-(ratio > 1) except costvol_bwd.gate_one (tests/test_graph_variants_launches_gpu.py says why).
+(ratio > 1) except costvol_bwd.gate_one (tests/launch_suites.py UNREJECTED says why).
 
 At `unsup` the untrained network's two directions disagree almost everywhere, so its mask keeps only a few hundred of the 2.36 M pixels
 per step.  test_unsup_loss_launches_on_partly_consistent_flows therefore also runs the two unsupervised launches on flows built to be
@@ -39,6 +39,7 @@ mask is empty: its photometric sum and bound are 0, so the FLOOR of 2^-100 divid
 consistent flows (coef at a masked pixel over the FLOOR), unsup_bwd.smooth_dropped 4.9e5 and 7.7e5, pack.unswapped 1.3e30,
 aug_params.step_frozen inf (the accepted attempts differ), augment.flow_unmapped 1.8e5, adam.decay_everywhere 1.0e8 - 1.2e18,
 adam.t_off_by_one 5.6e3.  Both poisoned replays bit-identical at every graph.  The file ran in 35 s: the four walks 7 - 10 s each."""
+import functools
 import time
 
 import pytest
@@ -46,88 +47,22 @@ import torch
 
 import conv_launch_ref as R
 import glue_launch_ref as G
-import pwc_options_ref as REF
+from launch_suites import CONV, FLOW_TRAIN, GLUE, PLANS, UNREJECTED, assert_within_bounds, bits, build, load_inputs, poison, report, \
+    targets, walk_plans
 from unsupervised_detection_b200 import _lib, engine as E
-from test_flow_train_launches_cpu import CONV, GLUE, GRAPHS, KEYS, PLANS, build
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(1800)]
 
-UNREJECTED = {'costvol_bwd.gate_one'}
-
-
-def _inputs(g, seed):
-    """Textured frames in [-0.5, 0.5] (tests/test_unsup_flow_gpu.py's construction) and a smooth ground truth of several pixels, at the
-    upload size."""
-    gen = torch.Generator().manual_seed(seed)
-    B, (ih, iw) = g.B, g.in_hw
-    fr = [(R.smooth(B, ih, iw, 3, 0.3, gen) + 0.2 * (torch.rand(B, ih, iw, 3, generator=gen) - 0.5)).clamp(-0.5, 0.5) for _ in range(2)]
-    gt = R.smooth(B, ih, iw, 2, 4.0, gen, div=24)
-    g.img1.copy_(fr[0])
-    g.img2.copy_(fr[1])
-    g.gt.copy_(gt)
-
 
 # ------------------------------------------------------------------------------------------------ poisoned replay
-def _targets(g):
-    """Acts and fp32 / fp64 tensors the plans of g write (inputs, parameters, m, v, step and lr excluded)."""
-    keep = {t.untyped_storage().data_ptr() for t in (g.store.flat, g.store.m, g.store.v, g.store.grad, g.step_state, g.lr) + tuple(g.inputs)}
-    acts, f32, seen = [], [], set()
-
-    def walk(o):
-        if o is None or id(o) in seen:
-            return
-        seen.add(id(o))
-        if isinstance(o, E.Act):
-            acts.append(o)
-            walk(o.grad)
-        elif isinstance(o, torch.Tensor):
-            if o.dtype in (torch.float32, torch.float64) and o.is_cuda and o.untyped_storage().data_ptr() not in keep:
-                f32.append(o)
-        elif isinstance(o, (list, tuple)):
-            for x in o:
-                walk(x)
-        elif isinstance(o, dict):
-            for x in o.values():
-                walk(x)
-        elif isinstance(o, E.ConvLayer):
-            for x in (o.dcat, o.dwp, o.colpart, o.dwp_hi):
-                walk(x)
-            for pk in o.tr_packs or ():
-                walk(pk.dwp)
-            if o.tr_planes is not None:
-                f32.append(o.tr_planes)
-    walk(g.bld.keep)
-    for _, p in ((n, getattr(g, n)) for n in PLANS):
-        walk(p.keep)
-    for L in g.pwc.all_layers():
-        walk(L)
+def _poison(g, sentinel):
+    """Poison what the plans of g write (not the inputs, parameters, m, v, step or lr) and the real entries of the flat gradient."""
+    st = g.store
     named = [g.flow, g.sums, g._scratch] + ([g.aug_params] + list(g.batch) if g.augment else [])
     named += [getattr(g, k) for k in ('warped', 'mask', 'coef', 'dflow') if hasattr(g, k)]
-    f32 += [t for t in named if all(t is not x for x in f32)]
-    return acts, f32
-
-
-def _poison(g, sentinel):
-    acts, f32 = _targets(g)
-    for a in acts:
-        idx = [a.c_off + p for p, m in enumerate(a.chanmap) if m >= 0]
-        if not idx:
-            continue
-        v = torch.full((a.N, a.H, a.W, len(idx)), sentinel, dtype=torch.bfloat16, device='cuda')
-        if sentinel == sentinel:
-            v[..., 1::2] = -sentinel
-        a.buf[:a.N].index_copy_(3, torch.tensor(idx, device='cuda'), v)
-    for t in f32:
-        t.fill_(sentinel)
-        if sentinel == sentinel:
-            t.view(-1)[1::2] = -sentinel
-    st = g.store
-    for name, _, n, off, _ in st.entries:
-        st.grad[off:off + n].fill_(sentinel)
-
-
-def _bits(t):
-    return t.view(torch.int32 if t.element_size() == 4 else torch.int64)
+    found = targets([g.bld.keep] + [getattr(g, p).keep for p in PLANS] + list(g.pwc.all_layers()), named,
+                    (st.flat, st.m, st.v, st.grad, g.step_state, g.lr) + tuple(g.inputs))
+    poison(found, [st], sentinel)
 
 
 def _poisoned_replays(g, clean):
@@ -137,10 +72,10 @@ def _poisoned_replays(g, clean):
     for sentinel in (float('nan'), 2.0 ** 100):
         _poison(g, sentinel)
         torch.cuda.synchronize()
-        poisoned = not torch.equal(_bits(g.store.grad), _bits(clean['grad']))
+        poisoned = not torch.equal(bits(g.store.grad), bits(clean['grad']))
         graph.replay()
         torch.cuda.synchronize()
-        out[sentinel] = (poisoned, all(torch.equal(_bits(getattr(g.store, 'grad') if k == 'grad' else g.sums), _bits(v))
+        out[sentinel] = (poisoned, all(torch.equal(bits(getattr(g.store, 'grad') if k == 'grad' else g.sums), bits(v))
                                        for k, v in clean.items()))
     return out
 
@@ -183,67 +118,50 @@ def _epe_check(g):
     return G.ratio(got, ref, b)
 
 
-def _walk_step(g, rec, step, out, poison=False):
-    glue = G.Glue(controls=True)
-    w = R.Walker(rec, controls=True, glue=glue)
-    counts = {}
-    for name in PLANS:
-        plan = getattr(g, name)
-        n, m = len(w.failures), len(glue.failures)
-        before = dict(glue.counts)
-        w.run(plan)
-        counts[name] = {k: v - before.get(k, 0) for k, v in glue.counts.items() if v - before.get(k, 0)}
-        out['failures'] += ['step %d %s: %s' % (step, name, f) for f in w.failures[n:] + glue.failures[m:]]
+def _walk_step(g, rec, plans, step, out):
+    def after(name, glue):
         if name == 'fwd' and g.loss == 'unsupervised':
             r, bad = _pack_check(g, glue)
             out['pack'] = max(out.get('pack', 0.0), r)
             glue._control('pack.unswapped', bad)
-        if name == 'fwd' and step == 1 and GRAPHS_EPE.get(out['key']):
+        if name == 'fwd' and step == 1 and out['key'] == 'default':
             out['epe'] = _epe_check(g)
-        if name == 'bwd' and poison:
+        if name == 'bwd' and step == 1:
             torch.cuda.synchronize()
             out['poison'] = _poisoned_replays(g, dict(grad=g.store.grad.clone(), sums=g.sums.clone()))
-    out['counts'].append(counts)
-    out['conv'].append(w.checked)
-    for k, v in dict(w.controls, **glue.controls).items():
+
+    r = walk_plans(rec, plans, controls=True, glue_controls=True, after=after)
+    out['failures'] += ['step %d %s: %s' % (step, name, f) for name, fs in r['failures'].items() for f in fs]
+    out['counts'].append(r['counts'])
+    out['conv'].append(r['conv'])
+    for k, v in r['controls'].items():
         out['controls'][k] = max(out['controls'].get(k, 0.0), v) if k not in UNREJECTED else v
-    for lab, v in list(w.summary().items()) + list(glue.summary().items()):
-        print('%-8s step %d %-44s count %4d  worst bound ratio %.3g' % (out['key'], step, lab, v['count'], v['worst']))
-        out['worst'][lab] = max(out['worst'].get(lab, 0.0), v['worst'])
-    if hasattr(glue, 'unsup_mask'):
-        print('%-8s step %d unsupervised mask vs fp64: %s' % (out['key'], step, glue.unsup_mask))
+    report('%s step %d' % (out['key'], step), r['summary'])
+    if r['unsup_mask'] is not None:
+        print('%-22s step %d unsupervised mask vs fp64: %s' % (out['key'], step, r['unsup_mask']))
 
 
-GRAPHS_EPE = {'default': True}
-_WALKS = {}
-
-
+@functools.lru_cache(maxsize=None)
 def walk(key):
-    if key in _WALKS:
-        return _WALKS[key]
     t0 = time.time()
-    g, rec, _ = build(key, 'cuda')
-    opts = GRAPHS[key][1].get('options')
-    g.load_params(REF.make_params(3, jitter=0.1, options=opts))
-    _inputs(g, 40 + KEYS.index(key))
-    g._ensure_packed()
-    out = dict(key=key, failures=[], counts=[], conv=[], controls={}, worst={}, tables=[])
+    g, rec, plans = build(key, 'cuda')
+    load_inputs(key, g)
+    out = dict(key=key, failures=[], counts=[], conv=[], controls={}, tables=[])
     for step in (1, 2):
-        _walk_step(g, rec, step, out, poison=step == 1)
+        _walk_step(g, rec, plans, step, out)
         if g.augment:
             out['tables'].append(g.aug_params.clone())
     out['step_state'] = int(g.step_state)
-    print('%-8s negative controls (ratio > 1 = rejected): %s' % (key, out['controls']))
-    print('%-8s %s conv and %s glue launches checked over two steps in %.1f s'
+    report(key, {}, out['controls'])
+    print('%-22s %s conv and %s glue launches checked over two steps in %.1f s'
           % (key, out['conv'], [sum(sum(c.values()) for c in s.values()) for s in out['counts']], time.time() - t0))
-    del g, rec
+    del g, rec, plans
     torch.cuda.synchronize()
     torch.cuda.empty_cache()
-    _WALKS[key] = out
     return out
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_every_launch_within_its_bound(key):
     r = walk(key)
     assert not r['failures'], '%s:\n%s' % (key, '\n'.join(r['failures'][:20]))
@@ -254,7 +172,7 @@ def test_every_launch_within_its_bound(key):
         assert r['pack'] == 0.0
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_negative_controls_are_rejected(key):
     c = walk(key)['controls']
     want = {'tile', 'fwd.halo', 'adam.decay_everywhere', 'adam.t_off_by_one'}
@@ -271,7 +189,7 @@ def test_negative_controls_are_rejected(key):
     assert not bad, (key, bad)
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', FLOW_TRAIN)
 def test_poisoned_graph_replay_is_bit_identical(key):
     for sentinel, (poisoned, same) in walk(key)['poison'].items():
         assert poisoned and same, (key, sentinel, poisoned, same)
@@ -307,16 +225,14 @@ def test_unsup_loss_launches_on_partly_consistent_flows():
     plan.add('cis_unsup_flow_loss', *ptrs, warped.data_ptr(), mask.data_ptr(), coef.data_ptr(), scratch.data_ptr(), out.data_ptr())
     norm = float(4 * H * W)
     plan.add('cis_unsup_flow_loss_bwd', *ptrs, warped.data_ptr(), coef.data_ptr(), 1.0 / norm, 3.0 / norm, dflow.data_ptr())
-    glue = G.Glue(controls=True)
-    R.Walker(R.Recorder(), glue=glue).run(plan)
-    for lab, v in glue.summary().items():
-        print('direct_unsup %-40s count %4d  worst bound ratio %.3g' % (lab, v['count'], v['worst']))
-    print('direct_unsup mask vs fp64: %s; controls %s' % (glue.unsup_mask, glue.controls))
-    assert not glue.failures, '\n'.join(glue.failures[:20])
-    assert dict(glue.counts) == {'cis_unsup_flow_loss': 1, 'cis_unsup_flow_loss_bwd': 1}
-    m = glue.unsup_mask
+    r = walk_plans(R.Recorder(), [('direct_unsup', plan)], glue_controls=True)
+    report('direct_unsup', r['summary'])
+    print('direct_unsup mask vs fp64: %s; controls %s' % (r['unsup_mask'], r['controls']))
+    assert_within_bounds(r)
+    assert r['counts']['direct_unsup'] == {'cis_unsup_flow_loss': 1, 'cis_unsup_flow_loss_bwd': 1}
+    m = r['unsup_mask']
     assert m['pixels'] - m['out'] - m['occluded'] >= 0.1 * m['pixels'] and m['out'] > 0 and m['occluded'] > 0, m
-    assert glue.controls['unsup.mask_ones'] > 1.0 and glue.controls['unsup_bwd.smooth_dropped'] > 1.0, glue.controls
+    assert r['controls']['unsup.mask_ones'] > 1.0 and r['controls']['unsup_bwd.smooth_dropped'] > 1.0, r['controls']
 
 
 def test_abs_sum_matches_fp64():

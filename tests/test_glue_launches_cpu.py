@@ -1,47 +1,22 @@
-"""Ownership of every launch of the benchmarked graphs, without a GPU: the graphs of tests/test_glue_launches_gpu.py are BUILT on CPU
-tensors (nothing is launched), and every entry point in their forward and backward plans must have exactly one owner -- the conv walker,
-the glue checker's reference table (tests/glue_launch_ref.py), a test that pins it elsewhere, or the structural ops.  A kernel added to
-the step without a per-launch reference fails here.  The per-graph launch counts of the GPU checks are pinned too."""
+"""Ownership of every launch of the benchmarked graphs, without a GPU: the graphs tests/test_conv_launches_gpu.py and
+tests/test_glue_launches_gpu.py check are BUILT on CPU tensors (nothing is launched), and every entry point in their forward and backward
+plans must have exactly one owner -- the conv walker, the glue checker's reference table (tests/glue_launch_ref.py), a test that pins it
+elsewhere, or the structural ops.  A kernel added to the step without a per-launch reference fails here.  The per-graph launch counts of
+the GPU checks are pinned too."""
 import collections
 
 import pytest
 
 import glue_launch_ref as G
+from launch_suites import GLUE, build
 from unsupervised_detection_b200 import _lib
-from unsupervised_detection_b200.models import functional as FN
-from unsupervised_detection_b200.step_graph import CISGraph
 
-CONFIG2 = {
-    'fwd': {'cis_resize_concat_bf16': 11, 'cis_warp_costvol': 5, 'cis_pack_f32_to_bf16': 3, 'cis_resize_bilinear_f32': 3,
-            'cis_upsample_nn2x': 2, 'cis_flow_stats': 1, 'cis_pack_generator_input': 1, 'cis_zero': 2},
-    'bwd_R': {'cis_dact_colsum': 23, 'cis_resize_concat_bf16_bwd': 14, 'cis_colsum': 9},
-    'bwd_G': {'cis_dact_colsum': 16, 'cis_dact_mul': 14, 'cis_resize_concat_bf16_bwd': 14, 'cis_add_slice': 3, 'cis_upsample_nn2x_bwd': 2,
-              'cis_colsum': 1},
-}
-PWC_BWD = {'cis_dact_colsum': 91, 'cis_colsum': 18, 'cis_parity_split_bf16': 8, 'cis_warp_costvol_bwd': 5, 'cis_zero': 5,
-           'cis_cast_bf16_to_f32': 2, 'cis_resize_f32_bwd_to_bf16_scaled': 1}
-PWC_FWD = {'cis_warp_costvol': 5, 'cis_pack_f32_to_bf16': 2, 'cis_resize_bilinear_f32': 1}
-# the flow given directly: no PWC-Net, no 384x640 inputs
-FLOW_GIVEN = dict(CONFIG2, fwd={'cis_resize_concat_bf16': 11, 'cis_pack_f32_to_bf16': 1, 'cis_upsample_nn2x': 2, 'cis_flow_stats': 1,
-                                'cis_pack_generator_input': 1, 'cis_zero': 2})
-BOXES = {'fwd': {'cis_resize_concat_bf16': 11, 'cis_warp_costvol': 5, 'cis_pack_f32_to_bf16': 3, 'cis_resize_bilinear_f32': 3, 'cis_zero': 1},
-         'bwd_R': CONFIG2['bwd_R']}
-
-
-def _graph(*a, **k):
-    g = CISGraph(*a, device='cpu', **k)
-    plans = {'fwd': g.fwd}
-    plans.update({'bwd_' + m: p for m, p in g.bwd.items()})
-    return g, plans
+KEYS = ['config2', 'defaults', 'odd', 'boxes', 'pwc_runner']
 
 
 @pytest.fixture(scope='module')
 def graphs():
-    r = FN._PWCRunner(2, 384, 640, 'cpu', 'pwcnet', trainable=True)
-    r.ensure_backward()
-    out = {'config2': _graph(256, 448, 4), 'defaults': _graph(192, 384, 16, with_pwc=False), 'odd': _graph(100, 172, 3, with_pwc=False),
-           'boxes': _graph(256, 448, 4, masks='boxes'), 'pwc_runner': (r, {'fwd': r.bld.fwd, 'bwd': r.bwd})}
-    return out
+    return {k: dict(build(k, 'cpu')[2]) for k in KEYS}
 
 
 def test_owner_sets_are_disjoint():
@@ -51,10 +26,10 @@ def test_owner_sets_are_disjoint():
             assert not sets[i] & sets[j], sets[i] & sets[j]
 
 
-@pytest.mark.parametrize('key', ['config2', 'defaults', 'odd', 'boxes', 'pwc_runner'])
+@pytest.mark.parametrize('key', KEYS)
 def test_every_launch_has_one_owner(graphs, key):
     owners = set(G.ARGS) | G.CONV_WALKER | set(G.PINNED_ELSEWHERE) | G.STRUCTURAL
-    for name, plan in graphs[key][1].items():
+    for name, plan in graphs[key].items():
         for op in plan.ops:
             assert op[2] in owners, (key, name, op[2])
 
@@ -66,10 +41,9 @@ def test_references_decode_the_abi():
         assert name in _lib._PROTOS
 
 
-@pytest.mark.parametrize('key,want', [('config2', CONFIG2), ('defaults', FLOW_GIVEN), ('odd', FLOW_GIVEN), ('boxes', BOXES),
-                                      ('pwc_runner', {'fwd': PWC_FWD, 'bwd': PWC_BWD})])
+@pytest.mark.parametrize('key,want', [(k, GLUE[k]) for k in KEYS])
 def test_glue_launch_counts(graphs, key, want):
-    plans = graphs[key][1]
+    plans = graphs[key]
     assert set(plans) == set(want)
     for name, plan in plans.items():
         assert dict(G.glue_counts(plan)) == want[name], (key, name)
@@ -78,11 +52,10 @@ def test_glue_launch_counts(graphs, key, want):
                 G.decode(op)
 
 
-def test_odd_geometry_runs_the_generic_resize():
+def test_odd_geometry_runs_the_generic_resize(graphs):
     """100x172: the recover decoder's 4x6 -> 7x11 -> 13x22 -> 25x43 resize-concats take the generic (non-x2) kernel and transpose."""
-    _, plans = _graph(100, 172, 3, with_pwc=False)
     kinds = collections.Counter()
-    for name, plan in plans.items():
+    for name, plan in graphs['odd'].items():
         for op in plan.ops:
             if op[2].startswith('cis_resize_concat_bf16'):
                 a = G.decode(op)

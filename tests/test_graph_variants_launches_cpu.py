@@ -18,82 +18,27 @@ import pytest
 
 import conv_launch_ref as R
 import glue_launch_ref as G
-from unsupervised_detection_b200 import _lib, engine as E
-from unsupervised_detection_b200.models import functional as FN
-from unsupervised_detection_b200.models.PWCNet.model_pwcnet import _DEFAULT_PWCNET_TEST_OPTIONS, A_TOTAL, CORR_OFF
-from unsupervised_detection_b200.step_graph import CISGraph
-from test_conv_launches_cpu import _attributed, _features
-from test_glue_launches_cpu import FLOW_GIVEN, PWC_BWD, PWC_FWD
-
-PWC_OPTIONS = {'r1': {'search_range': 1}, 'r2': {'search_range': 2}, 'r3': {'search_range': 3}, 'dense_off': {'use_dense_cx': False}}
-KEYS = ['gen_fwd', 'ensemble', 'odd'] + list(PWC_OPTIONS)
-
-# glue launches per plan ('masks' = _mask_plan, 'rest' = the other forward ops)
-GEN_FWD = {'masks': {'cis_zero': 1, 'cis_flow_stats': 1, 'cis_pack_generator_input': 1, 'cis_pack_f32_to_bf16': 1, 'cis_upsample_nn2x': 2},
-           'rest': {'cis_resize_concat_bf16': 11, 'cis_zero': 1}}
-ENSEMBLE = {'masks': {'cis_pack_f32_to_bf16': 3, 'cis_warp_costvol': 5, 'cis_resize_bilinear_f32': 3, 'cis_zero': 1, 'cis_flow_stats': 1,
-                      'cis_pack_generator_input': 1, 'cis_upsample_nn2x': 2},
-            'rest': {'cis_resize_concat_bf16': 11, 'cis_zero': 1}}
-# search ranges 1-3: the warp + cost-volume launches take the entry points with a range argument
-PWC_RANGE = {plan: {n + '_r' if n.startswith('cis_warp_costvol') else n: c for n, c in counts.items()}
-             for plan, counts in (('fwd', PWC_FWD), ('bwd', PWC_BWD))}
-GLUE = {'gen_fwd': GEN_FWD, 'ensemble': ENSEMBLE, 'odd': FLOW_GIVEN, 'r1': PWC_RANGE, 'r2': PWC_RANGE, 'r3': PWC_RANGE,
-        'dense_off': {'fwd': PWC_FWD, 'bwd': PWC_BWD}}
-# conv launches per graph (cis_conv_igemm + cis_conv_wgrad ops over its plans)
-CONV = {'gen_fwd': 49, 'ensemble': 158, 'odd': 185, 'r1': 357, 'r2': 357, 'r3': 357, 'dense_off': 357}
-
-
-def split_fwd(g):
-    """[('masks', _mask_plan), ('rest', the forward ops that are not in it, in plan order)].  Ops are matched by identity, counted: the
-    structural 'join' op is one shared tuple that can appear in both parts."""
-    left = collections.Counter(id(op) for op in g._mask_plan.ops)
-    rest = E.Plan('fwd_rest')
-    for op in g.fwd.ops:
-        if left[id(op)]:
-            left[id(op)] -= 1
-        else:
-            rest.ops.append(op)
-    assert not +left
-    rest.keep = g.fwd.keep
-    return [('masks', g._mask_plan), ('rest', rest)]
-
-
-def build(key, device):
-    """(graph or runner, conv Recorder, [(plan name, Plan)]) of one of KEYS."""
-    mp = pytest.MonkeyPatch()
-    with R.recorded(mp) as rec:
-        if key == 'gen_fwd':
-            g = CISGraph(128, 224, 1, device=device, with_pwc=False, train=False)
-            plans = split_fwd(g)
-        elif key == 'ensemble':
-            g = CISGraph(192, 384, 4, device=device, train=False, pwc_options=_DEFAULT_PWCNET_TEST_OPTIONS)
-            plans = split_fwd(g)
-        elif key == 'odd':
-            g = CISGraph(100, 172, 3, device=device, with_pwc=False)
-            plans = [('fwd', g.fwd), ('bwd_R', g.bwd['R']), ('bwd_G', g.bwd['G'])]
-        else:
-            g = FN._PWCRunner(2, 384, 640, device, 'pwcnet', trainable=True, options=PWC_OPTIONS[key])
-            g.ensure_backward()
-            plans = [('fwd', g.bld.fwd), ('bwd', g.bwd)]
-    return g, rec, plans
+from launch_suites import CONV, GLUE, VARIANTS, attributed, build, features
+from unsupervised_detection_b200 import _lib
+from unsupervised_detection_b200.models.PWCNet.model_pwcnet import A_TOTAL, CORR_OFF
 
 
 @pytest.fixture(scope='module')
 def graphs():
-    return {k: build(k, 'cpu') for k in KEYS}
+    return {k: build(k, 'cpu') for k in VARIANTS}
 
 
 def _checks(graphs, key):
-    return _attributed(graphs[key][1], [p for _, p in graphs[key][2]])
+    return attributed(graphs[key][1], [p for _, p in graphs[key][2]])
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', VARIANTS)
 def test_every_conv_op_is_attributed_once(graphs, key):
     checks = _checks(graphs, key)
     assert sum(len(R.conv_ops(p)) for _, p in graphs[key][2]) == sum(len(ck.ops) for ck in checks) == CONV[key]
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', VARIANTS)
 def test_every_launch_has_one_owner(graphs, key):
     owners = [set(G.ARGS), G.CONV_WALKER, set(G.PINNED_ELSEWHERE), G.STRUCTURAL]
     for name, plan in graphs[key][2]:
@@ -101,7 +46,7 @@ def test_every_launch_has_one_owner(graphs, key):
             assert sum(op[2] in s for s in owners) == 1, (key, name, op[2])
 
 
-@pytest.mark.parametrize('key', KEYS)
+@pytest.mark.parametrize('key', VARIANTS)
 def test_glue_launch_counts(graphs, key):
     plans = dict(graphs[key][2])
     want = GLUE[key]
@@ -145,7 +90,7 @@ def test_cost_volume_range_launches(graphs, key, r, pad):
 def test_ensemble_recover_split_k_over_batch_broadcast_concats(graphs):
     """The recover net of the ensemble runs at N = 12 (three calls of 4 crops); its flow heads read 3- and 4-source concats whose
     batch-broadcast sources repeat, split 6 and 7 ways over K."""
-    f = _features(_checks(graphs, 'ensemble'))
+    f = features(_checks(graphs, 'ensemble'))
     assert {('n_mod', 3, 6), ('n_mod', 4, 7)} <= f, sorted(x for x in f if isinstance(x, tuple) and x[0] == 'n_mod')
     big = [ck for ck in _checks(graphs, 'ensemble') if ck.layer.name.startswith('FlownetS/') and ck.descs()[0].splits >= 6
            and ck.descs()[0].nsrc == 4]
