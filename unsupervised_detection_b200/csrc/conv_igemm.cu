@@ -40,19 +40,29 @@ static constexpr int kBM = 128;       // GEMM rows per CTA
 static constexpr int kBK = 64;        // bf16 K elements per stage (128-byte swizzled rows)
 static constexpr int kAStage = kBM * 128;
 static constexpr int kThreads = 256;  // halo / wgrad kernels: 4 producer/epilogue warps + 1 MMA warpgroup
-// conv_halo_kernel<BN, NWG>: warps 0-3 producers + epilogue, then NWG MMA warpgroups.
-//   NWG = 1: BN >= 64 adds warps 4-7 (epilogue only: the wide epilogue is instruction-bound on its warps) before the MMA warpgroup.
+// conv_halo_kernel<BN, NWG>: warps 0-3 producers + epilogue, then NWG MMA warpgroups (warps 4-7, 4-11).
+//   NWG = 1: 256 threads, two CTAs per SM (128 registers per thread), so one CTA's prologue and epilogue overlap the other's main
+//   loop.  The producer warpgroup hands registers to the MMA warpgroup for the main loop (setmaxnreg: kProdRegs / kMmaRegs; 128
+//   accumulator columns need ~168) and both return to kLaunchRegs for the epilogue.  BN >= 64: the MMA warps join the epilogue once
+//   their accumulators are in shared memory (the wide epilogue is instruction-bound on its warps).
 //   NWG = 2 (BN >= 64): two MMA warpgroups (warps 4-11) consume every weight stage, so each weight byte fetched from L2 feeds twice
-//   the output rows; no epilogue-only warps (384 threads keep the 168-register budget of one warpgroup's 128 accumulator columns),
-//   the MMA warps join the epilogue once their accumulators are in shared memory.
+//   the output rows; 384 threads, one CTA per SM (the 168-register budget of one warpgroup's 128 accumulator columns), the MMA warps
+//   join the epilogue.
 template <int BN, int NWG> struct HaloCfg {
   static_assert(NWG == 1 || (NWG == 2 && BN >= 64), "two MMA warpgroups only for BN >= 64");
-  static constexpr int kMmaWarp = (NWG == 1 && BN >= 64) ? 8 : 4;     // first warp of the first MMA warpgroup
+  static constexpr int kMmaWarp = 4;                                   // first warp of the first MMA warpgroup
   static constexpr int kThreads = (kMmaWarp + 4 * NWG) * 32;
-  static constexpr int kEpiWarps = NWG == 1 ? kMmaWarp : kThreads / 32;   // warps 0 .. kEpiWarps-1 run the epilogue
+  static constexpr int kEpiWarps = (NWG == 1 && BN < 64) ? kMmaWarp : kThreads / 32;   // warps 0 .. kEpiWarps-1 run the epilogue
   static constexpr int kEpiParts = NWG == 1 ? (BN >= 64 ? 2 : 1) : BN / 32;   // column parts of a 32-row epilogue unit
   // accumulator registers per MMA thread: MT * BN <= kMaxAccCols (the host never stacks more tiles than that)
   static constexpr int kMaxMT = (128 / BN) < 4 ? (128 / BN) : 4;
+  static constexpr int kCtasPerSm = NWG == 1 ? 2 : 1;
+  static constexpr int kLaunchRegs = (65536 / (kCtasPerSm * kThreads)) & ~7;   // registers per thread under the launch bounds
+  // main-loop budgets of the producer and MMA warpgroups (0: no setmaxnreg; BN = 16 holds its 64 accumulator columns in kLaunchRegs)
+  static constexpr int kProdRegs = (NWG == 1 && BN >= 32) ? 88 : 0;
+  static constexpr int kMmaRegs = (NWG == 1 && BN >= 32) ? 168 : 0;
+  static_assert(kProdRegs == 0 || 128 * (kProdRegs + NWG * kMmaRegs) <= kThreads * kLaunchRegs,
+                "setmaxnreg.inc would wait for registers the CTA does not own");
 };
 static constexpr int kMaxAccCols = 128;   // fp32 accumulator columns one MMA warpgroup holds in registers (128 per thread)
 static constexpr int kGProducers = 256;   // gather kernel: 8 producer/epilogue warps (its cp.async address arithmetic is the bottleneck)
@@ -321,7 +331,10 @@ __device__ __forceinline__ void cluster_reduce_rows(const CisConv& p, const uint
   }
 }
 
-template <int BN>
+// CPS: co-resident CTAs per SM the registers allow.  CPS = 2 (80 registers per thread) up to BN = 64, where the producer warpgroups
+// lend 8 registers per thread to the MMA warpgroup for the main loop (setmaxnreg; 0 = none).  BN = 128 (128 accumulator columns next
+// to 8 gathering warps) and the one-per-SM BN = 64 instance (grids of at most one CTA per SM) are compiled for CPS = 1.
+template <int BN, int CPS>
 struct FwdCfg {
   // kLag + 1 K blocks of gathers are in flight per producer thread (the im2col loads are L2 round trips).  A deeper ring costs
   // co-resident CTAs on the thin layers.
@@ -330,11 +343,18 @@ struct FwdCfg {
   static constexpr int kBStage = BN * 128;
   static constexpr int kSmem = kStages * (kAStage + kBStage) + 1024;
   static_assert(kStages * (kAStage + kBStage) >= kBM * BN * 4, "the accumulator tile reuses the operand ring");
+  static_assert(CPS == 1 || BN <= 64, "128 accumulator columns do not fit two CTAs per SM");
+  static constexpr int kLaunchRegs = (65536 / (CPS * kGThreads)) & ~7;
+  static constexpr int kProdRegs = (BN == 64 && CPS == 2) ? 72 : 0;
+  static constexpr int kMmaRegs = (BN == 64 && CPS == 2) ? 96 : 0;
+  static_assert(kProdRegs == 0 || 128 * (kProdRegs * kGProducers / 128 + kMmaRegs) <= kGThreads * kLaunchRegs,
+                "setmaxnreg.inc would wait for registers the CTA does not own");
 };
 
-template <int BN>
-__global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_constant__ CisConv p) {
-  using Cfg = FwdCfg<BN>;
+// CPS = 1: no minimum CTA count in the launch bounds (ptxas then keeps its own register choice, 90 for BN = 64 instead of 118)
+template <int BN, int CPS>
+__global__ void __launch_bounds__(kGThreads, CPS == 1 ? 0 : CPS) conv_igemm_kernel(const __grid_constant__ CisConv p) {
+  using Cfg = FwdCfg<BN, CPS>;
   constexpr int S = Cfg::kStages;
   constexpr int kMmaWarp = kGProducers / 32;
   extern __shared__ uint8_t smem_raw[];
@@ -398,6 +418,7 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     // Per-row constants (this thread's 4 rows): top-left input pixel, and the linear pixel index of it in the plain and in the
     // batch-broadcast (n % n_mod) view of the sources.  The K loop below is division-free: with integer divisions / 64-bit address
     // arithmetic per (K block, row) the producer warps are issue-bound, not bound by the loads.
+    if constexpr (Cfg::kProdRegs > 0) setmaxnreg_dec<Cfg::kProdRegs>();
     int hb[4], wb[4], pre[4], prem[4];
     int nm0 = 0;                          // the batch-broadcast modulus (sources with n_mod > 0 share one; others: slow path)
     for (int i = 0; i < p.nsrc; ++i)
@@ -487,6 +508,10 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
       fence_proxy_async();
       mbar_arrive(bar_full + 8 * ((nkb - 1 - i) % S));
     }
+    if constexpr (Cfg::kProdRegs > 0) {   // the MMA warpgroup returns its share after its last MMA
+      named_bar_sync<2, kGProducers>();
+      setmaxnreg_inc<Cfg::kLaunchRegs>();
+    }
 
     // ------------------------------------------------------------------ epilogue: warps w and w + 4 share 32 accumulator rows and split the columns
     mbar_wait(bar_accum, 0);
@@ -519,6 +544,7 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     }
   } else {
     // ------------------------------------------------------------------ MMA warpgroup
+    if constexpr (Cfg::kMmaRegs > 0) setmaxnreg_inc<Cfg::kMmaRegs>();
     const int wtid = tid - kMmaWarp * 32;
     float acc[BN];
     const uint32_t dhi = desc_hi(1024);
@@ -538,6 +564,10 @@ __global__ void __launch_bounds__(kGThreads) conv_igemm_kernel(const __grid_cons
     }
     wg_wait<0>();
     acc_store<BN>(acc, tile_base, wtid);   // every operand stage has been consumed: the ring is dead
+    if constexpr (Cfg::kMmaRegs > 0) {
+      named_bar_sync<3, 128>();
+      setmaxnreg_dec<Cfg::kLaunchRegs>();
+    }
     mbar_arrive(bar_accum);
   }
   if (nsplit > 1 && p.sk_cluster) {
@@ -688,7 +718,7 @@ __device__ __forceinline__ void thin_halo_load(const CisConv& p, const Src* src,
 }
 
 template <int BN, int NWG>
-__global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
+__global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, HaloCfg<BN, NWG>::kCtasPerSm) conv_halo_kernel(const __grid_constant__ CisConv p, const int halo_stage_bytes, const int BS, const int NHS,
                                                         const __grid_constant__ HaloMaps maps, const int use_tma, const int G) {
   // One weight pipeline stage = the tiles of G consecutive taps of one 64-channel chunk (contiguous in the pre-tiled operand, ONE
   // bulk copy): the MMA warpgroup pays the per-stage cost (mbarrier wait, wgmma fence / commit / wait, release) once per 4*MT*G
@@ -780,10 +810,10 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
   if (tid == 0) CIS_TRACE_AT(0);
 
   if (warp < kHMmaWarp_) {
-   if (warp < 4) {
     // ------------------------------------------------------------------ producers
     // Two independent roles so neither stream throttles the other: warps 0-1 stream the per-chunk halos (2 stages), warps 2-3
     // stream the per-(tap, chunk) weight tiles (BS stages).
+    if constexpr (Cfg::kProdRegs > 0) setmaxnreg_dec<Cfg::kProdRegs>();
     if (use_tma) {
       if (tid == 0) {
         // halo through the TMA engine: one 4-D tiled load per 64-channel chunk (x phase), out-of-image pixels / channels are zero-filled
@@ -884,10 +914,14 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
       }
     }
     __syncwarp();
-   }
-
+    // back to the even split for the epilogue; the MMA warpgroup returns its share once its accumulators are in shared memory
+    if constexpr (Cfg::kProdRegs > 0) {
+      named_bar_sync<2, 128>();
+      setmaxnreg_inc<Cfg::kLaunchRegs>();
+    }
   } else {
     // ------------------------------------------------------------------ MMA warpgroup(s)
+    if constexpr (Cfg::kMmaRegs > 0) setmaxnreg_inc<Cfg::kMmaRegs>();
     const int wg = NWG > 1 ? (warp - kHMmaWarp_) >> 2 : 0;
     const int wtid = tid - (kHMmaWarp_ + 4 * wg) * 32;
     constexpr int MTM = Cfg::kMaxMT;
@@ -941,6 +975,10 @@ __global__ void __launch_bounds__(HaloCfg<BN, NWG>::kThreads, 1) conv_halo_kerne
 #pragma unroll
     for (int m = 0; m < MTM; ++m)
       if (m < MT) acc_store<BN>(acc[m], tile_base + (uint32_t)((wg * MT + m) * BN) * kAccColBytes, wtid);
+    if constexpr (Cfg::kMmaRegs > 0) {
+      named_bar_sync<3, 128>();
+      setmaxnreg_dec<Cfg::kLaunchRegs>();
+    }
     mbar_arrive(bar_accum);
   }
 
@@ -1773,12 +1811,12 @@ static cudaError_t launch_splitk_finish(const CisConv* d, dim3 main_grid, cudaSt
   return launch_pdl(splitk_finish_kernel<BN>, dim3(main_grid.x, main_grid.y, mt * kSub), dim3(kBlock), 0, st, *d);
 }
 
-template <int BN>
-static int launch_fwd(const CisConv* d, cudaStream_t st) {
-  using Cfg = FwdCfg<BN>;
+template <int BN, int CPS>
+static int launch_fwd_cps(const CisConv* d, cudaStream_t st) {
+  using Cfg = FwdCfg<BN, CPS>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem);
+    cudaError_t e = cudaFuncSetAttribute(conv_igemm_kernel<BN, CPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmem);
     if (e != cudaSuccess) return cis_set_cuda_error(e, "cudaFuncSetAttribute(conv_igemm)");
     attr_set = true;
   }
@@ -1791,14 +1829,24 @@ static int launch_fwd(const CisConv* d, cudaStream_t st) {
   }
   dim3 grid((M + kBM - 1) / kBM, d->n_tiles, splits);
   cudaError_t le = (splits > 1 && d->sk_cluster)
-                       ? launch_pdl_zcluster(conv_igemm_kernel<BN>, grid, dim3(kGThreads), Cfg::kSmem, st, splits, *d)
-                       : launch_pdl(conv_igemm_kernel<BN>, grid, dim3(kGThreads), Cfg::kSmem, st, *d);
+                       ? launch_pdl_zcluster(conv_igemm_kernel<BN, CPS>, grid, dim3(kGThreads), Cfg::kSmem, st, splits, *d)
+                       : launch_pdl(conv_igemm_kernel<BN, CPS>, grid, dim3(kGThreads), Cfg::kSmem, st, *d);
   if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(conv_igemm)");
   if (splits > 1 && !d->sk_cluster) {
     le = launch_splitk_finish<BN>(d, grid, st);
     if (le != cudaSuccess) return cis_set_cuda_error(le, "launch(splitk_finish)");
   }
   return cis_check_launch("conv_igemm");
+}
+// BN = 64 grids of at most one CTA per SM run the CPS = 1 instance: nothing overlaps there, and the producers' main-loop register
+// budget of the CPS = 2 instance costs time (H100 SXM at 700 W, 4x48x80, 96 input channels, 120 CTAs: 14.0 us at CPS = 1, 17.3 at 2)
+template <int BN>
+static int launch_fwd(const CisConv* d, cudaStream_t st) {
+  const long ncta = (long)((d->N * d->OH * d->OW + kBM - 1) / kBM) * d->n_tiles * (d->splits > 1 ? d->splits : 1);
+  if constexpr (BN == 64) {
+    if (ncta <= cis_num_sms()) return launch_fwd_cps<BN, 1>(d, st);
+  }
+  return launch_fwd_cps<BN, BN == 128 ? 1 : 2>(d, st);
 }
 
 
@@ -1849,6 +1897,19 @@ static int g_persist_mode = -1;   // -1: environment / default (1 = thin layers)
 extern "C" int cis_set_persist_mode(int mode) {
   g_persist_mode = mode;
   return CIS_OK;
+}
+
+// Largest dynamic shared memory (a multiple of 1 KB) with which two CTAs of `kernel` fit on one SM: half the SM's shared memory, less
+// the per-CTA reservation and the kernel's static shared memory (H100: 228 KB per SM, 1 KB reserved -> 112 KB).
+template <typename K>
+static int pair_smem_limit(K kernel) {
+  int dev = 0, per_sm = 0, reserved = 0;
+  cudaFuncAttributes fa;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+      cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess ||
+      cudaFuncGetAttributes(&fa, kernel) != cudaSuccess)
+    return 112 * 1024;
+  return (per_sm / 2 - reserved - (int)fa.sharedSizeBytes) & ~1023;
 }
 
 // wk: NULL = the weights are cis_pack_weights_tiled tiles at d->wpack; else (compact format) d->wpack is a gather launch's row pack
@@ -1909,13 +1970,17 @@ static int launch_halo(const CisConv* d, cudaStream_t st, const int16_t* wk = nu
   if (G < 1) G = 1;
   if (G > nst_max) G = nst_max;
   const int fixed = nhs * halo_stage + HP * 4 + 1024;
-  // two co-resident CTAs per SM overlap one CTA's epilogue with the other's main loop -- when the grid has that many CTAs
+  // two co-resident CTAs per SM (NWG = 1: HaloCfg's register budget) overlap one CTA's prologue and epilogue with the other's main
+  // loop -- when the grid has that many CTAs and each takes at most half the SM's shared memory.  NWG = 2 CTAs hold the register file
+  // alone; their launches keep the weight ring they were tuned with.
+  static const int lim_pair = HaloCfg<BN, NWG>::kCtasPerSm == 2 ? pair_smem_limit(conv_halo_kernel<BN, NWG>) : 113 * 1024;
   static const int lim_small_kb = getenv("CIS_HALO_SMALL_KB") ? atoi(getenv("CIS_HALO_SMALL_KB")) : 226;   // grids of <= one CTA per SM
-  static const int lim_kb_wide = getenv("CIS_HALO_LIMIT_KB") ? atoi(getenv("CIS_HALO_LIMIT_KB")) : 113;
-  static const int lim_kb_thin = getenv("CIS_HALO_LIMIT_THIN_KB") ? atoi(getenv("CIS_HALO_LIMIT_THIN_KB")) : 113;   // BN <= 32
+  static const int lim_kb_wide = getenv("CIS_HALO_LIMIT_KB") ? atoi(getenv("CIS_HALO_LIMIT_KB")) : 0;
+  static const int lim_kb_thin = getenv("CIS_HALO_LIMIT_THIN_KB") ? atoi(getenv("CIS_HALO_LIMIT_THIN_KB")) : 0;   // BN <= 32
   const int lim_kb = BN <= 32 ? lim_kb_thin : lim_kb_wide;
+  const int lim = lim_kb > 0 ? lim_kb * 1024 : lim_pair;
   const int nsm = cis_num_sms();
-  int limit = (ncta_all > nsm && fixed + 2 * kB <= lim_kb * 1024) ? lim_kb * 1024 : 226 * 1024;
+  int limit = (ncta_all > nsm && fixed + 2 * kB <= lim) ? lim : 226 * 1024;
   if (ncta_all <= nsm && fixed + 2 * kB <= lim_small_kb * 1024) limit = lim_small_kb * 1024;
   while (G > 1 && fixed + 2 * G * kB > limit) --G;
   const int groups = cper * ((nsub > 1 ? 1 : (nst_max + G - 1) / G));   // pipeline stages one CTA walks (grouped: at least one per chunk)

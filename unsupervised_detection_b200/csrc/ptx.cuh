@@ -108,6 +108,24 @@ __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// ---------------------------------------------------------------- per-warpgroup register budgets
+// Every thread of the warpgroup executes the same setmaxnreg at a converged point.  .dec returns registers to the CTA's pool; .inc waits
+// until the pool has them, so the counts of all warpgroups of a CTA must add up to no more than what it was launched with (a CTA of T
+// threads compiled to R registers owns T * R).  R: a multiple of 8 in [24, 256].  Between two setmaxnreg the warps of the warpgroup
+// must synchronise explicitly (named_bar_sync over the warpgroup).
+template <int ID, int N>
+__device__ __forceinline__ void named_bar_sync() {
+  asm volatile("bar.sync %0, %1;" ::"n"(ID), "n"(N) : "memory");
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+
 // ---------------------------------------------------------------- wgmma (sm_90a warpgroup MMA)
 // A warpgroup = 4 consecutive warps starting at a warp index that is a multiple of 4; all 128 threads issue every wgmma.
 __device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
