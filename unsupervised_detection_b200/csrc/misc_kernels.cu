@@ -483,6 +483,23 @@ struct RcArgs {
   CisSrc s[CIS_MAX_SRC];
   int nsrc;
 };
+// The source that concatenated 8-channel chunk ck falls in, with ck made relative to it.  Only constant indices into the argument
+// block: a run-time index into a by-value kernel parameter makes the compiler copy the whole block to a local-memory stack in every
+// thread, which costs more memory traffic than the pass itself.
+template <typename S, typename A>
+__device__ __forceinline__ S concat_src(const A& a, int& ck) {
+  S sd = a.s[0];
+  bool more = true;
+#pragma unroll
+  for (int k = 0; k < CIS_MAX_SRC - 1; ++k) {
+    more = more && k < a.nsrc - 1 && ck >= a.s[k].chunks;
+    if (more) {
+      ck -= a.s[k].chunks;
+      sd = a.s[k + 1];
+    }
+  }
+  return sd;
+}
 __global__ void resize_concat_bf16_kernel(const RcArgs a, int N, int H, int W, bf16* __restrict__ dst, int dp, int dc, int OH, int OW,
                                           int total_chunks) {
   // grid.y = destination row (n, oy), grid.x * 256 threads = (ox, 8-channel chunk) of that row: no 64-bit divisions per thread
@@ -494,15 +511,7 @@ __global__ void resize_concat_bf16_kernel(const RcArgs a, int N, int H, int W, b
   int ck = (int)(t - (unsigned)ox * (unsigned)total_chunks);
   const int n = (int)(blockIdx.y / (unsigned)OH), oy = (int)(blockIdx.y - (unsigned)n * (unsigned)OH);
   const int off = ck * 8;
-  int si = 0;
-  while (si < a.nsrc - 1 && ck >= a.s[si].chunks) {
-    ck -= a.s[si].chunks;
-    ++si;
-  }
-  CisSrc sd = a.s[0];
-  if (si == 1) sd = a.s[1];
-  if (si == 2) sd = a.s[2];
-  if (si == 3) sd = a.s[3];
+  const CisSrc sd = concat_src<CisSrc>(a, ck);
   const int ns = sd.n_mod ? n % sd.n_mod : n;
   const bf16* b = reinterpret_cast<const bf16*>(sd.ptr) + (size_t)ns * H * W * sd.pitch + sd.c_off + ck * 8;
   uint4* o = reinterpret_cast<uint4*>(dst + ((size_t)blockIdx.y * OW + ox) * dp + dc + off);
@@ -536,15 +545,7 @@ __global__ void resize_concat_x2_bf16_kernel(const RcArgs a, int N, int H, int W
   int ck = (int)(t - (unsigned)x * (unsigned)total_chunks);
   const int n = (int)(blockIdx.y / (unsigned)H), y = (int)(blockIdx.y - (unsigned)n * (unsigned)H);
   const int off = ck * 8;
-  int si = 0;
-  while (si < a.nsrc - 1 && ck >= a.s[si].chunks) {
-    ck -= a.s[si].chunks;
-    ++si;
-  }
-  CisSrc sd = a.s[0];
-  if (si == 1) sd = a.s[1];
-  if (si == 2) sd = a.s[2];
-  if (si == 3) sd = a.s[3];
+  const CisSrc sd = concat_src<CisSrc>(a, ck);
   const int ns = sd.n_mod ? n % sd.n_mod : n;
   const bf16* b = reinterpret_cast<const bf16*>(sd.ptr) + (size_t)ns * H * W * sd.pitch + sd.c_off + ck * 8;
   const int x1 = min(x + 1, W - 1), y1 = min(y + 1, H - 1);
@@ -588,15 +589,7 @@ __global__ void resize_concat_bf16_bwd_kernel(const bf16* __restrict__ dd, int d
   int ck = (int)(t - (unsigned)x * (unsigned)total_chunks);
   const int n = (int)(blockIdx.y / (unsigned)H), y = (int)(blockIdx.y - (unsigned)n * (unsigned)H);
   const int off = ck * 8;
-  int si = 0;
-  while (si < a.nsrc - 1 && ck >= a.s[si].chunks) {
-    ck -= a.s[si].chunks;
-    ++si;
-  }
-  RcGrad sd = a.s[0];
-  if (si == 1) sd = a.s[1];
-  if (si == 2) sd = a.s[2];
-  if (si == 3) sd = a.s[3];
+  const RcGrad sd = concat_src<RcGrad>(a, ck);
   if (!sd.want || (sd.n_mod && n >= sd.n_mod)) return;
   const int reps = sd.n_mod ? N / sd.n_mod : 1;
   float acc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tv[8];
@@ -608,6 +601,32 @@ __global__ void resize_concat_bf16_bwd_kernel(const bf16* __restrict__ dd, int d
 #pragma unroll
       for (int e = 0; e < 8; ++e) acc[e] += tv[e];
     }
+    *o = pack8(acc);
+    return;
+  }
+  if (OH == 2 * H && OW == 2 * W && reps == 1) {
+    // exact x2 without replicas (every recover-decoder gradient but the broadcast one): the whole window -- rows 2y-1 (y > 0), 2y, 2y+1,
+    // columns likewise -- is loaded before any arithmetic, then summed row by row, column by column with the weights of the loop below,
+    // so the result is bit-identical to it with nine loads in flight instead of one
+    const int j0 = y > 0 ? 0 : 1, k0 = x > 0 ? 0 : 1;
+    const float wy[3] = {0.5f, 1.f, y == H - 1 ? 1.f : 0.5f}, wx[3] = {0.5f, 1.f, x == W - 1 ? 1.f : 0.5f};
+    uint4 v[3][3];
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (j >= j0 && k >= k0)
+          v[j][k] = *reinterpret_cast<const uint4*>(dd + ((size_t)(n * OH + 2 * y - 1 + j) * OW + 2 * x - 1 + k) * dp + dc + off);
+#pragma unroll
+    for (int j = 0; j < 3; ++j)
+#pragma unroll
+      for (int k = 0; k < 3; ++k)
+        if (j >= j0 && k >= k0) {
+          const float wt = wy[j] * wx[k];
+          unpack8(v[j][k], tv);
+#pragma unroll
+          for (int e = 0; e < 8; ++e) acc[e] += wt * tv[e];
+        }
     *o = pack8(acc);
     return;
   }
@@ -730,7 +749,9 @@ __global__ void resize_f32_bwd_to_bf16_kernel(const float* __restrict__ dd, int 
       const float wt = wy * legacy_w(dx, x, W, sx);
       if (wt == 0.f) continue;
       const float* q = dd + ((size_t)(n * OH + dy) * OW + dx) * C;
-      for (int c = 0; c < C; ++c) a[c] += wt * q[c];
+#pragma unroll
+      for (int c = 0; c < 8; ++c)         // constant indices keep a[] in registers (a run-time index puts it on a local-memory stack)
+        if (c < C) a[c] += wt * q[c];
     }
   }
 #pragma unroll
