@@ -6,14 +6,15 @@ The pairs are the reader's own lists (Davis2016Reader.frame_pairs) for --train_p
 at --test_temporal_shift.  Frames are read unaugmented and uncropped at 384x640, PWC-Net (--flow_ckpt) runs on them in batches of
 --batch_size, and each pair's field is written as one Middlebury .flo file at 384x640, (u, v) = (-flow1, -flow0), the exact inverse
 of the readers' pwc_flow_from_uv, under the name data/davis2016_data_utils.flow_file gives it.  Under torchrun, rank r writes pairs
-r, r + world, ...: the ranks write disjoint files."""
+r, r + world, ...: the ranks write disjoint files.  --use_ema (ema_flags.py) runs the moving average of a pwcnet-<epoch> written by
+train_flow.py --ema_decay."""
 import os
 import sys
 from concurrent.futures import ThreadPoolExecutor
 
 from absl import flags as absl_flags
 
-from unsupervised_detection_b200 import flow_flags
+from unsupervised_detection_b200 import ema_flags, flow_flags  # noqa: F401  (ema_flags defines --use_ema)
 from unsupervised_detection_b200.common_flags import FLAGS
 
 

@@ -445,6 +445,14 @@ int cis_flow_multiscale_loss_bwd(const CisFlowPyr* pyr, const float* gt, int32_t
 int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, const int64_t* seg, int32_t nseg, float decay, const float* lr,
                 float beta1, float beta2, float eps, int64_t* step_state, cis_stream_t stream);
 
+/* ---- exponential moving average of the weights (tf.train.ExponentialMovingAverage(decay, num_updates=t)) ----
+ * t = step_state[0], read when the kernel runs: the step counter the optimiser launch just before this one (cis_clip_adam /
+ * cis_adam_l2) advanced, so CUDA-graph replays need no host.  d = min(decay, (1 + t) / (10 + t)) in fp64, rounded once to fp32; then
+ * over [0, n): shadow = shadow - (shadow - param) * (1 - d), each fp32 operation rounded on its own (no FMA), bit-identical to the
+ * same three numpy fp32 operations.  Padding entries included: zeros in both stay zero.  CIS_ERR_BAD_ARG for a NULL buffer, n < 1 or a
+ * decay outside (0, 1). */
+int cis_ema_update(float* shadow, const float* param, int64_t n, float decay, const int64_t* step_state, cis_stream_t stream);
+
 /* ---- Unsupervised fine-tuning of PWC-Net (occlusion-masked census + second-order smoothness, restated from UnFlow's published
  * recipe as defined in DESIGN.md: not checked against any other implementation) ----
  * img1, img2 = fp32 RGB [B, H, W, 3] in [-0.5, 0.5]; flow = fp32 [2B, H, W, 2] in PWC-Net's order and sign, pixels of H x W: direction

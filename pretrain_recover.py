@@ -1,8 +1,9 @@
 """Pretrains the recover network (the flow inpainter, scope FlownetS) on box-shaped flow occlusions: the recover step of train.py with one
 random box per sample in place of the generator's mask.  Same flags, seed and flag dump as train.py, plus --box_min / --box_max (box side
 range as fractions of each image side), --pretrain_flow (PWC-Net's flow, or the dataset's ground-truth flow: Flying Chairs' own, or the
-supplied flow of a mask dataset under --flow_dir) and --validate (held-out EPE
-every epoch, recover-best on improvement).  It writes <checkpoint_dir>/recover-<epoch> (TF V2 bundle + .pt), which
+supplied flow of a mask dataset under --flow_dir), --validate (held-out EPE
+every epoch, recover-best on improvement) and --ema_decay (a moving average of the recover net's weights, which the validation and
+recover-best use).  It writes <checkpoint_dir>/recover-<epoch> (TF V2 bundle + .pt), which
 `train.py --recover_ckpt=<checkpoint_dir>/recover-<epoch>` then starts adversarial training from.  Under torchrun every rank runs this
 file; only rank 0 prints."""
 import os
@@ -12,11 +13,11 @@ import sys
 from absl import flags as absl_flags
 
 from train import seed_everything
-from unsupervised_detection_b200 import flow_flags
+from unsupervised_detection_b200 import ema_flags, flow_flags
 from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES, define_validate
 from unsupervised_detection_b200.step_graph import box_sides
 
-PRETRAIN_FLAGS = ['box_min', 'box_max', 'pretrain_flow', 'validate', 'flow_dir']
+PRETRAIN_FLAGS = ['box_min', 'box_max', 'pretrain_flow', 'validate', 'flow_dir', 'ema_decay']
 if 'box_min' not in FLAGS:
     absl_flags.DEFINE_float('box_min', 0.1, 'smallest box side, as a fraction of the image side (per axis)')
     absl_flags.DEFINE_float('box_max', 0.5, 'largest box side, as a fraction of the image side (per axis)')
@@ -36,6 +37,7 @@ def check_flags(config):
     if not config.checkpoint_dir:
         raise absl_flags.IllegalFlagValueError('--checkpoint_dir is needed: the recover-<epoch> checkpoints are written there')
     flow_flags.check(config)
+    ema_flags.check(config)
     if config.pretrain_flow == 'gt' and not has_flow(config.dataset, config.flow_dir):
         raise absl_flags.IllegalFlagValueError('--pretrain_flow=gt needs a dataset with ground-truth flow (%s) or --flow_dir with %s, not %s'
                                                % (', '.join(FLOW_DATASETS), ' / '.join(MASK_DATASETS), config.dataset))

@@ -149,7 +149,13 @@ _PROTOS = {
     'cis_warp_costvol_bwd_r': [_p, _i32, _i32, _p, _i32, _i32, _p, _f32, _i32, _i32, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32, _p, _i32, _i32,
                                _p, _i32, _i32, _i32, _p, _p, _p, _i32],
 }
-EXPORTS = sorted(list(_PROTOS) + ['cis_last_error', 'cis_version', 'cis_set_persist_mode', 'cis_crc32c', 'cis_host_resize_bilinear_legacy',
+# The moving average of the weights (ema_flags.py --ema_decay), launched only by the optimiser plans of graphs built with ema_decay > 0.
+# Kept apart from _PROTOS, the entry points of the step as the per-launch census of tests/glue_launch_ref.py covers it: this one's
+# per-launch check is tests/test_ema_gpu.py's (the same harness, launch_suites.walk_plans, with its own reference).
+_EMA_PROTOS = {
+    'cis_ema_update': [_p, _p, _i64, _f32, _p],
+}
+EXPORTS = sorted(list(_PROTOS) + list(_EMA_PROTOS) + ['cis_last_error', 'cis_version', 'cis_set_persist_mode', 'cis_crc32c', 'cis_host_resize_bilinear_legacy',
                                   'cis_host_bgr8_to_rgb_resized', 'cis_conv_s2_phase_plan'])
 
 _lib = None
@@ -175,7 +181,7 @@ def load():
         lib.cis_host_bgr8_to_rgb_resized.restype = C.c_int
         lib.cis_conv_s2_phase_plan.argtypes = [C.POINTER(CisConv), C.POINTER(CisConv), C.POINTER(C.c_int16)]
         lib.cis_conv_s2_phase_plan.restype = C.c_int
-        for name, args in _PROTOS.items():
+        for name, args in list(_PROTOS.items()) + list(_EMA_PROTOS.items()):
             fn = getattr(lib, name)
             fn.argtypes = list(args) + [C.c_void_p]
             fn.restype = C.c_int

@@ -22,6 +22,7 @@ import numpy as np
 
 GEN_SCOPE, REC_SCOPE, PWC_SCOPE = 'MaskNet', 'FlownetS', 'pwcnet'
 GLOBAL_STEP_NAMES = ('train_op/global_step', 'global_step')
+EMA_SUFFIX = '/ExponentialMovingAverage'
 
 
 # creation order of generator_net's layers (models/nets.py:19-37); kept equal to models.nets.GEN_LAYERS by tests/test_tf_bundle.py
@@ -49,7 +50,14 @@ def generator_tf_names(sep='//'):
     return out
 
 
+def ema_name(internal):
+    """The name of a variable's moving average: tf.train.ExponentialMovingAverage's shadow name, `<var>/ExponentialMovingAverage`."""
+    return internal + EMA_SUFFIX
+
+
 def to_tf_name(internal, sep='//', _cache={}):
+    if internal.endswith(EMA_SUFFIX):
+        return to_tf_name(internal[:-len(EMA_SUFFIX)], sep) + EMA_SUFFIX
     if internal.startswith(GEN_SCOPE + '/'):
         if sep not in _cache:
             _cache[sep] = generator_tf_names(sep)

@@ -2119,6 +2119,29 @@ __global__ void adam_l2_kernel(float* __restrict__ param, float* __restrict__ m,
   v[i] = vi;
   param[i] = w - lr_t * mi / (sqrtf(vi) + eps);
 }
+// Moving average of the weights after an optimiser launch (cis_ema_update in cis_b200.h): d from the step counter that launch advanced,
+// every operation rounded on its own (no FMA contraction) so that a numpy fp32 restatement matches bit for bit.  Four elements per
+// thread, one float4 each way when both buffers are 16-byte aligned and the four are in range.
+__global__ void ema_update_kernel(float* __restrict__ shadow, const float* __restrict__ param, size_t n, float decay,
+                                  const long long* __restrict__ step, int vec) {
+  pdl_launch_dependents();
+  pdl_wait();
+  const size_t i0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) * 4;
+  if (i0 >= n) return;
+  const double t = (double)step[0];
+  const float k = __fsub_rn(1.f, (float)fmin((double)decay, (1.0 + t) / (10.0 + t)));
+  if (vec && i0 + 4 <= n) {
+    float4 s = *reinterpret_cast<const float4*>(shadow + i0);
+    const float4 p = *reinterpret_cast<const float4*>(param + i0);
+    s.x = __fsub_rn(s.x, __fmul_rn(__fsub_rn(s.x, p.x), k));
+    s.y = __fsub_rn(s.y, __fmul_rn(__fsub_rn(s.y, p.y), k));
+    s.z = __fsub_rn(s.z, __fmul_rn(__fsub_rn(s.z, p.z), k));
+    s.w = __fsub_rn(s.w, __fmul_rn(__fsub_rn(s.w, p.w), k));
+    *reinterpret_cast<float4*>(shadow + i0) = s;
+    return;
+  }
+  for (size_t i = i0; i < n && i < i0 + 4; ++i) shadow[i] = __fsub_rn(shadow[i], __fmul_rn(__fsub_rn(shadow[i], param[i]), k));
+}
 static int flow_loss_args(const char* what, const CisFlowPyr* pyr, const float* gt, int32_t B, int32_t H, int32_t W, int32_t GH, int32_t GW,
                           float s0, float s1, int32_t robust, float eps, float q, FlowLossArgs& a) {
   if (!pyr || !gt || B < 1 || B > 65535 || H < 64 || W < 64 || H % 64 || W % 64 || GH < 1 || GW < 1 || (robust != 0 && robust != 1))
@@ -2789,6 +2812,13 @@ int cis_adam_l2(float* param, float* m, float* v, const float* grad, int64_t n, 
              (const long long*)step_state);
   CIS_LAUNCH(step_inc_kernel, 1, 1, 0, ST, (long long*)step_state);
   return cis_check_launch("adam_l2");
+}
+int cis_ema_update(float* shadow, const float* param, int64_t n, float decay, const int64_t* step_state, cis_stream_t stream) {
+  if (!shadow || !param || !step_state || n < 1 || !(decay > 0.f && decay < 1.f))
+    return cis_set_error(CIS_ERR_BAD_ARG, "cis_ema_update: bad buffer, size or decay (needs 0 < decay < 1)");
+  const int vec = (((uintptr_t)shadow | (uintptr_t)param) & 15) == 0;
+  CIS_LAUNCH(ema_update_kernel, nblk(((size_t)n + 3) / 4), 256, 0, ST, shadow, param, (size_t)n, decay, (const long long*)step_state, vec);
+  return cis_check_launch("ema_update");
 }
 int cis_unsup_flow_loss(const float* flow, const float* img1, const float* img2, int32_t B, int32_t H, int32_t W, float* warped, float* mask,
                         float* coef, double* scratch, double* out, cis_stream_t stream) {

@@ -4,6 +4,7 @@ Networks are described once (shapes are static), which produces three launch lis
 step and backward for the generator step -- that are then replayed (optionally inside a CUDA graph) every iteration.
 PyTorch only owns device memory and streams here; there is no autograd and no torch compute on the hot path.
 """
+import contextlib
 import ctypes as C
 import dataclasses
 import os
@@ -13,6 +14,7 @@ import torch
 
 from . import _lib
 from ._lib import CisConv, CisWgrad, CisSrc, ACT_NONE, ACT_ELU, ACT_LEAKY
+from .checkpoint.tf_names import ema_name
 
 
 def ru(x, m):
@@ -631,7 +633,8 @@ def merge_parity_launches(descs):
 
 class ParamStore(object):
     """One flat fp32 parameter buffer (+ grad, Adam m/v) per variable scope; names follow the TF variable layout
-    (adversarial_learner.py:211-214 scopes 'MaskNet' / 'FlownetS'; model_pwcnet.py 'pwcnet')."""
+    (adversarial_learner.py:211-214 scopes 'MaskNet' / 'FlownetS'; model_pwcnet.py 'pwcnet').  add_shadow() adds `shadow`, the moving
+    average of `flat` (cis_ema_update), in the same layout."""
 
     def __init__(self, device):
         self.device = device
@@ -639,6 +642,7 @@ class ParamStore(object):
         self.index = {}
         self.size = 0
         self.flat = None
+        self.shadow = None
 
     def declare(self, name, shape, padded=None):
         n = int(np.prod(shape))
@@ -669,20 +673,67 @@ class ParamStore(object):
         _, shape, n, off, _ = self.entries[self.index[name]]
         return getattr(self, which)[off:off + n].view(shape)
 
+    def add_shadow(self):
+        """Allocate `shadow`, initialised from flat (padding included, so padded entries stay 0)."""
+        self.shadow = self.flat.clone()
+
     def load(self, params):
+        """Every variable from params[name]; with a shadow, its moving average from params[ema_name(name)], or from the loaded value
+        when params has none."""
         for name, shape, n, off, _ in self.entries:
             if name not in params:
                 raise KeyError('missing parameter ' + name)
-            t = params[name].detach().to(torch.float32).reshape(-1)
-            if t.numel() != n:
-                raise ValueError('shape mismatch for %s: %d vs %d' % (name, t.numel(), n))
-            self.flat[off:off + n].copy_(t)
+            self.flat[off:off + n].copy_(self._flat_value(params, name, n))
+            if self.shadow is not None:
+                avg = ema_name(name)
+                self.shadow[off:off + n].copy_(self._flat_value(params, avg, n) if avg in params else self.flat[off:off + n])
+
+    @staticmethod
+    def _flat_value(params, name, n):
+        t = params[name].detach().to(torch.float32).reshape(-1)
+        if t.numel() != n:
+            raise ValueError('shape mismatch for %s: %d vs %d' % (name, t.numel(), n))
+        return t
 
     def export(self, which='flat'):
         return {name: getattr(self, which)[off:off + n].view(shape).clone() for name, shape, n, off, _ in self.entries}
 
+    def export_all(self):
+        """export() plus, with a shadow, every moving average under its ema_name: what a checkpoint of this store holds."""
+        out = self.export()
+        if self.shadow is not None:
+            out.update((ema_name(k), v) for k, v in self.export('shadow').items())
+        return out
+
     def real_count(self):
         return sum(e[2] for e in self.entries)
+
+
+def check_ema_decay(decay):
+    """ValueError unless decay is 0 (no moving average) or 0 < decay < 1."""
+    if not (decay == 0 or 0 < decay < 1):
+        raise ValueError('ema_decay must be 0 (off) or in (0, 1), got %r' % (decay,))
+
+
+@contextlib.contextmanager
+def averaged_weights(graph, stores):
+    """Inside the block the flat buffer of each of `stores` holds its moving average (shadow), and graph._dirty makes the graph rebuild
+    its packed bf16 operands from it on first use.  The packs alone would not do: a conv without batch norm reads its bias from flat
+    when it runs.  On exit the live weights are copied back, bit for bit, and the operands marked for a re-pack, so training continues
+    from the live weights.  No stores: nothing changes."""
+    if not stores:
+        yield
+        return
+    live = [s.flat.clone() for s in stores]
+    for s in stores:
+        s.flat.copy_(s.shadow)
+    graph._dirty = True
+    try:
+        yield
+    finally:
+        for s, t in zip(stores, live):
+            s.flat.copy_(t)
+        graph._dirty = True
 
 
 @dataclasses.dataclass(eq=False)

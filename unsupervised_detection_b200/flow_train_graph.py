@@ -33,7 +33,7 @@ import ctypes as C
 import torch
 
 from . import _lib
-from .engine import Act, Builder, ParamStore, Plan
+from .engine import Act, Builder, ParamStore, Plan, averaged_weights, check_ema_decay
 from .step_graph import UploadSlots, capture_plans
 
 LEVELS = (6, 5, 4, 3, 2)                          # level i of the loss kernels is pyramid level LEVELS[i]
@@ -83,13 +83,16 @@ class FlowTrainGraph(object):
     the unsupervised loss; lr, beta1, beta2, adam_eps: TF-Adam.  With loss='unsupervised' the network batch is 2 * batch (forward pairs,
     then backward pairs) and self.flow holds both halves; the ground truth is only read by epe().
     augment: train_step augments each uploaded batch at in_hw before the step (supervised losses only); aug_ranges: a CisFlowAug
-    (flow_aug_ranges(); None = AUG_RANGES); sample_offset: the global index of this rank's first sample (rank * batch under data parallelism)."""
+    (flow_aug_ranges(); None = AUG_RANGES); sample_offset: the global index of this rank's first sample (rank * batch under data parallelism).
+    ema_decay: 0 (the default) keeps no moving average; 0 < ema_decay < 1 gives the store a shadow that one cis_ema_update after
+    cis_adam_l2 updates every step (averaged(), export_params())."""
 
     def __init__(self, H, W, batch, options=None, global_batch=None, device='cuda', in_hw=None, loss='multiscale', alphas=ALPHAS,
                  weight_decay=WEIGHT_DECAY, eps=ROBUST_EPS, q=ROBUST_Q, lr=1e-4, beta1=0.9, beta2=0.999, adam_eps=1e-8, name='pwcnet',
-                 smooth_weight=SMOOTH_WEIGHT, augment=False, aug_ranges=None, sample_offset=0):
+                 smooth_weight=SMOOTH_WEIGHT, augment=False, aug_ranges=None, sample_offset=0, ema_decay=0.0):
         from .models.PWCNet.model_pwcnet import PWCNetBuilder
         check_size(H, W)
+        check_ema_decay(ema_decay)
         if loss not in FLOW_LOSSES:
             raise ValueError('loss must be one of %s, got %r' % (FLOW_LOSSES, loss))
         if len(alphas) != 5:
@@ -175,6 +178,9 @@ class FlowTrainGraph(object):
         self.adam.add('cis_adam_l2', st.flat.data_ptr(), st.m.data_ptr(), st.v.data_ptr(), st.grad.data_ptr(), st.size, self._seg.data_ptr(),
                       len(self.kernel_seg), self.weight_decay, self.lr.data_ptr(), float(beta1), float(beta2), float(adam_eps),
                       self.step_state.data_ptr())
+        if ema_decay:
+            st.add_shadow()
+            self.adam.add('cis_ema_update', st.shadow.data_ptr(), st.flat.data_ptr(), st.size, ema_decay, self.step_state.data_ptr())
         # ---- bf16 operands (forward and data-gradient orientation), after backward planning decided what is needed
         pack = Plan('pack_P')
         for L in layers:
@@ -249,7 +255,13 @@ class FlowTrainGraph(object):
         self._dirty = True
 
     def export_params(self):
-        return self.store.export()
+        """Every variable, and with ema_decay its moving average under its ema_name."""
+        return self.store.export_all()
+
+    def averaged(self):
+        """Context manager: inside it the network runs on its moving average and export_params() holds it under the plain names too; the
+        live weights come back on exit (engine.averaged_weights).  Without averaging, nothing changes."""
+        return averaged_weights(self, [self.store] if self.store.shadow is not None else [])
 
     def set_lr(self, lr):
         """The learning rate of the following optimiser steps (a device value: captured CUDA graphs read it too)."""

@@ -10,6 +10,7 @@ ignored (there is no tf.Session).  Data parallelism (not in the reference): one 
 sharded over ranks and the active network's flat gradient buffer is summed with ONE NCCL all-reduce per step
 (SURVEY.md section 8e); clip / noise test / Adam then run identically on every rank.
 """
+import contextlib
 import math
 import os
 import time
@@ -24,6 +25,7 @@ from ..data.synthetic import SyntheticReader
 from .. import params_init
 from .. import checkpoint as ckpt_io
 from .. import flow_flags                               # defines --flow_dir for every script that drives the learner
+from .. import ema_flags                                # defines --ema_decay likewise
 from .utils.general_utils import compute_all_IoU
 
 
@@ -140,6 +142,15 @@ class AdversarialLearner(object):
             raise ValueError('batch_size must be divisible by the number of ranks')
         self.local_batch = self.config.batch_size // self.world
 
+    def _ema_decay(self):
+        """config.ema_decay: the decay of the weights' moving average, 0 (or absent) = none."""
+        return float(getattr(self.config, 'ema_decay', 0.0) or 0.0)
+
+    def _averaged(self):
+        """With config.ema_decay, graph.averaged(): inside it the trained networks run on their moving averages; else a context that
+        changes nothing."""
+        return self.graph.averaged() if self._ema_decay() else contextlib.nullcontext()
+
     def _cis_graph(self, **kw):
         """CISGraph at img_height x img_width on local_batch frame pairs, with PWC-Net's default options; kw = the graph's own arguments."""
         cfg = self.config
@@ -152,7 +163,7 @@ class AdversarialLearner(object):
         self._init_training_ranks()
         self.load_training_data()
         self.graph = self._cis_graph(global_batch=cfg.batch_size, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, train=True,
-                                     masks='generator', flow_source=self._flow_source())
+                                     masks='generator', flow_source=self._flow_source(), ema_decay=self._ema_decay())
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self.val_steps_per_epoch = int(np.ceil(float(self.num_samples_val) / cfg.batch_size))
         self._init_params()
@@ -203,6 +214,8 @@ class AdversarialLearner(object):
             # in the reference graph only through flow_saver, so it is optional here
             pr, gs = self._read_ckpt(ck, self._names('MaskNet', 'FlownetS'))
             p.update(pr)
+            if self._ema_decay():       # the moving averages, when the checkpoint has them; the graph starts the others from pr
+                p.update(self._read_ckpt(ck, [ckpt_io.ema_name(n) for n in self._names('MaskNet', 'FlownetS')], strict=False)[0])
             p.update(self._read_ckpt(ck, self._names('pwcnet'), strict=False)[0])
             self.global_step = int(gs or 0)
             print("Resumed training from model {}".format(ck))
@@ -220,10 +233,26 @@ class AdversarialLearner(object):
         if fc.startswith('synthetic'):
             return params_init.init_pwcnet(self.graph.pwc_store.entries)
         if self._is_ckpt(fc):
-            p = self._read_ckpt(fc, self._names('pwcnet'))[0]                    # flow_saver.restore, adversarial_learner.py:339-341
+            if self._use_ema():                                                 # a pwcnet-<epoch> of train_flow.py --ema_decay
+                p = self._read_averages(fc, self._names('pwcnet'))
+            else:
+                p = self._read_ckpt(fc, self._names('pwcnet'))[0]                # flow_saver.restore, adversarial_learner.py:339-341
             print("Flow net loaded from {}".format(fc))
             return p
         raise IOError("Could not find flow ckpt file. Aborting.")              # adversarial_learner.py:343
+
+    def _read_averages(self, path, names):
+        """--use_ema: the moving averages <var>/ExponentialMovingAverage of `names` in checkpoint `path` -> {var: tensor}; KeyError naming
+        the file and the first variable without one."""
+        got = self._read_ckpt(path, [ckpt_io.ema_name(n) for n in names], strict=False)[0]
+        miss = [n for n in names if ckpt_io.ema_name(n) not in got]
+        if miss:
+            raise KeyError('--use_ema: checkpoint %s holds no moving average of %d of %d variables, first %s (write it with --ema_decay)'
+                           % (path, len(miss), len(names), ckpt_io.ema_name(miss[0])))
+        return {n: got[ckpt_io.ema_name(n)] for n in names}
+
+    def _use_ema(self):
+        return bool(getattr(self.config, 'use_ema', False))
 
     @staticmethod
     def _latest_checkpoint(d):
@@ -250,7 +279,7 @@ class AdversarialLearner(object):
         state file.  train.py --recover_ckpt=<dir>/recover-<epoch> and a TF recover_saver.restore both read it.  epoch='best' writes
         recover-best (the lowest validation EPE so far), which later saves never delete."""
         base = 'recover-%s' % epoch
-        self._write_checkpoint(checkpoint_dir, base, self.graph.rec_store.export, None, "recover net to {}/{}".format(checkpoint_dir, base))
+        self._write_checkpoint(checkpoint_dir, base, self.graph.rec_store.export_all, None, "recover net to {}/{}".format(checkpoint_dir, base))
 
     def _write_checkpoint(self, checkpoint_dir, base, export, bundle_step, what):
         """On rank 0 only: prints ' [*] Saving <what>' and writes host copies of the tensors export() returns as <base>.pt + the <base>
@@ -435,21 +464,23 @@ class AdversarialLearner(object):
     def _save_and_validate(self, epoch, save, validate):
         """The epoch end of pretrain_recover and train_flow: save(checkpoint_dir, epoch) every save_freq epochs and after the last one.
         Then, with config.validate, validate() -> (value, text, tag), lower is better: rank 0 prints 'Epoch [e] ' + text and writes
-        value under tag at step epoch, and save(checkpoint_dir, 'best') runs whenever value is strictly below min_val_epe."""
+        value under tag at step epoch, and save(checkpoint_dir, 'best') runs whenever value is strictly below min_val_epe.  With
+        config.ema_decay the validation and the best checkpoint see the moving averages (graph.averaged())."""
         cfg = self.config
         if epoch % cfg.save_freq == 0 or epoch == cfg.max_epochs:
             save(cfg.checkpoint_dir, epoch)
         if not getattr(cfg, 'validate', False):
             return
-        value, text, tag = validate()
-        if self.rank == 0:
-            print("Epoch [{}] {}".format(epoch, text))
-            if self.summary_writer is not None:
-                self.summary_writer.add_scalar(tag, value)
-                self.summary_writer.flush_step(epoch)
-        if value < self.min_val_epe:                # the same all-reduced value on every rank
-            self.min_val_epe = value
-            save(cfg.checkpoint_dir, 'best')
+        with self._averaged():
+            value, text, tag = validate()
+            if self.rank == 0:
+                print("Epoch [{}] {}".format(epoch, text))
+                if self.summary_writer is not None:
+                    self.summary_writer.add_scalar(tag, value)
+                    self.summary_writer.flush_step(epoch)
+            if value < self.min_val_epe:                # the same all-reduced value on every rank
+                self.min_val_epe = value
+                save(cfg.checkpoint_dir, 'best')
 
     def train(self, config):
         """adversarial_learner.py:312-420 in _epoch_loop.  step() decides for itself when to fetch the losses and writes its summaries;
@@ -466,7 +497,14 @@ class AdversarialLearner(object):
             banner="Training completed successfully")
 
     def epoch_end_callback(self, sess, sv, epoch_num):
-        """adversarial_learner.py:422-448: validation IoU, save best / every save_freq epochs."""
+        """adversarial_learner.py:422-448: validation IoU, save best / every save_freq epochs.  With config.ema_decay the validation and
+        model.best see the moving averages (CISGraph.averaged()); model-<epoch> holds the live weights and the averages."""
+        with self._averaged():
+            self._validate_iou(sess, epoch_num)
+        if epoch_num % self.config.save_freq == 0:
+            self.save(sess, self.config.checkpoint_dir, epoch_num)
+
+    def _validate_iou(self, sess, epoch_num):
         validation_iou = 0.0
         vr = self.val_reader or self.reader
         for _ in range(self.val_steps_per_epoch):
@@ -492,8 +530,6 @@ class AdversarialLearner(object):
         if validation_iou > self.min_val_iou:
             self.save(sess, self.config.checkpoint_dir, 'best')
             self.min_val_iou = validation_iou
-        if epoch_num % self.config.save_freq == 0:
-            self.save(sess, self.config.checkpoint_dir, epoch_num)
 
     # ------------------------------------------------------------------------------------------------ recover-net pretraining
     def build_pretrain_graph(self):
@@ -516,7 +552,7 @@ class AdversarialLearner(object):
         # sample_offset: sample b of rank r is global sample r * local_batch + b, so a DP job draws the boxes of one GPU running the global batch
         self.graph = self._cis_graph(global_batch=cfg.batch_size, cbn=cfg.cbn, epsilon=cfg.epsilon, beta1=cfg.beta1, train=True,
                                      masks='boxes', box=box, sample_offset=self.rank * self.local_batch,
-                                     flow_source='input' if gt else 'pwc')
+                                     flow_source='input' if gt else 'pwc', ema_decay=self._ema_decay())
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         self._init_params()
 
@@ -656,6 +692,11 @@ class AdversarialLearner(object):
             p = params_init.init_recover()          # the mask path does not read the recover net; restored when present
             p.update(self._read_ckpt(ckpt_file, self._names('MaskNet', 'pwcnet'))[0])
             p.update(self._read_ckpt(ckpt_file, self._names('FlownetS'), strict=False)[0])
+            if self._use_ema():
+                # the averages of the adversarially trained networks; PWC-Net is frozen there and has none
+                p.update(self._read_averages(ckpt_file, self._names('MaskNet')))
+                avg = self._read_ckpt(ckpt_file, [ckpt_io.ema_name(n) for n in self._names('FlownetS')], strict=False)[0]
+                p.update({n: avg[ckpt_io.ema_name(n)] for n in self._names('FlownetS') if ckpt_io.ema_name(n) in avg})
         else:
             raise IOError("Checkpoint file not found")                         # test_generator.py:58
         self.graph.load_params(p)

@@ -49,7 +49,8 @@ class FlowLearner(AdversarialLearner):
                                     global_batch=cfg.batch_size, device=self.device, in_hw=(PWC_H, PWC_W),
                                     loss=loss, weight_decay=getattr(cfg, 'weight_decay', 4e-4),
                                     lr=self._rate(1), beta1=cfg.beta1, smooth_weight=getattr(cfg, 'smooth_weight', 3.0),
-                                    augment=getattr(cfg, 'flow_aug', False), sample_offset=self.rank * self.local_batch)
+                                    augment=getattr(cfg, 'flow_aug', False), sample_offset=self.rank * self.local_batch,
+                                    ema_decay=self._ema_decay())
         self._lr = self._rate(1)
         self.train_steps_per_epoch = int(math.ceil(cfg.num_samples_train / cfg.batch_size))
         names = [e[0] for e in self.graph.store.entries]
@@ -95,7 +96,8 @@ class FlowLearner(AdversarialLearner):
 
     def save_flow(self, checkpoint_dir, epoch):
         """`pwcnet-<epoch>`: a TF V2 bundle of the pwcnet/* variables only (no global_step, no Adam slots) plus the same tensors as a
-        native `.pt`, and the `checkpoint` state file.  epoch='best' writes pwcnet-best (the lowest validation EPE so far)."""
+        native `.pt`, and the `checkpoint` state file.  epoch='best' writes pwcnet-best (the lowest validation EPE so far).  With
+        --ema_decay each variable's moving average is there too, as <var>/ExponentialMovingAverage."""
         base = 'pwcnet-%s' % epoch
         self._write_checkpoint(checkpoint_dir, base, self.graph.export_params, None, "PWC-Net to {}/{}".format(checkpoint_dir, base))
 

@@ -9,7 +9,7 @@ With flow_source='input' a supplied flow field replaces PWC-Net, for either mask
 import torch
 
 from . import _lib
-from .engine import Builder, ParamStore, Plan, Act
+from .engine import Builder, ParamStore, Plan, Act, averaged_weights, check_ema_decay
 from .models.nets import GeneratorNet, RecoverNet
 from .models.PWCNet.model_pwcnet import PWCNetBuilder
 
@@ -106,7 +106,7 @@ class UploadSlots(object):
 class CISGraph(object):
     def __init__(self, img_height, img_width, batch, device='cuda', global_batch=None, flow_normalizer=80.0, cbn=0.5, epsilon=75.0,
                  beta1=0.9, with_pwc=True, train=True, pwc_hw=(PWC_H, PWC_W), seed=8964, pwc_options=None, masks=None, box=None,
-                 sample_offset=0, flow_source='pwc'):
+                 sample_offset=0, flow_source='pwc', ema_decay=0.0):
         """pwc_options: PWC-Net options (the reference's option keys; None = model_pwcnet._DEFAULT_PWCNET_TEST_OPTIONS).
         masks: 'generator' (the adversarial graph; None means it on PWC-Net's flow) or 'boxes' (pretraining of the recover net): one
         random box per sample, drawn on the device by cis_box_masks, replaces the generator's mask; the generator is neither run nor trained and only the recover step
@@ -119,7 +119,11 @@ class CISGraph(object):
         after take_stage is the 'pwc' graph's, and the stage, the pipelined schedule and the batch hand-over work on the pair
         (img1, flow_full) in place of (img1, img2).  Both mask sources and train=True / False accept it, named explicitly: supplied
         flow serves the recover-net pretraining (masks='boxes') as well as the adversarial graph (masks='generator'), and a graph that
-        silently became the other one would train the wrong network.  with_pwc=False does not accept it."""
+        silently became the other one would train the wrong network.  with_pwc=False does not accept it.
+        ema_decay: 0 (the default) keeps no moving average.  0 < ema_decay < 1 (train=True): every trained store gets a shadow, and one
+        cis_ema_update follows the optimiser launch of each step on the store that step trained; averaged() runs the graph on the
+        averages and export_params() adds them under their checkpoint names."""
+        check_ema_decay(ema_decay)
         if masks is None:
             if flow_source == 'input':
                 raise ValueError("flow_source='input' needs the mask source named: masks='generator' or masks='boxes'")
@@ -284,6 +288,9 @@ class CISGraph(object):
                     ad.add('cis_grad_avg_abs', store.grad.data_ptr(), self.seg.data_ptr(), len(store.seg_pairs), self.avg_abs.data_ptr())
                 ad.add('cis_clip_adam', store.flat.data_ptr(), store.m.data_ptr(), store.v.data_ptr(), store.grad.data_ptr(), store.size, 1.0,
                        0.2, 1e-4, beta1, 0.999, 1e-8, self.step_state.data_ptr(), self.avg_abs.data_ptr(), 1 if mode == 'G' else 0, seed)
+                if ema_decay:
+                    store.add_shadow()
+                    ad.add('cis_ema_update', store.shadow.data_ptr(), store.flat.data_ptr(), store.size, ema_decay, self.step_state.data_ptr())
                 self.adam[mode] = ad
         # packing of the trainable nets (forward + data-gradient orientation), after backward planning decided what is needed
         self.pack_gen, self.pack_rec = Plan('pack_gen'), Plan('pack_rec')
@@ -320,12 +327,18 @@ class CISGraph(object):
             self._pwc_packed = False
 
     def export_params(self):
+        """Every variable, and the moving average of every averaged one under its ema_name."""
         out = {}
-        out.update(self.gen_store.export())
-        out.update(self.rec_store.export())
+        out.update(self.gen_store.export_all())
+        out.update(self.rec_store.export_all())
         if self.with_pwc:
             out.update(self.pwc_store.export())
         return out
+
+    def averaged(self):
+        """Context manager: inside it the averaged networks run on their moving averages, and export_params() holds those averages
+        under the plain names too; the live weights come back on exit (engine.averaged_weights).  Without averaging, nothing changes."""
+        return averaged_weights(self, [s for s in (self.gen_store, self.rec_store) if s.shadow is not None])
 
     def param_count(self):
         return self.gen_store.real_count() + self.rec_store.real_count() + (self.pwc_store.real_count() if self.with_pwc else 0)
