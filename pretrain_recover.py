@@ -3,7 +3,7 @@ random box per sample in place of the generator's mask.  Same flags, seed and fl
 range as fractions of each image side), --pretrain_flow (PWC-Net's flow, or the dataset's ground-truth flow: Flying Chairs' own, or the
 supplied flow of a mask dataset under --flow_dir), --validate (held-out EPE
 every epoch, recover-best on improvement) and --ema_decay (a moving average of the recover net's weights, which the validation and
-recover-best use).  It writes <checkpoint_dir>/recover-<epoch> (TF V2 bundle + .pt), which
+recover-best use) and --resumable (continue an interrupted run from its last epoch).  It writes <checkpoint_dir>/recover-<epoch> (TF V2 bundle + .pt), which
 `train.py --recover_ckpt=<checkpoint_dir>/recover-<epoch>` then starts adversarial training from.  Under torchrun every rank runs this
 file; only rank 0 prints."""
 import os
@@ -13,11 +13,11 @@ import sys
 from absl import flags as absl_flags
 
 from train import seed_everything
-from unsupervised_detection_b200 import ema_flags, flow_flags
+from unsupervised_detection_b200 import ema_flags, flow_flags, resume_flags
 from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES, define_validate
 from unsupervised_detection_b200.step_graph import box_sides
 
-PRETRAIN_FLAGS = ['box_min', 'box_max', 'pretrain_flow', 'validate', 'flow_dir', 'ema_decay']
+PRETRAIN_FLAGS = ['box_min', 'box_max', 'pretrain_flow', 'validate', 'flow_dir', 'ema_decay', 'resumable']
 if 'box_min' not in FLAGS:
     absl_flags.DEFINE_float('box_min', 0.1, 'smallest box side, as a fraction of the image side (per axis)')
     absl_flags.DEFINE_float('box_max', 0.5, 'largest box side, as a fraction of the image side (per axis)')
@@ -38,6 +38,7 @@ def check_flags(config):
         raise absl_flags.IllegalFlagValueError('--checkpoint_dir is needed: the recover-<epoch> checkpoints are written there')
     flow_flags.check(config)
     ema_flags.check(config)
+    resume_flags.check(config)
     if config.pretrain_flow == 'gt' and not has_flow(config.dataset, config.flow_dir):
         raise absl_flags.IllegalFlagValueError('--pretrain_flow=gt needs a dataset with ground-truth flow (%s) or --flow_dir with %s, not %s'
                                                % (', '.join(FLOW_DATASETS), ' / '.join(MASK_DATASETS), config.dataset))
@@ -66,7 +67,10 @@ def main(argv):
         check_flags(FLAGS)
     except absl_flags.Error as err:
         sys.exit('%s\nUsage: %s ARGS\n%s' % (err, argv[0], FLAGS))
-    run(FLAGS)
+    try:
+        run(FLAGS)
+    except resume_flags.StateMismatch as err:          # the training state in --checkpoint_dir belongs to another run
+        sys.exit('%s\nUsage: %s ARGS\n%s' % (err, argv[0], FLAGS))
 
 
 if __name__ == "__main__":

@@ -5,7 +5,7 @@ unsupervised_detection_b200/flow_train_graph.py.  Same flags, seed and flag dump
 which the rate halves), --weight_decay (L2 on the conv kernels) and --validate (every epoch: the end-point error on Flying Chairs' val split,
 or the mean unsupervised objective over a video dataset's val pairs; pwcnet-best on improvement) and --flow_aug (random affine and
 photometric augmentation of every supervised training batch on the device, the ground-truth flow transformed to match) and --ema_decay (a moving average of
-the weights, which the validation and pwcnet-best use).  --flow_ckpt, when given, is the starting
+the weights, which the validation and pwcnet-best use) and --resumable (continue an interrupted run from its last epoch).  --flow_ckpt, when given, is the starting
 point (fine-tuning); otherwise training starts from params_init.init_pwcnet.  The network input is img_height x img_width (multiples of
 64, at least 128).
 
@@ -22,10 +22,10 @@ import sys
 from absl import flags as absl_flags
 
 from train import seed_everything
-from unsupervised_detection_b200 import ema_flags, flow_flags
+from unsupervised_detection_b200 import ema_flags, flow_flags, resume_flags
 from unsupervised_detection_b200.common_flags import FLAGS, FLAG_NAMES, define_validate
 
-TRAIN_FLOW_FLAGS = ['flow_loss', 'smooth_weight', 'learning_rate', 'lr_boundaries', 'weight_decay', 'validate', 'flow_aug', 'ema_decay']
+TRAIN_FLOW_FLAGS = ['flow_loss', 'smooth_weight', 'learning_rate', 'lr_boundaries', 'weight_decay', 'validate', 'flow_aug', 'ema_decay', 'resumable']
 UNSUP_DATASETS = ('FLYINGCHAIRS', 'DAVIS2016', 'FBMS', 'SEGTRACK')
 if 'flow_loss' not in FLAGS:
     absl_flags.DEFINE_enum('flow_loss', 'multiscale', ['multiscale', 'robust', 'unsupervised'], "flow loss: 'multiscale' = ||d||_2 to "
@@ -75,6 +75,7 @@ def check_flags(config):
         raise absl_flags.IllegalFlagValueError('--img_height / --img_width: %s' % err)
     flow_flags.check(config)
     ema_flags.check(config)
+    resume_flags.check(config)
     if not config.learning_rate > 0 or config.weight_decay < 0:
         raise absl_flags.IllegalFlagValueError('--learning_rate must be > 0 and --weight_decay >= 0')
     lr_boundaries(config)
@@ -110,7 +111,10 @@ def main(argv):
         check_flags(FLAGS)
     except absl_flags.Error as err:
         sys.exit('%s\nUsage: %s ARGS\n%s' % (err, argv[0], FLAGS))
-    run(FLAGS)
+    try:
+        run(FLAGS)
+    except resume_flags.StateMismatch as err:          # the training state in --checkpoint_dir belongs to another run
+        sys.exit('%s\nUsage: %s ARGS\n%s' % (err, argv[0], FLAGS))
 
 
 if __name__ == "__main__":

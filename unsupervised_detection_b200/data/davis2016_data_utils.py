@@ -158,7 +158,7 @@ class _Iter(object):
     `dataset.prefetch(3 * batch_size)`, davis2016_data_utils.py:226): host decoding / augmentation of the next batches overlaps the
     GPU step that consumes the current one.  For a constant batch size, order and content are the same with or without prefetching
     (one producer, FIFO queue, iterator-private random stream); changing the batch size restarts the producer and drops what it had
-    decoded ahead."""
+    decoded ahead.  state() / restore() save and resume the stream at the consumer's position, which resumable training stores."""
 
     def __init__(self, reader, pairs, train, shuffle, num_threads, prefetch=0):
         # Snapshot of the reader as it is NOW (file lists, temporal shift, crops): a later image_inputs()/test_inputs() call on the
@@ -175,6 +175,22 @@ class _Iter(object):
         self.prefetch = prefetch
         self._q = self._thread = self._qn = None
         self._stop = threading.Event()
+        self._at = self._position()                 # state(): the stream position of the next batch batch() returns
+
+    def _position(self):
+        return {'rng': self.rng.getstate(), 'pos': self.pos, 'order': list(self.order)}
+
+    def state(self):
+        """The stream position of the next batch batch() returns (not of what the background producer has drawn ahead): random state,
+        list position and order.  restore(state()) on an iterator over the same pairs makes it return the same batches from there."""
+        return self._at
+
+    def restore(self, state):
+        """Continue from a position state() returned; batches decoded ahead are dropped."""
+        self.close()
+        self.rng.setstate(state['rng'])
+        self.pos, self.order = state['pos'], list(state['order'])
+        self._at = self._position()
 
     def shard(self, rank, world, global_batch):
         """Data-parallel evaluation: global batch k is samples [k*B, (k+1)*B) of the ordered list (wrapping at the end, like
@@ -189,6 +205,7 @@ class _Iter(object):
         self.close()
         self.order = [(k * global_batch + rank * lb + j) % n for k in range(steps) for j in range(lb)]
         self.pos = 0
+        self._at = self._position()
         return self
 
     def _name_of(self, pair):
@@ -204,18 +221,21 @@ class _Iter(object):
         return i
 
     def _submit(self, n):
-        """Draw the next n samples (indices + augmentation seeds, in stream order) and hand them to the thread pool."""
+        """Draw the next n samples (indices + augmentation seeds, in stream order) and hand them to the thread pool -> (their futures, the
+        stream position after the draws)."""
         idx = [self._next_index() for _ in range(n)]
         fn = self.view._train_sample if self.train else self.view._test_sample
         seeds = [self.rng.getrandbits(32) for _ in idx]
-        return [self.pool.submit(fn, self.pairs[i], sd) for i, sd in zip(idx, seeds)]
+        return [self.pool.submit(fn, self.pairs[i], sd) for i, sd in zip(idx, seeds)], self._position()
 
     @staticmethod
-    def _collect(futs):
-        """-> [img1, img2, seg1, fnames] (+ [flow] when the samples carry a supplied flow field as a fifth element)."""
+    def _collect(drawn):
+        """_submit's (futures, position) -> ([img1, img2, seg1, fnames] (+ [flow] when the samples carry a supplied flow field as a fifth
+        element), position)."""
+        futs, at = drawn
         res = [f.result() for f in futs]
         out = [torch.from_numpy(np.stack([r[k] for r in res])) for k in range(3)] + [[r[3] for r in res]]
-        return out + [torch.from_numpy(np.stack([r[4] for r in res]))] if len(res[0]) > 4 else out
+        return (out + [torch.from_numpy(np.stack([r[4] for r in res]))] if len(res[0]) > 4 else out), at
 
     def _make(self, n):
         return self._collect(self._submit(n))
@@ -237,7 +257,7 @@ class _Iter(object):
                     continue
             if isinstance(item, Exception):
                 break
-        for futs in inflight:
+        for futs, _ in inflight:
             for f in futs:
                 f.cancel()
 
@@ -262,12 +282,13 @@ class _Iter(object):
                 self._q, self._qn = queue.Queue(maxsize=self.prefetch), n
                 self._thread = threading.Thread(target=self._producer, args=(n, self._q, self._stop), daemon=True)
                 self._thread.start()
-            out = self._q.get()
-            if isinstance(out, Exception):
+            item = self._q.get()
+            if isinstance(item, Exception):
                 self.close()
-                raise out
+                raise item
+            out, self._at = item
         else:
-            out = self._make(n)
+            out, self._at = self._make(n)
         ts = out[:3] + out[4:]
         if pinned and torch.cuda.is_available():
             ts = [t.pin_memory() for t in ts]

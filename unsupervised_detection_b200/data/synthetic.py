@@ -11,6 +11,13 @@ class SyntheticReader(object):
         self.gen = torch.Generator().manual_seed(seed)
         self.val_samples = num_val
 
+    def state(self):
+        """The position of the next batch: the generator's state.  restore(state()) makes the following batches repeat."""
+        return self.gen.get_state()
+
+    def restore(self, state):
+        self.gen.set_state(state)
+
     def _smooth(self, n, c, amp, div=32):
         lo = torch.randn(n, c, max(self.h // div, 2), max(self.w // div, 2), generator=self.gen)
         return F.interpolate(lo, size=(self.h, self.w), mode='bicubic', align_corners=False) * amp

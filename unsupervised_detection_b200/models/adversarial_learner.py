@@ -26,6 +26,9 @@ from .. import params_init
 from .. import checkpoint as ckpt_io
 from .. import flow_flags                               # defines --flow_dir for every script that drives the learner
 from .. import ema_flags                                # defines --ema_decay likewise
+from .. import resume_flags                             # and --resumable
+from .. import train_state
+from ..checkpoint.tf_bundle import crc32c
 from .utils.general_utils import compute_all_IoU
 
 
@@ -63,6 +66,8 @@ class AdversarialLearner(object):
     val_graph = None                                    # forward-only boxes graph of validate_recover, built on first use
     min_val_epe = math.inf
     _summary_img2 = None                                # frame 2 of the last summary step's batch (an input-flow graph has no img2)
+    _kind = None                                        # the training script, train_state.KINDS: what a --resumable state file belongs to
+    _frozen = None                                      # CRC-32C of the frozen PWC-Net parameters (--resumable)
 
     # ------------------------------------------------------------------------------------------------ data
     def load_training_data(self):
@@ -426,16 +431,30 @@ class AdversarialLearner(object):
         step(batch, next_batch, fetch) -> result.  fetch is True every summary_freq steps (the same decision on every rank); then rank 0
         prints 'Epoch: [e] [s/steps] time: t/it ' + text and writes the scalars, if any, at the result's global_step, where
         progress(result) -> (text, {tag: scalar}).  Each epoch ends with epoch_end(epoch); after the last one rank 0 prints `banner`
-        between rules and the loop returns."""
+        between rules and the loop returns.  With config.resumable the loop continues after the epoch of the newest training state
+        (_resume), with the step count and reader positions it left, and every epoch end writes one (_save_train_state)."""
         cfg, steps_per_epoch = self.config, self.train_steps_per_epoch
+        resumable = getattr(cfg, 'resumable', False)
+        done, readers = self._resume() if resumable else (0, None)
+        if done >= cfg.max_epochs:
+            if self.rank == 0:
+                print("The training state of epoch {} reaches --max_epochs={}: training is complete".format(done, cfg.max_epochs))
+            return
         if self.rank == 0:
             for line in header:
                 print(line)
                 print("-------------------------------------")
         w = self.collect_summaries()
+        if readers is not None:
+            self.reader.restore(readers['train'])
         batch = self.reader.batch(self.local_batch)
-        for k in count(start=1):
+        if readers is not None:
+            self.reader.restore(readers['train_now'])
+            if self.val_reader is not None:
+                self.val_reader.restore(readers['val'])
+        for k in count(start=done * steps_per_epoch + 1):
             start_time = time.time()
+            pending = self.reader.state() if resumable else None    # where `nxt` starts: the epoch's first batch still to train on
             # the next batch (already decoded by the reader's background prefetch) is copied to the device on the side stream while this
             # step computes -- the same step(batch, next_batch=...) pattern bench.py's end-to-end arm measures
             nxt = self.reader.batch(self.local_batch)
@@ -454,12 +473,79 @@ class AdversarialLearner(object):
             if k % steps_per_epoch == 0:
                 epoch = k // steps_per_epoch
                 epoch_end(epoch)
+                if resumable:
+                    self._save_train_state(epoch, pending)
                 if epoch == cfg.max_epochs:
                     if self.rank == 0:
                         print("-------------------------------")
                         print(banner)
                         print("-------------------------------")
                     return
+
+    # ------------------------------------------------------------------------------------------------ --resumable
+    def _trained_stores(self):
+        """{scope: ParamStore} of the networks the run trains."""
+        g = self.graph
+        if self._kind == 'flow':
+            return {'pwcnet': g.store}
+        if self._kind == 'pretrain_recover':
+            return {'FlownetS': g.rec_store}
+        return {'MaskNet': g.gen_store, 'FlownetS': g.rec_store}
+
+    def _frozen_crc(self):
+        """CRC-32C of the frozen PWC-Net parameters the graph reads; None when it reads none (PWC-Net training, supplied or ground-truth
+        flow)."""
+        g = self.graph
+        if self._kind == 'flow' or g.flow_source == 'input':
+            return None
+        return crc32c(g.pwc_store.flat.cpu().numpy())
+
+    def _resume(self):
+        """--resumable: loads the newest train_state file of checkpoint_dir into the built graph and the learner (weights, Adam moments,
+        averages, step counter, counters) -> (the epoch it ends, this rank's reader positions); (0, None) without one.  StateMismatch
+        when the file belongs to another run (train_state.check)."""
+        cfg = self.config
+        self._frozen = self._frozen_crc()
+        file = train_state.newest(cfg.checkpoint_dir)
+        if file is None:
+            if self.rank == 0:
+                print("No training state in {}: training starts from scratch".format(cfg.checkpoint_dir))
+            return 0, None
+        st = train_state.load(file)
+        train_state.check(st, file, self._kind, self.world, train_state.trajectory(cfg), self._frozen)
+        for scope, store in self._trained_stores().items():
+            for which, t in st['stores'][scope].items():
+                getattr(store, which).copy_(t)
+        self.graph._dirty = True                        # re-pack the bf16 operands from the restored weights, as load_params does
+        self.graph.step_state.copy_(st['step_state'])
+        self.global_step, self._step = st['global_step'], st['step']
+        self.min_val_iou, self.min_val_epe = st['min_val_iou'], st['min_val_epe']
+        if self.rank == 0:
+            print("Resumed training state from {} (epoch {})".format(file, st['epoch']))
+        return st['epoch'], st['readers'][self.rank]
+
+    def _save_train_state(self, epoch, pending):
+        """--resumable, at the end of `epoch` (after its checkpoints and validation, outside graph.averaged()): gathers every rank's
+        reader positions (`pending` = the training reader's position at the next batch to train on) and rank 0 writes the state file."""
+        cfg, g = self.config, self.graph
+        readers = {'train': pending, 'train_now': self.reader.state(),
+                   'val': self.val_reader.state() if self.val_reader is not None else None}
+        d = _dist()
+        if d is not None and self.world > 1:
+            every = [None] * self.world
+            d.all_gather_object(every, readers)
+        else:
+            every = [readers]
+        if self.rank != 0:
+            return
+        if torch.cuda.is_available():
+            torch.cuda.synchronize()
+        stores = {scope: {which: getattr(s, which).cpu() for which in ('flat', 'm', 'v', 'shadow') if getattr(s, which) is not None}
+                  for scope, s in self._trained_stores().items()}
+        st = dict(format=train_state.FORMAT, kind=self._kind, epoch=epoch, world=self.world, flags=train_state.trajectory(cfg),
+                  frozen_crc=self._frozen, global_step=self.global_step, step=self._step, min_val_iou=self.min_val_iou,
+                  min_val_epe=self.min_val_epe, stores=stores, step_state=g.step_state.cpu(), readers=every)
+        print(" [*] Saving training state to " + train_state.write(cfg.checkpoint_dir, st))
 
     def _save_and_validate(self, epoch, save, validate):
         """The epoch end of pretrain_recover and train_flow: save(checkpoint_dir, epoch) every save_freq epochs and after the last one.
@@ -486,6 +572,7 @@ class AdversarialLearner(object):
         """adversarial_learner.py:312-420 in _epoch_loop.  step() decides for itself when to fetch the losses and writes its summaries;
         every epoch ends with epoch_end_callback, which saves model-<epoch> every save_freq epochs (not after the last one)."""
         self.config = config
+        self._kind = 'adversarial'
         self.build_train_graph()
         self.min_val_iou = -1.0e12
         self._epoch_loop(
@@ -586,6 +673,7 @@ class AdversarialLearner(object):
         split, logged as the EPE inside the boxes and kept at its lowest in recover-best.  --flow_ckpt is mandatory unless
         pretrain_flow=gt, --recover_ckpt gives the starting weights (else the reference's initialisation)."""
         self.config = config
+        self._kind = 'pretrain_recover'
         self.build_pretrain_graph()
 
         def validate():

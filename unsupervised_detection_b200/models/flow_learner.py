@@ -64,6 +64,13 @@ class FlowLearner(AdversarialLearner):
             p = params_init.init_pwcnet(self.graph.store.entries)
         self.graph.load_params(p)
 
+    def _resume(self):
+        """AdversarialLearner._resume, then the learning rate of the next update."""
+        out = super()._resume()
+        self._lr = self._rate(self.global_step + 1)
+        self.graph.set_lr(self._lr)
+        return out
+
     def _rate(self, step):
         cfg = self.config
         return learning_rate_at(step, getattr(cfg, 'learning_rate', 1e-4), [int(b) for b in getattr(cfg, 'lr_boundaries', None) or ()])
@@ -107,6 +114,7 @@ class FlowLearner(AdversarialLearner):
         Chairs validate_flow(), logged as `Validation EPE (flow)`; on a mask dataset validate_unsup(), `Validation unsupervised flow
         loss`."""
         self.config = config
+        self._kind = 'flow'
         self.build_flow_graph()
         g = self.graph
 
